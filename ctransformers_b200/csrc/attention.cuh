@@ -6,6 +6,9 @@
 //               llama.cpp:2337-2400, ggml.c:11031 (F16 path), 2392-2426, 11390, 11925-11973, 12009-12078
 //   k_argmax    greedy pick on device (used by the fused decode loop; ties → lowest id)
 #pragma once
+#include <cmath>
+#include <vector>
+
 #include "device_types.cuh"
 
 namespace ctb {
@@ -91,6 +94,22 @@ __host__ __device__ inline int kv_ctx_pad(int n_ctx) { return (n_ctx + 255) & ~2
 __host__ __device__ inline size_t k_row(int kv_head, int pos, int n_ctx, int hd) { return ((size_t)kv_head * n_ctx + pos) * hd; }   // element offset of a K row
 __host__ __device__ inline int k_perm(int e, int hd) { return (e & 31) * (hd >> 5) + (e >> 5); }
 __host__ __device__ inline int v_perm(int t) { return (t & ~255) + (t & 31) * 8 + ((t >> 5) & 7); }
+
+// The (cos, sin) table [n_pos][hd/2] every RoPE kernel reads: the reference's theta recurrence with the same libm calls
+// (ggml.c:12482-12529), built on the host once.
+inline std::vector<float2> rope_table(int n_pos, int hd, int n_rot, float freq_base, float freq_scale) {
+  const int half = hd / 2;
+  std::vector<float2> tab((size_t)n_pos * half);
+  const float theta_scale = powf(freq_base, -2.0f / n_rot);
+  for (int p = 0; p < n_pos; p++) {
+    float theta = freq_scale * (float)p;
+    for (int i = 0; i < half; i++) {
+      tab[(size_t)p * half + i] = make_float2(cosf(theta), sinf(theta));
+      theta *= theta_scale;
+    }
+  }
+  return tab;
+}
 
 struct RopeKVParams {
   float* q;             // [N][n_head*hd]   rotated in place

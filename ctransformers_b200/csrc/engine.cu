@@ -403,16 +403,7 @@ void Engine::init(const GGUFFile& g) {
   }
   // ---- RoPE table: same recurrence, same libm calls as ggml.c:12482-12529
   {
-    const int half = hp_.head_dim() / 2;
-    std::vector<float2> tab((size_t)hp_.n_ctx * half);
-    const float theta_scale = powf(hp_.rope_base, -2.0f / hp_.n_rot);
-    for (int p = 0; p < hp_.n_ctx; p++) {
-      float theta = hp_.rope_scale * (float)p;
-      for (int i = 0; i < half; i++) {
-        tab[(size_t)p * half + i] = make_float2(cosf(theta), sinf(theta));
-        theta *= theta_scale;
-      }
-    }
+    const std::vector<float2> tab = rope_table(hp_.n_ctx, hp_.head_dim(), hp_.n_rot, hp_.rope_base, hp_.rope_scale);
     rope_ = (float2*)alloc(tab.size() * sizeof(float2));
     CTB_CUDA(cudaMemcpy(rope_, tab.data(), tab.size() * sizeof(float2), cudaMemcpyHostToDevice));
   }
@@ -747,8 +738,8 @@ void Engine::build_ops() {
     const int want = atoi(e);
     if (want >= ST_W && want < step_slots_ && want % ST_W == 0) { step_smem_ -= (size_t)(step_slots_ - want) * ST_SLOT; step_slots_ = want; }
   }
-  const bool ring_attn = st_attn_ring_ok(hp_.n_ctx, step_slots_) && !getenv("CTB_NO_RING_ATTN");
-  for (StepOp& op : ops_) if (op.ph.kind == PH_ATTN) op.ph.q6 = ring_attn ? 1 : 0;
+  ring_attn_ = st_attn_ring_ok(hp_.n_ctx, step_slots_) && !getenv("CTB_NO_RING_ATTN");
+  for (StepOp& op : ops_) if (op.ph.kind == PH_ATTN) op.ph.q6 = ring_attn_ ? 1 : 0;
   if (any_stream && step_slots_ < ST_W) throw std::runtime_error("model rows are too long for the step kernel's shared memory");
   if (any_stream) CTB_CUDA(step_set_smem_limit(step_smem_));
   else fused_ = false;
@@ -1047,6 +1038,15 @@ void Engine::decode_one(int token, int pos, int n_total, bool with_logits) {
   st[0] = token; st[1] = pos; st[2] = 0; st[3] = n_total;
   CTB_CUDA(cudaMemcpyAsync(d_state_, st, 16, cudaMemcpyHostToDevice, stream_));
   CTB_CUDA(cudaGraphLaunch(with_logits ? graph_full_ : graph_nolog_, stream_));
+  single_steps_++;
+}
+
+int Engine::paths(int* out, int cap) {
+  const int v[6] = {fused_ ? 1 : 0, fused_ && ring_attn_ ? 1 : 0, step_slots_, ensure_prefill() ? 1 : 0, (int)prefill_launches_, (int)single_steps_};
+  const int n = (int)(sizeof(v) / sizeof(v[0]));
+  if (cap < n) return -n;
+  std::copy(v, v + n, out);
+  return n;
 }
 
 void Engine::host_views() {
@@ -1227,10 +1227,7 @@ bool Engine::ensure_prefill() {
   P.n_phases = (int)prog.size();
   P.d_prog = (PPhase*)dalloc((prog.size() + 1) * sizeof(PPhase));
   CTB_CUDA(cudaMemcpy(P.d_prog, prog.data(), prog.size() * sizeof(PPhase), cudaMemcpyHostToDevice));
-  const size_t work = pb_work_bytes(K_max, hp_.n_ctx, hp_.head_dim()), room = pstep_max_dyn_smem();
-  if (work + 4 * (size_t)ST_SLOT > room) return false;
-  P.n_slots = (int)std::min<size_t>(ST_MAX_SLOTS, (room - work) / ST_SLOT) / PB_TEAMS * PB_TEAMS;   // whole per-team sub-rings
-  P.smem = (size_t)P.n_slots * ST_SLOT + work;
+  if (!pstep_shape(pb_work_bytes(K_max, hp_.n_ctx, hp_.head_dim()), P.n_slots, P.smem)) return false;
   CTB_CUDA(pstep_set_smem_limit(P.smem));
   P.ok = true;
   return true;
@@ -1249,6 +1246,7 @@ void Engine::prefill_batch(const int* tokens, const int* pos, const int* n_total
   st[PB_T * 4] = n;
   CTB_CUDA(cudaMemcpyAsync(P.d_state, st, (PB_T * 4 + 4) * 4, cudaMemcpyHostToDevice, stream_));
   CTB_CUDA(launch_pstep(step_grid_, P.n_slots, P.smem, stream_, P.d_prog, P.n_phases, d_sync_));
+  prefill_launches_++;
   if (last) {
     const StepOp& head = ops_[n_body_];
     CTB_CUDA(cudaMemcpyAsync(const_cast<float*>(head.ph.mv.x), P.x_final + (size_t)(n - 1) * hp_.n_embd, (size_t)hp_.n_embd * 4, cudaMemcpyDeviceToDevice, stream_));

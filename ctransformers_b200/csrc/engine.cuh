@@ -74,6 +74,8 @@ class Engine {
   double time_matvec_only(int reps, long* launches, unsigned mask = 0);
   int profile_step(int token, int n_past, double ms_by_kind[4], int count_by_kind[4]);
   long trace_step(int token, int n_past, unsigned long long* out, long cap_words);
+  // Which implementations the evals run (include/ctransformers_b200.h ctb_llm_paths): entries written, or -needed.
+  int paths(int* out, int cap);
 
   // Host views of the last token's logits / hidden state (the reference hands out ctx->logits.data(), mutable by the caller,
   // llama.cc:47-51).  Until a caller asks for one, nothing is copied per eval (lazy); from the first request on every eval
@@ -162,6 +164,7 @@ class Engine {
   int step_grid_ = 0, step_slots_ = 0;   // launch shape of the step kernel: CTAs, ring slots,
   size_t step_smem_ = 0;                 // dynamic shared memory
   bool fused_ = true;            // CTB_STEP_FUSE=0: one kernel per op
+  bool ring_attn_ = false;       // the step kernel's attention phases take cached K / V through the ring (st_attn_ring_ok)
   void build_ops();
   void push_matvec(struct MVParams& p, int kind);
   void upload_prog(Phase* dst, int* dst_bounds, const std::vector<StepOp>& ops);
@@ -178,6 +181,8 @@ class Engine {
   struct PrefillState* pf_ = nullptr;
   bool prefill_on_ = true;       // CTB_NO_PREFILL=1: prompts run through the single-token kernel
   int prefill_min_ = 4;          // shortest run of consecutive tokens worth a batched launch
+  long prefill_launches_ = 0;    // k_pstep launches so far
+  long single_steps_ = 0;        // tokens of batch_eval that went through the single-token step
   bool ensure_prefill();
   void prefill_batch(const int* tokens, const int* pos, const int* n_total, int n, bool last);
   void decode_one(int token, int pos, int n_total, bool with_logits);

@@ -294,6 +294,15 @@ long ctb_llm_trace_step(LLM* llm, int token, int n_past, unsigned long long* out
   }
 }
 
+long ctb_llm_paths(LLM* llm, int* out, int cap) {
+  try {
+    return llm->engine->paths(out, cap);
+  } catch (const std::exception& e) {
+    fprintf(stderr, "ctransformers-b200: paths failed: %s\n", e.what());
+    return -100;
+  }
+}
+
 double ctb_llm_time_matvec_only(LLM* llm, int reps, long* launches) { return ctb_llm_time_matvec_kinds(llm, reps, launches, 0); }
 
 double ctb_llm_time_matvec_kinds(LLM* llm, int reps, long* launches, unsigned kind_mask) {

@@ -13,6 +13,7 @@
 #include "../../include/ctransformers_b200.h"
 #include "attention.cuh"
 #include "matvec.cuh"
+#include "prefill.cuh"
 #include "repack.cuh"
 #include "stream.cuh"
 #include "tables.hpp"
@@ -106,10 +107,16 @@ int sm_count() {
   return n_sm;
 }
 
-// a program of phases through the persistent step kernel, exactly as the engine launches it
-void run_phases(std::vector<Phase> phs) {
+// grid-barrier words of the persistent kernels (k_step and k_pstep both leave them zeroed when they end)
+unsigned* sync_words() {
   static unsigned* d_sync = nullptr;
   if (!d_sync) { OPS_CUDA(cudaMalloc((void**)&d_sync, 64)); OPS_CUDA(cudaMemset(d_sync, 0, 64)); }
+  return d_sync;
+}
+
+// a program of phases through the persistent step kernel, exactly as the engine launches it
+void run_phases(std::vector<Phase> phs) {
+  unsigned* d_sync = sync_words();
   const StepLaunch L = step_launch_shape(phs.data(), (int)phs.size(), sm_count(), step_max_dyn_smem());
   const std::vector<int> hb = step_bounds(phs.data(), (int)phs.size(), L.grid);
   DevBuf dbounds(hb.size() * 4);
@@ -194,6 +201,28 @@ void stage_to_host(const float* x, const float* w, const float* b, float* y_norm
   if (y_norm) OPS_CUDA(cudaMemcpy(y_norm, dy.p, (size_t)K * 4, cudaMemcpyDeviceToHost));
 }
 
+// KV caches in the reference's layouts (K [pos][n_kv*hd], V transposed [n_kv*hd][v_ld]), positions [0, n_pos)  <->  the
+// device layouts of attention.cuh for a context of n_ctx (k_row / k_perm, kv_ctx_pad / v_perm); unset device entries are 0
+void kv_to_device(const uint16_t* kref, const uint16_t* vref, int v_ld, int n_pos, int n_kv, int hd, int n_ctx, std::vector<uint16_t>& kp,
+                  std::vector<uint16_t>& vp) {
+  const int cp = kv_ctx_pad(n_ctx);
+  kp.assign((size_t)n_ctx * n_kv * hd, 0);
+  vp.assign((size_t)n_kv * hd * cp, 0);
+  for (int t = 0; t < n_pos; t++)
+    for (int kh = 0; kh < n_kv; kh++)
+      for (int e = 0; e < hd; e++) kp[k_row(kh, t, n_ctx, hd) + k_perm(e, hd)] = kref[((size_t)t * n_kv + kh) * hd + e];
+  for (int ch = 0; ch < n_kv * hd; ch++)
+    for (int t = 0; t < n_pos; t++) vp[(size_t)ch * cp + v_perm(t)] = vref[(size_t)ch * v_ld + t];
+}
+void kv_from_device(const std::vector<uint16_t>& kp, const std::vector<uint16_t>& vp, int n_kv, int hd, int n_ctx, uint16_t* kref, uint16_t* vref) {
+  const int cp = kv_ctx_pad(n_ctx);
+  for (int t = 0; t < n_ctx; t++)
+    for (int kh = 0; kh < n_kv; kh++)
+      for (int e = 0; e < hd; e++) kref[((size_t)t * n_kv + kh) * hd + e] = kp[k_row(kh, t, n_ctx, hd) + k_perm(e, hd)];
+  for (int ch = 0; ch < n_kv * hd; ch++)
+    for (int t = 0; t < n_ctx; t++) vref[(size_t)ch * n_ctx + t] = vp[(size_t)ch * cp + v_perm(t)];
+}
+
 }  // namespace
 
 extern "C" {
@@ -262,12 +291,7 @@ int ctb_norm(int mode, const float* x, const float* w, const float* b, float* y,
 int ctb_rope(float* x, int n_heads, int head_dim, int pos, int mode, float freq_base, float freq_scale) {
   return guarded("ctb_rope", [&] {
     const int half = head_dim / 2;
-    std::vector<float2> tab((size_t)(pos + 1) * half);
-    const float theta_scale = powf(freq_base, -2.0f / head_dim);
-    for (int p = 0; p <= pos; p++) {
-      float theta = freq_scale * (float)p;
-      for (int i = 0; i < half; i++) { tab[(size_t)p * half + i] = make_float2(cosf(theta), sinf(theta)); theta *= theta_scale; }
-    }
+    const std::vector<float2> tab = rope_table(pos + 1, head_dim, head_dim, freq_base, freq_scale);
     const size_t nq = (size_t)n_heads * head_dim;
     DevBuf dq(nq * 4), dtab(tab.size() * 8), dst(16);
     OPS_CUDA(cudaMemcpy(dq.p, x, nq * 4, cudaMemcpyHostToDevice));
@@ -288,16 +312,9 @@ int ctb_attention(const float* q, const uint16_t* kcache, const uint16_t* vcache
   return guarded("ctb_attention", [&] {
     if (head_dim != 64 && head_dim != 128) throw std::runtime_error("head_dim must be 64 or 128");
     if (n_total < T) n_total = T;
-    const int cp = kv_ctx_pad(n_total);
     const size_t nq = (size_t)n_head * head_dim;
-    // reference layouts in (K [T][n_kv*hd], V transposed [n_kv*hd][T]) -> our permuted device layouts
-    std::vector<uint16_t> kp((size_t)n_total * n_kv * head_dim, 0), vp((size_t)n_kv * head_dim * cp, 0);
-    for (int t = 0; t < T; t++)
-      for (int kh = 0; kh < n_kv; kh++)
-        for (int e = 0; e < head_dim; e++)
-          kp[k_row(kh, t, n_total, head_dim) + k_perm(e, head_dim)] = kcache[((size_t)t * n_kv + kh) * head_dim + e];
-    for (int ch = 0; ch < n_kv * head_dim; ch++)
-      for (int t = 0; t < T; t++) vp[(size_t)ch * cp + v_perm(t)] = vcache[(size_t)ch * T + t];
+    std::vector<uint16_t> kp, vp;
+    kv_to_device(kcache, vcache, T, T, n_kv, head_dim, n_total, kp, vp);
     // the kernel fuses RoPE + KV store for the current position: feed it an identity rotation (cos 1, sin 0 is exact) and the
     // current position's k/v taken back out of the caller's caches (f16 -> f32 -> f16 round-trips exactly)
     const int pos = T - 1;
@@ -326,6 +343,86 @@ int ctb_attention(const float* q, const uint16_t* kcache, const uint16_t* vcache
     k_attn<<<dim3(n_head, 1, head_dim / ATTN_CH), ATTN_THREADS, smem>>>(ap);
     OPS_CUDA(cudaGetLastError());
     OPS_CUDA(cudaMemcpy(out, dout.p, nq * 4, cudaMemcpyDeviceToHost));
+  });
+}
+
+int ctb_attention_path(int path, const float* q, const float* k_new, const float* v_new, uint16_t* kcache, uint16_t* vcache, float* out,
+                       int n_head, int n_kv, int head_dim, int n_ctx, int pos0, int n_tok, const int* n_total, int rope_mode, float freq_base,
+                       float kq_scale) {
+  return guarded("ctb_attention_path", [&] {
+    const int hd = head_dim;
+    if (path < 0 || path > 3) throw std::runtime_error("unknown attention path " + std::to_string(path));
+    if (hd != 64 && hd != 128) throw std::runtime_error("head_dim must be 64 or 128");
+    if (n_head < 1 || n_kv < 1 || n_head % n_kv) throw std::runtime_error("n_head must be a multiple of n_kv");
+    if (n_tok < 1 || pos0 < 0 || pos0 + n_tok > n_ctx) throw std::runtime_error("the tokens' positions must lie inside the context");
+    for (int i = 0; i < n_tok; i++)
+      if (n_total[i] <= pos0 + i || n_total[i] > n_ctx) throw std::runtime_error("n_total[i] must lie in [position + 1, n_ctx]");
+    const size_t nq = (size_t)n_head * hd, nkv = (size_t)n_kv * hd;
+    std::vector<uint16_t> kp, vp;
+    kv_to_device(kcache, vcache, n_ctx, n_ctx, n_kv, hd, n_ctx, kp, vp);
+    const std::vector<float2> tab = rope_table(n_ctx, hd, hd, freq_base, 1.0f);
+    // device state per token {token, position, step, n_total}; the batched kernel reads PB_T rows + the valid-token count
+    std::vector<int> st((size_t)std::max(n_tok, PB_T) * 4 + 4, 0);
+    for (int i = 0; i < std::max(n_tok, PB_T); i++) {
+      const int k = std::min(i, n_tok - 1);
+      st[(size_t)i * 4 + 1] = pos0 + k; st[(size_t)i * 4 + 3] = n_total[k];
+    }
+    if (path == 3) st[(size_t)PB_T * 4] = n_tok;
+    DevBuf dq(nq * n_tok * 4), dk(nkv * n_tok * 4), dv(nkv * n_tok * 4), dkc(kp.size() * 2), dvc(vp.size() * 2), dout(nq * n_tok * 4),
+        dtab(tab.size() * 8), dst(st.size() * 4);
+    OPS_CUDA(cudaMemcpy(dq.p, q, nq * n_tok * 4, cudaMemcpyHostToDevice));
+    OPS_CUDA(cudaMemcpy(dk.p, k_new, nkv * n_tok * 4, cudaMemcpyHostToDevice));
+    OPS_CUDA(cudaMemcpy(dv.p, v_new, nkv * n_tok * 4, cudaMemcpyHostToDevice));
+    OPS_CUDA(cudaMemcpy(dkc.p, kp.data(), kp.size() * 2, cudaMemcpyHostToDevice));
+    OPS_CUDA(cudaMemcpy(dvc.p, vp.data(), vp.size() * 2, cudaMemcpyHostToDevice));
+    OPS_CUDA(cudaMemcpy(dtab.p, tab.data(), tab.size() * 8, cudaMemcpyHostToDevice));
+    OPS_CUDA(cudaMemcpy(dst.p, st.data(), st.size() * 4, cudaMemcpyHostToDevice));
+    OPS_CUDA(cudaMemset(dout.p, 0, nq * n_tok * 4));
+    AttnParams ap{};
+    ap.q = dq.as<float>(); ap.k = dk.as<float>(); ap.v = dv.as<float>(); ap.kc = dkc.as<uint16_t>(); ap.vc = dvc.as<uint16_t>();
+    ap.out = dout.as<float>(); ap.exp_tab = tables().ex; ap.rope = dtab.as<float2>(); ap.state = dst.as<int>(); ap.kq_scale = kq_scale;
+    ap.n_head = n_head; ap.n_kv = n_kv; ap.hd = hd; ap.n_ctx = n_ctx; ap.q_stride = (int)nq; ap.kv_stride = (int)nkv; ap.neox = (rope_mode & 2) ? 1 : 0;
+    if (path == 3) {   // one k_pstep launch of the engine's KV + ATTN phases (prefill_batch), with the engine's launch shape
+      if (n_tok > PB_T) throw std::runtime_error("the batched kernel takes at most 32 tokens");
+      int n_slots = 0;
+      size_t smem = 0;
+      // (the engine's scratch also holds the widest activation; a model with these heads has n_embd >= n_head * hd)
+      if (!pstep_shape(pb_work_bytes((int)nq, n_ctx, hd), n_slots, smem)) throw std::runtime_error("n_ctx too long for the batched kernel's attention scratch");
+      PPhase ph{};
+      ph.at = ap; ph.state = dst.as<int>();
+      PPhase prog[2] = {ph, ph};
+      prog[0].kind = PP_KV; prog[1].kind = PP_ATTN;
+      DevBuf dprog(sizeof(prog));
+      OPS_CUDA(cudaMemcpy(dprog.p, prog, sizeof(prog), cudaMemcpyHostToDevice));
+      OPS_CUDA(pstep_set_smem_limit(smem));
+      OPS_CUDA(launch_pstep(sm_count(), n_slots, smem, 0, dprog.as<PPhase>(), 2, sync_words()));
+    } else {   // one launch per token, in order, like decode_one
+      if (path == 1) {
+        Phase ph{};
+        ph.kind = PH_ATTN; ph.q6 = 1; ph.at = ap;
+        const StepLaunch L = step_launch_shape(&ph, 1, sm_count(), step_max_dyn_smem());
+        if (!st_attn_ring_ok(n_ctx, L.n_slots)) throw std::runtime_error("the step kernel's ring cannot carry K / V at this n_ctx");
+      }
+      const size_t smem = attn_smem_bytes(n_ctx, hd);
+      if (path == 0) OPS_CUDA(cudaFuncSetAttribute(k_attn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)std::max<size_t>(smem, 48 * 1024)));
+      for (int i = 0; i < n_tok; i++) {
+        AttnParams a = ap;
+        a.q += (size_t)i * nq; a.k += (size_t)i * nkv; a.v += (size_t)i * nkv; a.out += (size_t)i * nq; a.state += (size_t)i * 4;
+        if (path == 0) {
+          k_attn<<<dim3(n_head, 1, hd / ATTN_CH), ATTN_THREADS, smem>>>(a);
+          OPS_CUDA(cudaGetLastError());
+        } else {
+          Phase ph{};
+          ph.kind = PH_ATTN; ph.q6 = path == 1 ? 1 : 0; ph.at = a;
+          run_phases({ph});
+        }
+      }
+    }
+    OPS_CUDA(cudaDeviceSynchronize());
+    OPS_CUDA(cudaMemcpy(out, dout.p, nq * n_tok * 4, cudaMemcpyDeviceToHost));
+    OPS_CUDA(cudaMemcpy(kp.data(), dkc.p, kp.size() * 2, cudaMemcpyDeviceToHost));
+    OPS_CUDA(cudaMemcpy(vp.data(), dvc.p, vp.size() * 2, cudaMemcpyDeviceToHost));
+    kv_from_device(kp, vp, n_kv, hd, n_ctx, kcache, vcache);
   });
 }
 

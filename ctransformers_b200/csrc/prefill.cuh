@@ -583,6 +583,15 @@ static inline size_t pstep_max_dyn_smem() {
   cudaDeviceGetAttribute(&optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, dev);
   return (size_t)optin > fa.sharedSizeBytes ? (size_t)optin - fa.sharedSizeBytes : 0;
 }
+// launch shape of k_pstep around `work` bytes of scratch: whole per-team sub-rings in what shared memory has left.  false
+// when fewer than 4 slots fit (the attention scratch of a long context): the caller then has no batched prefill.
+inline bool pstep_shape(size_t work, int& n_slots, size_t& smem) {
+  const size_t room = pstep_max_dyn_smem();
+  if (work + 4 * (size_t)ST_SLOT > room) return false;
+  n_slots = (int)std::min<size_t>(ST_MAX_SLOTS, (room - work) / ST_SLOT) / PB_TEAMS * PB_TEAMS;
+  smem = (size_t)n_slots * ST_SLOT + work;
+  return true;
+}
 static inline cudaError_t pstep_set_smem_limit(size_t bytes) { return cudaFuncSetAttribute(k_pstep, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes); }
 static inline cudaError_t launch_pstep(int grid, int n_slots, size_t smem, cudaStream_t st, const PPhase* d_prog, int n_phases, unsigned* d_sync) {
   PStepArgs a;

@@ -99,6 +99,12 @@ double ctb_llm_time_matvec_only(LLM* llm, int reps, long* launches);
 /* Same, restricted to the launches whose kind bit is set in kind_mask (bit 0 QKV, 1 attention output, 2 FFN gate+up,
  * 3 FFN down, 4 output head; 0 = all): per-projection timing under in-graph launch conditions. */
 double ctb_llm_time_matvec_kinds(LLM* llm, int reps, long* launches, unsigned kind_mask);
+/* Which implementations this model's evals run, so a caller can tell what a context length and the CTB_* environment
+ * switches selected.  out = {decode steps fused into the step kernel (0: one kernel per op, CTB_STEP_FUSE=0), attention of
+ * the step kernel fed by its K / V ring (0: attn_body from global memory, or k_attn when not fused), ring slots of the step
+ * kernel (ST_W per slot depth), batched prefill available (tries to set it up), batched prefill launches so far, tokens
+ * evaluated by single-token steps so far}.  Returns the entries written (6), or -6 when cap is smaller, < 0 on error. */
+long ctb_llm_paths(LLM* llm, int* out, int cap);
 
 /* Host-only pieces of the boundary, callable without a GPU: the GGUF vocabulary with its SPM / BPE tokenizer
  * (llama.cpp:1648-1760, 3080-3427, 6151-6187) and the sampler chain of llama_llm::Sample (llama.cc:53-84). */
@@ -129,6 +135,22 @@ int ctb_rope(float* x, int n_heads, int head_dim, int pos, int mode, float freq_
  * over rows of that length and splits them at n_total & ~31 between its SIMD lanes and a scalar tail. */
 int ctb_attention(const float* q, const uint16_t* kcache, const uint16_t* vcache, float* out, int n_head, int n_kv, int head_dim,
                   int T, int n_total, float kq_scale);
+/* n_tok query tokens at positions pos0 .. pos0+n_tok-1 through one of the engine's four attention implementations, each
+ * launched the way the engine launches it, RoPE and the KV-cache store included:
+ *   path 0  standalone k_attn (un-fused steps, non-K-quant models), one launch per token
+ *   path 1  attention phase of the persistent step kernel with cached K / V carried by its shared-memory ring, one launch per
+ *           token; fails when the ring cannot carry this n_ctx (st_attn_ring_ok)
+ *   path 2  the same phase reading K / V from global memory (attn_body; contexts past the ring's reach), one launch per token
+ *   path 3  the batched prefill kernel's KV + attention phases, all tokens in one launch (n_tok <= 32); fails when its
+ *           attention scratch does not fit shared memory at this n_ctx
+ * q [n_tok][n_head*hd], k_new / v_new [n_tok][n_kv*hd]: projections NOT yet rotated; RoPE mode 0 or 2 (neox), freq_base,
+ * freq_scale 1.  kcache [n_ctx][n_kv*hd] fp16 (rotated K) and vcache TRANSPOSED [n_kv*hd][n_ctx] fp16, the reference's layouts
+ * (llama.cpp:2323-2335): they hold positions < pos0 on entry and the new tokens' rows as well on return.  n_total[i] = n_past + N
+ * of the eval chunk token i belongs to (position + 1 <= n_total[i] <= n_ctx).  out [n_tok][n_head*hd].  0 on success, -1 (with
+ * a message on stderr) when the path cannot take the shape. */
+int ctb_attention_path(int path, const float* q, const float* k_new, const float* v_new, uint16_t* kcache, uint16_t* vcache,
+                       float* out, int n_head, int n_kv, int head_dim, int n_ctx, int pos0, int n_tok, const int* n_total,
+                       int rope_mode, float freq_base, float kq_scale);
 /* silu(W1 x) * (W3 x) with the fp16 SiLU table (ggml.c:3625-3632) — the fused FFN gate. */
 int ctb_ffn_gate(int type, const void* w1_blocks, const void* w3_blocks, const float* x, float* out, int K, int M);
 /* ggml_get_rows on a quantized table (ggml.c:11615-11642). */

@@ -10,7 +10,8 @@ Contents
   host_logic.npz   tokenizer ids for a set of strings, detokenized pieces, and sampler picks for seeded logits
   reference_blocks.npz  blocks written by the reference's quantizer, the pool of refs.reference_quantized_blocks
   reference_runs.npz  what the reference computed for each test that compares with it (tests/test_model_gpu.py,
-                   tests/test_oracle.py), so those tests run where the reference is not available
+                   tests/test_oracle.py, tests/test_long_context_gpu.py), so those tests run where the reference is not
+                   available.  `python make_golden.py long_context` adds the long-context runs to the existing file.
 """
 import ctypes as C
 import json
@@ -184,6 +185,26 @@ def reference_runs(tmp):
     np.savez_compressed(HERE / "reference_runs.npz", **out)
 
 
+def long_context_runs(tmp):
+    """Adds the reference's results for modelcases.LONG_RUNS to reference_runs.npz as keys long_<run>_*; every key already in
+    the file keeps its bytes (the rest of reference_runs() also rebuilds the 7B-shaped bench models)."""
+    old = dict(refs.golden_runs())
+    out = dict(old)
+
+    for key, (name, ctx, n_prompt, bs, n_new) in modelcases.LONG_RUNS.items():
+        path, _ = modelcases.build(name, tmp)
+        run = modelcases.run_greedy(ref_llm(path, ctx, threads=min(16, os.cpu_count() or 1)), modelcases.seeded_prompt(name, n_prompt), n_new,
+                                    batch_size=bs)
+        first_logits, first_embd, toks, last_logits, _ = run
+        for k, v in (("first_logits", first_logits), ("first_embd", first_embd), ("last_logits", last_logits)):
+            out[f"long_{key}_{k}"] = np.array(refs.digest(v))
+        out[f"long_{key}_tokens"] = np.array(toks, np.int32)
+        print(key, "tokens", toks[:8])
+    np.savez_compressed(HERE / "reference_runs.npz", **out)
+    new = refs.golden_runs()
+    assert all(np.array_equal(new[k], v) and new[k].dtype == v.dtype for k, v in old.items()), "an existing key changed"
+
+
 if __name__ == "__main__":
     assert refs.have_ref(), "build oracle/_ref first: make -C oracle ref"
     import sys
@@ -196,7 +217,9 @@ if __name__ == "__main__":
                 reference_blocks()
             if "reference_runs" in only:
                 reference_runs(tmp)
-            cases = [o for o in only if o not in ("kat", "reference_blocks", "reference_runs")]
+            if "long_context" in only:
+                long_context_runs(tmp)
+            cases = [o for o in only if o not in ("kat", "reference_blocks", "reference_runs", "long_context")]
             if cases:
                 models(tmp, cases)
         else:

@@ -48,6 +48,48 @@ def long_prompt(name, bos=True):
     return ids
 
 
+def seeded_prompt(name, n, seed=17):
+    """n seeded token ids for a model case (BOS first on llama): the prompts of the long-context runs."""
+    arch, shape, _, _ = CASES[name]
+    ids = np.random.default_rng(seed).integers(259 if arch == "llama" else 0, shape.n_vocab, n).tolist()
+    if arch == "llama":
+        ids[0] = 1
+    return ids
+
+
+# Long-context runs: key -> (model case, context_length, prompt tokens, batch_size, greedy steps).  What the engine does at each
+# length (tests/test_long_context_gpu.py asserts it through ctb_llm_paths):
+#   c2304_p1100  batched prefill (35 launches), then ring decode at T 1101..1124 (nchv 5, cv 3); with CTB_NO_PREFILL=1 the ring
+#                step runs at every T from 1, through every cv step up to T = 1025
+#   c2304_p2280  the context fills exactly: the last step attends over 2304 positions (V items fill the ring slot, cv 2)
+#   c3072        the V items of 12 chunks do not fit the ring: attention reads K / V from global memory (attn_body in the step)
+#   c1152_bs3    chunks of 3 tokens: every token's n_total is its chunk's end, past the token for the first two of each chunk
+#   c4096        the batched kernel's attention scratch does not fit shared memory: no batched prefill
+#   c8192        the attention scratch leaves room for one ring slot per consumer warp (10 slots)
+LONG_RUNS = {
+    "llama_tiny_q4km_c2304_p1100": ("llama_tiny_q4km", 2304, 1100, 512, 24),
+    "falcon_tiny_q5km_c2304_p1100": ("falcon_tiny_q5km", 2304, 1100, 512, 24),
+    "llama_gqa_q5km_c2304_p520": ("llama_gqa_q5km", 2304, 520, 512, 8),
+    "llama_tiny_q4km_c2304_p2280": ("llama_tiny_q4km", 2304, 2280, 512, 24),
+    "llama_tiny_q4km_c3072_p600": ("llama_tiny_q4km", 3072, 600, 512, 8),
+    "llama_tiny_q4km_c1152_p1100_bs3": ("llama_tiny_q4km", 1152, 1100, 3, 4),
+    "falcon_tiny_q5km_c4096_p300": ("falcon_tiny_q5km", 4096, 300, 64, 8),
+    "llama_tiny_q4km_c8192_p300": ("llama_tiny_q4km", 8192, 300, 64, 8),
+    "llama_tiny_q4km_c1024_p600": ("llama_tiny_q4km", 1024, 600, 512, 8),
+}
+
+
+def oracle_greedy(model, prompt, n_new, batch_size):
+    """run_greedy's results from an oracle model (refs.OracleModel): greedy = the first largest logit."""
+    model.eval(prompt, batch_size=batch_size)
+    first_logits, first_embd = model.logits.copy(), model.embd.copy()
+    toks = []
+    for _ in range(n_new):
+        toks.append(int(np.argmax(model.logits)))
+        model.eval([toks[-1]])
+    return first_logits, first_embd, toks, model.logits.copy(), None
+
+
 REALQ_PROMPT = [1] + np.random.default_rng(0).integers(259, 1024, 30).tolist()
 
 

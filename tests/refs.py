@@ -152,6 +152,34 @@ def ref_vec_dot(t, k, wrow, act):
     return float(s[0])
 
 
+def attention_expected(q, k_new, v_new, kcache, vcache, n_head, n_kv, hd, pos0, n_total, mode, freq_base, kq_scale):
+    """What the reference's attention block computes for an eval chunk of n_tok tokens at positions pos0.. (llama.cpp:2303-2400),
+    from oracle pieces: orc_rope on q and k, the chunk's K rows and V columns stored as fp16 before any token attends, then
+    orc_attn_head_n per head over the chunk row length n_total[i].  Arguments as ctb_attention_path (kcache [n_ctx][n_kv*hd],
+    vcache [n_kv*hd][n_ctx], uint16 fp16 bits); returns (out [n_tok][n_head*hd], kcache, vcache) with the new rows stored."""
+    o = oracle()
+    o.orc_attn_head_n.argtypes = [C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p, C.c_size_t, C.c_int, C.c_int, C.c_int, C.c_float, C.c_void_p]
+    n_tok, n_ctx = q.shape[0], kcache.shape[0]
+    kc, vc = kcache.copy(), vcache.copy()
+    for i in range(n_tok):
+        kr = np.ascontiguousarray(k_new[i], np.float32).copy()
+        o.orc_rope(ptr(kr), n_kv, hd, pos0 + i, mode, freq_base, 1.0)
+        kc[pos0 + i] = kr.astype(np.float16).view(np.uint16)
+        vc[:, pos0 + i] = np.asarray(v_new[i], np.float32).astype(np.float16).view(np.uint16)
+    out = np.zeros((n_tok, n_head * hd), np.float32)
+    group = n_head // n_kv
+    for i in range(n_tok):
+        T = pos0 + i + 1
+        assert T <= n_total[i] <= n_ctx
+        qr = np.ascontiguousarray(q[i], np.float32).copy()
+        o.orc_rope(ptr(qr), n_head, hd, pos0 + i, mode, freq_base, 1.0)
+        for h in range(n_head):
+            kvh = h // group
+            o.orc_attn_head_n(ptr(qr[h * hd:]), kc.ctypes.data + kvh * hd * 2, n_kv * hd, vc.ctypes.data + kvh * hd * n_ctx * 2, n_ctx, hd, T,
+                              int(n_total[i]), float(kq_scale), out.ctypes.data + (i * n_head + h) * hd * 4)
+    return out, kc, vc
+
+
 # --------------------------------------------------------------------------------------------------------------
 # Whole-model oracle (oracle/llama_oracle.c) driven from a GGUF file
 def read_gguf(path):

@@ -5,6 +5,7 @@ Bar: BIT-EXACT everywhere.  The oracle reproduces the reference's AVX2 accumulat
 bit for bit against the compiled reference in tests/test_oracle.py), and the CUDA kernels reproduce the same order, so
 quantizers, norms, RoPE, embedding rows, every quantized dot product and the attention block must match to the last bit."""
 import ctypes as C
+import functools
 
 import numpy as np
 import pytest
@@ -177,6 +178,109 @@ def test_attention_bit_exact(lib, n_head, n_kv, hd, T, n_total):
         vslice = np.ascontiguousarray(vpad[kvh * hd:(kvh + 1) * hd])
         o.orc_attn_head_n(ptr(q[h]), ptr(kslice), hd, ptr(vslice), n_total, hd, T, n_total, float(scale), ptr(want[h]))
     _same_bits(got, want)
+
+
+# ---- every attention implementation of the engine (ctb_attention_path), RoPE and the KV-cache store included
+ATTN_PATHS = {0: "k_attn", 1: "step_ring", 2: "step_global", 3: "prefill"}
+# (n_head, n_kv, hd, n_ctx, pos0, n_tok, chunk, extra, rope mode, hard).  The call evaluates n_tok tokens at positions pos0..;
+# chunk: they form one eval chunk, n_total = pos0 + n_tok + extra for all of them; else each is a chunk of its own with
+# n_total = position + 1 + extra.  hard: scores over a wide range (most exp-table entries flush to 0) and all-zero V channels.
+ATTN_CASES = {
+    # T (= position + 1) across the edges of the step kernel's ring geometry: V chunks of 256 positions (nchv), channels per V
+    # item (cv 8 -> 6 -> 4 -> 3 -> 2 at T 513 / 769 / 1025 / 1537), K items of 36 rows (hd 128), V items that fill a slot (T 2304)
+    "T1-2": (8, 2, 128, 2304, 0, 2, False, 0, 0, False),
+    "T31-33": (8, 2, 128, 2304, 30, 3, False, 0, 0, False),
+    "T36-37": (8, 2, 128, 2304, 35, 2, False, 0, 0, False),
+    "T255-257": (8, 2, 128, 2304, 254, 3, False, 0, 0, False),
+    "T512-513": (8, 2, 128, 2304, 511, 2, False, 0, 0, False),
+    "T768-769": (8, 2, 128, 2304, 767, 2, False, 0, 0, False),
+    "T1024-1025": (8, 2, 128, 2304, 1023, 2, False, 0, 0, False),
+    "T1536-1537": (8, 2, 128, 2304, 1535, 2, False, 0, 0, False),
+    "T2047-2048": (8, 2, 128, 2304, 2046, 2, False, 0, 0, False),
+    "T2304-full": (8, 2, 128, 2304, 2303, 1, False, 0, 0, False),
+    # hd 64, MQA, neox: K items of 72 rows, a batch straddling a 256-position chunk, a full 32-token batch that fills the context
+    "mqa-T72-73": (8, 1, 64, 2304, 71, 2, False, 0, 2, False),
+    "mqa-straddle256": (8, 1, 64, 2304, 254, 5, True, 0, 2, False),
+    "mqa-T513": (8, 1, 64, 2304, 512, 1, False, 0, 2, False),
+    "mqa-T769": (8, 1, 64, 2304, 768, 1, False, 0, 2, False),
+    "mqa-T1025": (8, 1, 64, 2304, 1024, 1, False, 0, 2, False),
+    "mqa-T1537": (8, 1, 64, 2304, 1536, 1, False, 0, 2, False),
+    "mqa-batch32-full": (8, 1, 64, 2304, 2272, 32, True, 0, 2, False),
+    # more (head, channel group) tasks than SMs: Falcon-7B heads (71 x 2 = 142 tasks), 40 heads of 128 (160 tasks)
+    "falcon7b-heads": (71, 1, 64, 2304, 1100, 5, True, 0, 2, False),
+    "falcon7b-heads-ctx2000": (71, 1, 64, 2000, 300, 1, False, 0, 2, False),
+    "40x128": (40, 40, 128, 1100, 1040, 3, False, 0, 0, False),
+    # n_total > T: the V·P dot's split between SIMD lanes and the scalar tail; n_ctx not a multiple of 256
+    "ntotal-tail": (4, 4, 128, 1000, 39, 1, False, 20, 0, False),
+    "ntotal-lanes": (4, 4, 128, 1000, 39, 1, False, 30, 0, False),
+    "ntotal-chunk": (16, 2, 64, 2304, 700, 5, True, 57, 0, False),
+    "gqa8-batch32-ctx777": (16, 2, 64, 777, 600, 32, True, 0, 0, False),
+    "batch1": (4, 4, 128, 600, 299, 1, True, 0, 0, False),
+    # hard inputs
+    "hard-hd128": (8, 2, 128, 1500, 1200, 3, True, 0, 0, True),
+    "hard-hd64": (8, 1, 64, 600, 300, 5, True, 0, 2, True),
+    # past the ring's reach (n_ctx > 2304) and past the batched kernel's scratch (n_ctx 4096)
+    "ctx2305": (8, 2, 128, 2305, 2000, 2, False, 0, 0, False),
+    "ctx3072": (8, 1, 64, 3072, 2900, 3, True, 0, 2, False),
+    "ctx4096": (8, 1, 64, 4096, 4000, 2, True, 0, 2, False),
+}
+
+
+def _attn_inputs(n_head, n_kv, hd, n_ctx, pos0, n_tok, chunk, extra, mode, hard):
+    rng = np.random.default_rng(n_head * 7919 + hd * 31 + n_ctx + pos0 * 3 + n_tok)
+    q = rng.standard_normal((n_tok, n_head * hd)).astype(np.float32) * (40.0 if hard else 1.0)
+    k = (rng.standard_normal((n_tok, n_kv * hd)) * 0.7).astype(np.float32)
+    v = rng.standard_normal((n_tok, n_kv * hd)).astype(np.float32)
+    kc = (rng.standard_normal((n_ctx, n_kv * hd)) * 0.7).astype(np.float16).view(np.uint16)
+    vc = rng.standard_normal((n_kv * hd, n_ctx)).astype(np.float16).view(np.uint16)
+    if hard:   # a whole channel group of V and a few more channels are zero
+        zero = list(range(32)) + [40, 77 % hd]
+        vc[zero] = 0
+        v[:, zero] = 0.0
+    pos = pos0 + np.arange(n_tok)
+    n_total = (np.full(n_tok, pos0 + n_tok + extra) if chunk else pos + 1 + extra).astype(np.int32)
+    return q, k, v, kc, vc, n_total
+
+
+@functools.lru_cache(maxsize=None)
+def _attn_expected(case):
+    n_head, n_kv, hd, n_ctx, pos0, n_tok, chunk, extra, mode, hard = ATTN_CASES[case]
+    q, k, v, kc, vc, n_total = _attn_inputs(*ATTN_CASES[case])
+    return refs.attention_expected(q, k, v, kc, vc, n_head, n_kv, hd, pos0, n_total, mode, 10000.0, np.float32(1.0 / np.sqrt(np.float32(hd))))
+
+
+@pytest.mark.parametrize("case", list(ATTN_CASES))
+@pytest.mark.parametrize("path", list(ATTN_PATHS), ids=list(ATTN_PATHS.values()))
+def test_attention_paths_bit_exact(lib, case, path):
+    """Each attention implementation, launched as the engine launches it, on n_tok new tokens against the reference's attention
+    block restated from oracle pieces: output, K cache and V cache identical to the last bit.  A path that cannot take the
+    shape (the ring past 2304 positions, the batched kernel past its scratch or beyond 32 tokens) must refuse it."""
+    n_head, n_kv, hd, n_ctx, pos0, n_tok, chunk, extra, mode, hard = ATTN_CASES[case]
+    q, k, v, kc, vc, n_total = _attn_inputs(*ATTN_CASES[case])
+    out = np.zeros((n_tok, n_head * hd), np.float32)
+    scale = np.float32(1.0 / np.sqrt(np.float32(hd)))
+    rc = lib.ctb_attention_path(path, ptr(q), ptr(k), ptr(v), ptr(kc), ptr(vc), ptr(out), n_head, n_kv, hd, n_ctx, pos0, n_tok, ptr(n_total),
+                                mode, 10000.0, float(scale))
+    refused = (path == 1 and n_ctx > 2304) or (path == 3 and (n_ctx >= 4096 or n_tok > 32))
+    if refused:
+        assert rc == -1, "the path must refuse this shape"
+        return
+    assert rc == 0
+    want, want_kc, want_vc = _attn_expected(case)
+    _same_bits(out, want)
+    assert np.array_equal(kc, want_kc), f"K cache: {int((kc != want_kc).sum())} entries differ"
+    assert np.array_equal(vc, want_vc), f"V cache: {int((vc != want_vc).sum())} entries differ"
+
+
+def test_attention_path_rejects_n_total_outside_the_context(lib):
+    """n_total outside [position + 1, n_ctx] is refused, not run."""
+    n_head, n_kv, hd, n_ctx, pos0, n_tok, *_ = ATTN_CASES["batch1"]
+    q, k, v, kc, vc, _ = _attn_inputs(*ATTN_CASES["batch1"])
+    out = np.zeros((n_tok, n_head * hd), np.float32)
+    for bad in (pos0, n_ctx + 1):
+        nt = np.array([bad], np.int32)
+        assert lib.ctb_attention_path(2, ptr(q), ptr(k), ptr(v), ptr(kc), ptr(vc), ptr(out), n_head, n_kv, hd, n_ctx, pos0, n_tok, ptr(nt), 0,
+                                      10000.0, 0.125) == -1
 
 
 @pytest.mark.parametrize("t", [Q4_K, Q5_K, Q4_0, Q5_0])

@@ -143,6 +143,21 @@ def test_full_eval_matches_reference_golden(name, tmp_path_factory):
     assert toks == gold["tokens"][:6].tolist()
 
 
+@pytest.mark.parametrize("key", list(modelcases.LONG_RUNS))
+def test_long_context_runs_match_reference(key, tmp_path_factory):
+    """The long-context runs of tests/test_long_context_gpu.py (contexts up to 8192, prompts up to 2280 tokens, chunks of 3 to
+    512): the oracle's logits and hidden state after the prompt, greedy tokens and last logits are the reference's bits, so the
+    GPU tests' comparisons with the oracle rest on the reference."""
+    name, ctx, n_prompt, bs, n_new = modelcases.LONG_RUNS[key]
+    path, _ = modelcases.build(name, tmp_path_factory.mktemp("orc_long"))
+    first_logits, first_embd, toks, last_logits, _ = modelcases.oracle_greedy(refs.OracleModel(path, ctx), modelcases.seeded_prompt(name, n_prompt),
+                                                                              n_new, bs)
+    gold = refs.golden_runs()
+    assert toks == gold[f"long_{key}_tokens"].tolist()
+    for k, v in (("first_logits", first_logits), ("first_embd", first_embd), ("last_logits", last_logits)):
+        assert refs.digest(v) == str(gold[f"long_{key}_{k}"]), k
+
+
 @pytest.mark.parametrize("name", ["llama_tiny_q4km", "falcon_tiny_q5km"])
 def test_full_eval_matches_live_reference_for_any_chunking(name, tmp_path_factory):
     """70-token prompt (so the V·P f16 dot uses both its SIMD part and its scalar tail), three chunkings, then 3 decode steps,
