@@ -174,6 +174,16 @@ __global__ void __launch_bounds__(MV_THREADS) k_gate_dump(const float* gate, con
   for (int i = threadIdx.x; i < M; i += MV_THREADS) out[i] = f[i];
 }
 
+// RoPE in place of the fp32 rows of blockIdx.x = 0 .. n_head-1 at position pos, as the attention kernels rotate q and k before
+// rounding them to f16; block = hd/2 threads, one pair each
+__global__ void k_rope_dump(float* x, const float2* rope, int pos, int hd, int neox) {
+  float* row = x + (size_t)blockIdx.x * hd;
+  int i0, i1;
+  float o0, o1;
+  rope_head_pair(row, threadIdx.x, hd, neox, rope[(size_t)pos * (hd / 2) + threadIdx.x], i0, i1, o0, o1);
+  row[i0] = o0; row[i1] = o1;
+}
+
 int guarded(const char* what, const std::function<void()>& fn) {
   try {
     int ndev = 0;
@@ -293,15 +303,10 @@ int ctb_rope(float* x, int n_heads, int head_dim, int pos, int mode, float freq_
     const int half = head_dim / 2;
     const std::vector<float2> tab = rope_table(pos + 1, head_dim, head_dim, freq_base, freq_scale);
     const size_t nq = (size_t)n_heads * head_dim;
-    DevBuf dq(nq * 4), dtab(tab.size() * 8), dst(16);
+    DevBuf dq(nq * 4), dtab(tab.size() * 8);
     OPS_CUDA(cudaMemcpy(dq.p, x, nq * 4, cudaMemcpyHostToDevice));
     OPS_CUDA(cudaMemcpy(dtab.p, tab.data(), tab.size() * 8, cudaMemcpyHostToDevice));
-    const int st[4] = {0, pos, 0, pos + 1};
-    OPS_CUDA(cudaMemcpy(dst.p, st, 16, cudaMemcpyHostToDevice));
-    RopeKVParams rp{};
-    rp.q = dq.as<float>(); rp.rope = dtab.as<float2>(); rp.state = dst.as<int>(); rp.n_head = n_heads; rp.n_kv = 1; rp.hd = head_dim;
-    rp.n_ctx = pos + 1; rp.neox = (mode & 2) ? 1 : 0; rp.q_stride = (int)nq; rp.kv_stride = (int)nq;
-    k_rope_kv<<<dim3(1, n_heads), half>>>(rp);   // grid.y == n_head: only the Q-head blocks exist, no KV store happens
+    k_rope_dump<<<n_heads, half>>>(dq.as<float>(), dtab.as<float2>(), pos, head_dim, (mode & 2) ? 1 : 0);
     OPS_CUDA(cudaGetLastError());
     OPS_CUDA(cudaMemcpy(x, dq.p, nq * 4, cudaMemcpyDeviceToHost));
   });

@@ -6,7 +6,7 @@
 //   ggml_compute_forward_mul_mat over Q4_K / Q5_K / Q6_K weights with Q8_K activations   ggml.c:11031-11245
 //   ggml_vec_dot_q4_K_q8_K / q5_K / q6_K, AVX2 variants                                  k_quants.c:2651-2714, 3174-3262, 3794-3872
 //   norm + quantize prologue and residual / SiLU / GELU epilogue                         matvec.cuh (shared with k_matvec)
-//   RoPE, KV store, K·q, softmax, V·p                                                    attention.cuh attn_body
+//   RoPE, KV store, K·q, softmax, V·p                                                    attention.cuh (attn_body, or st_attn_task below)
 //
 // Structure of a CTA (ST_W consumer warps + 1 producer warp):
 //   producer warp   walks the phase list ahead of everybody else and keeps a ring of ST_SLOT-byte shared-memory slots full:
@@ -593,19 +593,22 @@ __device__ __forceinline__ TileInfo tile_info(const TileSpace& ts, const MVParam
 // memory.  What is left on the critical path is one L2 round trip for q/k/v, one for the exp table, and arithmetic.
 //   K item  up to rows_per_item consecutive cached rows of the task's KV head (head-major cache: one contiguous bulk copy)
 //   V item  cv of the task's ATTN_CH channels, nchv 256-position chunks each (one bulk copy per channel)
-struct AttnRing { int pos, T, lim, n_k, rpi, n_v, cv, nchv; };
+struct AttnRingV { int nchv, cv, n_v; };   // V items of a task over T > 0 positions (the host asks for T = n_ctx)
+__host__ __device__ inline AttnRingV attn_ring_v(int T) {
+  AttnRingV v;
+  v.nchv = (T + 255) >> 8;
+  v.cv = max(1, min(8, ST_SLOT / (v.nchv * 512)));
+  v.n_v = (ATTN_CH + v.cv - 1) / v.cv;
+  return v;
+}
+struct AttnRing : AttnPos, AttnRingV { int n_k, rpi; };
 __device__ __forceinline__ AttnRing attn_ring_geom(const AttnParams& p) {
   AttnRing g;
-  g.pos = p.state[1];
-  g.T = g.pos + 1;
+  static_cast<AttnPos&>(g) = attn_pos(p, p.state);
   g.rpi = ST_SLOT / (p.hd * 2);
-  if (g.pos >= p.n_ctx) { g.T = 0; g.lim = 0; g.n_k = 0; g.n_v = 0; g.cv = 1; g.nchv = 0; return g; }
-  const int n_total = max(g.T, min(p.state[3], p.n_ctx));
-  g.lim = min(g.T, n_total & ~31);
+  if (g.T == 0) { g.n_k = 0; g.n_v = 0; g.cv = 1; g.nchv = 0; return g; }
+  static_cast<AttnRingV&>(g) = attn_ring_v(g.T);
   g.n_k = (g.pos + g.rpi - 1) / g.rpi;
-  g.nchv = (g.T + 255) >> 8;
-  g.cv = max(1, min(8, ST_SLOT / (g.nchv * 512)));
-  g.n_v = (ATTN_CH + g.cv - 1) / g.cv;
   return g;
 }
 
@@ -613,7 +616,7 @@ __device__ __forceinline__ AttnRing attn_ring_geom(const AttnParams& p) {
 __device__ __forceinline__ void st_attn_produce(const AttnParams& p, uint8_t* ring, uint64_t* full_bar, uint64_t* empty_bar, uint32_t S, uint32_t& seq) {
   const int lane = threadIdx.x & 31;
   const AttnRing g = attn_ring_geom(p);
-  const int n_cg = p.hd / ATTN_CH, n_tasks = p.n_head * n_cg, group = p.n_head / p.n_kv, cp = kv_ctx_pad(p.n_ctx);
+  const int n_cg = p.hd / ATTN_CH, n_tasks = p.n_head * n_cg, group = p.n_head / p.n_kv;
   for (int task = blockIdx.x; task < n_tasks; task += gridDim.x) {
     const int h = task / n_cg, cg = task % n_cg, kvh = h / group;
     const int step = min(32, ST_W * (int)S);   // lanes of one batch never share a slot (see st_producer)
@@ -636,160 +639,40 @@ __device__ __forceinline__ void st_attn_produce(const AttnParams& p, uint8_t* ri
       mbar_wait(&empty_bar[slot], st_parity(n, S) ^ 1u, 7, (int)n);
       mbar_expect_tx(&full_bar[slot], bytes * nch);
       for (int q = 0; q < nch; q++)
-        bulk_g2s(ring + (size_t)slot * ST_SLOT + (size_t)q * bytes, p.vc + ((size_t)kvh * p.hd + cg * ATTN_CH + iv * g.cv + q) * cp, bytes, &full_bar[slot]);
+        bulk_g2s(ring + (size_t)slot * ST_SLOT + (size_t)q * bytes, p.vc + v_chan(kvh, cg * ATTN_CH + iv * g.cv + q, p.n_ctx, p.hd), bytes, &full_bar[slot]);
     }
     __syncwarp();
     seq += (uint32_t)g.n_v;
   }
 }
 
-// consumer side: one (head, channel group) task, K / V of the older positions read from the ring.  Same arithmetic, same
-// order as attn_body (attention.cuh), which stays the reference implementation of the un-fused path.
+// consumer side: one (head, channel group) task, K / V of the older positions read from the ring, this position's from k16 / v16
 __device__ __forceinline__ void st_attn_task(const AttnParams& p, uint8_t* smem, const uint8_t* ring, uint64_t* full_bar, uint64_t* empty_bar, uint32_t S, uint32_t seq0,
                                              const AttnRing& g, int h, int cg, float* red_f, double* red_d) {
-  constexpr int NW = ST_W;
-  const int hd = p.hd, per = hd >> 5;
-  const int pos = g.pos, T = g.T, lim = g.lim;
-  const int group = p.n_head / p.n_kv, kvh = h / group;
-  const bool kv_writer = (h % group) == 0;
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int cp = kv_ctx_pad(p.n_ctx);
-  float* sc = (float*)smem;                             // [cp] scores, then exp values
-  uint16_t* p16 = (uint16_t*)(smem + (size_t)cp * 4);   // [cp] f16 probabilities, V-permuted order
-  uint16_t* q16 = p16 + cp;                             // [hd] f16 rotated query, K-permuted order
-  uint16_t* k16 = q16 + hd;                             // [hd] f16 rotated key of this position
-  uint16_t* v16 = k16 + hd;                             // [hd] f16 value of this position
-  {  // RoPE (pairs) + f16 conversion of q, k, v for this position; K / V rows of this position go to the cache
-    const float* qv = p.q + (size_t)h * hd;
-    const float* kv = p.k + (size_t)kvh * hd;
-    const float* vv = p.v + (size_t)kvh * hd;
-    uint16_t* kd = p.kc + k_row(kvh, pos, p.n_ctx, hd);
-    for (int i = threadIdx.x; i < hd / 2; i += ST_NT) {
-      const float2 cs = p.rope[(size_t)pos * (hd / 2) + i];
-      const int i0 = p.neox ? i : 2 * i, i1 = p.neox ? i + hd / 2 : 2 * i + 1;
-      float o0, o1;
-      rope_pair(__ldcg(qv + i0), __ldcg(qv + i1), cs, p.neox, o0, o1);
-      q16[k_perm(i0, hd)] = f2h(o0); q16[k_perm(i1, hd)] = f2h(o1);
-      rope_pair(__ldcg(kv + i0), __ldcg(kv + i1), cs, p.neox, o0, o1);
-      const uint16_t h0 = f2h(o0), h1 = f2h(o1);
-      k16[k_perm(i0, hd)] = h0; k16[k_perm(i1, hd)] = h1;
-      if (kv_writer && cg == 0) { kd[k_perm(i0, hd)] = h0; kd[k_perm(i1, hd)] = h1; }
-    }
-    for (int c = threadIdx.x; c < hd; c += ST_NT) {
-      const uint16_t hv = f2h(__ldcg(vv + c));
-      v16[c] = hv;
-      if (kv_writer && c / ATTN_CH == cg) p.vc[((size_t)kvh * hd + c) * cp + v_perm(pos)] = hv;
-    }
-  }
+  const AttnScratch s = attn_scratch(smem, p.n_ctx, p.hd, true);
+  attn_stage<ST_NT>(p, s, 0, h, cg, g.pos, attn_cs0<ST_NT>(p, g.pos));
   bar_sync<ST_BAR, ST_NT>();
-  // ---- scores: K item i belongs to warp i % NW (which also frees its slot); the current position comes from k16
-  for (int i = (int)(((uint32_t)warp + NW - seq0 % NW) % NW); i < g.n_k; i += NW) {   // K item i = ring item seq0 + i: its warp is (seq0 + i) % ST_W
+  // ---- scores: K item i = ring item seq0 + i belongs to warp (seq0 + i) % ST_W (which also frees its slot)
+  for (int i = (int)(((uint32_t)warp + ST_W - seq0 % ST_W) % ST_W); i < g.n_k; i += ST_W) {
     const uint32_t n = seq0 + (uint32_t)i, slot = st_slot(n, S);
-    const uint16_t* rows = (const uint16_t*)(ring + (size_t)slot * ST_SLOT);
-    const int r0 = i * g.rpi, nr = min(g.rpi, pos - r0);
+    const int r0 = i * g.rpi;
     mbar_wait(&full_bar[slot], st_parity(n, S), 8, (int)n);
-    if (per == 4) {
-      const uint2 qq = *(const uint2*)(q16 + lane * 4);
-      const float q0 = h2f((uint16_t)(qq.x & 0xffff)), q1 = h2f((uint16_t)(qq.x >> 16)), q2 = h2f((uint16_t)(qq.y & 0xffff)), q3 = h2f((uint16_t)(qq.y >> 16));
-      for (int t0 = 0; t0 < nr; t0 += 8) {
-        uint2 kk[8];
-#pragma unroll
-        for (int j = 0; j < 8; j++) kk[j] = *(const uint2*)(rows + (size_t)min(t0 + j, nr - 1) * hd + lane * 4);
-#pragma unroll
-        for (int j = 0; j < 8; j++) {
-          float s = 0.f;
-          s = __fmaf_rn(h2f((uint16_t)(kk[j].x & 0xffff)), q0, s);
-          s = __fmaf_rn(h2f((uint16_t)(kk[j].x >> 16)), q1, s);
-          s = __fmaf_rn(h2f((uint16_t)(kk[j].y & 0xffff)), q2, s);
-          s = __fmaf_rn(h2f((uint16_t)(kk[j].y >> 16)), q3, s);
-          s = attn_reduce_f32x8(s);
-          if (lane == 0 && t0 + j < nr) sc[r0 + t0 + j] = __fmul_rn(s, p.kq_scale);
-        }
-      }
-    } else {
-      for (int t = 0; t < nr; t++) {
-        const uint16_t* kr = rows + (size_t)t * hd + lane * per;
-        float s = 0.f;
-        for (int e = 0; e < per; e++) s = __fmaf_rn(h2f(kr[e]), h2f(q16[lane * per + e]), s);
-        s = attn_reduce_f32x8(s);
-        if (lane == 0) sc[r0 + t] = __fmul_rn(s, p.kq_scale);
-      }
-    }
+    attn_scores(p.hd, (const uint16_t*)(ring + (size_t)slot * ST_SLOT), min(g.rpi, g.pos - r0), 0, 8, s.q16, p.kq_scale, s.sc + r0);
     __syncwarp();
     if (lane == 0) mbar_arrive(&empty_bar[slot]);
   }
-  if (warp == (int)((seq0 + (uint32_t)g.n_k) % NW)) {   // the current position
-    float s = 0.f;
-    for (int e = 0; e < per; e++) s = __fmaf_rn(h2f(k16[lane * per + e]), h2f(q16[lane * per + e]), s);
-    s = attn_reduce_f32x8(s);
-    if (lane == 0) sc[pos] = __fmul_rn(s, p.kq_scale);
-  }
+  if (warp == (int)((seq0 + (uint32_t)g.n_k) % ST_W)) attn_scores(p.hd, s.k16, 1, 0, 8, s.q16, p.kq_scale, s.sc + g.pos);   // the current position
   bar_sync<ST_BAR, ST_NT>();
-  // ---- soft_max: max, fp16 exp table, fp64 sum, * (float)(1/sum)   (ggml.c:12047-12069)
-  float mx = -INFINITY;
-  for (int t = threadIdx.x; t < T; t += ST_NT) mx = fmaxf(mx, sc[t]);
-  mx = warp_max(mx);
-  if (lane == 0) red_f[warp] = mx;
-  bar_sync<ST_BAR, ST_NT>();
-  mx = red_f[0];
-#pragma unroll
-  for (int w = 1; w < NW; w++) mx = fmaxf(mx, red_f[w]);
-  double sum = 0.0;
-  for (int t = threadIdx.x; t < T; t += ST_NT) {
-    const float val = h2f(__ldg(p.exp_tab + f2h(__fsub_rn(sc[t], mx))));
-    sc[t] = val;
-    sum += (double)val;
-  }
-  sum = warp_sum(sum);
-  if (lane == 0) red_d[warp] = sum;
-  bar_sync<ST_BAR, ST_NT>();
-  sum = 0.0;
-#pragma unroll
-  for (int w = 0; w < NW; w++) sum += red_d[w];
-  const float inv = (float)(1.0 / sum);
-  const int t_end = (T + 255) & ~255;
-  for (int t = threadIdx.x; t < t_end; t += ST_NT) p16[v_perm(t)] = t < T ? f2h(__fmul_rn(sc[t], inv)) : (uint16_t)0;
-  bar_sync<ST_BAR, ST_NT>();
-  // ---- V·P for this task's channels (lane part + the leftover positions added one by one in double, ggml.c:2415-2418)
-  const int n_vec_eff = lim;                          // positions below it go through the 32 lanes (lim = min(T, n_vec))
-  const int n_total = max(T, min(p.state[3], p.n_ctx));
-  const int n_vec = n_total & ~31;
-  const int left = T - n_vec;                         // <= 31; <= 0 when the eval chunk extends past this token
-  const int ch_left = n_vec >> 8, i_left = (n_vec & 255) >> 5;
-  for (int cc = warp; cc < ATTN_CH; cc += NW) {
+  attn_softmax<ST_NT, ST_BAR>(s.sc, s.p16, g.T, p.exp_tab, red_f, red_d);
+  // ---- V·P for this task's channels
+  for (int cc = warp; cc < ATTN_CH; cc += ST_W) {
     const int c = cg * ATTN_CH + cc;
-    const int iv = cc / g.cv;
-    const uint32_t n = seq0 + (uint32_t)(g.n_k + iv), slot = st_slot(n, S);
+    const uint32_t n = seq0 + (uint32_t)(g.n_k + cc / g.cv), slot = st_slot(n, S);
     mbar_wait(&full_bar[slot], st_parity(n, S), 9, (int)n);
     const uint16_t* vrow = (const uint16_t*)(ring + (size_t)slot * ST_SLOT + (size_t)(cc % g.cv) * g.nchv * 512);
-    const uint16_t vcur = v16[c];
-    float s = 0.f;
-    for (int ch = 0; ch * 256 < n_vec_eff; ch++) {
-      const uint4 vv = *(const uint4*)(vrow + ch * 256 + lane * 8);
-      const uint4 pp = *(const uint4*)(p16 + ch * 256 + lane * 8);
-      const uint32_t vw[4] = {vv.x, vv.y, vv.z, vv.w}, pw[4] = {pp.x, pp.y, pp.z, pp.w};
-#pragma unroll
-      for (int i = 0; i < 8; i++) {
-        const int t = ch * 256 + 32 * i + lane;
-        if (t < n_vec_eff) {
-          uint16_t vh = (uint16_t)((vw[i >> 1] >> ((i & 1) * 16)) & 0xffff);
-          const uint16_t ph16 = (uint16_t)((pw[i >> 1] >> ((i & 1) * 16)) & 0xffff);
-          if (t == pos) vh = vcur;
-          s = __fmaf_rn(h2f(vh), h2f(ph16), s);
-        }
-      }
-    }
-    s = attn_reduce_f32x8(s);
-    double sumf = (double)s;
-    if (left > 0) {
-      const int t = n_vec + lane;
-      uint16_t vh = vrow[ch_left * 256 + lane * 8 + i_left];
-      const uint16_t ph16 = p16[ch_left * 256 + lane * 8 + i_left];
-      if (t == pos) vh = vcur;
-      const float term = __fmul_rn(h2f(vh), h2f(ph16));
-      for (int l = 0; l < left; l++) sumf += (double)__shfl_sync(0xffffffffu, term, l);
-    }
-    if (lane == 0) p.out[(size_t)h * hd + c] = (float)sumf;
+    const float o = attn_vp(vrow, s.p16, g, g.pos, s.v16[c]);
+    if (lane == 0) p.out[(size_t)h * p.hd + c] = o;
   }
   bar_sync<ST_BAR, ST_NT>();
   if (threadIdx.x < g.n_v) {
@@ -1086,11 +969,7 @@ inline std::vector<int> step_bounds(const Phase* phs, int n, int grid) {
 
 // can the attention phases of a model with this context feed K / V through a ring of n_slots slots?  A task holds all its V
 // items until it ends (its K items are released one by one), so they must fit beside a couple of slots of slack.
-inline bool st_attn_ring_ok(int n_ctx, int n_slots) {
-  const int nchv = (n_ctx + 255) / 256;
-  const int cv = std::max(1, std::min(8, ST_SLOT / (nchv * 512)));
-  return (ATTN_CH + cv - 1) / cv <= n_slots;
-}
+inline bool st_attn_ring_ok(int n_ctx, int n_slots) { return attn_ring_v(n_ctx).n_v <= n_slots; }
 
 // a mat-vec phase the step kernel can run: all matrices K-quant (→ Q8_K activations), K a multiple of 256
 inline bool step_supports(const MVParams& p) {
