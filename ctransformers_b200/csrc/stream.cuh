@@ -12,7 +12,8 @@
 //   producer warp   walks the phase list ahead of everybody else and keeps a ring of ST_SLOT-byte shared-memory slots full:
 //                   one cp.async.bulk (TMA bulk copy, completion on an mbarrier) per work item.  Weights do not depend on
 //                   activations, so the copies for the next phases are already in flight (or landed) while the consumers
-//                   still wait at a grid barrier, stage an activation vector or run attention: HBM never idles.
+//                   still wait at a grid barrier, stage an activation vector or run attention, until the ring is full
+//                   (one ring is about 8 us of HBM time on an H100; DESIGN.md §5.2 has what the boundaries cost).
 //   work item       (16-row tile, chunk of 3-4 consecutive 256-weight blocks): 16 x {144,176,210} bytes per block, contiguous
 //                   in the STREAM layout written at load time (k_repack_stream).  Items are numbered in one sequence that both
 //                   sides enumerate identically; item n belongs to consumer warp n % ST_W and lives in one of that warp's slots.
@@ -150,6 +151,16 @@ __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity, int co
 // global → shared bulk copy (TMA, SASS UBLKCP), completion counted in bytes on `bar`
 __device__ __forceinline__ void bulk_g2s(void* dst, const void* src, uint32_t bytes, uint64_t* bar) {
   asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];" ::"r"(st_smem(dst)), "l"(src), "r"(bytes), "r"(st_smem(bar)) : "memory");
+}
+// the same with an L2 cache policy (createpolicy) for the lines it reads
+__device__ __forceinline__ void bulk_g2s_hint(void* dst, const void* src, uint32_t bytes, uint64_t* bar, uint64_t pol) {
+  asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes.L2::cache_hint [%0], [%1], %2, [%3], %4;" ::"r"(st_smem(dst)), "l"(src), "r"(bytes),
+               "r"(st_smem(bar)), "l"(pol) : "memory");
+}
+__device__ __forceinline__ uint64_t l2_policy_evict_first() {
+  uint64_t p;
+  asm volatile("createpolicy.fractional.L2::evict_first.b64 %0, 1.0;" : "=l"(p));
+  return p;
 }
 // D(16x8, s32) = A(16x32, u8, row) · B(32x8, s8, col) + C.  Fragments (PTX ISA, m16n8k32 8-bit): a0 = row g, k 4t..4t+3; a1 = row
 // g+8, same k; a2 = row g, k 16+4t..; a3 = row g+8, k 16+4t..;  b0 = k 4t..4t+3, col g;  b1 = k 16+4t.., col g;  d0/d1 = row g,
@@ -681,10 +692,14 @@ __device__ __forceinline__ void st_attn_task(const AttnParams& p, uint8_t* smem,
   }
 }
 
-// Producer warp: the same enumeration as the consumers, one bulk copy per item, as far ahead as the ring allows.
+// Producer warp: the same enumeration as the consumers, one bulk copy per item, as far ahead as the ring allows.  The weight
+// copies read with an L2 evict-first policy: a weight line is dead once its ring copy has read it (the next read is a step
+// later, 4 GB of stream away), so the stream's lines go first and the step's live data (KV cache, activation vectors, exp
+// table) stays in L2.  K / V items keep the default policy.
 __device__ __forceinline__ void st_producer(const StepArgs& args, uint8_t* ring, uint64_t* full_bar, uint64_t* empty_bar) {
   const int lane = threadIdx.x & 31;
   const uint32_t S = (uint32_t)(args.n_slots / ST_W);   // ring depth per consumer warp
+  const uint64_t weight_pol = l2_policy_evict_first();
   uint32_t seq = 0;
   for (int ip = 0; ip < args.n_phases; ip++) {
     const Phase* ph = args.prog + ip;
@@ -720,7 +735,7 @@ __device__ __forceinline__ void st_producer(const StepArgs& args, uint8_t* ring,
             const uint32_t bytes = (uint32_t)(nblk * bb);
             mbar_wait(&empty_bar[slot], st_parity(n, S) ^ 1u, 4, (int)n);
             mbar_expect_tx(&full_bar[slot], bytes);
-            bulk_g2s(ring + (size_t)slot * ST_SLOT, src, bytes, &full_bar[slot]);
+            bulk_g2s_hint(ring + (size_t)slot * ST_SLOT, src, bytes, &full_bar[slot], weight_pol);
           }
           __syncwarp();
         }
