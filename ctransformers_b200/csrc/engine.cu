@@ -1206,20 +1206,8 @@ bool Engine::ensure_prefill() {
       ph.kind = PP_KV; prog.push_back(ph);
       ph.kind = PP_ATTN; prog.push_back(ph);
     } else {
-      const MVParams& m = op.ph.mv;
-      K_max = std::max(K_max, m.K);
-      ph.mv = m;
-      ph.mv.norm_out = nullptr;
-      ph.mv.x = bat(m.x, ph.x_ld);
-      ph.mv.x2 = bat(m.x2, ph.x2_ld);
-      ph.qbuf = (uint8_t*)dalloc(pb_qbuf_bytes(m.K));   // one buffer per phase: nothing stale can sit in an L1
-      ph.kind = PP_QUANT; prog.push_back(ph);
-      for (int sgi = 0; sgi < m.nseg; sgi++) {
-        ph.mv.seg[sgi].out = bat(m.seg[sgi].out, ph.out_ld[sgi]);
-        ph.mv.seg[sgi].res = bat(m.seg[sgi].res, ph.res_ld[sgi]);
-        ph.mv.seg[sgi].res2 = bat(m.seg[sgi].res2, ph.res2_ld[sgi]);
-      }
-      ph.kind = PP_GEMM; prog.push_back(ph);
+      K_max = std::max(K_max, op.ph.mv.K);
+      pb_matvec_phases(op.ph.mv, (uint8_t*)dalloc(pb_qbuf_bytes(op.ph.mv.K)), P.d_state, bat, prog);
     }
   }
   int ld;

@@ -431,6 +431,90 @@ int ctb_attention_path(int path, const float* q, const float* k_new, const float
   });
 }
 
+int ctb_prefill_mul_mat(int nseg, const int* types, const void* const* w_blocks, const int* rows, int K, int n_tok, const float* x,
+                        const float* x2, int norm_mode, const float* norm_w, const float* norm_b, float eps, const int* epi,
+                        const float* res, const float* res2, float* out, int n_ctx, int head_dim, int* n_slots) {
+  return guarded("ctb_prefill_mul_mat", [&] {
+    if (nseg < 1 || nseg > MV_MAX_SEG) throw std::runtime_error("1 to 3 segments");
+    if (K < 256 || K % 256) throw std::runtime_error("K must be a positive multiple of 256");
+    if (n_tok < 1) throw std::runtime_error("n_tok must be at least 1");
+    if (norm_mode < NORM_NONE || norm_mode > NORM_LAYER || (x2 && norm_mode != NORM_NONE)) throw std::runtime_error("norm mode 0, 1 or 2, and 0 with x2");
+    if ((norm_mode != NORM_NONE && !norm_w) || (norm_mode == NORM_LAYER && !norm_b)) throw std::runtime_error("RMSNorm needs norm_w, LayerNorm norm_w and norm_b");
+    if (norm_mode == NORM_NONE) norm_w = nullptr;   // the prologue applies whatever weight and bias it is given: only the mode's own
+    if (norm_mode != NORM_LAYER) norm_b = nullptr;
+    if (head_dim != 64 && head_dim != 128) throw std::runtime_error("head_dim must be 64 or 128");
+    if (n_ctx < 1) throw std::runtime_error("n_ctx must be at least 1");
+    int off[MV_MAX_SEG + 1] = {0};
+    for (int s = 0; s < nseg; s++) {
+      if (!type_is_kquant(types[s])) throw std::runtime_error("the batched kernel takes K-quant weights only");
+      if (rows[s] < 1) throw std::runtime_error("every segment needs at least one row");
+      if (epi[s] < EPI_STORE || epi[s] > EPI_SILU) throw std::runtime_error("unknown epilogue");
+      if ((epi[s] == EPI_ADD || epi[s] == EPI_ADD2) && !res) throw std::runtime_error("ADD / ADD2 need res");
+      if (epi[s] == EPI_ADD2 && !res2) throw std::runtime_error("ADD2 needs res2");
+      off[s + 1] = off[s] + rows[s];
+    }
+    const int W = off[nseg];
+    int slots = 0;
+    size_t smem = 0;
+    if (!pstep_shape(pb_work_bytes(K, n_ctx, head_dim), slots, smem)) throw std::runtime_error("no batched prefill at this n_ctx: its attention scratch does not fit");
+    std::unique_ptr<OwnedMat> mats[MV_MAX_SEG];
+    for (int s = 0; s < nseg; s++) {
+      mats[s].reset(new OwnedMat());
+      upload(*mats[s], types[s], w_blocks[s], K, rows[s]);
+    }
+    // PB_T-row token buffers, reused by every launch like the engine's batched buffers (rows past a short batch keep the previous
+    // launch's values), and the QUANT phase's qbuf zeroed like the engine's
+    DevBuf dx((size_t)PB_T * K * 4), dx2((size_t)PB_T * K * 4), dout((size_t)PB_T * W * 4), dres((size_t)PB_T * W * 4), dres2((size_t)PB_T * W * 4),
+        dnw((size_t)K * 4), dnb((size_t)K * 4), dq(pb_qbuf_bytes(K)), dst((PB_T * 4 + 4) * 4);
+    OPS_CUDA(cudaMemset(dq.p, 0, pb_qbuf_bytes(K)));
+    OPS_CUDA(cudaMemset(dout.p, 0, (size_t)PB_T * W * 4));
+    if (norm_w) OPS_CUDA(cudaMemcpy(dnw.p, norm_w, (size_t)K * 4, cudaMemcpyHostToDevice));
+    if (norm_b) OPS_CUDA(cudaMemcpy(dnb.p, norm_b, (size_t)K * 4, cudaMemcpyHostToDevice));
+    MVParams m{};
+    m.x = dx.as<float>(); m.x2 = x2 ? dx2.as<float>() : nullptr; m.x_mode = x2 ? 1 : 0;
+    m.norm_w = norm_w ? dnw.as<float>() : nullptr; m.norm_b = norm_b ? dnb.as<float>() : nullptr; m.norm_mode = norm_mode; m.eps = eps;
+    m.K = K; m.act = ACT_Q8_K; m.nseg = nseg; m.silu_tab = tables().silu; m.gelu_tab = tables().gelu;
+    for (int s = 0; s < nseg; s++) {
+      m.seg[s].w = mats[s]->m; m.seg[s].out = dout.as<float>() + off[s]; m.seg[s].epi = epi[s];
+      if (epi[s] == EPI_ADD || epi[s] == EPI_ADD2) m.seg[s].res = dres.as<float>() + off[s];
+      if (epi[s] == EPI_ADD2) m.seg[s].res2 = dres2.as<float>() + off[s];
+    }
+    struct Rows { const float* p; int ld; };
+    const Rows bufs[5] = {{dx.as<float>(), K}, {dx2.as<float>(), K}, {dout.as<float>(), W}, {dres.as<float>(), W}, {dres2.as<float>(), W}};
+    auto bat = [&](const float* p, int& ld) -> float* {
+      ld = 0;
+      if (!p) return nullptr;
+      for (const Rows& b : bufs)
+        if (p >= b.p && p < b.p + (size_t)PB_T * b.ld) { ld = b.ld; return const_cast<float*>(p); }
+      throw std::runtime_error("pointer outside the token buffers");
+    };
+    std::vector<PPhase> prog;
+    pb_matvec_phases(m, dq.as<uint8_t>(), dst.as<int>(), bat, prog);
+    DevBuf dprog((prog.size() + 1) * sizeof(PPhase));
+    OPS_CUDA(cudaMemcpy(dprog.p, prog.data(), prog.size() * sizeof(PPhase), cudaMemcpyHostToDevice));
+    OPS_CUDA(pstep_set_smem_limit(smem));
+    // launches of at most PB_T tokens over the same program and buffers, as eval_list cuts a run of prompt tokens
+    for (int b = 0; b < n_tok; b += PB_T) {
+      const int n = std::min(PB_T, n_tok - b);
+      std::vector<int> st(PB_T * 4 + 4, 0);
+      for (int i = 0; i < PB_T; i++) {
+        const int k = std::min(i, n - 1);
+        st[i * 4 + 1] = b + k; st[i * 4 + 3] = b + k + 1;
+      }
+      st[PB_T * 4] = n;
+      OPS_CUDA(cudaMemcpy(dst.p, st.data(), st.size() * 4, cudaMemcpyHostToDevice));
+      OPS_CUDA(cudaMemcpy(dx.p, x + (size_t)b * K, (size_t)n * K * 4, cudaMemcpyHostToDevice));
+      if (x2) OPS_CUDA(cudaMemcpy(dx2.p, x2 + (size_t)b * K, (size_t)n * K * 4, cudaMemcpyHostToDevice));
+      if (res) OPS_CUDA(cudaMemcpy(dres.p, res + (size_t)b * W, (size_t)n * W * 4, cudaMemcpyHostToDevice));
+      if (res2) OPS_CUDA(cudaMemcpy(dres2.p, res2 + (size_t)b * W, (size_t)n * W * 4, cudaMemcpyHostToDevice));
+      OPS_CUDA(launch_pstep(sm_count(), slots, smem, 0, dprog.as<PPhase>(), (int)prog.size(), sync_words()));
+      OPS_CUDA(cudaDeviceSynchronize());
+      OPS_CUDA(cudaMemcpy(out + (size_t)b * W, dout.p, (size_t)n * W * 4, cudaMemcpyDeviceToHost));
+    }
+    if (n_slots) *n_slots = slots;
+  });
+}
+
 int ctb_ffn_gate(int type, const void* w1_blocks, const void* w3_blocks, const float* x, float* out, int K, int M) {
   return guarded("ctb_ffn_gate", [&] {
     OwnedMat w1, w3;

@@ -500,6 +500,26 @@ inline bool pstep_shape(size_t work, int& n_slots, size_t& smem) {
   smem = (size_t)n_slots * ST_SLOT + work;
   return true;
 }
+// The QUANT + GEMM phase pair of one mat-vec m over PB_T-token buffers.  bat(p, ld) maps each activation pointer of m (x, x2, a
+// segment's out / res / res2) to its PB_T-row buffer and sets ld to the floats between token rows (null: null, 0).  qbuf holds
+// pb_qbuf_bytes(m.K), one per pair: nothing stale of another phase can sit in an L1.
+template <typename Bat>
+inline void pb_matvec_phases(const MVParams& m, uint8_t* qbuf, const int* state, Bat&& bat, std::vector<PPhase>& prog) {
+  PPhase ph{};
+  ph.state = state;
+  ph.mv = m;
+  ph.mv.norm_out = nullptr;
+  ph.mv.x = bat(m.x, ph.x_ld);
+  ph.mv.x2 = bat(m.x2, ph.x2_ld);
+  ph.qbuf = qbuf;
+  ph.kind = PP_QUANT; prog.push_back(ph);
+  for (int s = 0; s < m.nseg; s++) {
+    ph.mv.seg[s].out = bat(m.seg[s].out, ph.out_ld[s]);
+    ph.mv.seg[s].res = bat(m.seg[s].res, ph.res_ld[s]);
+    ph.mv.seg[s].res2 = bat(m.seg[s].res2, ph.res2_ld[s]);
+  }
+  ph.kind = PP_GEMM; prog.push_back(ph);
+}
 static inline cudaError_t pstep_set_smem_limit(size_t bytes) { return cudaFuncSetAttribute(k_pstep, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes); }
 static inline cudaError_t launch_pstep(int grid, int n_slots, size_t smem, cudaStream_t st, const PPhase* d_prog, int n_phases, unsigned* d_sync) {
   PStepArgs a;

@@ -151,6 +151,23 @@ int ctb_attention(const float* q, const uint16_t* kcache, const uint16_t* vcache
 int ctb_attention_path(int path, const float* q, const float* k_new, const float* v_new, uint16_t* kcache, uint16_t* vcache,
                        float* out, int n_head, int n_kv, int head_dim, int n_ctx, int pos0, int n_tok, const int* n_total,
                        int rope_mode, float freq_base, float kq_scale);
+/* n_tok activation rows through one mat-vec of the batched prefill kernel (k_pstep: its QUANT + GEMM phase pair), launched the
+ * way the engine launches it: the engine's grid, the ring depth pstep_shape gives a model of this n_ctx and head_dim, one
+ * quantized-activation buffer and PB_T-row token buffers reused by launches of at most 32 tokens (70 tokens run as 32 + 32 + 6).
+ * Equals ggml_mul_mat with n_tok columns (ggml.c:11031-11245) plus the engine's prologue and epilogues:
+ *   input  row i of x [n_tok][K]; x2 non-null: x * x2 (ggml_mul, the down projection's silu(gate) * up); norm_mode 1 RMSNorm * w,
+ *          2 LayerNorm * w + b (norm_w / norm_b [K], eps; a mode ignores what it does not use), 0 none (required with x2); then
+ *          quantize_row_q8_K
+ *   rows   nseg (1..3) K-quant matrices (types[s] 12 Q4_K, 13 Q5_K, 14 Q6_K; w_blocks[s]: rows[s] rows of K weights in the
+ *          reference's block layout) whose outputs sit side by side: out [n_tok][W], W = rows[0] + .. + rows[nseg-1]
+ *   epi[s] 0 STORE v, 1 ADD v + res, 3 ADD2 (v + res) + res2, 2 GELU / 4 SILU: the fp16 table of v (ggml.c:3600-3632);
+ *          res / res2 [n_tok][W] in out's layout, read only by the segments that add them
+ * *n_slots (if non-null) gets the ring slots used.  0 on success, -1 (with a message on stderr) for what the kernel cannot take: a
+ * type other than Q4_K / Q5_K / Q6_K, K not a multiple of 256, more than 3 segments, n_tok < 1, or an n_ctx whose attention
+ * scratch leaves no ring (the engine then has no batched prefill). */
+int ctb_prefill_mul_mat(int nseg, const int* types, const void* const* w_blocks, const int* rows, int K, int n_tok, const float* x,
+                        const float* x2, int norm_mode, const float* norm_w, const float* norm_b, float eps, const int* epi,
+                        const float* res, const float* res2, float* out, int n_ctx, int head_dim, int* n_slots);
 /* silu(W1 x) * (W3 x) with the fp16 SiLU table (ggml.c:3625-3632) — the fused FFN gate. */
 int ctb_ffn_gate(int type, const void* w1_blocks, const void* w3_blocks, const float* x, float* out, int K, int M);
 /* ggml_get_rows on a quantized table (ggml.c:11615-11642). */

@@ -11,7 +11,8 @@ Contents
   reference_blocks.npz  blocks written by the reference's quantizer, the pool of refs.reference_quantized_blocks
   reference_runs.npz  what the reference computed for each test that compares with it (tests/test_model_gpu.py,
                    tests/test_oracle.py, tests/test_long_context_gpu.py), so those tests run where the reference is not
-                   available.  `python make_golden.py long_context` adds the long-context runs to the existing file.
+                   available.  `python make_golden.py long_context` adds the long-context runs to the existing file,
+                   `python make_golden.py realq_prefill` the reference-quantized Q5_K_M prefill runs.
 """
 import ctypes as C
 import json
@@ -205,6 +206,25 @@ def long_context_runs(tmp):
     assert all(np.array_equal(new[k], v) and new[k].dtype == v.dtype for k, v in old.items()), "an existing key changed"
 
 
+def realq_prefill_runs(tmp):
+    """Adds the reference's results for modelcases.REALQ_PREFILL to reference_runs.npz as keys prefill_<key>_*; every key already
+    in the file keeps its bytes."""
+    old = dict(refs.golden_runs())
+    out = dict(old)
+    for key, (arch, ftype) in modelcases.REALQ_PREFILL.items():
+        path = modelcases.build_realq(tmp, arch, ftype)
+        run = modelcases.run_greedy(ref_llm(path, modelcases.REALQ_PREFILL_CTX), modelcases.realq_prompt(arch), modelcases.REALQ_PREFILL_NEW,
+                                    batch_size=512)
+        first_logits, first_embd, toks, last_logits, _ = run
+        for k, v in (("first_logits", first_logits), ("first_embd", first_embd), ("last_logits", last_logits)):
+            out[f"prefill_{key}_{k}"] = np.array(refs.digest(v))
+        out[f"prefill_{key}_tokens"] = np.array(toks, np.int32)
+        print(key, "tokens", toks)
+    np.savez_compressed(HERE / "reference_runs.npz", **out)
+    new = refs.golden_runs()
+    assert all(np.array_equal(new[k], v) and new[k].dtype == v.dtype for k, v in old.items()), "an existing key changed"
+
+
 if __name__ == "__main__":
     assert refs.have_ref(), "build oracle/_ref first: make -C oracle ref"
     import sys
@@ -219,7 +239,9 @@ if __name__ == "__main__":
                 reference_runs(tmp)
             if "long_context" in only:
                 long_context_runs(tmp)
-            cases = [o for o in only if o not in ("kat", "reference_blocks", "reference_runs", "long_context")]
+            if "realq_prefill" in only:
+                realq_prefill_runs(tmp)
+            cases = [o for o in only if o not in ("kat", "reference_blocks", "reference_runs", "long_context", "realq_prefill")]
             if cases:
                 models(tmp, cases)
         else:

@@ -93,15 +93,32 @@ def oracle_greedy(model, prompt, n_new, batch_size):
 REALQ_PROMPT = [1] + np.random.default_rng(0).integers(259, 1024, 30).tolist()
 
 
-def build_realq(directory):
-    """A Q4_K_M Llama whose weights are blocks of the reference's quantizer (refs.reference_quantized_blocks)."""
+def build_realq(directory, arch="llama", ftype="Q4_K_M"):
+    """A model whose weights are blocks of the reference's quantizer (refs.reference_quantized_blocks): Q4_K_M Llama by default."""
     import refs
-    path = Path(directory) / "realq.gguf"
+    path = Path(directory) / ("realq.gguf" if (arch, ftype) == ("llama", "Q4_K_M") else f"realq_{arch}_{ftype.lower()}.gguf")
     if not path.exists():
-        shape = synth.LlamaShape(n_vocab=1024, n_embd=512, n_head=4, n_head_kv=4, n_ff=1536, n_layer=2, n_ctx_train=128)
-        synth.write_llama(path, shape, "Q4_K_M", seed=3, sigma=0.05,
-                          quantizer=lambda t, w: refs.reference_quantized_blocks(t, w.shape[1], w.shape[0], seed=w.shape[0] * 7 + t))
+        if arch == "llama":
+            shape = synth.LlamaShape(n_vocab=1024, n_embd=512, n_head=4, n_head_kv=4, n_ff=1536, n_layer=2, n_ctx_train=128)
+        else:
+            shape = synth.FalconShape(n_vocab=1024, n_embd=512, n_head=8, n_head_kv=1, n_ff=2048, n_layer=2, n_ctx_train=128)
+        (synth.write_llama if arch == "llama" else synth.write_falcon)(
+            path, shape, ftype, seed=3, sigma=0.05,
+            quantizer=lambda t, w: refs.reference_quantized_blocks(t, w.shape[1], w.shape[0], seed=w.shape[0] * 7 + t))
     return path
+
+
+# Reference-quantized Q5_K_M models through batched prefill: key -> (arch, ftype).  Their Q5_K blocks have mins that differ from
+# their scales, which no random-block model has.  A 70-token prompt at batch_size 512: launches of 32 + 32 + 6 tokens.
+REALQ_PREFILL = {"realq_llama_q5km": ("llama", "Q5_K_M"), "realq_falcon_q5km": ("falcon", "Q5_K_M")}
+REALQ_PREFILL_CTX, REALQ_PREFILL_NEW = 96, 6
+
+
+def realq_prompt(arch):
+    ids = np.random.default_rng(9).integers(259 if arch == "llama" else 0, 1024, 70).tolist()
+    if arch == "llama":
+        ids[0] = 1
+    return ids
 
 
 def run_greedy(llm, prompt, n_new, batch_size=8):

@@ -119,6 +119,60 @@ def reference_quantized_blocks(t, k, m, seed):
     return np.ascontiguousarray(pool[idx].reshape(-1))
 
 
+def _f16_edge(rng, n):
+    """n f16 bit patterns of both signs: mostly normal values 2^-16 .. 2^-6, a fifth subnormal (bits 1 .. 1023), a few zeros."""
+    mag = np.exp2(rng.uniform(-16, -6, n)).astype(np.float16).view(np.uint16)
+    kind = rng.integers(0, 10, n)
+    mag[kind < 2] = rng.integers(1, 1024, int((kind < 2).sum()))
+    mag[kind == 9] = 0
+    return mag | (rng.integers(0, 2, n).astype(np.uint16) << 15)
+
+
+def edge_blocks(t, k, m, seed):
+    """m rows of k weights of type t (Q4_K / Q5_K / Q6_K bytes) at the edges of the block formats, where random_blocks and the
+    reference's quantizer do not go.  Sub-block scales and mins are drawn from shuffled runs of all their values, independently
+    of each other: blocks 8i .. 8i+7 together hold every 6-bit scale and every 6-bit min (Q4_K / Q5_K), blocks 16i .. 16i+15
+    every Q6_K scale -128..127.  Whole sub-blocks have all-zero or all-set quants (and for Q5_K / Q6_K only the low or only the high bits set),
+    d and dmin have both signs and reach f16 subnormals and zero; no inf or NaN."""
+    rng = np.random.default_rng(seed)
+    bs, sz = BLOCK[t]
+    nb = m * (k // bs)
+    nsub, qmax, consts = {Q4_K: (8, 15, (0, 15)), Q5_K: (8, 31, (0, 31, 15, 16)), Q6_K: (16, 63, (0, 63, 15, 48))}[t]
+
+    def runs(values, n):   # n draws: concatenated shuffles of all values
+        return np.concatenate([rng.permutation(values) for _ in range(-(-n // len(values)))])[:n].reshape(nb, -1)
+
+    q = rng.integers(0, qmax + 1, (nb, nsub, 256 // nsub))
+    pat = np.arange(nb * nsub).reshape(nb, nsub) % (2 * len(consts))   # every other sub-block random, the rest cycle the constants
+    for i, c in enumerate(consts):
+        q[pat == 2 * i + 1] = c
+    q = q.reshape(nb, 256)
+    out = np.zeros((nb, sz), np.uint8)
+    if t in (Q4_K, Q5_K):
+        sc, mn = runs(np.arange(64), nb * 8), runs(np.arange(64), nb * 8)
+        out[:, 0:2] = _f16_edge(rng, nb).view(np.uint8).reshape(nb, 2)
+        out[:, 2:4] = _f16_edge(rng, nb).view(np.uint8).reshape(nb, 2)
+        s = out[:, 4:16]                                                  # inverse of get_scale_min_k4 (k_quants.c:306-313)
+        s[:, 0:4] = sc[:, 0:4] | ((sc[:, 4:8] >> 4) << 6)
+        s[:, 4:8] = mn[:, 0:4] | ((mn[:, 4:8] >> 4) << 6)
+        s[:, 8:12] = (sc[:, 4:8] & 0xF) | ((mn[:, 4:8] & 0xF) << 4)
+        qs = out[:, 16:144] if t == Q4_K else out[:, 48:176]
+        for j in range(4):                                                # 64 weights per 32 bytes: sub-block 2j low nibbles, 2j+1 high
+            lo, hi = q[:, 64 * j:64 * j + 32], q[:, 64 * j + 32:64 * j + 64]
+            qs[:, 32 * j:32 * j + 32] = (lo & 15) | ((hi & 15) << 4)
+            if t == Q5_K:                                                 # qh bit 2j / 2j+1 of byte l: 5th bit of weight l of those sub-blocks
+                out[:, 16:48] |= ((lo >> 4) << (2 * j) | (hi >> 4) << (2 * j + 1)).astype(np.uint8)
+    else:   # Q6_K: ql[128] qh[64] scales[16] d (dequantize_row_q6_K, k_quants.c:1083-1117)
+        out[:, 192:208] = runs(np.arange(-128, 128), nb * 16).astype(np.int8).view(np.uint8)
+        out[:, 208:210] = _f16_edge(rng, nb).view(np.uint8).reshape(nb, 2)
+        for n in range(2):
+            for j in range(4):
+                v = q[:, 128 * n + 32 * j:128 * n + 32 * j + 32]
+                out[:, 64 * n + 32 * (j & 1):64 * n + 32 * (j & 1) + 32] |= ((v & 15) << (4 * (j >> 1))).astype(np.uint8)
+                out[:, 128 + 32 * n:128 + 32 * n + 32] |= ((v >> 4) << (2 * j)).astype(np.uint8)
+    return np.ascontiguousarray(out.reshape(-1))
+
+
 def ref_traits(t):
     tr = ref().ggml_internal_get_type_traits(t)
     to_float = C.CFUNCTYPE(None, C.c_void_p, C.c_void_p, C.c_int)(tr.to_float) if tr.to_float else None

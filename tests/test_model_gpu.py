@@ -198,6 +198,31 @@ def test_prefill_against_live_reference(name, bs, model_dir):
     same_as_reference(f"prefill_{name}_bs{bs}", modelcases.run_greedy(load(path, 96), modelcases.long_prompt(name), 6, batch_size=bs))
 
 
+@pytest.mark.parametrize("key", list(modelcases.REALQ_PREFILL))
+def test_prefill_real_quantized_q5km(key, model_dir, monkeypatch):
+    """Q5_K_M weights from the reference's quantizer (Q5_K mins that differ from the scales) through a 70-token prompt at
+    batch_size 512: once through the batched kernel (3 launches) and once token by token (CTB_NO_PREFILL=1), each equal to the
+    oracle and to the reference's digests."""
+    arch, ftype = modelcases.REALQ_PREFILL[key]
+    path = modelcases.build_realq(model_dir, arch, ftype)
+    prompt, ctx, n_new = modelcases.realq_prompt(arch), modelcases.REALQ_PREFILL_CTX, modelcases.REALQ_PREFILL_NEW
+    want = modelcases.oracle_greedy(refs.OracleModel(path, ctx), prompt, n_new, 512)
+    for env, launches in (({}, 3), ({"CTB_NO_PREFILL": "1"}, 0)):
+        with monkeypatch.context() as mp:
+            for k, v in env.items():
+                mp.setenv(k, v)
+            llm = load(path, ctx)
+            run = modelcases.run_greedy(llm, prompt, n_new, batch_size=512)
+        paths = (C.c_int * 6)()
+        assert llm.ctb_llm_paths(paths, 6) == 6
+        assert paths[4] == launches, f"batched prefill launches {paths[4]}, expected {launches}"
+        for i, what in ((0, "logits after the prompt"), (1, "hidden state after the prompt"), (3, "logits after the last step")):
+            got, exp = np.ascontiguousarray(run[i], np.float32), np.ascontiguousarray(want[i], np.float32)
+            assert np.array_equal(got.view(np.uint32), exp.view(np.uint32)), f"{env}: {what} differ from the oracle"
+        assert run[2] == want[2]
+        same_as_reference(f"prefill_{key}", run)
+
+
 def test_prefill_equals_single_token_path(model_dir, monkeypatch):
     """The batched kernel and the single-token kernel are two implementations of the same arithmetic: identical bits."""
     path, _ = modelcases.build("llama_wide_q4km", model_dir)

@@ -283,12 +283,15 @@ def test_attention_path_rejects_n_total_outside_the_context(lib):
                                       10000.0, 0.125) == -1
 
 
-@pytest.mark.parametrize("t", [Q4_K, Q5_K, Q4_0, Q5_0])
-def test_ffn_gate_vs_oracle(lib, t):
+@pytest.mark.parametrize("t,src", [pytest.param(t, "random", id=str(t)) for t in (Q4_K, Q5_K, Q4_0, Q5_0)] +
+                         [pytest.param(t, "edge", id=f"{t}-edge") for t in (Q4_K, Q5_K)])
+def test_ffn_gate_vs_oracle(lib, t, src):
+    """src "edge": refs.edge_blocks, every scale and min value and the quant extremes."""
     o = refs.oracle()
     k, m = 4096, 96
     rng = np.random.default_rng(t)
-    w1, w3 = _rand_weights(t, k, m, 1), _rand_weights(t, k, m, 2)
+    gen = _rand_weights if src == "random" else refs.edge_blocks
+    w1, w3 = gen(t, k, m, 1), gen(t, k, m, 2)
     x = _act(rng, k)
     g, u = np.zeros(m, np.float32), np.zeros(m, np.float32)
     o.orc_mul_mat(t, ptr(w1), ptr(x), ptr(g), k, m, 1)
@@ -321,16 +324,186 @@ def test_get_row_bit_exact(lib, t):
         assert np.array_equal(got.view(np.uint32), np.ascontiguousarray(want[r]).view(np.uint32))
 
 
-@pytest.mark.parametrize("t", [Q4_K, Q5_K, Q6_K, Q4_0, Q5_0, Q8_0])
+@pytest.mark.parametrize("t,src", [pytest.param(t, "refq", id=str(t)) for t in (Q4_K, Q5_K, Q6_K, Q4_0, Q5_0, Q8_0)] +
+                         [pytest.param(t, "edge", id=f"{t}-edge") for t in (Q4_K, Q5_K, Q6_K)])
 @pytest.mark.parametrize("k", [512, 1024, 2816])
-def test_mul_mat_real_quantized_weights(lib, t, k):
-    """Weights produced by the reference's quantizer (all scale/min bit patterns occur, unlike the random-block generator)."""
+def test_mul_mat_real_quantized_weights(lib, t, src, k):
+    """src "refq": weights produced by the reference's quantizer (scale / min bit patterns the random-block generator does not
+    write); "edge": refs.edge_blocks, every scale and min value (the pool's 6-bit scales stop at 26), all-zero and all-set quants,
+    negative and subnormal d / dmin."""
     o = refs.oracle()
     rng = np.random.default_rng(k + t)
     m = 48
-    w = refs.reference_quantized_blocks(t, k, m, seed=k + t)
+    w = (refs.reference_quantized_blocks if src == "refq" else refs.edge_blocks)(t, k, m, seed=k + t)
     x = _act(rng, k)[None]
     want, got = np.zeros((1, m), np.float32), np.zeros((1, m), np.float32)
     assert o.orc_mul_mat(t, ptr(w), ptr(x), ptr(want), k, m, 1) == 0
     assert lib.ctb_mul_mat(t, ptr(w), ptr(x), ptr(got), k, m, 1) == 0
     _same_bits(got, want)
+
+
+# ---- the batched prefill kernel's mat-mul (csrc/prefill.cuh k_pstep, QUANT + GEMM phases) through ctb_prefill_mul_mat.  Its
+# integer part is a second implementation of the K-quant dot products (scale digits on tensor cores), with its own mins chains,
+# short-batch bookkeeping and epilogue; the expected values are orc_mul_mat with N = n_tok columns, prologue and epilogue from
+# oracle pieces in the reference's order.
+STORE, ADD, GELU, ADD2, SILU = 0, 1, 2, 3, 4
+PF_SOURCES = {"random": _rand_weights, "refq": refs.reference_quantized_blocks, "edge": refs.edge_blocks}
+PF_TOKENS = [1, 2, 7, 8, 9, 31, 32, 70]   # 70: launches of 32 + 32 + 6 on the same buffers, the short one after full ones
+# name: (segments [(type, rows, epilogue)], K, n_tok, norm mode, x2 (x_mode 1), weight source)
+PF_SHAPES = {
+    "k256-m5": ([(Q5_K, 5, STORE)], 256, 70, 1, False, "edge"),
+    "k256-m1": ([(Q6_K, 1, STORE)], 256, 9, 0, False, "edge"),            # one tile in the whole grid: one CTA, one team idle
+    "k11008-m3-add": ([(Q4_K, 3, ADD)], 11008, 33, 0, False, "refq"),
+    "3seg-mixed-epilogues": ([(Q4_K, 17, GELU), (Q5_K, 40, SILU), (Q6_K, 9, ADD2)], 1024, 40, 2, False, "edge"),
+    "x2-add": ([(Q5_K, 50, ADD)], 2816, 12, 0, True, "edge"),
+    # the bench's Llama-2-7B Q4_K_M layer (QKV with the more-bits V in Q6_K; gate + up; down on silu(gate) * up)
+    "7b-qkv": ([(Q4_K, 4096, STORE), (Q4_K, 1024, STORE), (Q6_K, 1024, STORE)], 4096, 5, 1, False, "random"),
+    "7b-gate-up": ([(Q4_K, 11008, SILU), (Q4_K, 11008, STORE)], 4096, 5, 1, False, "random"),
+    "7b-down": ([(Q6_K, 4096, ADD)], 11008, 5, 0, True, "random"),
+    # the Falcon-7B-shaped Q5_K_M layer: LayerNorm + fused wqkv and up (GELU), down + attention output + layer input
+    "falcon7b-qkv-up": ([(Q5_K, 4736, STORE), (Q5_K, 18432, GELU)], 4608, 3, 2, False, "random"),
+    "falcon7b-down": ([(Q6_K, 4608, ADD2)], 18432, 3, 0, False, "random"),
+}
+
+
+def _pf_inputs(segs, k, n_tok, norm, with_x2, src, seed):
+    rng = np.random.default_rng(seed)
+    ws = [np.ascontiguousarray(PF_SOURCES[src](t, k, m, seed + 10 * i)) for i, (t, m, _) in enumerate(segs)]
+    x = np.stack([_act(rng, k, [1e-3, 1.0, 300.0][i % 3]) for i in range(n_tok)])
+    x[0, :256] = 0.0                                                  # an all-zero block: Q8_K d = 0
+    x2 = np.stack([_act(rng, k, 0.5) for _ in range(n_tok)]) if with_x2 else None
+    nw = (1 + 0.1 * rng.standard_normal(k)).astype(np.float32)
+    nb = (0.1 * rng.standard_normal(k)).astype(np.float32)
+    W = sum(m for _, m, _ in segs)
+    res = (rng.standard_normal((n_tok, W)) * 2).astype(np.float32)
+    res2 = (rng.standard_normal((n_tok, W)) * 2).astype(np.float32)
+    return ws, x, x2, nw, nb, res, res2
+
+
+def _pf_expected(segs, ws, k, x, x2, norm, nw, nb, res, res2, eps=1e-5):
+    o = refs.oracle()
+    n_tok = x.shape[0]
+    y = np.zeros_like(x)
+    for i in range(n_tok):
+        if norm == 1:
+            o.orc_rms_norm_mul(ptr(x[i]), ptr(nw), ptr(y[i]), k, eps)
+        elif norm == 2:
+            o.orc_layer_norm_mul_add(ptr(x[i]), ptr(nw), ptr(nb), ptr(y[i]), k, eps)
+        else:
+            y[i] = x[i] if x2 is None else x[i] * x2[i]
+    outs, off = [], 0
+    for (t, m, epi), w in zip(segs, ws):
+        v = np.zeros((n_tok, m), np.float32)
+        assert o.orc_mul_mat(t, ptr(w), ptr(y), ptr(v), k, m, n_tok) == 0
+        if epi == ADD:
+            v = v + res[:, off:off + m]
+        elif epi == ADD2:
+            v = (v + res[:, off:off + m]) + res2[:, off:off + m]
+        elif epi in (GELU, SILU):
+            a = np.zeros_like(v)
+            (o.orc_gelu if epi == GELU else o.orc_silu)(ptr(v), ptr(a), v.size)
+            v = a
+        outs.append(v)
+        off += m
+    return np.concatenate(outs, axis=1)
+
+
+def _pf_run(lib, segs, ws, k, x, x2, norm, nw, nb, res, res2, n_ctx=512, hd=128, eps=1e-5):
+    """ctb_prefill_mul_mat on the first n_tok rows; returns (rc, out, ring slots)."""
+    n_tok = x.shape[0]
+    nseg = len(segs)
+    types, rows, epi = (np.array([s[j] for s in segs], np.int32) for j in range(3))
+    wp = (C.c_void_p * max(nseg, 1))(*[w.ctypes.data for w in ws])
+    out = np.full((n_tok, int(rows.sum())), np.nan, np.float32)
+    slots = np.zeros(1, np.int32)
+    rc = lib.ctb_prefill_mul_mat(nseg, ptr(types), C.cast(wp, C.c_void_p), ptr(rows), k, n_tok, ptr(x), None if x2 is None else ptr(x2),
+                                 norm, ptr(nw), ptr(nb), eps, ptr(epi), ptr(res), ptr(res2), ptr(out), n_ctx, hd, ptr(slots))
+    return rc, out, int(slots[0])
+
+
+@functools.lru_cache(maxsize=None)
+def _pf_case(t, src):
+    segs = [(t, 37, STORE)]
+    ws, x, x2, nw, nb, res, res2 = _pf_inputs(segs, 11008, max(PF_TOKENS), 0, False, src, seed=t)
+    return segs, ws, x, res, res2, nw, nb, _pf_expected(segs, ws, 11008, x, None, 0, nw, nb, res, res2)
+
+
+@pytest.mark.parametrize("src", list(PF_SOURCES))
+@pytest.mark.parametrize("t", [Q4_K, Q5_K, Q6_K])
+def test_prefill_mul_mat_types_and_weight_sources(lib, t, src):
+    """Every K-quant type on random blocks, the reference's quantizer's blocks and the edge blocks (every scale and min, quant
+    extremes, negative and subnormal d / dmin); K = 11008 (43 blocks: a ragged last work item for every chunk size 4 / 3 / 2),
+    M = 37 (a partial last tile), and 1 .. 70 tokens: partial token groups, one full launch, and a short launch after full ones.
+    Token i is the same row in every run, so each run is checked against the first rows of one 70-column oracle mat-mul."""
+    segs, ws, x, res, res2, nw, nb, want = _pf_case(t, src)
+    for n in PF_TOKENS:
+        rc, got, _ = _pf_run(lib, segs, ws, 11008, x[:n], None, 0, nw, nb, res[:n], res2[:n])
+        assert rc == 0
+        try:
+            _same_bits(got, want[:n])
+        except AssertionError as e:
+            raise AssertionError(f"n_tok {n}: {e}") from None
+
+
+@functools.lru_cache(maxsize=None)
+def _pf_shape_expected(case):
+    segs, k, n_tok, norm, with_x2, src = PF_SHAPES[case]
+    ws, x, x2, nw, nb, res, res2 = _pf_inputs(segs, k, n_tok, norm, with_x2, src, seed=len(case) * 131 + k)
+    return (ws, x, x2, nw, nb, res, res2), _pf_expected(segs, ws, k, x, x2, norm, nw, nb, res, res2)
+
+
+@pytest.mark.parametrize("case", list(PF_SHAPES))
+def test_prefill_mul_mat_shapes(lib, case):
+    """Rows below one tile, single-tile grids, several segments of different types and epilogues in one phase, x_mode 1, RMSNorm
+    and LayerNorm prologues, and the 7B-shaped projections the prefill2048 bench runs: bit-exact with the oracle."""
+    segs, k, n_tok, norm, with_x2, src = PF_SHAPES[case]
+    (ws, x, x2, nw, nb, res, res2), want = _pf_shape_expected(case)
+    rc, got, _ = _pf_run(lib, segs, ws, k, x, x2, norm, nw, nb, res, res2)
+    assert rc == 0
+    _same_bits(got, want)
+
+
+def _pf_accepts(lib, n_ctx, hd):
+    w = refs.edge_blocks(Q4_K, 256, 1, 0)
+    x = np.ones((1, 256), np.float32)
+    z = np.zeros((1, 1), np.float32)
+    return _pf_run(lib, [(Q4_K, 1, STORE)], [w], 256, x, None, 0, x[0], x[0], z, z, n_ctx=n_ctx, hd=hd)
+
+
+def test_prefill_mul_mat_deepest_and_shallowest_ring(lib):
+    """The ring depth follows n_ctx: the batched kernel's attention scratch shares shared memory with it.  The same mat-mul at the
+    deepest ring (a short context) and at the shallowest one an engine can pick (the longest context that still gets batched
+    prefill: 2 slots per team, so every slot's phase parity flips on every other item), one context longer being refused."""
+    hd = 64
+    lo, hi = 64, 8192
+    assert _pf_accepts(lib, lo, hd)[0] == 0 and _pf_accepts(lib, hi, hd)[0] == -1
+    while hi - lo > 1:
+        mid = (lo + hi) // 2
+        if _pf_accepts(lib, mid, hd)[0] == 0:
+            lo = mid
+        else:
+            hi = mid
+    segs = [(Q6_K, 40, STORE), (Q5_K, 24, ADD), (Q4_K, 20, SILU)]
+    ws, x, x2, nw, nb, res, res2 = _pf_inputs(segs, 11008, 70, 1, False, "edge", seed=5)
+    want = _pf_expected(segs, ws, 11008, x, None, 1, nw, nb, res, res2)
+    depths = {}
+    for n_ctx in (16, lo):
+        rc, got, depths[n_ctx] = _pf_run(lib, segs, ws, 11008, x, None, 1, nw, nb, res, res2, n_ctx=n_ctx, hd=hd)
+        assert rc == 0
+        _same_bits(got, want)
+    assert depths[lo] == 4 and depths[16] > depths[lo], depths
+
+
+def test_prefill_mul_mat_refuses_what_the_kernel_cannot_take(lib):
+    w = refs.edge_blocks(Q4_K, 512, 16, 0)
+    x = np.ones((2, 512), np.float32)
+    r = np.zeros((2, 64), np.float32)
+    ok = _pf_run(lib, [(Q4_K, 16, STORE)], [w], 512, x, None, 0, x[0], x[0], r, r)
+    assert ok[0] == 0
+    assert _pf_run(lib, [(Q8_0, 16, STORE)], [_rand_weights(Q8_0, 512, 16, 0)], 512, x, None, 0, x[0], x[0], r, r)[0] == -1
+    x384 = np.ones((2, 384), np.float32)
+    assert lib.ctb_prefill_mul_mat(1, ptr(np.array([Q4_K], np.int32)), C.cast((C.c_void_p * 1)(w.ctypes.data), C.c_void_p),
+                                   ptr(np.array([16], np.int32)), 384, 2, ptr(x384), None, 0, None, None, 1e-5, ptr(np.zeros(1, np.int32)),
+                                   None, None, ptr(r), 512, 128, None) == -1
+    assert _pf_run(lib, [(Q4_K, 4, STORE)] * 4, [w] * 4, 512, x, None, 0, x[0], x[0], r, r)[0] == -1
+    assert _pf_run(lib, [(Q4_K, 16, STORE)], [w], 512, x[:0], None, 0, x[0], x[0], r, r)[0] == -1

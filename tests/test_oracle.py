@@ -82,6 +82,64 @@ def test_fp16_conversions_exhaustive():
     assert np.array_equal(np.array([o.orc_fp32_to_fp16(float(v)) for v in x], np.uint16), x.astype(np.float16).view(np.uint16))
 
 
+def _decode_k_blocks(t, blocks):
+    """(scales, mins, quants, d, dmin) of K-quant blocks, read from their bytes the way the reference's dequantizers read them
+    (get_scale_min_k4, k_quants.c:306-313; dequantize_row_q4_K / q5_K / q6_K).  Quants per weight, scales per sub-block."""
+    b = blocks.reshape(-1, refs.BLOCK[t][1]).astype(np.int64)
+    nb = b.shape[0]
+    f16 = lambda lo: (b[:, lo] | (b[:, lo + 1] << 8)).astype(np.uint16)
+    q = np.zeros((nb, 256), np.int64)
+    if t in (Q4_K, Q5_K):
+        s = b[:, 4:16]
+        sc = np.concatenate([s[:, 0:4] & 63, (s[:, 8:12] & 15) | ((s[:, 0:4] >> 6) << 4)], 1)
+        mn = np.concatenate([s[:, 4:8] & 63, (s[:, 8:12] >> 4) | ((s[:, 4:8] >> 6) << 4)], 1)
+        qs, qh = (b[:, 16:144], None) if t == Q4_K else (b[:, 48:176], b[:, 16:48])
+        for j in range(4):
+            q[:, 64 * j:64 * j + 32] = qs[:, 32 * j:32 * j + 32] & 15
+            q[:, 64 * j + 32:64 * j + 64] = qs[:, 32 * j:32 * j + 32] >> 4
+            if qh is not None:
+                q[:, 64 * j:64 * j + 32] += ((qh >> (2 * j)) & 1) << 4
+                q[:, 64 * j + 32:64 * j + 64] += ((qh >> (2 * j + 1)) & 1) << 4
+        return sc, mn, q, f16(0), f16(2)
+    ql, qh = b[:, 0:128], b[:, 128:192]
+    for n in range(2):
+        for j in range(4):
+            lo = ql[:, 64 * n + 32 * (j & 1):64 * n + 32 * (j & 1) + 32] >> (4 * (j >> 1))
+            q[:, 128 * n + 32 * j:128 * n + 32 * j + 32] = (lo & 15) | (((qh[:, 32 * n:32 * n + 32] >> (2 * j)) & 3) << 4)
+    return blocks.reshape(nb, -1)[:, 192:208].view(np.int8).astype(np.int64), None, q, f16(208), None
+
+
+@pytest.mark.parametrize("t", [Q4_K, Q5_K, Q6_K])
+@pytest.mark.parametrize("k,m", [(512, 48), (11008, 37)])
+def test_edge_blocks_cover_every_scale_min_and_quant_edge(t, k, m):
+    """refs.edge_blocks reaches what random_blocks (scales 32..63, mins = scales) and the reference-quantized pool (scales 26..63)
+    do not: checked on the bytes, decoded as the reference decodes them, at the sizes the mat-mul tests draw."""
+    w = refs.edge_blocks(t, k, m, seed=k + t)
+    sc, mn, q, d, dmin = _decode_k_blocks(t, w)
+    deq = np.zeros(w.size // refs.BLOCK[t][1] * 256, np.float32)
+    getattr(refs.oracle(), "orc_dequantize_row_" + refs.TYPE_NAME[t])(ptr(w), ptr(deq), deq.size)
+    assert np.isfinite(deq).all()
+    nsub = sc.shape[1]
+    scale_of = np.repeat(sc, 256 // nsub, axis=1)
+    f = lambda h: h.view(np.float16).astype(np.float32)[:, None]
+    if t == Q6_K:
+        assert sorted(set(sc.ravel())) == list(range(-128, 128))
+        want = f(d) * scale_of * (q - 32)
+    else:
+        assert sorted(set(sc.ravel())) == list(range(64)) and sorted(set(mn.ravel())) == list(range(64))
+        assert (sc == mn).mean() < 0.05, "mins must be drawn independently of the scales"
+        want = f(d) * scale_of * q - f(dmin) * np.repeat(mn, 32, axis=1)
+    assert np.allclose(deq.reshape(want.shape), want, rtol=1e-6, atol=0), "decoder and the reference's dequantizer disagree"
+    edges = {Q4_K: (0, 15), Q5_K: (0, 31, 15, 16), Q6_K: (0, 63, 15, 48)}[t]
+    per_sub = q.reshape(q.shape[0], nsub, -1)
+    for c in edges:   # whole sub-blocks of q = c: all bits clear, all set, only the low 4 or only the high bits set
+        assert (per_sub == c).all(axis=2).any(), c
+    for h in (d,) if dmin is None else (d, dmin):
+        assert not ((h & 0x7c00) == 0x7c00).any(), "no inf or NaN"
+        assert (h >> 15).any() and not (h >> 15).all(), "both signs"
+        assert (((h & 0x7c00) == 0) & ((h & 0x3ff) != 0)).any(), "subnormal f16 values"
+
+
 class TestAgainstCompiledReference:
     """Against what the compiled reference returned for the same inputs (tests/golden/reference_runs.npz)."""
 
@@ -156,6 +214,20 @@ def test_long_context_runs_match_reference(key, tmp_path_factory):
     assert toks == gold[f"long_{key}_tokens"].tolist()
     for k, v in (("first_logits", first_logits), ("first_embd", first_embd), ("last_logits", last_logits)):
         assert refs.digest(v) == str(gold[f"long_{key}_{k}"]), k
+
+
+@pytest.mark.parametrize("key", list(modelcases.REALQ_PREFILL))
+def test_realq_prefill_runs_match_reference(key, tmp_path_factory):
+    """The reference-quantized Q5_K_M runs of tests/test_model_gpu.py: the oracle gives the reference's bits, so the GPU test's
+    comparison with the oracle rests on the reference."""
+    arch, ftype = modelcases.REALQ_PREFILL[key]
+    path = modelcases.build_realq(tmp_path_factory.mktemp("orc_realq"), arch, ftype)
+    run = modelcases.oracle_greedy(refs.OracleModel(path, modelcases.REALQ_PREFILL_CTX), modelcases.realq_prompt(arch), modelcases.REALQ_PREFILL_NEW, 512)
+    first_logits, first_embd, toks, last_logits, _ = run
+    gold = refs.golden_runs()
+    assert toks == gold[f"prefill_{key}_tokens"].tolist()
+    for k, v in (("first_logits", first_logits), ("first_embd", first_embd), ("last_logits", last_logits)):
+        assert refs.digest(v) == str(gold[f"prefill_{key}_{k}"]), k
 
 
 @pytest.mark.parametrize("name", ["llama_tiny_q4km", "falcon_tiny_q5km"])
