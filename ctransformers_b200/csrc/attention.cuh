@@ -77,12 +77,17 @@ __device__ __forceinline__ float dequant_elem(int type, const uint8_t* row, int 
   return 0.f;
 }
 
+struct EmbedParams { const uint8_t* table; size_t row_bytes; const int* tokens; float* out; int type, K, n_vocab; };
+
+// the embedding row of token id `tok` (clamped to the vocabulary) into out[K], by threads tid, tid + nt, ...
+__device__ __forceinline__ void embed_row(const EmbedParams& em, int tok, float* out, int tid, int nt) {
+  const uint8_t* row = em.table + (size_t)min(max(tok, 0), em.n_vocab - 1) * em.row_bytes;
+  for (int e = tid; e < em.K; e += nt) out[e] = dequant_elem(em.type, row, e);
+}
+
 // grid = N tokens; out[n][K]
-static __global__ void k_embed(const uint8_t* table, int type, size_t row_bytes, int K, int n_vocab, const int* tokens, float* out) {
-  const int tok = tokens[blockIdx.x];
-  const uint8_t* row = table + (size_t)min(max(tok, 0), n_vocab - 1) * row_bytes;
-  float* o = out + (size_t)blockIdx.x * K;
-  for (int e = threadIdx.x; e < K; e += blockDim.x) o[e] = dequant_elem(type, row, e);
+static __global__ void k_embed(const EmbedParams em) {
+  embed_row(em, em.tokens[blockIdx.x], em.out + (size_t)blockIdx.x * em.K, threadIdx.x, blockDim.x);
 }
 
 // ---------------------------------------------------------------------------------------- rope+kv
@@ -449,15 +454,15 @@ static __global__ void __launch_bounds__(ATTN_THREADS) k_attn(const AttnParams p
 }
 
 // ----------------------------------------------------------------------------------------- argmax
-// single block; writes the id of the largest logit (lowest id on ties) to out[0] and the number of logits equal to it to out[1]
-static __global__ void k_argmax(const float* logits, int n, int* out) {
-  __shared__ float bv[32];
-  __shared__ int bi[32];
-  __shared__ int ties;
-  float best = -INFINITY;
-  int idx = 0x7fffffff;
-  for (int i = threadIdx.x; i < n; i += blockDim.x) {
-    const float v = logits[i];
+// Greedy pick over logits[0, n) by the first NT threads (named barrier BAR): the largest value, the lowest id among equal ones.
+// Thread 0 ends with the result in best / idx.  CG: the logits were written earlier in the same kernel (read them from L2).
+template <int NT, int BAR, bool CG>
+__device__ __forceinline__ void block_argmax(const float* logits, int n, float* bv /* [NT / 32] smem */, int* bi /* [NT / 32] smem */, float& best, int& idx) {
+  best = -INFINITY;
+  idx = 0x7fffffff;
+#pragma unroll(CG ? 4 : 1)   // the step kernel's 320 threads keep 4 loads in flight each; k_argmax's 1024 threads need no more registers for it
+  for (int i = threadIdx.x; i < n; i += NT) {
+    const float v = CG ? __ldcg(logits + i) : logits[i];
     if (v > best) { best = v; idx = i; }
   }
 #pragma unroll
@@ -467,10 +472,32 @@ static __global__ void k_argmax(const float* logits, int n, int* out) {
     if (ov > best || (ov == best && oi < idx)) { best = ov; idx = oi; }
   }
   if ((threadIdx.x & 31) == 0) { bv[threadIdx.x >> 5] = best; bi[threadIdx.x >> 5] = idx; }
-  __syncthreads();
-  if (threadIdx.x == 0) {
-    for (int w = 1; w < (int)(blockDim.x >> 5); w++)
+  bar_sync<BAR, NT>();
+  if (threadIdx.x == 0)
+    for (int w = 1; w < NT / 32; w++)
       if (bv[w] > best || (bv[w] == best && bi[w] < idx)) { best = bv[w]; idx = bi[w]; }
+}
+
+// the decode state {token, position, step, n_total} after a greedy pick: the pick is the next token (and goes to
+// out_tokens[step]); a single-token eval's attention rows have length position + 1
+__device__ __forceinline__ void advance_state(int* state, int* out_tokens, int pick) {
+  out_tokens[state[2]] = pick;
+  state[0] = pick;
+  state[1] += 1;
+  state[2] += 1;
+  state[3] = state[1] + 1;
+}
+
+constexpr int ARGMAX_THREADS = 1024;
+// single block; writes the id of the largest logit (lowest id on ties) to out[0] and the number of logits equal to it to out[1]
+static __global__ void k_argmax(const float* logits, int n, int* out) {
+  __shared__ float bv[ARGMAX_THREADS / 32];
+  __shared__ int bi[ARGMAX_THREADS / 32];
+  __shared__ int ties;
+  float best;
+  int idx;
+  block_argmax<ARGMAX_THREADS, 0, false>(logits, n, bv, bi, best, idx);
+  if (threadIdx.x == 0) {
     out[0] = idx;
     bv[0] = best;
     ties = 0;

@@ -8,12 +8,12 @@
 //   Other types: per-tensor planes so that every lane of a warp issues 16-byte-aligned, fully coalesced loads no
 //   matter how odd the source block size is (Q4_0 = 18 B, Q8_0 = 34 B):
 //
-//   type   plane qs (per row)          plane qh (per row)   plane sc (per row)               plane d (per row)
-//   Q4_0   nb x 16 B nibbles           -                    -                                 nb x fp16
-//   Q5_0   nb x 16 B nibbles           nb x 4 B fifth bits  -                                 nb x fp16
-//   Q8_0   nb x 32 B int8              -                    -                                 nb x fp16
-//   F16    K x 2 B                     -                    -                                 -
-//   F32    K x 4 B                     -                    -                                 -
+//   type   plane qs (per row)          plane qh (per row)   plane d (per row)
+//   Q4_0   nb x 16 B nibbles           -                    nb x fp16
+//   Q5_0   nb x 16 B nibbles           nb x 4 B fifth bits  nb x fp16
+//   Q8_0   nb x 32 B int8              -                    nb x fp16
+//   F16    K x 2 B                     -                    -
+//   F32    K x 4 B                     -                    -
 //
 // Block contents are exactly the reference's (k_quants.h:76-117, ggml.c:888-925); only their placement
 // changes.  Activations are quantized on the fly to the reference's Q8_K / Q8_0 (bit-exact) into
@@ -22,6 +22,7 @@
 #include <cstdint>
 #include <cuda_fp16.h>
 #include <cuda_runtime.h>
+#include <utility>
 
 namespace ctb {
 
@@ -33,9 +34,10 @@ struct DevMat {
   int nb = 0;           // quant blocks per row
   const uint8_t* qs = nullptr;
   const uint8_t* qh = nullptr;
-  const uint8_t* sc = nullptr;
+  const void* unused = nullptr;   // no plane; the step kernel's phase descriptors embed DevMats, and dropping these 8 bytes moved
+                                  // its dynamic shared memory by 32 B, which cost 2.5 % decode speed (H100 80GB HBM3, 700 W)
   const uint16_t* d = nullptr;
-  const uint8_t* st = nullptr;   // K-quants: the stream layout of stream.cuh (16-row tiles, block-major; qs/qh/sc/d stay null)
+  const uint8_t* st = nullptr;   // K-quants: the stream layout of stream.cuh (16-row tiles, block-major; qs/qh/d stay null)
   size_t bytes = 0;     // total bytes of all planes (= GGUF tensor bytes)
 };
 
@@ -53,28 +55,38 @@ __host__ __device__ inline int act_format_for(int t) {
 __device__ __forceinline__ float h2f(uint16_t h) { return __half2float(__ushort_as_half(h)); }
 __device__ __forceinline__ uint16_t f2h(float f) { return __half_as_ushort(__float2half_rn(f)); }
 
-__device__ __forceinline__ int4 ldg_stream16(const void* p) {
-  int4 r;
-  asm volatile("ld.global.nc.L1::no_allocate.v4.s32 {%0,%1,%2,%3}, [%4];" : "=r"(r.x), "=r"(r.y), "=r"(r.z), "=r"(r.w) : "l"(p));
-  return r;
-}
-// read-only 16-byte load that keeps its place in program order (block headers: re-used by the 4 lanes of a row, L1 may keep them)
-__device__ __forceinline__ int4 ldg_keep16(const void* p) {
-  int4 r;
-  asm volatile("ld.global.nc.v4.s32 {%0,%1,%2,%3}, [%4];" : "=r"(r.x), "=r"(r.y), "=r"(r.z), "=r"(r.w) : "l"(p));
-  return r;
-}
-__device__ __forceinline__ int2 ldg_stream8(const void* p) {
-  int2 r;
-  asm volatile("ld.global.nc.L1::no_allocate.v2.s32 {%0,%1}, [%2];" : "=r"(r.x), "=r"(r.y) : "l"(p));
-  return r;
-}
-
 // Programmatic dependent launch (sm_90+): a kernel lets its successor's CTAs start early (they prefetch weights and set up
 // while this one drains) and the successor blocks in pdl_wait() until the whole predecessor grid has finished and its
 // writes are visible.  Both are no-ops for a kernel launched without the programmatic-serialization attribute.
 __device__ __forceinline__ void pdl_trigger() { asm volatile("griddepcontrol.launch_dependents;"); }
 __device__ __forceinline__ void pdl_wait() { asm volatile("griddepcontrol.wait;" ::: "memory"); }
+
+// launch with the programmatic-serialization attribute when pdl is set (the kernel may then start while its predecessor drains)
+template <typename... KArgs, typename... Args>
+static inline cudaError_t launch_kernel(void (*kernel)(KArgs...), dim3 grid, dim3 block, size_t smem, cudaStream_t st, bool pdl, Args&&... args) {
+  cudaLaunchConfig_t cfg{};
+  cfg.gridDim = grid; cfg.blockDim = block; cfg.dynamicSmemBytes = smem; cfg.stream = st;
+  cudaLaunchAttribute at[1];
+  at[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
+  at[0].val.programmaticStreamSerializationAllowed = 1;
+  cfg.attrs = at; cfg.numAttrs = pdl ? 1 : 0;
+  return cudaLaunchKernelEx(&cfg, kernel, std::forward<Args>(args)...);
+}
+
+// dynamic shared memory a kernel can opt in to on the current device: the per-block limit less its static shared memory
+template <typename Kernel>
+static inline size_t max_dyn_smem(Kernel kernel) {
+  cudaFuncAttributes fa{};
+  if (cudaFuncGetAttributes(&fa, kernel) != cudaSuccess) return 0;
+  int dev = 0, optin = 0;
+  cudaGetDevice(&dev);
+  cudaDeviceGetAttribute(&optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, dev);
+  return (size_t)optin > fa.sharedSizeBytes ? (size_t)optin - fa.sharedSizeBytes : 0;
+}
+
+// named barrier over the first NT threads of the CTA (BAR = 0 with NT = blockDim.x is __syncthreads)
+template <int BAR, int NT>
+__device__ __forceinline__ void bar_sync() { asm volatile("bar.sync %0, %1;" ::"n"(BAR), "n"(NT) : "memory"); }
 
 __device__ __forceinline__ unsigned long long globaltimer_ns() {
   unsigned long long t;

@@ -32,11 +32,7 @@ static std::string watchdog_note() {
   const int* d = g_watchdog_words;
   if (!d) return " [no watchdog words]";
   if (d[0] == 0) return " [watchdog words clear]";
-  static const char* const what[] = {"?", "mbarrier", "grid barrier (aux = phase)", "fold hand-off flag (aux = chunk)", "producer: free weight slot (aux = item)",
-                                     "consumer: weight item (aux = item)", "producer: free K slot (attention)", "producer: free V slot (attention)",
-                                     "consumer: K item (attention)", "consumer: V item (attention)", "tensor-parallel exchange: a peer's element (aux = exchange number)", "?",
-                                     "prefill grid barrier (aux = phase)", "?", "prefill producer: free slot", "prefill consumer: weight item"};
-  const char* w = (d[0] > 0 && d[0] < (int)(sizeof(what) / sizeof(what[0]))) ? what[d[0]] : "?";
+  const char* w = (d[0] > 0 && d[0] < W_CODES) ? WAIT_TEXT[d[0]] : "?";
   return " [step-kernel watchdog: wait " + std::to_string(d[0]) + " (" + w + ") timed out in CTA " + std::to_string(d[1]) + ", aux " + std::to_string(d[2]) + ", thread " +
          std::to_string(d[3]) + "]";
 }
@@ -63,16 +59,8 @@ struct StepOp {
   bool stream = false;  // PH_MATVEC: runs inside the step kernel
 };
 
-// advance the on-device decode state after a greedy pick: state = {token, n_past, step}
-// state = {token, position, step, n_total}; pick lives in state[4]
-__global__ void k_advance(int* state, int* out_tokens) {
-  const int t = state[4];
-  out_tokens[state[2]] = t;
-  state[0] = t;
-  state[1] += 1;
-  state[2] += 1;
-  state[3] = state[1] + 1;   // a single-token eval: the attention rows have length position + 1
-}
+// advance the on-device decode state after k_argmax's greedy pick (state[4])
+__global__ void k_advance(int* state, int* out_tokens) { advance_state(state, out_tokens, state[4]); }
 
 // ---- batched prefill (prefill.cuh): the per-token schedule rewritten over PB_T-row buffers
 struct PrefillState {
@@ -224,7 +212,7 @@ DevMat Engine::upload_matrix(const GGUFTensor& t, Uploader& up, int want_K, int 
       const size_t blk0 = (size_t)r0 * m.nb;
       const int grid = (int)std::min<size_t>((n_u16 + 255) / 256, (size_t)sm_count_ * 32);
       uint16_t* qdst = qs + ((m.type == GT_Q4_0 || m.type == GT_Q5_0) ? blk0 * 8 : (m.type == GT_Q8_0 ? blk0 * 16 : (size_t)r0 * row_bytes / 2));
-      k_repack<<<grid, 256, 0, up.st[slot]>>>(m.type, (const uint16_t*)up.dev[slot], n_u16, qdst, qh ? qh + blk0 * 2 : nullptr, nullptr, d ? d + blk0 : nullptr);
+      k_repack<<<grid, 256, 0, up.st[slot]>>>(m.type, (const uint16_t*)up.dev[slot], n_u16, qdst, qh ? qh + blk0 * 2 : nullptr, d ? d + blk0 : nullptr);
     }
     CTB_CUDA(cudaGetLastError());
     up.finish(slot);
@@ -243,36 +231,6 @@ const float* Engine::upload_vector(const GGUFFile& g, const std::string& name, b
   float* d = (float*)alloc(t->nbytes);
   CTB_CUDA(cudaMemcpy(d, t->data, t->nbytes, cudaMemcpyHostToDevice));
   return d;
-}
-
-// fp16 <-> fp32 on the host through the F16C-equivalent software path (bit-identical to the device's and the reference's)
-static inline float host_h2f(uint16_t h) {
-  uint32_t sign = (uint32_t)(h & 0x8000u) << 16, exp = (h >> 10) & 0x1f, man = h & 0x3ffu, bits;
-  if (exp == 0) {
-    if (!man) bits = sign;
-    else { int e = -1; do { man <<= 1; e++; } while (!(man & 0x400u)); man &= 0x3ffu; bits = sign | ((uint32_t)(127 - 15 - e) << 23) | (man << 13); }
-  } else if (exp == 31) bits = sign | 0x7f800000u | (man << 13);
-  else bits = sign | ((exp + 112) << 23) | (man << 13);
-  float f; memcpy(&f, &bits, 4); return f;
-}
-static inline uint16_t host_f2h(float f) {
-  uint32_t x; memcpy(&x, &f, 4);
-  const uint32_t sign = (x >> 16) & 0x8000u, ax = x & 0x7fffffffu;
-  if (ax >= 0x7f800000u) return (uint16_t)(sign | 0x7c00u | (ax > 0x7f800000u ? (0x200u | ((ax >> 13) & 0x3ffu)) : 0));
-  if (ax >= 0x477ff000u) return (uint16_t)(sign | 0x7c00u);
-  if (ax < 0x33000001u) return (uint16_t)sign;
-  const int32_t e = (int32_t)(ax >> 23) - 127;
-  const uint32_t m = (ax & 0x7fffffu) | 0x800000u;
-  if (e < -14) {
-    const uint32_t shift = (uint32_t)(13 + (-14 - e));
-    uint32_t r = m >> shift; const uint32_t rem = m & ((1u << shift) - 1), half = 1u << (shift - 1);
-    if (rem > half || (rem == half && (r & 1))) r++;
-    return (uint16_t)(sign | r);
-  }
-  uint32_t hb = ((uint32_t)(e + 15) << 10) | ((m >> 13) & 0x3ffu);
-  const uint32_t rem = m & 0x1fffu;
-  if (rem > 0x1000u || (rem == 0x1000u && (hb & 1))) hb++;
-  return (uint16_t)(sign | hb);
 }
 
 TPShard tp_shard(int n_embd, int n_head, int n_head_kv, int n_ff, int rank, int world) {
@@ -389,17 +347,11 @@ void Engine::init(const GGUFFile& g) {
 
   // ---- lookup tables, built with the host libm exactly like ggml_init does (ggml.c:4319-4333)
   {
-    std::vector<uint16_t> silu(65536), gelu(65536), ex(65536);
-    for (int i = 0; i < 65536; i++) {
-      const float f = host_h2f((uint16_t)i);
-      silu[i] = host_f2h(host_silu(f));
-      gelu[i] = host_f2h(host_gelu(f));
-      ex[i] = host_f2h(expf(f));
-    }
+    const HostTables t = host_tables();
     silu_tab_ = (uint16_t*)alloc(65536 * 2); gelu_tab_ = (uint16_t*)alloc(65536 * 2); exp_tab_ = (uint16_t*)alloc(65536 * 2);
-    CTB_CUDA(cudaMemcpy(silu_tab_, silu.data(), 65536 * 2, cudaMemcpyHostToDevice));
-    CTB_CUDA(cudaMemcpy(gelu_tab_, gelu.data(), 65536 * 2, cudaMemcpyHostToDevice));
-    CTB_CUDA(cudaMemcpy(exp_tab_, ex.data(), 65536 * 2, cudaMemcpyHostToDevice));
+    CTB_CUDA(cudaMemcpy(silu_tab_, t.silu.data(), 65536 * 2, cudaMemcpyHostToDevice));
+    CTB_CUDA(cudaMemcpy(gelu_tab_, t.gelu.data(), 65536 * 2, cudaMemcpyHostToDevice));
+    CTB_CUDA(cudaMemcpy(exp_tab_, t.ex.data(), 65536 * 2, cudaMemcpyHostToDevice));
   }
   // ---- RoPE table: same recurrence, same libm calls as ggml.c:12482-12529
   {
@@ -732,7 +684,7 @@ void Engine::build_ops() {
   for (const StepOp& op : ops_) any_stream |= op.ph.kind == PH_MATVEC && op.stream;
   std::vector<Phase> phs;
   for (const StepOp& op : ops_) if (op.ph.kind != PH_XCHG && (op.ph.kind != PH_MATVEC || op.stream)) phs.push_back(op.ph);
-  const StepLaunch sl = step_launch_shape(phs.data(), (int)phs.size(), sm_count_, step_max_dyn_smem());
+  const StepLaunch sl = step_launch_shape(phs.data(), (int)phs.size(), sm_count_, max_dyn_smem(k_step<true>));
   step_grid_ = sl.grid; step_slots_ = sl.n_slots; step_smem_ = sl.smem;
   if (const char* e = getenv("CTB_ST_SLOTS")) {   // A/B knob: fewer ring slots = less prefetch in flight
     const int want = atoi(e);
@@ -783,28 +735,21 @@ void Engine::enqueue_ops(const std::vector<StepOp>& ops, const Phase* d_prog, co
     mark(-1);
     switch (op.ph.kind) {
       case PH_EMBED:
-        k_embed<<<1, 256, 0, stream_>>>(op.ph.em.table, op.ph.em.type, op.ph.em.row_bytes, op.ph.em.K, op.ph.em.n_vocab, op.ph.em.tokens, op.ph.em.out);
+        k_embed<<<1, 256, 0, stream_>>>(op.ph.em);
         launches_per_step_++;
         mark(3);
         break;
-      case PH_ATTN: {
-        cudaLaunchConfig_t cfg{};
-        cfg.gridDim = dim3(nh_, 1, hp_.head_dim() / ATTN_CH); cfg.blockDim = dim3(ATTN_THREADS);
-        cfg.dynamicSmemBytes = attn_smem_bytes(hp_.n_ctx, hp_.head_dim()); cfg.stream = stream_;
-        cudaLaunchAttribute at[1];
-        at[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-        at[0].val.programmaticStreamSerializationAllowed = 1;
-        cfg.attrs = at; cfg.numAttrs = pdl_ ? 1 : 0;
-        CTB_CUDA(cudaLaunchKernelEx(&cfg, k_attn, op.ph.at));
+      case PH_ATTN:
+        CTB_CUDA(launch_kernel(k_attn, dim3(nh_, 1, hp_.head_dim() / ATTN_CH), dim3(ATTN_THREADS), attn_smem_bytes(hp_.n_ctx, hp_.head_dim()), stream_, pdl_, op.ph.at));
         launches_per_step_++;
         mark(1);
-      } break;
+        break;
       case PH_XCHG:
         tp_all_reduce(op.ph.em.out, op.ph.em.K);
         mark(3);
         break;
       case PH_PICK:
-        k_argmax<<<1, 1024, 0, stream_>>>(d_logits_, hp_.n_vocab, d_state_ + 4);
+        k_argmax<<<1, ARGMAX_THREADS, 0, stream_>>>(d_logits_, hp_.n_vocab, d_state_ + 4);
         k_advance<<<1, 1, 0, stream_>>>(d_state_, d_tokens_out_);
         launches_per_step_ += 2;
         mark(3);
@@ -988,7 +933,7 @@ void Engine::after_eval(int next_pos) {
   // the look-ahead step writes K/V slot next_pos: only when nothing valid can live there (append-only decoding).  A caller
   // that re-evaluates an earlier position and later continues past it keeps its cache contents.
   if (!spec_on_ || next_pos >= hp_.n_ctx || next_pos < kv_high_) return;
-  k_argmax<<<1, 1024, 0, stream_>>>(d_logits_, hp_.n_vocab, d_state_ + 4);
+  k_argmax<<<1, ARGMAX_THREADS, 0, stream_>>>(d_logits_, hp_.n_vocab, d_state_ + 4);
   k_advance<<<1, 1, 0, stream_>>>(d_state_, d_tokens_out_);
   CTB_CUDA(cudaMemcpyAsync(h_spec_tok_, d_state_ + 4, 8, cudaMemcpyDeviceToHost, stream_));   // {greedy pick, how many logits equal the maximum}
   CTB_CUDA(cudaEventRecord(ev_pick_, stream_));

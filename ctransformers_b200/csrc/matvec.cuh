@@ -30,20 +30,40 @@ constexpr int MV_MAX_SEG = 3;
 enum : int { NORM_NONE = 0, NORM_RMS = 1, NORM_LAYER = 2 };
 enum : int { EPI_STORE = 0, EPI_ADD = 1, EPI_GELU = 2, EPI_ADD2 = 3, EPI_SILU = 4 };   // GELU / SILU: the reference's fp16-table activation of the row value
 
-// Every spin in the persistent kernels is bounded: a wait that lasts longer than ST_WATCHDOG_NS writes {code, CTA, aux} into
-// host-mapped memory and traps — a protocol bug then ends as a launch failure with a message, not as a hung GPU.
+// Every spin in the persistent kernels is bounded (bounded_wait): a wait that lasts longer than ST_WATCHDOG_NS writes
+// {code, CTA, aux, thread} into host-mapped memory and traps — a protocol bug then ends as a launch failure with a message,
+// not as a hung GPU.
 #ifndef ST_WATCHDOG_NS
 #define ST_WATCHDOG_NS 4000000000ull
 #endif
+#ifndef XC_WATCHDOG_NS
+#define XC_WATCHDOG_NS 30000000000ull   // a peer rank may start its launch late (host jitter): 30 s
+#endif
+// what a timed-out wait was waiting for (the code st_fail records), and the text the host reports for it
+enum WaitCode : int {
+  W_GRID_BARRIER = 1, W_FOLD_FLAG, W_FREE_WEIGHT_SLOT, W_WEIGHT_ITEM, W_FREE_K_SLOT, W_FREE_V_SLOT, W_K_ITEM, W_V_ITEM, W_XCHG,
+  W_PF_GRID_BARRIER, W_PF_FREE_SLOT, W_PF_WEIGHT_ITEM, W_CODES
+};
+constexpr const char* WAIT_TEXT[] = {"?", "grid barrier (aux = phase)", "fold hand-off flag (aux = chunk)", "producer: free weight slot (aux = item)",
+                                     "consumer: weight item (aux = item)", "producer: free K slot (attention)", "producer: free V slot (attention)",
+                                     "consumer: K item (attention)", "consumer: V item (attention)", "tensor-parallel exchange: a peer's element (aux = exchange number)",
+                                     "prefill grid barrier (aux = phase)", "prefill producer: free slot (aux = item)", "prefill consumer: weight item (aux = item)"};
+static_assert(sizeof(WAIT_TEXT) / sizeof(WAIT_TEXT[0]) == W_CODES, "one text per wait code");
+
 static __device__ int* g_st_dbg = nullptr;   // set by the host (st_set_debug_words): 4 ints of mapped pinned host memory, or null
-static __device__ __noinline__ void st_fail(int code, int aux) {
+static __device__ __noinline__ void st_fail(WaitCode code, int aux) {
   int* d = g_st_dbg;
   if (d) { d[0] = code; d[1] = (int)blockIdx.x; d[2] = aux; d[3] = (int)threadIdx.x; __threadfence_system(); }
   __trap();
 }
-#ifndef XC_WATCHDOG_NS
-#define XC_WATCHDOG_NS 30000000000ull   // a peer rank may start its launch late (host jitter): 30 s
-#endif
+// spin until done() holds; one try before the timer is read, st_fail(code, aux) once the wait has lasted limit_ns
+template <typename Done>
+__device__ __forceinline__ void bounded_wait(Done&& done, WaitCode code, int aux, unsigned long long limit_ns = ST_WATCHDOG_NS) {
+  if (done()) return;
+  const unsigned long long t0 = globaltimer_ns();
+  while (!done())
+    if (globaltimer_ns() - t0 > limit_ns) st_fail(code, aux);
+}
 
 struct MVSeg {
   DevMat w;
@@ -132,10 +152,6 @@ __device__ __forceinline__ void load16(const float* p, int valid, float (&v)[16]
   }
 }
 
-// named barrier over the first NT threads of the CTA (BAR = 0 with NT = blockDim.x is __syncthreads)
-template <int BAR, int NT>
-__device__ __forceinline__ void bar_sync() { asm volatile("bar.sync %0, %1;" ::"n"(BAR), "n"(NT) : "memory"); }
-
 template <int NT, int BAR>
 __device__ __forceinline__ double block_sum_f64(double s, double* red /* [NT / 32] smem */) {
   s = warp_sum(s);
@@ -158,8 +174,7 @@ __device__ __forceinline__ uint32_t pack4(const int* q) {
 // 16 consecutive {value, number} elements of one rank's partial vector; spins until all carry `epoch`
 __device__ __forceinline__ void load16_ll(const uint2* p, unsigned epoch, float (&u)[16]) {
   uint4 q[8];
-  unsigned long long t0 = 0;
-  for (;;) {
+  bounded_wait([&] {
     bool ok = true;
 #pragma unroll
     for (int j = 0; j < 8; j++) {
@@ -167,10 +182,8 @@ __device__ __forceinline__ void load16_ll(const uint2* p, unsigned epoch, float 
     }
 #pragma unroll
     for (int j = 0; j < 8; j++) ok &= q[j].y == epoch && q[j].w == epoch;
-    if (ok) break;
-    if (!t0) t0 = globaltimer_ns();
-    else if (globaltimer_ns() - t0 > XC_WATCHDOG_NS) st_fail(10, (int)epoch);
-  }
+    return ok;
+  }, W_XCHG, (int)epoch, XC_WATCHDOG_NS);
 #pragma unroll
   for (int j = 0; j < 8; j++) { u[2 * j] = __uint_as_float(q[j].x); u[2 * j + 1] = __uint_as_float(q[j].z); }
 }
@@ -205,16 +218,20 @@ __device__ __forceinline__ void load16x(const MVParams& xs, int base, int valid,
 // Norm weight / bias of this thread's first 16 elements: constants of the model, so they are fetched before the kernel waits
 // for its predecessor (pdl_wait) and are in registers when the input vector arrives.
 struct NormPre { float w0[16], bias0[16]; };
-__device__ __forceinline__ void preload_norm(NormPre& np, const float* nw, const float* nb_, int norm_mode, int K) {
+__device__ __forceinline__ void preload_norm(NormPre& np, const MVParams& p) {
   const int t = threadIdx.x;
-  if (norm_mode != NORM_NONE && nw) load16(nw + t * 16, K - t * 16, np.w0);
-  if (norm_mode != NORM_NONE && nb_) load16(nb_ + t * 16, K - t * 16, np.bias0);
+  if (p.norm_mode != NORM_NONE && p.norm_w) load16(p.norm_w + t * 16, p.K - t * 16, np.w0);
+  if (p.norm_mode != NORM_NONE && p.norm_b) load16(p.norm_b + t * 16, p.K - t * 16, np.bias0);
 }
 
 // The first NT threads of the CTA must call (named barrier BAR); each owns 16 consecutive elements per pass.
 template <int NT, int BAR, bool XC = false>   // XC: the input may be a tensor-parallel exchange (x_mode 2); compiled out otherwise
-__device__ __forceinline__ void stage_activation(const MVParams& xs, const NormPre& np, const float* nw, const float* nb_, float* norm_out, int norm_mode, float eps,
-                                                  int K, int act, uint8_t* smem, double* red, bool write_norm, unsigned epoch = 0) {
+__device__ __forceinline__ void stage_activation(const MVParams& xs, const NormPre& np, int act, uint8_t* smem, double* red, bool write_norm, unsigned epoch = 0) {
+  const float* nw = xs.norm_w;
+  const float* nb_ = xs.norm_b;
+  float* norm_out = xs.norm_out;
+  const int norm_mode = xs.norm_mode, K = xs.K;
+  const float eps = xs.eps;
   const int t = threadIdx.x, lane = t & 31;
   const int passes = (K + NT * 16 - 1) / (NT * 16);
   // ---- statistics (fp64 sums like ggml.c:10700-10703 / 10630-10645; the order of a double sum does not reach the float result)
@@ -480,14 +497,16 @@ __device__ __forceinline__ float dot_f32_row(const DevMat& w, int row, const uin
 
 __device__ __forceinline__ float table_f16(const uint16_t* tab, float x) { return h2f(__ldg(tab + f2h(x))); }
 
-// residuals may have been written earlier in the same (persistent) kernel: L2-coherent loads
-__device__ __forceinline__ void store_epilogue(const MVSeg& sg, const MVParams& p, int row, float v) {
-  if (sg.epi == EPI_ADD) v = __fadd_rn(v, __ldcg(sg.res + row));
-  else if (sg.epi == EPI_ADD2) v = __fadd_rn(__fadd_rn(v, __ldcg(sg.res + row)), __ldcg(sg.res2 + row));
-  else if (sg.epi == EPI_GELU) v = table_f16(p.gelu_tab, v);
-  else if (sg.epi == EPI_SILU) v = table_f16(p.silu_tab, v);
-  sg.out[row] = v;
+// The value an output element stores: the row's sum v with the segment's epilogue.  res / res2 point at this element's
+// residuals (read by EPI_ADD / EPI_ADD2 only); they may have been written earlier in the same persistent kernel: L2-coherent loads.
+__device__ __forceinline__ float epilogue(int epi, float v, const float* res, const float* res2, const MVParams& p) {
+  if (epi == EPI_ADD) return __fadd_rn(v, __ldcg(res));
+  if (epi == EPI_ADD2) return __fadd_rn(__fadd_rn(v, __ldcg(res)), __ldcg(res2));
+  if (epi == EPI_GELU) return table_f16(p.gelu_tab, v);
+  if (epi == EPI_SILU) return table_f16(p.silu_tab, v);
+  return v;
 }
+__device__ __forceinline__ void store_epilogue(const MVSeg& sg, const MVParams& p, int row, float v) { sg.out[row] = epilogue(sg.epi, v, sg.res + row, sg.res2 + row, p); }
 
 // rows one warp task covers for a (non-K-quant) weight type
 __host__ __device__ inline int rows_per_unit(int type) { return (type == GT_F16 || type == GT_F32) ? 1 : MV_ROWS; }
@@ -500,9 +519,9 @@ static __global__ void __launch_bounds__(MV_THREADS, 1) k_matvec(const __grid_co
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   pdl_trigger();
   NormPre np;
-  preload_norm(np, p.norm_w, p.norm_b, p.norm_mode, p.K);
+  preload_norm(np, p);
   pdl_wait();   // everything above touched only weights and shared memory; the input vector is the predecessor's output
-  stage_activation<MV_THREADS, 0>(p, np, p.norm_w, p.norm_b, p.norm_out, p.norm_mode, p.eps, p.K, p.act, smem, red, blockIdx.x == 0);
+  stage_activation<MV_THREADS, 0>(p, np, p.act, smem, red, blockIdx.x == 0);
   const ActView a = act_view(p.act, p.K, smem);
   const int gw = blockIdx.x * MV_WARPS + warp, nw = gridDim.x * MV_WARPS;
   int first = gw;   // global striding continues across segments so all warps stay busy
@@ -540,13 +559,7 @@ constexpr int MV_SMEM_LIMIT = 200 * 1024;
 
 // static: each translation unit launches / configures ITS OWN instantiation of the (static) kernel
 static inline cudaError_t launch_matvec_kernel(const MVLaunch& L, cudaStream_t st, const MVParams& p, bool pdl = false) {
-  cudaLaunchConfig_t cfg{};
-  cfg.gridDim = dim3(L.grid); cfg.blockDim = dim3(MV_THREADS); cfg.dynamicSmemBytes = L.smem; cfg.stream = st;
-  cudaLaunchAttribute at[1];
-  at[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-  at[0].val.programmaticStreamSerializationAllowed = 1;
-  cfg.attrs = at; cfg.numAttrs = pdl ? 1 : 0;
-  return cudaLaunchKernelEx(&cfg, k_matvec, p);
+  return launch_kernel(k_matvec, dim3(L.grid), dim3(MV_THREADS), L.smem, st, pdl, p);
 }
 static inline cudaError_t matvec_set_smem_limit(int bytes) {
   return cudaFuncSetAttribute(k_matvec, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes);

@@ -40,21 +40,15 @@ struct OpsTables {
   uint16_t *silu = nullptr, *gelu = nullptr, *ex = nullptr;
 };
 
-// built once per process, on the host with libm, like ggml_init (ggml.c:4319-4333)
+// built once per process, like the engine's
 OpsTables& tables() {
   static OpsTables t;
   if (!t.silu) {
-    std::vector<uint16_t> s(65536), g(65536), e(65536);
-    for (int i = 0; i < 65536; i++) {
-      const float f = __half2float(__ushort_as_half((uint16_t)i));
-      s[i] = __half_as_ushort(__float2half_rn(host_silu(f)));
-      g[i] = __half_as_ushort(__float2half_rn(host_gelu(f)));
-      e[i] = __half_as_ushort(__float2half_rn(expf(f)));
-    }
+    const HostTables h = host_tables();
     OPS_CUDA(cudaMalloc(&t.silu, 65536 * 2)); OPS_CUDA(cudaMalloc(&t.gelu, 65536 * 2)); OPS_CUDA(cudaMalloc(&t.ex, 65536 * 2));
-    OPS_CUDA(cudaMemcpy(t.silu, s.data(), 65536 * 2, cudaMemcpyHostToDevice));
-    OPS_CUDA(cudaMemcpy(t.gelu, g.data(), 65536 * 2, cudaMemcpyHostToDevice));
-    OPS_CUDA(cudaMemcpy(t.ex, e.data(), 65536 * 2, cudaMemcpyHostToDevice));
+    OPS_CUDA(cudaMemcpy(t.silu, h.silu.data(), 65536 * 2, cudaMemcpyHostToDevice));
+    OPS_CUDA(cudaMemcpy(t.gelu, h.gelu.data(), 65536 * 2, cudaMemcpyHostToDevice));
+    OPS_CUDA(cudaMemcpy(t.ex, h.ex.data(), 65536 * 2, cudaMemcpyHostToDevice));
   }
   return t;
 }
@@ -92,13 +86,13 @@ void upload(OwnedMat& o, int type, const void* blocks, int K, int M) {
     return;
   }
   const PlaneSizes ps = plane_sizes(type, M, o.m.nb, bytes);
-  uint16_t* pl[4] = {nullptr, nullptr, nullptr, nullptr};
-  const size_t sz[4] = {ps.qs, ps.qh, ps.sc, ps.d};
-  for (int i = 0; i < 4; i++)
+  uint16_t* pl[3] = {nullptr, nullptr, nullptr};
+  const size_t sz[3] = {ps.qs, ps.qh, ps.d};
+  for (int i = 0; i < 3; i++)
     if (sz[i]) { OPS_CUDA(cudaMalloc((void**)&pl[i], sz[i])); o.bufs.push_back(pl[i]); }
-  k_repack<<<(int)std::min<size_t>((bytes / 2 + 255) / 256, 4096), 256>>>(type, raw.as<uint16_t>(), bytes / 2, pl[0], pl[1], pl[2], pl[3]);
+  k_repack<<<(int)std::min<size_t>((bytes / 2 + 255) / 256, 4096), 256>>>(type, raw.as<uint16_t>(), bytes / 2, pl[0], pl[1], pl[2]);
   OPS_CUDA(cudaDeviceSynchronize());
-  o.m.qs = (const uint8_t*)pl[0]; o.m.qh = (const uint8_t*)pl[1]; o.m.sc = (const uint8_t*)pl[2]; o.m.d = pl[3];
+  o.m.qs = (const uint8_t*)pl[0]; o.m.qh = (const uint8_t*)pl[1]; o.m.d = pl[2];
 }
 
 int sm_count() {
@@ -117,7 +111,7 @@ unsigned* sync_words() {
 // a program of phases through the persistent step kernel, exactly as the engine launches it
 void run_phases(std::vector<Phase> phs) {
   unsigned* d_sync = sync_words();
-  const StepLaunch L = step_launch_shape(phs.data(), (int)phs.size(), sm_count(), step_max_dyn_smem());
+  const StepLaunch L = step_launch_shape(phs.data(), (int)phs.size(), sm_count(), max_dyn_smem(k_step<true>));
   const std::vector<int> hb = step_bounds(phs.data(), (int)phs.size(), L.grid);
   DevBuf dbounds(hb.size() * 4);
   OPS_CUDA(cudaMemcpy(dbounds.p, hb.data(), hb.size() * 4, cudaMemcpyHostToDevice));
@@ -148,30 +142,25 @@ void run_matvec(MVParams& p) {
 }
 
 // standalone wrappers around the prologue pieces, so the activation quantizers can be checked bit-for-bit
-__global__ void __launch_bounds__(MV_THREADS) k_stage_dump(const float* x, const float* nw, const float* nb, float* norm_out, int mode, float eps, int K, int act,
-                                                            uint8_t* dump) {
+__global__ void __launch_bounds__(MV_THREADS) k_stage_dump(const __grid_constant__ MVParams q, int act, uint8_t* dump) {
   extern __shared__ __align__(16) uint8_t smem[];
   __shared__ double red[MV_WARPS];
-  MVParams q{};
-  q.x = x;
   NormPre np;
-  preload_norm(np, nw, nb, mode, K);
-  stage_activation<MV_THREADS, 0>(q, np, nw, nb, norm_out, mode, eps, K, act, smem, red, true);
-  const size_t n = act_smem_bytes(act, K);
+  preload_norm(np, q);
+  stage_activation<MV_THREADS, 0>(q, np, act, smem, red, true);
+  const size_t n = act_smem_bytes(act, q.K);
   for (size_t i = threadIdx.x; i < n; i += MV_THREADS) dump[i] = smem[i];
 }
 
 // the x_mode = 1 input path of the prologue on its own: out[i] = gate_act[i] * up[i] (gate_act = silu_table(gate), from the epilogue)
-__global__ void __launch_bounds__(MV_THREADS) k_gate_dump(const float* gate, const float* up, const uint16_t* silu_tab, int M, float* out) {
+__global__ void __launch_bounds__(MV_THREADS) k_gate_dump(const __grid_constant__ MVParams q, float* out) {
   extern __shared__ __align__(16) uint8_t smem[];
   __shared__ double red[MV_WARPS];
-  MVParams q{};
-  q.x = gate; q.x2 = up; q.x_mode = 1; q.silu_tab = silu_tab;
   NormPre np;
-  preload_norm(np, nullptr, nullptr, NORM_NONE, M);
-  stage_activation<MV_THREADS, 0>(q, np, nullptr, nullptr, nullptr, NORM_NONE, 0.f, M, ACT_F32, smem, red, false);
+  preload_norm(np, q);
+  stage_activation<MV_THREADS, 0>(q, np, ACT_F32, smem, red, false);
   const float* f = (const float*)smem;
-  for (int i = threadIdx.x; i < M; i += MV_THREADS) out[i] = f[i];
+  for (int i = threadIdx.x; i < q.K; i += MV_THREADS) out[i] = f[i];
 }
 
 // RoPE in place of the fp32 rows of blockIdx.x = 0 .. n_head-1 at position pos, as the attention kernels rotate q and k before
@@ -204,7 +193,10 @@ void stage_to_host(const float* x, const float* w, const float* b, float* y_norm
   const size_t n = act_smem_bytes(act, K);
   DevBuf dd(n);
   if (n > 48 * 1024) OPS_CUDA(cudaFuncSetAttribute(k_stage_dump, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)n));
-  k_stage_dump<<<1, MV_THREADS, n>>>(dx.as<float>(), w ? dw.as<float>() : nullptr, b ? db.as<float>() : nullptr, dy.as<float>(), mode, eps, K, act, dd.as<uint8_t>());
+  MVParams q{};
+  q.x = dx.as<float>(); q.norm_w = w ? dw.as<float>() : nullptr; q.norm_b = b ? db.as<float>() : nullptr; q.norm_out = dy.as<float>();
+  q.norm_mode = mode; q.eps = eps; q.K = K;
+  k_stage_dump<<<1, MV_THREADS, n>>>(q, act, dd.as<uint8_t>());
   OPS_CUDA(cudaGetLastError());
   dump.resize(n);
   OPS_CUDA(cudaMemcpy(dump.data(), dd.p, n, cudaMemcpyDeviceToHost));
@@ -405,7 +397,7 @@ int ctb_attention_path(int path, const float* q, const float* k_new, const float
       if (path == 1) {
         Phase ph{};
         ph.kind = PH_ATTN; ph.q6 = 1; ph.at = ap;
-        const StepLaunch L = step_launch_shape(&ph, 1, sm_count(), step_max_dyn_smem());
+        const StepLaunch L = step_launch_shape(&ph, 1, sm_count(), max_dyn_smem(k_step<true>));
         if (!st_attn_ring_ok(n_ctx, L.n_slots)) throw std::runtime_error("the step kernel's ring cannot carry K / V at this n_ctx");
       }
       const size_t smem = attn_smem_bytes(n_ctx, hd);
@@ -529,7 +521,9 @@ int ctb_ffn_gate(int type, const void* w1_blocks, const void* w3_blocks, const f
     run_matvec(p);
     const size_t smem = (size_t)M * 4 + 64;
     OPS_CUDA(cudaFuncSetAttribute(k_gate_dump, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)std::max<size_t>(smem, 48 * 1024)));
-    k_gate_dump<<<1, MV_THREADS, smem>>>(dg.as<float>(), du.as<float>(), tables().silu, M, dy.as<float>());
+    MVParams q{};
+    q.x = dg.as<float>(); q.x2 = du.as<float>(); q.x_mode = 1; q.norm_mode = NORM_NONE; q.K = M;
+    k_gate_dump<<<1, MV_THREADS, smem>>>(q, dy.as<float>());
     OPS_CUDA(cudaGetLastError());
     OPS_CUDA(cudaMemcpy(out, dy.p, (size_t)M * 4, cudaMemcpyDeviceToHost));
   });
@@ -553,8 +547,7 @@ int ctb_matvec_partition(const int* types, const int* rows, int nseg, int K, int
     long items = 0;
     for (int tile = first_tile[c]; tile < first_tile[c + 1]; tile++) {
       int tl = tile;
-      const int kb = st_chunk_blocks(types[ts.locate(tl)]);
-      items += (nb + kb - 1) / kb;
+      items += st_chunks(types[ts.locate(tl)], nb);
     }
     max_items = std::max(max_items, items);
   }
@@ -569,7 +562,9 @@ int ctb_get_row(int type, const void* table_blocks, int K, int n_rows, int row, 
     DevBuf dt(rb * n_rows), dtok(4), dout((size_t)K * 4);
     OPS_CUDA(cudaMemcpy(dt.p, table_blocks, rb * n_rows, cudaMemcpyHostToDevice));
     OPS_CUDA(cudaMemcpy(dtok.p, &row, 4, cudaMemcpyHostToDevice));
-    k_embed<<<1, 256>>>(dt.as<uint8_t>(), type, rb, K, n_rows, dtok.as<int>(), dout.as<float>());
+    EmbedParams em{};
+    em.table = dt.as<uint8_t>(); em.row_bytes = rb; em.tokens = dtok.as<int>(); em.out = dout.as<float>(); em.type = type; em.K = K; em.n_vocab = n_rows;
+    k_embed<<<1, 256>>>(em);
     OPS_CUDA(cudaGetLastError());
     OPS_CUDA(cudaMemcpy(out, dout.p, (size_t)K * 4, cudaMemcpyDeviceToHost));
   });

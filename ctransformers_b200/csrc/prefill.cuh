@@ -233,7 +233,7 @@ __device__ __forceinline__ void pb_chunk(const uint8_t* slot, int nblk, int b0, 
 }
 
 // end of a tile: the team's 4 warps publish their accumulators, then its 128 threads finish 16 rows x PB_T tokens:
-// hsum_float_8's tree over the 8 lanes (ggml.c:609-615), the mins tail, the epilogue (store_epilogue of matvec.cuh per token row)
+// hsum_float_8's tree over the 8 lanes (ggml.c:609-615), the mins tail, the epilogue (matvec.cuh) per token row
 template <int BARID>
 __device__ __forceinline__ void pb_finish(const PBState& st, float* xch, int type, int lane, int lp, int tid_team, const PPhase& ph, int n_tok, int seg, int row0) {
   const int g = lane >> 2, t = lane & 3;
@@ -259,19 +259,12 @@ __device__ __forceinline__ void pb_finish(const PBState& st, float* xch, int typ
     if (type == GT_Q4_K) v = __fadd_rn(v, __fadd_rn(__fadd_rn(x[8 * L], x[10 * L]), __fadd_rn(x[9 * L], x[11 * L])));
     else if (type == GT_Q5_K) v = __fadd_rn(v, x[8 * L]);
     const int grow = row0 + row;
-    if (grow < sg.w.M && tok < n_tok) {
-      if (sg.epi == EPI_ADD) v = __fadd_rn(v, __ldcg(sg.res + (size_t)tok * rld + grow));
-      else if (sg.epi == EPI_ADD2) v = __fadd_rn(__fadd_rn(v, __ldcg(sg.res + (size_t)tok * rld + grow)), __ldcg(sg.res2 + (size_t)tok * r2ld + grow));
-      else if (sg.epi == EPI_GELU) v = table_f16(ph.mv.gelu_tab, v);
-      else if (sg.epi == EPI_SILU) v = table_f16(ph.mv.silu_tab, v);
-      sg.out[(size_t)tok * old + grow] = v;
-    }
+    if (grow < sg.w.M && tok < n_tok) sg.out[(size_t)tok * old + grow] = epilogue(sg.epi, v, sg.res + (size_t)tok * rld + grow, sg.res2 + (size_t)tok * r2ld + grow, ph.mv);
   }
 }
 
 // ---------------------------------------------------------------------------------------------
-// Ring addressing: every team has its own slots (team t's i-th item: slot (i % depth) * PB_TEAMS + t, phase parity (i / depth) & 1),
-// so the team that waits for an item is the one that consumed the slot's previous occupant (see st_slot in stream.cuh).
+// Ring addressing: every team owns PB_TEAMS-strided slots of the ring (ring_pos in stream.cuh); cnt[t] counts team t's items.
 __device__ __forceinline__ void pb_producer(const PStepArgs& args, uint8_t* ring, uint64_t* full_bar, uint64_t* empty_bar) {
   const int lane = threadIdx.x & 31;
   const uint32_t D = (uint32_t)(args.n_slots / PB_TEAMS);
@@ -290,24 +283,20 @@ __device__ __forceinline__ void pb_producer(const PStepArgs& args, uint8_t* ring
       const int ntw = min(PB_TEAMS, T1 - w0);
       const TileInfo ti = tile_info(ts, p, w0 + lane, nb, lane < ntw);
       for (int kc = 0;; kc++) {
-        unsigned mask = __ballot_sync(0xffffffffu, kc < ti.nch);
+        const unsigned mask = __ballot_sync(0xffffffffu, kc < ti.nch);
         if (!mask) break;
-        while (mask) {
-          const int j = __ffs(mask) - 1;   // = the team
-          mask &= mask - 1;
+#pragma unroll
+        for (int j = 0; j < PB_TEAMS; j++) {   // tile w0 + j belongs to team j
+          if (!((mask >> j) & 1u)) continue;
           const int seg = __shfl_sync(0xffffffffu, ti.seg, j), til = __shfl_sync(0xffffffffu, ti.til, j), type = __shfl_sync(0xffffffffu, ti.type, j);
-          const uint32_t i = j == 0 ? cnt[0] : cnt[1];
           if (lane == 0) {
-            const int kb = st_chunk_blocks(type), bb = st_block_bytes(type);
-            const int nblk = min(kb, nb - kc * kb);
-            const uint8_t* base = seg == 0 ? p.seg[0].w.st : (seg == 1 ? p.seg[1].w.st : p.seg[2].w.st);
-            const uint8_t* src = base + ((size_t)til * nb + (size_t)kc * kb) * bb;
-            const uint32_t slot = (i % D) * PB_TEAMS + (uint32_t)j, bytes = (uint32_t)(nblk * bb);
-            mbar_wait(&empty_bar[slot], ((i / D) & 1u) ^ 1u, 14, (int)i);
-            mbar_expect_tx(&full_bar[slot], bytes);
-            bulk_g2s(ring + (size_t)slot * ST_SLOT, src, bytes, &full_bar[slot]);
+            const RingPos rp = ring_pos(cnt[j], (uint32_t)j, PB_TEAMS, D);
+            const StItem it = st_item(p, seg, type, til, kc, nb);
+            mbar_wait(&empty_bar[rp.slot], rp.parity ^ 1u, W_PF_FREE_SLOT, (int)cnt[j]);
+            mbar_expect_tx(&full_bar[rp.slot], it.bytes);
+            bulk_g2s(ring + (size_t)rp.slot * ST_SLOT, it.src, it.bytes, &full_bar[rp.slot]);
           }
-          if (j == 0) cnt[0]++; else cnt[1]++;
+          cnt[j]++;
         }
       }
     }
@@ -337,16 +326,16 @@ __device__ __forceinline__ void pb_gemm_phase(const PPhase& ph, int n_tok, uint8
       const unsigned mask = __ballot_sync(0xffffffffu, kc < ti.nch);
       if (!mask) break;
       if ((mask >> team) & 1u) {
-        const uint32_t slot = (cnt % D) * PB_TEAMS + (uint32_t)team;
+        const RingPos rp = ring_pos(cnt, (uint32_t)team, PB_TEAMS, D);
         const int kb = st_chunk_blocks(my_type);
         const int b0 = kc * kb, nblk = min(kb, nb - b0);
-        const uint8_t* sp = ring + (size_t)slot * ST_SLOT;
-        mbar_wait(&full_bar[slot], (cnt / D) & 1u, 15, (int)cnt);
+        const uint8_t* sp = ring + (size_t)rp.slot * ST_SLOT;
+        mbar_wait(&full_bar[rp.slot], rp.parity, W_PF_WEIGHT_ITEM, (int)cnt);
         if (my_type == GT_Q4_K) pb_chunk<GT_Q4_K>(sp, nblk, b0, ph.qbuf, nb, lane, lp, (n_tok + 7) >> 3, st);
         else if (my_type == GT_Q6_K) pb_chunk<GT_Q6_K>(sp, nblk, b0, ph.qbuf, nb, lane, lp, (n_tok + 7) >> 3, st);
         else pb_chunk<GT_Q5_K>(sp, nblk, b0, ph.qbuf, nb, lane, lp, (n_tok + 7) >> 3, st);
         __syncwarp();
-        if (lane == 0) mbar_arrive(&empty_bar[slot]);   // 4 arrivals (the team's warps) free the slot
+        if (lane == 0) mbar_arrive(&empty_bar[rp.slot]);   // 4 arrivals (the team's warps) free the slot
         cnt++;
       }
     }
@@ -405,11 +394,7 @@ static __global__ void __launch_bounds__(PB_THREADS, 1) k_pstep(const __grid_con
   const int warp = threadIdx.x >> 5;
   uint8_t* ring = smem;
   uint8_t* work = smem + (size_t)args.n_slots * ST_SLOT;   // activation image (QUANT) / team exchange buffers (GEMM) / attention scratch
-  if (threadIdx.x == 0) {
-    for (int s = 0; s < args.n_slots; s++) { mbar_init(&full_bar[s], 1); mbar_init(&empty_bar[s], 4); }
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-  }
-  __syncthreads();
+  ring_init(full_bar, empty_bar, args.n_slots, 4);
   if (warp == PB_W) {
     pb_producer(args, ring, full_bar, empty_bar);
     return;
@@ -428,10 +413,7 @@ static __global__ void __launch_bounds__(PB_THREADS, 1) k_pstep(const __grid_con
     bar_sync<PB_BAR, PB_NT>();
     if (threadIdx.x == 0 && ip > 0) {
       const unsigned target = (unsigned)ip * G;
-      const unsigned long long t0 = globaltimer_ns();
-      while (ld_acquire_u32(args.sync) < target) {
-        if (globaltimer_ns() - t0 > ST_WATCHDOG_NS) st_fail(12, ip);
-      }
+      bounded_wait([&] { return ld_acquire_u32(args.sync) >= target; }, W_PF_GRID_BARRIER, ip);
     }
     bar_sync<PB_BAR, PB_NT>();
     const int n_tok = min(PB_T, ph.state[PB_T * 4]);
@@ -443,8 +425,8 @@ static __global__ void __launch_bounds__(PB_THREADS, 1) k_pstep(const __grid_con
         q.x = ph.mv.x + (size_t)tok * ph.x_ld;
         if (q.x2) q.x2 = ph.mv.x2 + (size_t)tok * ph.x2_ld;
         NormPre np;
-        preload_norm(np, q.norm_w, q.norm_b, q.norm_mode, q.K);
-        stage_activation<PB_NT, PB_BAR>(q, np, q.norm_w, q.norm_b, nullptr, q.norm_mode, q.eps, q.K, ACT_Q8_K, work, red, false);
+        preload_norm(np, q);
+        stage_activation<PB_NT, PB_BAR>(q, np, ACT_Q8_K, work, red, false);
         pb_quant_store<PB_NT, PB_BAR>(work, q.K, tok, ph.qbuf);
       }
     } else if (ph.kind == PP_KV) {
@@ -457,23 +439,11 @@ static __global__ void __launch_bounds__(PB_THREADS, 1) k_pstep(const __grid_con
         pb_attn_warp_task(ph.at, ph.state + tok * 4, tok, task % ph.at.n_head, wsm);
       }
     } else if (ph.kind == PP_EMBED) {
-      for (int tok = blockIdx.x; tok < n_tok; tok += G) {
-        const int id = ph.state[tok * 4];
-        const uint8_t* row = ph.em.table + (size_t)min(max(id, 0), ph.em.n_vocab - 1) * ph.em.row_bytes;
-        float* o = ph.em.out + (size_t)tok * ph.em.K;
-        for (int e = threadIdx.x; e < ph.em.K; e += PB_NT) o[e] = dequant_elem(ph.em.type, row, e);
-      }
+      for (int tok = blockIdx.x; tok < n_tok; tok += G) embed_row(ph.em, ph.state[tok * 4], ph.em.out + (size_t)tok * ph.em.K, threadIdx.x, PB_NT);
     }
   }
   bar_sync<PB_BAR, PB_NT>();
-  if (threadIdx.x == 0) {
-    __threadfence();
-    if (atomicAdd(args.sync + 1, 1u) == G - 1) {
-      args.sync[0] = 0u;
-      args.sync[1] = 0u;
-      __threadfence();
-    }
-  }
+  grid_rearm(args.sync);
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -483,18 +453,10 @@ inline size_t pb_work_bytes(int K_max, int n_ctx, int hd) {
   w = std::max(w, (size_t)PB_W * pb_attn_warp_bytes(n_ctx, hd));
   return (w + 127) & ~(size_t)127;
 }
-static inline size_t pstep_max_dyn_smem() {
-  cudaFuncAttributes fa{};
-  if (cudaFuncGetAttributes(&fa, k_pstep) != cudaSuccess) return 0;
-  int dev = 0, optin = 0;
-  cudaGetDevice(&dev);
-  cudaDeviceGetAttribute(&optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, dev);
-  return (size_t)optin > fa.sharedSizeBytes ? (size_t)optin - fa.sharedSizeBytes : 0;
-}
 // launch shape of k_pstep around `work` bytes of scratch: whole per-team sub-rings in what shared memory has left.  false
 // when fewer than 4 slots fit (the attention scratch of a long context): the caller then has no batched prefill.
 inline bool pstep_shape(size_t work, int& n_slots, size_t& smem) {
-  const size_t room = pstep_max_dyn_smem();
+  const size_t room = max_dyn_smem(k_pstep);
   if (work + 4 * (size_t)ST_SLOT > room) return false;
   n_slots = (int)std::min<size_t>(ST_MAX_SLOTS, (room - work) / ST_SLOT) / PB_TEAMS * PB_TEAMS;
   smem = (size_t)n_slots * ST_SLOT + work;

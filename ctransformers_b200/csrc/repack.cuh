@@ -5,20 +5,20 @@
 
 namespace ctb {
 
-struct PlaneSizes { size_t qs, qh, sc, d; };
+struct PlaneSizes { size_t qs, qh, d; };
 
 inline PlaneSizes plane_sizes(int type, int M, int nb, size_t raw_bytes) {
   const size_t nblk = (size_t)M * nb;
   switch (type) {
-    case GT_Q4_0: return {nblk * 16, 0, 0, nblk * 2};
-    case GT_Q5_0: return {nblk * 16, nblk * 4, 0, nblk * 2};
-    case GT_Q8_0: return {nblk * 32, 0, 0, nblk * 2};
-    default: return {raw_bytes, 0, 0, 0};
+    case GT_Q4_0: return {nblk * 16, 0, nblk * 2};
+    case GT_Q5_0: return {nblk * 16, nblk * 4, nblk * 2};
+    case GT_Q8_0: return {nblk * 32, 0, nblk * 2};
+    default: return {raw_bytes, 0, 0};
   }
 }
 
 // GGUF array-of-blocks → planes (device_types.cuh), 2 bytes per thread-iteration (non-K-quant types; K-quants: stream.cuh).
-static __global__ void k_repack(int type, const uint16_t* __restrict__ raw, size_t n_u16, uint16_t* qs, uint16_t* qh, uint16_t* sc, uint16_t* d) {
+static __global__ void k_repack(int type, const uint16_t* __restrict__ raw, size_t n_u16, uint16_t* qs, uint16_t* qh, uint16_t* d) {
   for (size_t idx = (size_t)blockIdx.x * blockDim.x + threadIdx.x; idx < n_u16; idx += (size_t)gridDim.x * blockDim.x) {
     const uint16_t v = raw[idx];
     switch (type) {

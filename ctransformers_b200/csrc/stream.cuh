@@ -51,8 +51,6 @@ constexpr int ST_ROWS = 16;
 constexpr int ST_BAR = 1;               // named barrier of the consumer warps
 constexpr int ST_STATE = 6;             // floats of fold state per thread: 4 AVX-lane accumulators + up to 2 mins accumulators
 
-__host__ __device__ inline int st_row_block_bytes(int type) { return type == GT_Q4_K ? 144 : (type == GT_Q5_K ? 176 : 210); }
-__host__ __device__ inline int st_block_bytes(int type) { return ST_ROWS * st_row_block_bytes(type); }   // 2304 / 2816 / 3360
 #ifndef CTB_CHUNK_Q4
 #define CTB_CHUNK_Q4 4
 #endif
@@ -62,9 +60,24 @@ __host__ __device__ inline int st_block_bytes(int type) { return ST_ROWS * st_ro
 #ifndef CTB_CHUNK_Q6
 #define CTB_CHUNK_Q6 2
 #endif
-static_assert(CTB_CHUNK_Q4 * 2304 <= ST_SLOT && CTB_CHUNK_Q5 * 2816 <= ST_SLOT && CTB_CHUNK_Q6 * 3360 <= ST_SLOT, "a work item must fit one ring slot");
-__host__ __device__ inline int st_chunk_blocks(int type) { return type == GT_Q4_K ? CTB_CHUNK_Q4 : (type == GT_Q5_K ? CTB_CHUNK_Q5 : CTB_CHUNK_Q6); }
-__host__ __device__ inline int st_tile_cost(int type) { return type == GT_Q6_K ? 105 : (type == GT_Q5_K ? 88 : 72); }   // bytes per row-block / 2
+// Per K-quant type: bytes of one row's 256-weight block, blocks per work item (one ring slot), mins accumulators of the fold
+struct StType { int rb, kb, nm; };
+__host__ __device__ constexpr StType st_type(int type) {
+  return type == GT_Q4_K ? StType{144, CTB_CHUNK_Q4, 2} : (type == GT_Q5_K ? StType{176, CTB_CHUNK_Q5, 1} : StType{210, CTB_CHUNK_Q6, 0});
+}
+template <int TYPE> struct StTraits {
+  static constexpr int KB = st_type(TYPE).kb, BB = ST_ROWS * st_type(TYPE).rb, NM = st_type(TYPE).nm;
+  static_assert(KB * BB <= ST_SLOT, "a work item must fit one ring slot");
+};
+__host__ __device__ inline int st_row_block_bytes(int type) { return st_type(type).rb; }
+__host__ __device__ inline int st_block_bytes(int type) { return ST_ROWS * st_type(type).rb; }   // 2304 / 2816 / 3360
+__host__ __device__ inline int st_chunk_blocks(int type) { return st_type(type).kb; }
+__host__ __device__ inline int st_tile_cost(int type) { return st_type(type).rb / 2; }
+// work items of a row of nb blocks (constant divisors)
+__host__ __device__ inline int st_chunks(int type, int nb) {
+  constexpr int K4 = StTraits<GT_Q4_K>::KB, K5 = StTraits<GT_Q5_K>::KB, K6 = StTraits<GT_Q6_K>::KB;
+  return type == GT_Q4_K ? (nb + K4 - 1) / K4 : (type == GT_Q5_K ? (nb + K5 - 1) / K5 : (nb + K6 - 1) / K6);
+}
 __host__ __device__ inline size_t st_matrix_bytes(int type, int M, int nb) { return (size_t)((M + ST_ROWS - 1) / ST_ROWS) * nb * st_block_bytes(type); }
 
 // ---------------------------------------------------------------------------------------------
@@ -120,13 +133,15 @@ static __global__ void k_repack_stream(int type, const uint8_t* __restrict__ raw
 }
 
 // ---------------------------------------------------------------------------------------------
-// Ring addressing.  Item n (one global sequence, enumerated identically by the producer and the consumers) belongs to
-// consumer warp n % ST_W and lives in one of THAT warp's own `depth` slots: slot = ((n / ST_W) % depth) * ST_W + n % ST_W,
-// mbarrier phase parity ((n / ST_W) / depth) & 1.  The warp that waits for item n is the warp that consumed the slot's
-// previous occupant, so it can never be a whole barrier phase ahead of the data (a parity wait cannot tell phase r from
-// phase r + 2: with slots shared between warps a fast warp saw "full" on a slot whose previous item was still landing).
-__device__ __forceinline__ uint32_t st_slot(uint32_t n, uint32_t depth) { return ((n / ST_W) % depth) * ST_W + n % ST_W; }
-__device__ __forceinline__ uint32_t st_parity(uint32_t n, uint32_t depth) { return ((n / ST_W) / depth) & 1u; }
+// Ring addressing.  Every owner (a consumer warp here, a team of warps in prefill.cuh) has its own `depth` slots: its i-th
+// item lives in slot (i % depth) * owners + owner with mbarrier phase parity (i / depth) & 1.  The owner that waits for an item
+// is the one that consumed the slot's previous occupant, so it can never be a whole barrier phase ahead of the data (a parity
+// wait cannot tell phase r from phase r + 2: with slots shared between owners a fast warp saw "full" on a slot whose previous
+// item was still landing).
+struct RingPos { uint32_t slot, parity; };
+__device__ __forceinline__ RingPos ring_pos(uint32_t i, uint32_t owner, uint32_t owners, uint32_t depth) { return {(i % depth) * owners + owner, (i / depth) & 1u}; }
+// the step kernel's items form one sequence that the producer and the consumers enumerate identically; item n belongs to warp n % ST_W
+__device__ __forceinline__ RingPos st_ring(uint32_t n, uint32_t depth) { return ring_pos(n / ST_W, n % ST_W, ST_W, depth); }
 
 // ---------------------------------------------------------------------------------------------
 // PTX: mbarrier, bulk copy, tensor-core mma
@@ -141,12 +156,17 @@ __device__ __forceinline__ bool mbar_try_wait(uint64_t* bar, uint32_t parity) {
   asm volatile("{\n .reg .pred p;\n mbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n selp.u32 %0, 1, 0, p;\n}" : "=r"(ok) : "r"(st_smem(bar)), "r"(parity) : "memory");
   return ok != 0;
 }
-__device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity, int code = 1, int aux = 0) {
-  if (mbar_try_wait(bar, parity)) return;
-  const unsigned long long t0 = globaltimer_ns();
-  while (!mbar_try_wait(bar, parity)) {
-    if (globaltimer_ns() - t0 > ST_WATCHDOG_NS) st_fail(code, aux);
+__device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity, WaitCode code, int aux) {
+  bounded_wait([&] { return mbar_try_wait(bar, parity); }, code, aux);
+}
+// the ring's barriers, by thread 0 before the CTA's first barrier: a full barrier completes on the producer's arrive and the
+// bytes of its copy, an empty barrier on the arrives of the consumers that share a slot
+__device__ __forceinline__ void ring_init(uint64_t* full_bar, uint64_t* empty_bar, int n_slots, int consumers_per_slot) {
+  if (threadIdx.x == 0) {
+    for (int s = 0; s < n_slots; s++) { mbar_init(&full_bar[s], 1); mbar_init(&empty_bar[s], consumers_per_slot); }
+    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
+  __syncthreads();
 }
 // global → shared bulk copy (TMA, SASS UBLKCP), completion counted in bytes on `bar`
 __device__ __forceinline__ void bulk_g2s(void* dst, const void* src, uint32_t bytes, uint64_t* bar) {
@@ -391,11 +411,6 @@ __device__ __forceinline__ void block_terms<GT_Q6_K>(const uint8_t* blk, int b, 
   }
 }
 
-template <int TYPE> struct StTraits;
-template <> struct StTraits<GT_Q4_K> { static constexpr int KB = CTB_CHUNK_Q4, BB = 2304, NM = 2; };
-template <> struct StTraits<GT_Q5_K> { static constexpr int KB = CTB_CHUNK_Q5, BB = 2816, NM = 1; };
-template <> struct StTraits<GT_Q6_K> { static constexpr int KB = CTB_CHUNK_Q6, BB = 3360, NM = 0; };
-
 // One work item: blocks [b0, b0 + nblk) of the 16-row tile whose pieces lie in `slot`.  Integer work first (the slot is
 // released as soon as the last weight word has been read), then the ordered fp32 fold: state in from the mailbox unless this
 // is the tile's first chunk, blocks folded in order, state out unless it is the last chunk — then hsum_float_8 and the epilogue.
@@ -419,12 +434,7 @@ __device__ __forceinline__ void run_item(const uint8_t* slot, uint64_t* empty_ba
 
   float acc[4] = {0.f, 0.f, 0.f, 0.f}, accm[2] = {0.f, 0.f};
   if (kc > 0) {
-    if (lane == 0 && *flag < kc) {
-      const unsigned long long t0 = globaltimer_ns();
-      while (*flag < kc) {
-        if (globaltimer_ns() - t0 > ST_WATCHDOG_NS) st_fail(3, kc);
-      }
-    }
+    if (lane == 0) bounded_wait([&] { return *flag >= kc; }, W_FOLD_FLAG, kc);
     __syncwarp();
     __threadfence_block();
 #pragma unroll
@@ -478,8 +488,7 @@ __device__ __forceinline__ void run_item(const uint8_t* slot, uint64_t* empty_ba
     const int row = row0 + g + 8 * t;
     if (row < sg.w.M) {
       if (XC && a.xc) {   // tensor-parallel partial sum: {value (+ residual on the rank that carries it), exchange number} to every rank
-        float v = t ? out[1] : out[0];
-        if (sg.epi == EPI_ADD) v = __fadd_rn(v, __ldcg(sg.res + row));
+        const float v = epilogue(sg.epi, t ? out[1] : out[0], sg.res + row, sg.res2 + row, p);
         const XchgParams& xc = *a.xc;
         const size_t at = ((size_t)(a.epoch & 1u) * xc.world + xc.rank) * xc.n + row;
         for (int r = 0; r < xc.world; r++)
@@ -548,7 +557,6 @@ struct XchgParams {
   int role;                            // 0 none, 1 this phase consumes the exchange (sums it while staging), 2 it produces it
   uint2* ll[XC_MAX_WORLD];             // region base of every rank as mapped here
 };
-struct EmbedParams { const uint8_t* table; size_t row_bytes; const int* tokens; float* out; int type, K, n_vocab; };
 struct PickParams { const float* logits; int* state; int* out_tokens; int n; };
 struct alignas(16) Phase {
   int kind;
@@ -592,9 +600,18 @@ __device__ __forceinline__ TileInfo tile_info(const TileSpace& ts, const MVParam
     ti.seg = ts.locate(tl);
     ti.til = tl;
     ti.type = ti.seg == 0 ? p.seg[0].w.type : (ti.seg == 1 ? p.seg[1].w.type : p.seg[2].w.type);
-    ti.nch = ti.type == GT_Q4_K ? (nb + CTB_CHUNK_Q4 - 1) / CTB_CHUNK_Q4 : (ti.type == GT_Q5_K ? (nb + CTB_CHUNK_Q5 - 1) / CTB_CHUNK_Q5 : (nb + CTB_CHUNK_Q6 - 1) / CTB_CHUNK_Q6);   // ceil(nb / st_chunk_blocks): constant divisors
+    ti.nch = st_chunks(ti.type, nb);
   }
   return ti;
+}
+
+// source and bytes of work item (chunk kc of tile til) of segment seg, whose type is `type`
+struct StItem { const uint8_t* src; uint32_t bytes; };
+__device__ __forceinline__ StItem st_item(const MVParams& p, int seg, int type, int til, int kc, int nb) {
+  const int kb = st_chunk_blocks(type), bb = st_block_bytes(type);
+  const int nblk = min(kb, nb - kc * kb);
+  const uint8_t* base = seg == 0 ? p.seg[0].w.st : (seg == 1 ? p.seg[1].w.st : p.seg[2].w.st);
+  return {base + ((size_t)til * nb + (size_t)kc * kb) * bb, (uint32_t)(nblk * bb)};
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -634,23 +651,25 @@ __device__ __forceinline__ void st_attn_produce(const AttnParams& p, uint8_t* ri
     for (int i0 = 0; i0 < g.n_k; i0 += step) {
       const int i = i0 + lane;
       if (lane < step && i < g.n_k) {
-        const uint32_t n = seq + (uint32_t)i, slot = st_slot(n, S);
+        const uint32_t n = seq + (uint32_t)i;
+        const RingPos rp = st_ring(n, S);
         const int rows = min(g.rpi, g.pos - i * g.rpi);
-        mbar_wait(&empty_bar[slot], st_parity(n, S) ^ 1u, 6, (int)n);
-        mbar_expect_tx(&full_bar[slot], (uint32_t)(rows * p.hd * 2));
-        bulk_g2s(ring + (size_t)slot * ST_SLOT, p.kc + k_row(kvh, i * g.rpi, p.n_ctx, p.hd), (uint32_t)(rows * p.hd * 2), &full_bar[slot]);
+        mbar_wait(&empty_bar[rp.slot], rp.parity ^ 1u, W_FREE_K_SLOT, (int)n);
+        mbar_expect_tx(&full_bar[rp.slot], (uint32_t)(rows * p.hd * 2));
+        bulk_g2s(ring + (size_t)rp.slot * ST_SLOT, p.kc + k_row(kvh, i * g.rpi, p.n_ctx, p.hd), (uint32_t)(rows * p.hd * 2), &full_bar[rp.slot]);
       }
       __syncwarp();
     }
     seq += (uint32_t)g.n_k;
     for (int iv = lane; iv < g.n_v; iv += 32) {   // n_v <= 32 / cv <= S is checked on the host (st_attn_ring_ok)
-      const uint32_t n = seq + (uint32_t)iv, slot = st_slot(n, S);
+      const uint32_t n = seq + (uint32_t)iv;
+      const RingPos rp = st_ring(n, S);
       const int nch = min(g.cv, ATTN_CH - iv * g.cv);
       const uint32_t bytes = (uint32_t)(g.nchv * 512);
-      mbar_wait(&empty_bar[slot], st_parity(n, S) ^ 1u, 7, (int)n);
-      mbar_expect_tx(&full_bar[slot], bytes * nch);
+      mbar_wait(&empty_bar[rp.slot], rp.parity ^ 1u, W_FREE_V_SLOT, (int)n);
+      mbar_expect_tx(&full_bar[rp.slot], bytes * nch);
       for (int q = 0; q < nch; q++)
-        bulk_g2s(ring + (size_t)slot * ST_SLOT + (size_t)q * bytes, p.vc + v_chan(kvh, cg * ATTN_CH + iv * g.cv + q, p.n_ctx, p.hd), bytes, &full_bar[slot]);
+        bulk_g2s(ring + (size_t)rp.slot * ST_SLOT + (size_t)q * bytes, p.vc + v_chan(kvh, cg * ATTN_CH + iv * g.cv + q, p.n_ctx, p.hd), bytes, &full_bar[rp.slot]);
     }
     __syncwarp();
     seq += (uint32_t)g.n_v;
@@ -666,12 +685,13 @@ __device__ __forceinline__ void st_attn_task(const AttnParams& p, uint8_t* smem,
   bar_sync<ST_BAR, ST_NT>();
   // ---- scores: K item i = ring item seq0 + i belongs to warp (seq0 + i) % ST_W (which also frees its slot)
   for (int i = (int)(((uint32_t)warp + ST_W - seq0 % ST_W) % ST_W); i < g.n_k; i += ST_W) {
-    const uint32_t n = seq0 + (uint32_t)i, slot = st_slot(n, S);
+    const uint32_t n = seq0 + (uint32_t)i;
+    const RingPos rp = st_ring(n, S);
     const int r0 = i * g.rpi;
-    mbar_wait(&full_bar[slot], st_parity(n, S), 8, (int)n);
-    attn_scores(p.hd, (const uint16_t*)(ring + (size_t)slot * ST_SLOT), min(g.rpi, g.pos - r0), 0, 8, s.q16, p.kq_scale, s.sc + r0);
+    mbar_wait(&full_bar[rp.slot], rp.parity, W_K_ITEM, (int)n);
+    attn_scores(p.hd, (const uint16_t*)(ring + (size_t)rp.slot * ST_SLOT), min(g.rpi, g.pos - r0), 0, 8, s.q16, p.kq_scale, s.sc + r0);
     __syncwarp();
-    if (lane == 0) mbar_arrive(&empty_bar[slot]);
+    if (lane == 0) mbar_arrive(&empty_bar[rp.slot]);
   }
   if (warp == (int)((seq0 + (uint32_t)g.n_k) % ST_W)) attn_scores(p.hd, s.k16, 1, 0, 8, s.q16, p.kq_scale, s.sc + g.pos);   // the current position
   bar_sync<ST_BAR, ST_NT>();
@@ -679,16 +699,17 @@ __device__ __forceinline__ void st_attn_task(const AttnParams& p, uint8_t* smem,
   // ---- V·P for this task's channels
   for (int cc = warp; cc < ATTN_CH; cc += ST_W) {
     const int c = cg * ATTN_CH + cc;
-    const uint32_t n = seq0 + (uint32_t)(g.n_k + cc / g.cv), slot = st_slot(n, S);
-    mbar_wait(&full_bar[slot], st_parity(n, S), 9, (int)n);
-    const uint16_t* vrow = (const uint16_t*)(ring + (size_t)slot * ST_SLOT + (size_t)(cc % g.cv) * g.nchv * 512);
+    const uint32_t n = seq0 + (uint32_t)(g.n_k + cc / g.cv);
+    const RingPos rp = st_ring(n, S);
+    mbar_wait(&full_bar[rp.slot], rp.parity, W_V_ITEM, (int)n);
+    const uint16_t* vrow = (const uint16_t*)(ring + (size_t)rp.slot * ST_SLOT + (size_t)(cc % g.cv) * g.nchv * 512);
     const float o = attn_vp(vrow, s.p16, g, g.pos, s.v16[c]);
     if (lane == 0) p.out[(size_t)h * p.hd + c] = o;
   }
   bar_sync<ST_BAR, ST_NT>();
   if (threadIdx.x < g.n_v) {
     const uint32_t n = seq0 + (uint32_t)(g.n_k + threadIdx.x);
-    mbar_arrive(&empty_bar[st_slot(n, S)]);
+    mbar_arrive(&empty_bar[st_ring(n, S).slot]);
   }
 }
 
@@ -727,15 +748,12 @@ __device__ __forceinline__ void st_producer(const StepArgs& args, uint8_t* ring,
         // lane of the same (converged) warp could fill
         for (int base = 0; base < cnt; base += ST_W * (int)S) {
           if (((mask >> lane) & 1u) && rank >= base && rank < base + ST_W * (int)S) {
-            const uint32_t n = seq + (uint32_t)rank, slot = st_slot(n, S);
-            const int kb = st_chunk_blocks(ti.type), bb = st_block_bytes(ti.type);
-            const int nblk = min(kb, nb - kc * kb);
-            const uint8_t* base_p = ti.seg == 0 ? p.seg[0].w.st : (ti.seg == 1 ? p.seg[1].w.st : p.seg[2].w.st);
-            const uint8_t* src = base_p + ((size_t)ti.til * nb + (size_t)kc * kb) * bb;
-            const uint32_t bytes = (uint32_t)(nblk * bb);
-            mbar_wait(&empty_bar[slot], st_parity(n, S) ^ 1u, 4, (int)n);
-            mbar_expect_tx(&full_bar[slot], bytes);
-            bulk_g2s_hint(ring + (size_t)slot * ST_SLOT, src, bytes, &full_bar[slot], weight_pol);
+            const uint32_t n = seq + (uint32_t)rank;
+            const RingPos rp = st_ring(n, S);
+            const StItem it = st_item(p, ti.seg, ti.type, ti.til, kc, nb);
+            mbar_wait(&empty_bar[rp.slot], rp.parity ^ 1u, W_FREE_WEIGHT_SLOT, (int)n);
+            mbar_expect_tx(&full_bar[rp.slot], it.bytes);
+            bulk_g2s_hint(ring + (size_t)rp.slot * ST_SLOT, it.src, it.bytes, &full_bar[rp.slot], weight_pol);
           }
           __syncwarp();
         }
@@ -756,7 +774,7 @@ __device__ __forceinline__ void st_matvec_phase(const Phase& ph, const NormPre& 
   const MVParams& p = ph.mv;
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const unsigned epoch = XC ? xc_base + (unsigned)ph.xc.index + 1u : 0u;   // number of the exchange this phase consumes / produces (if any)
-  stage_activation<ST_NT, ST_BAR, XC>(p, np, p.norm_w, p.norm_b, p.norm_out, p.norm_mode, p.eps, p.K, ACT_Q8_K, act_smem, red, blockIdx.x == 0, epoch);
+  stage_activation<ST_NT, ST_BAR, XC>(p, np, ACT_Q8_K, act_smem, red, blockIdx.x == 0, epoch);
   StAct a = st_act_extras<ST_NT, ST_BAR>(act_smem, p.K, ph.q6 != 0);
   a.xc = XC && ph.xc.role == 2 ? &ph.xc : nullptr;
   a.epoch = epoch;
@@ -787,19 +805,20 @@ __device__ __forceinline__ void st_matvec_phase(const Phase& ph, const NormPre& 
         const int j = __ffs(mr) - 1;
         const int seg = __shfl_sync(0xffffffffu, ti.seg, j), til = __shfl_sync(0xffffffffu, ti.til, j), type = __shfl_sync(0xffffffffu, ti.type, j);
         const int nch = __shfl_sync(0xffffffffu, ti.nch, j);
-        const uint32_t n = seq + (uint32_t)r, slot = st_slot(n, S);
+        const uint32_t n = seq + (uint32_t)r;
+        const RingPos rp = st_ring(n, S);
         const int kb = st_chunk_blocks(type);
         const int b0 = kc * kb, nblk = min(kb, nb - b0);
         const MVSeg& sg = p.seg[seg];
-        const uint8_t* sp = ring + (size_t)slot * ST_SLOT;
-        mbar_wait(&full_bar[slot], st_parity(n, S), 5, (int)n);
+        const uint8_t* sp = ring + (size_t)rp.slot * ST_SLOT;
+        mbar_wait(&full_bar[rp.slot], rp.parity, W_WEIGHT_ITEM, (int)n);
         if (first_item) { tr[2] = globaltimer_ns(); first_item = false; }
         volatile float* mail = mailbox[j];
         volatile int* flag = flags + j;
         const bool last = kc == nch - 1;
-        if (type == GT_Q4_K) run_item<GT_Q4_K, XC>(sp, &empty_bar[slot], nblk, b0, kc, last, a, lane, mail, flag, sg, p, til * ST_ROWS);
-        else if (type == GT_Q6_K) run_item<GT_Q6_K, XC>(sp, &empty_bar[slot], nblk, b0, kc, last, a, lane, mail, flag, sg, p, til * ST_ROWS);
-        else run_item<GT_Q5_K, XC>(sp, &empty_bar[slot], nblk, b0, kc, last, a, lane, mail, flag, sg, p, til * ST_ROWS);
+        if (type == GT_Q4_K) run_item<GT_Q4_K, XC>(sp, &empty_bar[rp.slot], nblk, b0, kc, last, a, lane, mail, flag, sg, p, til * ST_ROWS);
+        else if (type == GT_Q6_K) run_item<GT_Q6_K, XC>(sp, &empty_bar[rp.slot], nblk, b0, kc, last, a, lane, mail, flag, sg, p, til * ST_ROWS);
+        else run_item<GT_Q5_K, XC>(sp, &empty_bar[rp.slot], nblk, b0, kc, last, a, lane, mail, flag, sg, p, til * ST_ROWS);
       }
       seq += (uint32_t)cnt;
     }
@@ -808,30 +827,26 @@ __device__ __forceinline__ void st_matvec_phase(const Phase& ph, const NormPre& 
 
 // greedy pick + state advance (k_argmax + k_advance of the un-fused path), CTA 0 only
 __device__ __forceinline__ void st_pick_phase(const PickParams& pk, float* bv, int* bi) {
-  float best = -INFINITY;
-  int idx = 0x7fffffff;
-  for (int i = threadIdx.x; i < pk.n; i += ST_NT) {
-    const float v = __ldcg(pk.logits + i);
-    if (v > best) { best = v; idx = i; }
-  }
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) {
-    const float ov = __shfl_xor_sync(0xffffffffu, best, o);
-    const int oi = __shfl_xor_sync(0xffffffffu, idx, o);
-    if (ov > best || (ov == best && oi < idx)) { best = ov; idx = oi; }
-  }
-  if ((threadIdx.x & 31) == 0) { bv[threadIdx.x >> 5] = best; bi[threadIdx.x >> 5] = idx; }
-  bar_sync<ST_BAR, ST_NT>();
+  float best;
+  int idx;
+  block_argmax<ST_NT, ST_BAR, true>(pk.logits, pk.n, bv, bi, best, idx);
   if (threadIdx.x == 0) {
-    for (int w = 1; w < ST_W; w++)
-      if (bv[w] > best || (bv[w] == best && bi[w] < idx)) { best = bv[w]; idx = bi[w]; }
-    int* st = pk.state;   // {token, position, step, n_total, pick}
-    st[4] = idx;
-    pk.out_tokens[st[2]] = idx;
-    st[0] = idx;
-    st[1] += 1;
-    st[2] += 1;
-    st[3] = st[1] + 1;
+    pk.state[4] = idx;   // state = {token, position, step, n_total, pick}
+    advance_state(pk.state, pk.out_tokens, idx);
+  }
+}
+
+// End of a persistent launch, after the CTA's last barrier: the last CTA to get here re-arms the grid-barrier words for the
+// next launch (sync[0] arrivals, sync[1] finished CTAs) and, when set_xc, stores the tensor-parallel exchange count in sync[2].
+__device__ __forceinline__ void grid_rearm(unsigned* sync, bool set_xc = false, unsigned xc = 0) {
+  if (threadIdx.x == 0) {
+    __threadfence();
+    if (atomicAdd(sync + 1, 1u) == gridDim.x - 1) {
+      sync[0] = 0u;
+      sync[1] = 0u;
+      if (set_xc) sync[2] = xc;
+      __threadfence();
+    }
   }
 }
 
@@ -850,11 +865,7 @@ static __global__ void __launch_bounds__(ST_THREADS, 1) k_step(const __grid_cons
   const int warp = threadIdx.x >> 5;
   uint8_t* ring = smem;
   uint8_t* act_smem = smem + (size_t)args.n_slots * ST_SLOT;
-  if (threadIdx.x == 0) {
-    for (int s = 0; s < args.n_slots; s++) { mbar_init(&full_bar[s], 1); mbar_init(&empty_bar[s], 1); }
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-  }
-  __syncthreads();
+  ring_init(full_bar, empty_bar, args.n_slots, 1);
   pdl_trigger();
   pdl_wait();           // (the producer reads device state too: the position decides how many K / V items an attention phase has)
   if (warp == ST_W) {
@@ -886,12 +897,7 @@ static __global__ void __launch_bounds__(ST_THREADS, 1) k_step(const __grid_cons
       const unsigned target = (unsigned)ip * G;
       asm volatile("red.release.gpu.global.add.u32 [%0], 1;" ::"l"(args.sync) : "memory");
       if (tr) tr[5] = globaltimer_ns();
-      if (ld_relaxed_u32(args.sync) < target) {
-        const unsigned long long t0 = globaltimer_ns();
-        while (ld_relaxed_u32(args.sync) < target) {
-          if (globaltimer_ns() - t0 > ST_WATCHDOG_NS) st_fail(2, ip);
-        }
-      }
+      bounded_wait([&] { return ld_relaxed_u32(args.sync) >= target; }, W_GRID_BARRIER, ip);
       if (tr) { tr[6] = globaltimer_ns(); tr[7] = tr[6]; }
       // no acquire fence: everything the other CTAs produced is read with ld.global.cg (L2, never a stale L1 line), and those
       // loads are issued after the CTA barrier below, i.e. after this poll has returned
@@ -903,7 +909,7 @@ static __global__ void __launch_bounds__(ST_THREADS, 1) k_step(const __grid_cons
     const Phase& ph = ph_s[ip & 1];
     fetch_phase(ip + 1);
     NormPre np;
-    if (ph.kind == PH_MATVEC) preload_norm(np, ph.mv.norm_w, ph.mv.norm_b, ph.mv.norm_mode, ph.mv.K);
+    if (ph.kind == PH_MATVEC) preload_norm(np, ph.mv);
     if (tr && threadIdx.x == 0) tr[0] = globaltimer_ns();
     if (XC && ph.kind == PH_MATVEC && ph.xc.role == 1) xc_done++;
     if (ph.kind == PH_MATVEC) {
@@ -925,11 +931,7 @@ static __global__ void __launch_bounds__(ST_THREADS, 1) k_step(const __grid_cons
         }
       }
     } else if (ph.kind == PH_EMBED) {
-      if (blockIdx.x == 0) {
-        const int tok = ph.em.tokens[0];
-        const uint8_t* row = ph.em.table + (size_t)min(max(tok, 0), ph.em.n_vocab - 1) * ph.em.row_bytes;
-        for (int e = threadIdx.x; e < ph.em.K; e += ST_NT) ph.em.out[e] = dequant_elem(ph.em.type, row, e);
-      }
+      if (blockIdx.x == 0) embed_row(ph.em, ph.em.tokens[0], ph.em.out, threadIdx.x, ST_NT);
     } else if (ph.kind == PH_PICK) {
       if (blockIdx.x == 0) st_pick_phase(ph.pk, pick_v, pick_i);
     }
@@ -939,15 +941,7 @@ static __global__ void __launch_bounds__(ST_THREADS, 1) k_step(const __grid_cons
     }
   }
   bar_sync<ST_BAR, ST_NT>();
-  if (threadIdx.x == 0) {
-    __threadfence();
-    if (atomicAdd(args.sync + 1, 1u) == G - 1) {   // every CTA is past its last barrier: re-arm for the next launch
-      args.sync[0] = 0u;
-      args.sync[1] = 0u;
-      if (XC) args.sync[2] = xc_base + xc_done;
-      __threadfence();
-    }
-  }
+  grid_rearm(args.sync, XC, xc_base + xc_done);
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -1002,14 +996,6 @@ inline Phase matvec_phase(const MVParams& p) {
   return ph;
 }
 
-static inline size_t step_max_dyn_smem() {
-  cudaFuncAttributes fa{};
-  if (cudaFuncGetAttributes(&fa, k_step<true>) != cudaSuccess) return 0;   // (the two builds share their static shared memory)
-  int dev = 0, optin = 0;
-  cudaGetDevice(&dev);
-  cudaDeviceGetAttribute(&optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, dev);
-  return (size_t)optin > fa.sharedSizeBytes ? (size_t)optin - fa.sharedSizeBytes : 0;
-}
 // point the kernels' watchdog at 4 ints of host-mapped memory (each translation unit has its own copy of the symbol)
 static inline cudaError_t st_set_debug_words(int* dev_ptr) { return cudaMemcpyToSymbol(g_st_dbg, &dev_ptr, sizeof(int*)); }
 static inline cudaError_t step_set_smem_limit(size_t bytes) {
@@ -1021,13 +1007,7 @@ static inline cudaError_t launch_step(const StepLaunch& L, cudaStream_t st, cons
                                       unsigned long long* trace = nullptr, bool xchg = false) {
   StepArgs a;
   a.prog = d_prog; a.bounds = d_bounds; a.n_phases = n_phases; a.n_slots = L.n_slots; a.sync = d_sync; a.trace = trace;
-  cudaLaunchConfig_t cfg{};
-  cfg.gridDim = dim3(L.grid); cfg.blockDim = dim3(ST_THREADS); cfg.dynamicSmemBytes = L.smem; cfg.stream = st;
-  cudaLaunchAttribute at[1];
-  at[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-  at[0].val.programmaticStreamSerializationAllowed = 1;
-  cfg.attrs = at; cfg.numAttrs = pdl ? 1 : 0;
-  return xchg ? cudaLaunchKernelEx(&cfg, k_step<true>, a) : cudaLaunchKernelEx(&cfg, k_step<false>, a);
+  return launch_kernel(xchg ? k_step<true> : k_step<false>, dim3(L.grid), dim3(ST_THREADS), L.smem, st, pdl, a);
 }
 
 }  // namespace ctb
