@@ -163,6 +163,24 @@ __device__ __forceinline__ double block_sum_f64(double s, double* red /* [NT / 3
   for (int w = 0; w < NT / 32; w++) t += red[w];
   return t;
 }
+// two sums and a maximum at the price of one sum (red: [3 * NT / 32]); the sums are added in the order block_sum_f64 uses
+template <int NT, int BAR>
+__device__ __forceinline__ void block_sum2_max_f64(double& s, double& a, double& g, double* red) {
+  constexpr int NW = NT / 32;
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) {
+    s += __shfl_xor_sync(0xffffffffu, s, o);
+    a += __shfl_xor_sync(0xffffffffu, a, o);
+    g = fmax(g, __shfl_xor_sync(0xffffffffu, g, o));
+  }
+  bar_sync<BAR, NT>();
+  if ((threadIdx.x & 31) == 0) { red[threadIdx.x >> 5] = s; red[NW + (threadIdx.x >> 5)] = a; red[2 * NW + (threadIdx.x >> 5)] = g; }
+  bar_sync<BAR, NT>();
+  s = 0.0;
+  a = 0.0;
+#pragma unroll
+  for (int w = 0; w < NW; w++) { s += red[w]; a += red[NW + w]; g = fmax(g, red[2 * NW + w]); }
+}
 
 __device__ __forceinline__ uint32_t pack4(const int* q) {
   return (uint32_t)(q[0] & 0xff) | ((uint32_t)(q[1] & 0xff) << 8) | ((uint32_t)(q[2] & 0xff) << 16) | ((uint32_t)(q[3] & 0xff) << 24);
@@ -224,7 +242,70 @@ __device__ __forceinline__ void preload_norm(NormPre& np, const MVParams& p) {
   if (p.norm_mode != NORM_NONE && p.norm_b) load16(p.norm_b + t * 16, p.K - t * 16, np.bias0);
 }
 
+// One norm statistic, (float)(Σ term(x_i) / K), as the reference computes it: its double sum runs over the elements one after
+// another (ggml.c:10700-10703 / 10630-10645).  The threads add the same terms in another order (16-element chains, the warp
+// butterfly, the warps in order), and a double sum of float terms is not exact once they span more than about 53 - 24 -
+// log2(K) bits: then the two orders can round the float statistic differently.  Every order of K terms lies within
+// γ_K·Σ|t_i| of the exact sum (γ_K = K·u / (1 - K·u), u = 2^-53; an addition of an exact 0 is exact), so the reference's sum
+// lies within 2γ_K·A of the parallel one S, with A = Σ|t_i| (from below, A ≥ (1 - γ_K)·A_exact; the factor below covers that
+// for K ≤ 2^20).  Division and rounding to float are monotone: when both ends of [S - e, S + e] give the same float, so does
+// the reference's sum and S is used.  Otherwise (about K·2^-26 of normalisations by the bound) warp 0 adds the terms in
+// element order and broadcasts the sum.  s / a: this thread's partial sums of the terms / of |terms| (a_is_s: the terms are
+// never negative, so A = S and a is not reduced).  Every thread, and every CTA, sees the same S and A and takes the same branch.
+// LayerNorm's Σx of an input whose mean is near 0 fails the bound (|S| << A) too often; there every term is usually a multiple
+// of the smallest term's lsb, 1 / g, and A < 2^52 / g: then no partial sum in any order rounds and S is exact.  g: the largest
+// 1 / lsb over this thread's terms (lsb_inv; a_is_s: unused).
+__device__ __forceinline__ unsigned min_exp(unsigned emin, float t) {   // smallest exponent field of a non-zero term (subnormal: 1)
+  const unsigned bits = __float_as_uint(t) & 0x7fffffffu;
+  return bits ? min(emin, max(bits >> 23, 1u)) : emin;
+}
+__device__ __forceinline__ double lsb_inv(unsigned emin) { return ldexp(1.0, 150 - (int)emin); }
+
+enum : int { NORM_TERM_SQ = 0, NORM_TERM_X = 1, NORM_TERM_DEV = 2 };   // x², x, (x - mean)²
+// The statistic's sum in element order, by warp 0: it loads 512 elements at a time and every lane adds all of them.  Out of
+// line, one copy for the three statistics: it runs on few normalisations and would otherwise grow every kernel's hot code.
+// It takes the input's fields by value, so a caller's MVParams never has to live in local memory for its sake.
+template <bool XC>
+static __device__ __noinline__ double seq_sum_warp0(const float* x, const float* x2, int x_mode, int x_parts, int x_stride, int K, int kind,
+                                                    float mean, unsigned epoch) {
+  MVParams xs;
+  xs.x = x; xs.x2 = x2; xs.x_mode = x_mode; xs.x_parts = x_parts; xs.x_stride = x_stride;
+  const int lane = threadIdx.x & 31;
+  double seq = 0.0;
+  for (int base = 0; base < K; base += 512) {
+    float v[16];
+    load16x<XC>(xs, base + lane * 16, K - base - lane * 16, v, epoch);
+    for (int l = 0; l < 32; l++)
+#pragma unroll
+      for (int i = 0; i < 16; i++) {
+        float t = __shfl_sync(0xffffffffu, v[i], l);
+        if (kind == NORM_TERM_DEV) t = __fsub_rn(t, mean);
+        if (base + l * 16 + i < K) seq += kind == NORM_TERM_X ? (double)t : (double)__fmul_rn(t, t);
+      }
+  }
+  return seq;
+}
+
+template <int NT, int BAR, bool XC>
+__device__ __forceinline__ float norm_stat(double s, double a, double g, bool a_is_s, int kind, float mean, const MVParams& xs, double* red,
+                                           unsigned epoch) {
+  const int K = xs.K;
+  if (a_is_s) a = s = block_sum_f64<NT, BAR>(s, red);
+  else block_sum2_max_f64<NT, BAR>(s, a, g, red);
+  // inf / NaN terms give the same sum in every order (a double sum of float terms cannot overflow); so does an exact sum
+  if (!isfinite(s) || (!a_is_s && __dmul_ru(a, g) < 0x1p52)) return (float)(s / (double)K);
+  const double e = __dmul_ru(a, (double)K * 0x1.0000001p-52);   // ≥ 2γ_K / (1 - γ_K) · A, rounded up
+  const float lo = (float)(__dsub_rd(s, e) / (double)K), hi = (float)(__dadd_ru(s, e) / (double)K);
+  if (lo == hi) return lo;
+  const double seq = threadIdx.x < 32 ? seq_sum_warp0<XC>(xs.x, xs.x2, xs.x_mode, xs.x_parts, xs.x_stride, K, kind, mean, epoch) : 0.0;
+  bar_sync<BAR, NT>();   // every thread has read the partials out of red
+  if (threadIdx.x == 0) red[0] = seq;
+  bar_sync<BAR, NT>();
+  return (float)(red[0] / (double)K);
+}
+
 // The first NT threads of the CTA must call (named barrier BAR); each owns 16 consecutive elements per pass.
+// red: 3 * NT / 32 doubles of shared memory.
 template <int NT, int BAR, bool XC = false>   // XC: the input may be a tensor-parallel exchange (x_mode 2); compiled out otherwise
 __device__ __forceinline__ void stage_activation(const MVParams& xs, const NormPre& np, int act, uint8_t* smem, double* red, bool write_norm, unsigned epoch = 0) {
   const float* nw = xs.norm_w;
@@ -234,7 +315,7 @@ __device__ __forceinline__ void stage_activation(const MVParams& xs, const NormP
   const float eps = xs.eps;
   const int t = threadIdx.x, lane = t & 31;
   const int passes = (K + NT * 16 - 1) / (NT * 16);
-  // ---- statistics (fp64 sums like ggml.c:10700-10703 / 10630-10645; the order of a double sum does not reach the float result)
+  // ---- statistics: fp64 sums, the reference's float result (norm_stat)
   float mean = 0.f, scale = 1.f;
   float v0[16];                          // pass 0's x stays in registers
   load16x<XC>(xs, t * 16, K - t * 16, v0, epoch);
@@ -251,21 +332,24 @@ __device__ __forceinline__ void stage_activation(const MVParams& xs, const NormP
 #pragma unroll
       for (int e = 0; e < 16; e++) ss += (double)__fmul_rn(v[e], v[e]);
     }
-    ss = block_sum_f64<NT, BAR>(ss, red);
-    const float m = (float)(ss / (double)K);
+    const float m = norm_stat<NT, BAR, XC>(ss, ss, 0.0, true, NORM_TERM_SQ, 0.f, xs, red, epoch);
     scale = __fdiv_rn(1.0f, __fsqrt_rn(__fadd_rn(m, eps)));
   } else if (norm_mode == NORM_LAYER) {
-    double s1 = 0.0;
+    double s1 = 0.0, a1 = 0.0;
+    unsigned emin = 255;
     for (int ps = 0; ps < passes; ps++) {
       const int base = (ps * NT + t) * 16;
       if ((base & ~511) >= K) continue;
       float v[16];
       load16x<XC>(xs, base, K - base, v, epoch);
 #pragma unroll
-      for (int e = 0; e < 16; e++) s1 += (double)v[e];
+      for (int e = 0; e < 16; e++) {
+        s1 += (double)v[e];
+        a1 += (double)fabsf(v[e]);
+        emin = min_exp(emin, v[e]);
+      }
     }
-    s1 = block_sum_f64<NT, BAR>(s1, red);
-    mean = (float)(s1 / (double)K);
+    mean = norm_stat<NT, BAR, XC>(s1, a1, lsb_inv(emin), false, NORM_TERM_X, 0.f, xs, red, epoch);
     double s2 = 0.0;
     for (int ps = 0; ps < passes; ps++) {
       const int base = (ps * NT + t) * 16;
@@ -275,8 +359,7 @@ __device__ __forceinline__ void stage_activation(const MVParams& xs, const NormP
 #pragma unroll
       for (int e = 0; e < 16; e++) { const float d = (base + e < K) ? __fsub_rn(v[e], mean) : 0.f; s2 += (double)__fmul_rn(d, d); }
     }
-    s2 = block_sum_f64<NT, BAR>(s2, red);
-    const float var = (float)(s2 / (double)K);
+    const float var = norm_stat<NT, BAR, XC>(s2, s2, 0.0, true, NORM_TERM_DEV, mean, xs, red, epoch);
     scale = __fdiv_rn(1.0f, __fsqrt_rn(__fadd_rn(var, eps)));
   }
   // ---- normalise + quantize
@@ -515,7 +598,7 @@ __host__ __device__ inline int rows_per_unit(int type) { return (type == GT_F16 
 // Q4_0 / Q8_0 / F16 / F32 weights.  Persistent: one CTA per SM, warp tasks strided over all warps of the grid.
 static __global__ void __launch_bounds__(MV_THREADS, 1) k_matvec(const __grid_constant__ MVParams p) {
   extern __shared__ __align__(16) uint8_t smem[];
-  __shared__ double red[MV_WARPS];
+  __shared__ double red[3 * MV_WARPS];
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   pdl_trigger();
   NormPre np;

@@ -144,7 +144,7 @@ void run_matvec(MVParams& p) {
 // standalone wrappers around the prologue pieces, so the activation quantizers can be checked bit-for-bit
 __global__ void __launch_bounds__(MV_THREADS) k_stage_dump(const __grid_constant__ MVParams q, int act, uint8_t* dump) {
   extern __shared__ __align__(16) uint8_t smem[];
-  __shared__ double red[MV_WARPS];
+  __shared__ double red[3 * MV_WARPS];
   NormPre np;
   preload_norm(np, q);
   stage_activation<MV_THREADS, 0>(q, np, act, smem, red, true);
@@ -155,7 +155,7 @@ __global__ void __launch_bounds__(MV_THREADS) k_stage_dump(const __grid_constant
 // the x_mode = 1 input path of the prologue on its own: out[i] = gate_act[i] * up[i] (gate_act = silu_table(gate), from the epilogue)
 __global__ void __launch_bounds__(MV_THREADS) k_gate_dump(const __grid_constant__ MVParams q, float* out) {
   extern __shared__ __align__(16) uint8_t smem[];
-  __shared__ double red[MV_WARPS];
+  __shared__ double red[3 * MV_WARPS];
   NormPre np;
   preload_norm(np, q);
   stage_activation<MV_THREADS, 0>(q, np, ACT_F32, smem, red, false);
@@ -287,6 +287,34 @@ int ctb_norm(int mode, const float* x, const float* w, const float* b, float* y,
   return guarded("ctb_norm", [&] {
     std::vector<uint8_t> dump;
     stage_to_host(x, w, b, y, mode, eps, n, ACT_F32, dump);
+  });
+}
+
+int ctb_norm_path(int path, int mode, const float* x, const float* w, const float* b, float* y, int n, float eps) {
+  return guarded("ctb_norm_path", [&] {
+    if (path < 0 || path > 1) throw std::runtime_error("unknown norm path " + std::to_string(path));
+    if (mode != NORM_RMS && mode != NORM_LAYER) throw std::runtime_error("norm mode 1 or 2");
+    if (path == 0) {
+      std::vector<uint8_t> dump;
+      stage_to_host(x, w, b, y, mode, eps, n, ACT_F32, dump);
+      return;
+    }
+    if (n < 256 || n % 256) throw std::runtime_error("the step kernel takes n a positive multiple of 256");
+    // one mat-vec phase of the step kernel over 16 all-zero Q4_K rows: what is checked is the normalised vector CTA 0 writes
+    const std::vector<uint8_t> zeros(raw_row_bytes(GT_Q4_K, n) * 16, 0);
+    OwnedMat wm;
+    upload(wm, GT_Q4_K, zeros.data(), n, 16);
+    DevBuf dx((size_t)n * 4), dw((size_t)n * 4), db((size_t)n * 4), dy((size_t)n * 4), dout(16 * 4);
+    OPS_CUDA(cudaMemcpy(dx.p, x, (size_t)n * 4, cudaMemcpyHostToDevice));
+    if (w) OPS_CUDA(cudaMemcpy(dw.p, w, (size_t)n * 4, cudaMemcpyHostToDevice));
+    if (b) OPS_CUDA(cudaMemcpy(db.p, b, (size_t)n * 4, cudaMemcpyHostToDevice));
+    MVParams p{};
+    p.x = dx.as<float>(); p.norm_w = w ? dw.as<float>() : nullptr; p.norm_b = b && mode == NORM_LAYER ? db.as<float>() : nullptr;
+    p.norm_out = dy.as<float>(); p.norm_mode = mode; p.eps = eps; p.K = n; p.act = ACT_Q8_K; p.nseg = 1;
+    p.seg[0].w = wm.m; p.seg[0].out = dout.as<float>(); p.seg[0].epi = EPI_STORE;
+    p.silu_tab = tables().silu; p.gelu_tab = tables().gelu;
+    run_phases({matvec_phase(p)});
+    OPS_CUDA(cudaMemcpy(y, dy.p, (size_t)n * 4, cudaMemcpyDeviceToHost));
   });
 }
 

@@ -389,7 +389,7 @@ static __global__ void __launch_bounds__(PB_THREADS, 1) k_pstep(const __grid_con
   extern __shared__ __align__(16) uint8_t smem[];
   __shared__ __align__(8) uint64_t full_bar[ST_MAX_SLOTS];
   __shared__ __align__(8) uint64_t empty_bar[ST_MAX_SLOTS];
-  __shared__ double red[PB_W];
+  __shared__ double red[3 * PB_W];
   __shared__ __align__(16) PPhase ph;
   const int warp = threadIdx.x >> 5;
   uint8_t* ring = smem;

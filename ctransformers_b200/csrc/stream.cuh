@@ -855,7 +855,7 @@ static __global__ void __launch_bounds__(ST_THREADS, 1) k_step(const __grid_cons
   extern __shared__ __align__(16) uint8_t smem[];
   __shared__ __align__(8) uint64_t full_bar[ST_MAX_SLOTS];
   __shared__ __align__(8) uint64_t empty_bar[ST_MAX_SLOTS];
-  __shared__ double red[ST_W];
+  __shared__ double red[3 * ST_W];
   __shared__ __align__(16) float mailbox[ST_MAXT][ST_STATE * 32];
   __shared__ int flags[ST_MAXT];
   __shared__ float pick_v[ST_W];

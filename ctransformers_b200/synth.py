@@ -244,8 +244,19 @@ def _weight_producer(t, ne0, rows, sigma, seed, quantizer: Optional[Callable]):
     return produce
 
 
-def write_llama(path, shape: LlamaShape = LLAMA2_7B, ftype="Q4_K_M", seed=0, quantizer=None, sigma=0.02, emb_sigma=1.0):
-    """Llama-architecture GGUF.  Returns dict(path, weight_bytes_per_token, tensor_types)."""
+def _f32_table(n_vocab, E, sigma, seed, token_rows):
+    """token_embd as F32 rows: N(0, sigma²) values, with token_rows {token id: row [E]} in place of the drawn rows."""
+    def produce():
+        table = np.random.default_rng(seed).standard_normal((n_vocab, E), dtype=np.float32) * np.float32(sigma)
+        for tok, row in token_rows.items():
+            table[tok] = np.asarray(row, np.float32)
+        return table
+    return produce
+
+
+def write_llama(path, shape: LlamaShape = LLAMA2_7B, ftype="Q4_K_M", seed=0, quantizer=None, sigma=0.02, emb_sigma=1.0, token_rows=None):
+    """Llama-architecture GGUF.  Returns dict(path, weight_bytes_per_token, tensor_types).  token_rows {token id: row}: token_embd
+    is written as F32 with these rows (the rest drawn), so a test can choose exactly what the first layer's norm sees."""
     main, more, out_t, emb_t = _type_plan(ftype)
     w = GGUFWriter(path)
     a = "llama"
@@ -287,7 +298,12 @@ def write_llama(path, shape: LlamaShape = LLAMA2_7B, ftype="Q4_K_M", seed=0, qua
         s = sid[0]
         w.add_tensor(name, F32, (n,), lambda: (base + 0.1 * np.random.default_rng(s).standard_normal(n, dtype=np.float32)).astype(np.float32))
 
-    mat("token_embd.weight", emb_t, E, shape.n_vocab, emb_sigma, count=False)
+    if token_rows is None:
+        mat("token_embd.weight", emb_t, E, shape.n_vocab, emb_sigma, count=False)
+    else:
+        sid[0] += 1
+        w.add_tensor("token_embd.weight", F32, (E, shape.n_vocab), _f32_table(shape.n_vocab, E, emb_sigma, sid[0], token_rows))
+        types_used["token_embd.weight"] = F32
     for il in range(shape.n_layer):
         b = f"blk.{il}."
         mb = use_more_bits(il, shape.n_layer)
@@ -306,8 +322,8 @@ def write_llama(path, shape: LlamaShape = LLAMA2_7B, ftype="Q4_K_M", seed=0, qua
     return dict(path=str(path), weight_bytes_per_token=per_token[0], tensor_types=types_used)
 
 
-def write_falcon(path, shape: FalconShape = FALCON_7B_SHAPED, ftype="Q5_K_M", seed=0, quantizer=None, sigma=0.02, emb_sigma=1.0):
-    """Falcon-architecture GGUF (fused attn_qkv, LayerNorm with bias, gpt2/BPE vocabulary)."""
+def write_falcon(path, shape: FalconShape = FALCON_7B_SHAPED, ftype="Q5_K_M", seed=0, quantizer=None, sigma=0.02, emb_sigma=1.0, token_rows=None):
+    """Falcon-architecture GGUF (fused attn_qkv, LayerNorm with bias, gpt2/BPE vocabulary); token_rows as for write_llama."""
     main, more, _, emb_t = _type_plan(ftype)
     out_t = Q8_0 if ftype not in ("F16", "F32") else main
     w = GGUFWriter(path)
@@ -349,7 +365,12 @@ def write_falcon(path, shape: FalconShape = FALCON_7B_SHAPED, ftype="Q5_K_M", se
         s = sid[0]
         w.add_tensor(name, F32, (n,), lambda: (base + 0.1 * np.random.default_rng(s).standard_normal(n, dtype=np.float32)).astype(np.float32))
 
-    mat("token_embd.weight", emb_t, E, shape.n_vocab, emb_sigma, count=False)
+    if token_rows is None:
+        mat("token_embd.weight", emb_t, E, shape.n_vocab, emb_sigma, count=False)
+    else:
+        sid[0] += 1
+        w.add_tensor("token_embd.weight", F32, (E, shape.n_vocab), _f32_table(shape.n_vocab, E, emb_sigma, sid[0], token_rows))
+        types_used["token_embd.weight"] = F32
     for il in range(shape.n_layer):
         b = f"blk.{il}."
         mb = use_more_bits(il, shape.n_layer)

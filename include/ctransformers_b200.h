@@ -126,6 +126,12 @@ int ctb_quantize_row_q8_K(const float* x, void* y, int k);
 int ctb_quantize_row_q8_0(const float* x, void* y, int k);
 /* ggml_rms_norm + ggml_mul (mode 1) or ggml_norm + ggml_mul + ggml_add (mode 2) (ggml.c:10674-10720, 10605-10654). */
 int ctb_norm(int mode, const float* x, const float* w, const float* b, float* y, int n, float eps);
+/* The same norm (mode 1 or 2) through one of the kernels that normalise a mat-vec's input:
+ *   path 0  what ctb_norm runs: the prologue of k_matvec (MV_THREADS threads)
+ *   path 1  one mat-vec phase of the persistent step kernel launched as the engine launches it (16 all-zero Q4_K rows); y is
+ *           the normalised vector CTA 0 writes, as the engine's result_norm / embeddings; n a positive multiple of 256
+ * 0 on success, -1 (with a message on stderr) otherwise. */
+int ctb_norm_path(int path, int mode, const float* x, const float* w, const float* b, float* y, int n, float eps);
 /* ggml_rope_custom on [n_heads][head_dim] at position pos; mode 0 or 2 (neox) (ggml.c:12430-12566). */
 int ctb_rope(float* x, int n_heads, int head_dim, int pos, int mode, float freq_base, float freq_scale);
 /* One query token (at position T-1) against T cached positions, all heads, exactly as the reference's attention block:

@@ -12,7 +12,8 @@ Contents
   reference_runs.npz  what the reference computed for each test that compares with it (tests/test_model_gpu.py,
                    tests/test_oracle.py, tests/test_long_context_gpu.py), so those tests run where the reference is not
                    available.  `python make_golden.py long_context` adds the long-context runs to the existing file,
-                   `python make_golden.py realq_prefill` the reference-quantized Q5_K_M prefill runs.
+                   `python make_golden.py realq_prefill` the reference-quantized Q5_K_M prefill runs, `python make_golden.py
+                   norm_order` the runs of the models with planted norm rows (tests/test_norm_order_gpu.py).
 """
 import ctypes as C
 import json
@@ -225,6 +226,24 @@ def realq_prefill_runs(tmp):
     assert all(np.array_equal(new[k], v) and new[k].dtype == v.dtype for k, v in old.items()), "an existing key changed"
 
 
+def norm_order_runs(tmp):
+    """Adds the reference's results for modelcases.NORM_ORDER_MODELS to reference_runs.npz as keys norm_<case>_*; every key
+    already in the file keeps its bytes."""
+    old = dict(refs.golden_runs())
+    out = dict(old)
+    for name in modelcases.NORM_ORDER_MODELS:
+        path, ctx = modelcases.build_norm_order(name, tmp)
+        states, toks = modelcases.norm_order_llm_run(ref_llm(path, ctx), name)
+        for i, (logits, embd) in enumerate(states):
+            out[f"norm_{name}_{i}_logits"] = np.array(refs.digest(logits))
+            out[f"norm_{name}_{i}_embd"] = np.array(refs.digest(embd))
+        out[f"norm_{name}_tokens"] = np.array(toks, np.int32)
+        print(name, "tokens", toks)
+    np.savez_compressed(HERE / "reference_runs.npz", **out)
+    new = refs.golden_runs()
+    assert all(np.array_equal(new[k], v) and new[k].dtype == v.dtype for k, v in old.items()), "an existing key changed"
+
+
 if __name__ == "__main__":
     assert refs.have_ref(), "build oracle/_ref first: make -C oracle ref"
     import sys
@@ -241,7 +260,9 @@ if __name__ == "__main__":
                 long_context_runs(tmp)
             if "realq_prefill" in only:
                 realq_prefill_runs(tmp)
-            cases = [o for o in only if o not in ("kat", "reference_blocks", "reference_runs", "long_context", "realq_prefill")]
+            if "norm_order" in only:
+                norm_order_runs(tmp)
+            cases = [o for o in only if o not in ("kat", "reference_blocks", "reference_runs", "long_context", "realq_prefill", "norm_order")]
             if cases:
                 models(tmp, cases)
         else:

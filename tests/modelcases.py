@@ -136,3 +136,61 @@ def run_greedy(llm, prompt, n_new, batch_size=8):
         toks.append(int(t))
         llm.eval([t])
     return first_logits, first_embd, toks, np.array(llm.logits, dtype=np.float32), gaps
+
+
+# Models whose token_embd (F32) holds rows that break the kernels' order of the first layer's norm sums (refs.norm_order_rows):
+# model case -> norm mode.  Q4_K_M Llama: step kernel and batched prefill; Q4_0 Llama: k_matvec; Q5_K_M Falcon: LayerNorm, with
+# rows that break Σx and rows that break Σ(x - mean)² alone.  The prompt is one 40-token chunk, which the batched prefill runs as
+# a full 32-token launch and a short 8-token one, with planted tokens in both; then every planted token is a decode step of its
+# own, then greedy steps.
+NORM_ORDER_MODELS = {"llama_tiny_q4km": 1, "llama_tiny_q4_0": 1, "falcon_tiny_q5km": 2}
+NORM_ORDER_PLANTED = list(range(300, 308))
+NORM_ORDER_AT = [3, 17, 30, 33, 36, 39]   # prompt positions of planted tokens: 3 in the full launch, 3 in the short one
+NORM_ORDER_PROMPT, NORM_ORDER_GREEDY = 40, 4
+
+
+def build_norm_order(name, directory):
+    import refs
+    arch, shape, ftype, ctx = CASES[name]
+    path = Path(directory) / f"{name}_norm_order.gguf"
+    if not path.exists():
+        rows, _, _ = refs.norm_order_rows(NORM_ORDER_MODELS[name], shape.n_embd, seed=shape.n_embd)
+        rows = np.resize(rows, (len(NORM_ORDER_PLANTED), shape.n_embd))
+        (synth.write_llama if arch == "llama" else synth.write_falcon)(path, shape, ftype, seed=11,
+                                                                      token_rows=dict(zip(NORM_ORDER_PLANTED, rows)))
+    return path, ctx
+
+
+def norm_order_prompt(name):
+    ids = seeded_prompt(name, NORM_ORDER_PROMPT, seed=23)
+    for i, p in enumerate(NORM_ORDER_AT):
+        ids[p] = NORM_ORDER_PLANTED[i % len(NORM_ORDER_PLANTED)]
+    return ids
+
+
+def norm_order_run(eval_fn, state_fn, pick_fn, name):
+    """The prompt in one chunk, every planted token as a decode step, then greedy steps.  eval_fn(tokens, batch_size), state_fn()
+    -> (logits, embeddings), pick_fn() -> greedy token.  Returns ([(logits, embeddings) after the prompt and after every step],
+    greedy tokens)."""
+    eval_fn(norm_order_prompt(name), 512)
+    states = [state_fn()]
+    for t in NORM_ORDER_PLANTED:
+        eval_fn([t], 512)
+        states.append(state_fn())
+    toks = []
+    for _ in range(NORM_ORDER_GREEDY):
+        toks.append(int(pick_fn()))
+        eval_fn([toks[-1]], 512)
+        states.append(state_fn())
+    return states, toks
+
+
+def norm_order_llm_run(llm, name):
+    return norm_order_run(lambda t, bs: llm.eval(t, batch_size=bs),
+                          lambda: (np.array(llm.logits, np.float32), np.array(llm.embeddings, np.float32)),
+                          lambda: llm.sample(top_k=1, repetition_penalty=1.0, seed=0), name)
+
+
+def norm_order_oracle_run(model, name):
+    return norm_order_run(lambda t, bs: model.eval(t, batch_size=bs), lambda: (model.logits.copy(), model.embd.copy()),
+                          lambda: int(np.argmax(model.logits)), name)

@@ -370,3 +370,142 @@ class OracleModel:
         if getattr(self, "m", None):
             self.o.orc_model_free(self.m)
             self.m = None
+
+
+# --------------------------------------------------------------------------------------------------------------
+# The order of the norms' fp64 sums (csrc/matvec.cuh stage_activation / norm_stat).  The reference adds the terms one after
+# another; the kernels' threads add them in chains, a warp butterfly and warp order.  Rows whose terms span many binary orders
+# of magnitude round the float statistic differently in the two orders; norm_order_rows plants such rows.
+def seq_sum(terms):
+    """The reference's order: terms[..., 0] + terms[..., 1] + ... in double (np.cumsum adds in sequence; np.sum is pairwise)."""
+    return np.cumsum(np.asarray(terms, np.float64), axis=-1)[..., -1]
+
+
+def kernel_order_sum(terms, nt):
+    """The parallel order of stage_activation + block_sum_f64 with nt threads: thread t adds, starting from 0.0, elements
+    (ps*nt + t)*16 .. +15 of every pass ps in pass-major order; the warp butterfly adds the lane sums with xor offsets 16, 8,
+    4, 2, 1; the warp sums are then added from 0.0 in warp order."""
+    t = np.asarray(terms, np.float64)
+    rows = t.reshape(-1, t.shape[-1])
+    R, K = rows.shape
+    passes = -(-K // (nt * 16))
+    pad = np.zeros((R, passes * nt * 16))
+    pad[:, :K] = rows
+    per = pad.reshape(R, passes, nt, 16).transpose(0, 2, 1, 3).reshape(R, nt, passes * 16)
+    lane = np.cumsum(per, axis=-1)[..., -1].reshape(R, nt // 32, 32)
+    idx = np.arange(32)
+    for o in (16, 8, 4, 2, 1):
+        lane = lane + lane[..., idx ^ o]
+    return np.cumsum(lane[..., 0], axis=-1)[..., -1].reshape(t.shape[:-1])
+
+
+def norm_emulated(mode, x, w, b, eps, summer):
+    """RMSNorm * w (mode 1) or LayerNorm * w + b (mode 2) of rows x in float32, as orc_rms_norm_mul / orc_layer_norm_mul_add
+    compute them, with summer(terms) adding the fp64 sums.  Returns (y, the float statistics: (mean of squares,) or (mean, var))."""
+    x = np.atleast_2d(np.asarray(x, np.float32))
+    K = x.shape[-1]
+    stat = lambda t: (summer(t.astype(np.float64)) / K).astype(np.float32)[:, None]
+    f32 = np.float32
+    if mode == 1:
+        m = stat(x * x)
+        scale = f32(1) / np.sqrt(m + f32(eps))
+        return (x * scale) * w, (m,)
+    mean = stat(x)
+    d = x - mean
+    var = stat(d * d)
+    scale = f32(1) / np.sqrt(var + f32(eps))
+    return ((d * scale) * w) + b, (mean, var)
+
+
+NORM_ORDER_THREADS = tuple(range(64, 1025, 32))   # every CTA size a build can give the kernels (k_step 320, k_pstep 256, k_matvec 512)
+NORM_ORDER_EPS = 1e-5
+
+
+def _planted_row(kind, K, where, rng):
+    """One row that breaks the statistic `kind` ("rms": Σx², "mean": Σx, "var": Σ(x - mean)²) in the kernel orders, or None.
+    A cluster of large elements carries the sum: x1 and x2 tune it to just below a float rounding boundary of sum / K, and x0
+    comes last.  The reference's order then drops every small term after x0 (each is less than half an ulp of the running sum)
+    and rounds down; the kernels add the small terms to each other first, keep them and round up.  For "var" every value comes
+    with its negation right after it (x0's, the chain of 16 elements it starts holds nothing else), so Σx is exactly 0 in any of
+    these orders, the mean is 0 and only Σx² breaks."""
+    c = {"start": 0, "middle": K // 2 + 16 * int(rng.integers(0, 8)) + 5, "warp": 509 if K >= 1024 else 13, "end": K - 99}[where]
+    sq, var = kind != "mean", kind == "var"
+    if var:
+        c -= 2                                                     # x0 stays at the same place: the last of its thread's chain
+    x = np.zeros(K, np.float32)
+    cl = [c, c + 1, c + 2, c + 3, c + 4, c + 5] if var else [c, c + 1, c + 2]
+    e_small = float(rng.choice([-27.0, -27.5, -28.0])) if sq else float(rng.choice([-54.0, -55.0, -56.0]))
+    small = (np.exp2(e_small) * rng.uniform(0.75, 1.0, K)).astype(np.float32)   # squares (or values) below 2^-54 · x0^2 (x0)
+    if var:
+        taken = np.zeros(K, bool)
+        taken[cl] = True
+        xz = cl[-1]
+        taken[xz:(xz // 16 + 1) * 16] = True                       # nothing after -x0 in its chain
+        for j in range(0, K - 1, 2):
+            if not taken[j] and not taken[j + 1]:
+                x[j], x[j + 1] = small[j], -small[j]
+    else:
+        x[:] = small * (rng.choice([-1, 1], K).astype(np.float32) if kind == "rms" else 1)
+        x[cl] = 0
+    x0 = np.float32(2 + rng.integers(0, 2048) / 1024.0) if not sq else np.float32(1.5 + rng.integers(0, 1024) / 2048.0)
+    i0 = cl[-2] if var else cl[-1]
+    x[i0] = x0
+    if var:
+        x[cl[-1]] = -x0
+
+    def terms(r):
+        return (r * r).astype(np.float64) if sq else r.astype(np.float64)
+
+    s = seq_sum(terms(x))
+    m = np.float32(s / K)
+    M = (np.float64(m) + np.float64(np.nextafter(m, np.float32(np.inf)))) / 2   # the rounding boundary above m
+    r = M * K - s - 2 * np.spacing(s)                              # what x1 and x2 add, a little short of the boundary
+    if var:
+        r /= 2
+    if r <= 0:
+        return None
+    f = (lambda v: float(np.float32(v) * np.float32(v))) if sq else float
+    parts = []
+    for _ in range(2):
+        v = np.float32(np.sqrt(r) if sq else r)
+        while v > 0 and f(v) > r:
+            v = np.nextafter(v, np.float32(0))
+        parts.append(v)
+        r -= f(v)
+    if var:
+        x[cl[0]], x[cl[1]], x[cl[2]], x[cl[3]] = parts[0], -parts[0], parts[1], -parts[1]
+    else:
+        x[cl[0]], x[cl[1]] = parts
+    p2 = np.float32(2.0 ** int(np.ceil(np.log2(np.sqrt(K)) if sq else np.log2(K))))   # statistic of order 1: eps does not absorb it
+    return x * p2
+
+
+def _order_breaks(mode, x, w, b):
+    """True when, for every thread count in NORM_ORDER_THREADS, the kernel order changes the float statistics and y."""
+    want, stats = norm_emulated(mode, x, w, b, NORM_ORDER_EPS, seq_sum)
+    for nt in NORM_ORDER_THREADS:
+        got, kstats = norm_emulated(mode, x, w, b, NORM_ORDER_EPS, lambda t: kernel_order_sum(t, nt))
+        if all(np.array_equal(a, c) for a, c in zip(stats, kstats)) or np.array_equal(got.view(np.uint32), want.view(np.uint32)):
+            return False
+    return True
+
+
+def norm_order_rows(mode, K, seed):
+    """Planted rows of width K for norm mode 1 (RMSNorm: rows that break Σx²) or 2 (LayerNorm: rows that break Σx, and rows that
+    break only Σ(x - mean)²), with the norm weight w and bias b they were checked with.  The cluster of large elements sits at the
+    start, in the middle, across a warp boundary (a thread boundary when K < 1024) and near the end; the small terms' size varies
+    with the seed.  Every row is checked (_order_breaks) to change the float statistic and y at every thread count."""
+    rng = np.random.default_rng(seed)
+    w = (1 + 0.1 * rng.standard_normal(K)).astype(np.float32)
+    b = (0.1 * rng.standard_normal(K)).astype(np.float32)
+    rows = []
+    for kind in (("rms",) if mode == 1 else ("mean", "var")):
+        for where in ("start", "middle", "warp", "end"):
+            for _ in range(64):
+                x = _planted_row(kind, K, where, rng)
+                if x is not None and _order_breaks(mode, x, w, b):
+                    rows.append(x)
+                    break
+            else:
+                raise AssertionError(f"no {kind} row at {where} for K {K}")
+    return np.stack(rows), w, b
