@@ -1,5 +1,5 @@
 // Non-matmul stages of the eval graph, each reproducing the reference's rounding points:
-//   k_embed     ggml_get_rows on a quantized token_embd            ggml.c:11615-11642 + dequantize_row_* (k_quants.c:784-821, 984-1026, 1123-1166; ggml.c:1483-1608)
+//   k_embed     ggml_get_rows on a quantized token_embd            ggml.c:11615-11642 + dequantize_row_* (k_quants.c:784-821, 984-1026, 1123-1166; ggml.c:1483-1610)
 //   RoPE        rope_pair / rope_head_pair / rope_k_pair (mode 0 / neox), K row and V channel store   ggml.c:12430-12566, llama.cpp:2303-2335
 //   attention   the helpers attn_stage / attn_scores / attn_softmax / attn_vp: RoPE + KV store, K·q (fp16 operands, fp32
 //               acc) → scale → causal mask → fp16-table softmax (fp64 sum) → P→fp16 → V·P, with the reference's AVX2
@@ -42,6 +42,17 @@ __device__ __forceinline__ float dequant_elem(int type, const uint8_t* row, int 
       const int byte = blk[6 + (r & 15)];
       const int nib = r < 16 ? (byte & 0xF) : (byte >> 4);
       return __fmul_rn((float)((nib | (int)(((qh >> r) & 1u) << 4)) - 16), d);
+    }
+    case GT_Q4_1: case GT_Q5_1: {   // dequantize_row_q4_1 / q5_1 (ggml.c:1538-1557, 1585-1610): x*d + m, unsigned quants
+      const bool q5 = type == GT_Q5_1;
+      const uint8_t* blk = row + (size_t)(e >> 5) * (q5 ? 24 : 20);
+      const int r = e & 31;
+      const float d = h2f((uint16_t)(blk[0] | (blk[1] << 8)));
+      const float m = h2f((uint16_t)(blk[2] | (blk[3] << 8)));
+      const int byte = blk[(q5 ? 8 : 4) + (r & 15)];
+      int q = r < 16 ? (byte & 0xF) : (byte >> 4);
+      if (q5) q |= ((blk[4 + (r >> 3)] >> (r & 7)) & 1) << 4;
+      return __fmaf_rn((float)q, d, m);   // q*d is exact in fp32, so this equals the reference's x*d + m in either form
     }
     case GT_Q8_0: {
       const uint8_t* blk = row + (size_t)(e >> 5) * 34;

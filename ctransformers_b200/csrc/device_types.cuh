@@ -11,12 +11,14 @@
 //   type   plane qs (per row)          plane qh (per row)   plane d (per row)
 //   Q4_0   nb x 16 B nibbles           -                    nb x fp16
 //   Q5_0   nb x 16 B nibbles           nb x 4 B fifth bits  nb x fp16
+//   Q4_1   nb x 16 B nibbles           -                    nb x fp16      + plane mn: nb x fp16 mins
+//   Q5_1   nb x 16 B nibbles           nb x 4 B fifth bits  nb x fp16      + plane mn: nb x fp16 mins
 //   Q8_0   nb x 32 B int8              -                    nb x fp16
 //   F16    K x 2 B                     -                    -
 //   F32    K x 4 B                     -                    -
 //
 // Block contents are exactly the reference's (k_quants.h:76-117, ggml.c:888-925); only their placement
-// changes.  Activations are quantized on the fly to the reference's Q8_K / Q8_0 (bit-exact) into
+// changes.  Activations are quantized on the fly to the reference's Q8_K / Q8_0 / Q8_1 (bit-exact) into
 // shared memory (struct ActView) and never touch HBM.
 #pragma once
 #include <cstdint>
@@ -26,7 +28,7 @@
 
 namespace ctb {
 
-enum : int { GT_F32 = 0, GT_F16 = 1, GT_Q4_0 = 2, GT_Q5_0 = 6, GT_Q8_0 = 8, GT_Q4_K = 12, GT_Q5_K = 13, GT_Q6_K = 14 };
+enum : int { GT_F32 = 0, GT_F16 = 1, GT_Q4_0 = 2, GT_Q4_1 = 3, GT_Q5_0 = 6, GT_Q5_1 = 7, GT_Q8_0 = 8, GT_Q4_K = 12, GT_Q5_K = 13, GT_Q6_K = 14 };
 
 struct DevMat {
   int type = -1;
@@ -34,8 +36,8 @@ struct DevMat {
   int nb = 0;           // quant blocks per row
   const uint8_t* qs = nullptr;
   const uint8_t* qh = nullptr;
-  const void* unused = nullptr;   // no plane; the step kernel's phase descriptors embed DevMats, and dropping these 8 bytes moved
-                                  // its dynamic shared memory by 32 B, which cost 2.5 % decode speed (H100 80GB HBM3, 700 W)
+  const uint16_t* mn = nullptr;  // Q4_1 / Q5_1: the min plane.  The step kernel's phase descriptors embed DevMats, and dropping
+                                 // these 8 bytes moved its dynamic shared memory by 32 B, which cost 2.5 % decode speed (H100 80GB HBM3, 700 W)
   const uint16_t* d = nullptr;
   const uint8_t* st = nullptr;   // K-quants: the stream layout of stream.cuh (16-row tiles, block-major; qs/qh/d stay null)
   size_t bytes = 0;     // total bytes of all planes (= GGUF tensor bytes)
@@ -43,10 +45,11 @@ struct DevMat {
 
 __host__ __device__ inline bool type_is_kquant(int t) { return t == GT_Q4_K || t == GT_Q5_K || t == GT_Q6_K; }
 // activation format each weight type is multiplied with (reference: type_traits vec_dot_type, ggml.c:1638-1808)
-enum : int { ACT_Q8_K = 0, ACT_Q8_0 = 1, ACT_F16 = 2, ACT_F32 = 3 };
+enum : int { ACT_Q8_K = 0, ACT_Q8_0 = 1, ACT_F16 = 2, ACT_F32 = 3, ACT_Q8_1 = 4 };
 __host__ __device__ inline int act_format_for(int t) {
   if (type_is_kquant(t)) return ACT_Q8_K;
   if (t == GT_Q4_0 || t == GT_Q5_0 || t == GT_Q8_0) return ACT_Q8_0;
+  if (t == GT_Q4_1 || t == GT_Q5_1) return ACT_Q8_1;
   if (t == GT_F16) return ACT_F16;
   return ACT_F32;
 }

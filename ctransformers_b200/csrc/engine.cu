@@ -85,7 +85,8 @@ constexpr size_t UP_CHUNK = (size_t)32 << 20;   // upload pipeline: chunk bytes 
 constexpr int UP_BUFS = 3;
 
 static bool supported_matrix_type(uint32_t t) {
-  return t == T_F32 || t == T_F16 || t == T_Q4_0 || t == T_Q5_0 || t == T_Q8_0 || t == T_Q4_K || t == T_Q5_K || t == T_Q6_K;
+  return t == T_F32 || t == T_F16 || t == T_Q4_0 || t == T_Q4_1 || t == T_Q5_0 || t == T_Q5_1 || t == T_Q8_0 || t == T_Q4_K || t == T_Q5_K ||
+         t == T_Q6_K;
 }
 
 size_t engine_arena_bytes(const GGUFFile& g, const HParams& hp) {
@@ -187,7 +188,7 @@ DevMat Engine::upload_matrix(const GGUFTensor& t, Uploader& up, int want_K, int 
   }
   int rows_per_chunk = (int)std::max<size_t>(ST_ROWS, UP_CHUNK / row_bytes / ST_ROWS * ST_ROWS);   // whole 16-row tiles
   if (row_bytes * ST_ROWS > UP_CHUNK) throw std::runtime_error("tensor '" + t.name + "': rows too long for the upload staging buffers");
-  uint16_t *st = nullptr, *qs = nullptr, *qh = nullptr, *d = nullptr;
+  uint16_t *st = nullptr, *qs = nullptr, *qh = nullptr, *d = nullptr, *mn = nullptr;
   const bool kq = type_is_kquant(m.type);
   if (kq) {
     st = (uint16_t*)alloc(st_matrix_bytes(m.type, m.M, m.nb));
@@ -197,7 +198,8 @@ DevMat Engine::upload_matrix(const GGUFTensor& t, Uploader& up, int want_K, int 
     qs = (uint16_t*)alloc(ps.qs);
     if (ps.qh) qh = (uint16_t*)alloc(ps.qh);
     if (ps.d) d = (uint16_t*)alloc(ps.d);
-    m.qs = (const uint8_t*)qs; m.qh = (const uint8_t*)qh; m.d = d;
+    if (ps.mn) mn = (uint16_t*)alloc(ps.mn);
+    m.qs = (const uint8_t*)qs; m.qh = (const uint8_t*)qh; m.d = d; m.mn = mn;
   }
   for (int r0 = 0; r0 < m.M; r0 += rows_per_chunk) {
     const int rows = std::min(rows_per_chunk, m.M - r0);
@@ -211,8 +213,10 @@ DevMat Engine::upload_matrix(const GGUFTensor& t, Uploader& up, int want_K, int 
       const size_t n_u16 = n / 2;
       const size_t blk0 = (size_t)r0 * m.nb;
       const int grid = (int)std::min<size_t>((n_u16 + 255) / 256, (size_t)sm_count_ * 32);
-      uint16_t* qdst = qs + ((m.type == GT_Q4_0 || m.type == GT_Q5_0) ? blk0 * 8 : (m.type == GT_Q8_0 ? blk0 * 16 : (size_t)r0 * row_bytes / 2));
-      k_repack<<<grid, 256, 0, up.st[slot]>>>(m.type, (const uint16_t*)up.dev[slot], n_u16, qdst, qh ? qh + blk0 * 2 : nullptr, d ? d + blk0 : nullptr);
+      const bool nib = m.type == GT_Q4_0 || m.type == GT_Q5_0 || m.type == GT_Q4_1 || m.type == GT_Q5_1;   // 16 B of nibbles per block
+      uint16_t* qdst = qs + (nib ? blk0 * 8 : (m.type == GT_Q8_0 ? blk0 * 16 : (size_t)r0 * row_bytes / 2));
+      k_repack<<<grid, 256, 0, up.st[slot]>>>(m.type, (const uint16_t*)up.dev[slot], n_u16, qdst, qh ? qh + blk0 * 2 : nullptr, d ? d + blk0 : nullptr,
+                                              mn ? mn + blk0 : nullptr);
     }
     CTB_CUDA(cudaGetLastError());
     up.finish(slot);

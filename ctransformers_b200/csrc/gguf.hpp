@@ -46,7 +46,8 @@ inline int type_block_bytes(uint32_t t) {
 }
 inline const char* type_name(uint32_t t) {
   switch (t) {
-    case T_F32: return "f32"; case T_F16: return "f16"; case T_Q4_0: return "q4_0"; case T_Q5_0: return "q5_0"; case T_Q8_0: return "q8_0";
+    case T_F32: return "f32"; case T_F16: return "f16"; case T_Q4_0: return "q4_0"; case T_Q4_1: return "q4_1"; case T_Q5_0: return "q5_0";
+    case T_Q5_1: return "q5_1"; case T_Q8_0: return "q8_0";
     case T_Q4_K: return "q4_K"; case T_Q5_K: return "q5_K"; case T_Q6_K: return "q6_K";
   }
   return "unsupported";

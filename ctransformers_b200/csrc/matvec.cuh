@@ -2,10 +2,11 @@
 //
 //   stage_activation<NT, BAR>  the prologue of every mat-vec: RMSNorm / LayerNorm with fp64 reductions + separate weight (+bias)
 //                              multiply (ggml.c:10674-10720, 10605-10654) and the activation quantization to Q8_K (K-quants,
-//                              k_quants.c:1191-1226) or Q8_0 (Q4_0/Q8_0, ggml.c:1232-1268) into shared memory, never HBM
-//   k_matvec                   y[M] = W[M,K]·x[K] for the non-K-quant weight types (Q4_0 / Q8_0 / F16 / F32): one CTA per SM,
-//                              warp tasks strided over the grid, the reference kernels' lane order restated
-//                              (Q4_0 ggml.c:2500-2525 · Q8_0 3379-3402 · F16 2392-2426 · F32 2330-2365)
+//                              k_quants.c:1191-1226), Q8_0 (Q4_0/Q5_0/Q8_0, ggml.c:1232-1268) or Q8_1 (Q4_1/Q5_1, ggml.c:1420-1481)
+//                              into shared memory, never HBM
+//   k_matvec                   y[M] = W[M,K]·x[K] for the non-K-quant weight types (Q4_0 / Q5_0 / Q8_0 / Q4_1 / Q5_1 / F16 / F32):
+//                              one CTA per SM, warp tasks strided over the grid, the reference kernels' lane order restated
+//                              (Q4_0 ggml.c:2500-2525 · Q4_1 2770-2803 · Q5_1 3234-3259 · Q8_0 3379-3402 · F16 2392-2426 · F32 2330-2365)
 //   store_epilogue             store | + residual (ggml_add, llama.cpp:2415, 2453) | SiLU / GELU fp16 table (ggml.c:3568-3632)
 //
 // K-quant weights (Q4_K / Q5_K / Q6_K — everything a Q4_K_M / Q5_K_M file multiplies per token) go through the persistent
@@ -101,6 +102,7 @@ struct MVParams {
 //   Q8_K: qs is stored lane-major per block: byte offset of int8 word (sub-block s, lane l) = ((b*2 + (s>>2))*8 + l)*16 + (s&3)*4,
 //         so GPU lane l reads its 8 words of a block with two conflict-free 16-byte loads.  d: per block.  bs: bsums, natural.
 //   Q8_0: natural order; d per 32 (already rounded through fp16).
+//   Q8_1: natural order; {d, s} float pairs per 32 at d (d[2b] = d, d[2b + 1] = s of block b).
 struct ActView {
   const int8_t* qs;
   const float* d;
@@ -111,6 +113,7 @@ __host__ __device__ inline size_t act_smem_bytes(int act, int K) {
   switch (act) {
     case ACT_Q8_K: return (size_t)K + (((size_t)(K / 256) * 4 + 15) & ~(size_t)15) + (size_t)(K / 16) * 2 + 16;
     case ACT_Q8_0: return (size_t)K + (size_t)(K / 32) * 4 + 16;
+    case ACT_Q8_1: return (size_t)K + (size_t)(K / 32) * 8 + 16;
     case ACT_F16: return (size_t)K * 2;
     default: return (size_t)K * 4;
   }
@@ -457,6 +460,24 @@ __device__ __forceinline__ void stage_activation(const MVParams& xs, const NormP
         *(uint4*)(qs + base) = make_uint4(pack4(q), pack4(q + 4), pack4(q + 8), pack4(q + 12));
         if ((lane & 1) == 0) dd[base >> 5] = h2f(f2h(d));
       }
+    } else if (act == ACT_Q8_1) {
+      // quantize_row_q8_1, AVX2 variant (ggml.c:1420-1481): as Q8_0, but d = amax/127 stays a float, and s = d * (float)Σq
+      // over the block (an exact integer sum; the two threads of a block add their halves)
+      float amax = 0.f;
+#pragma unroll
+      for (int e = 0; e < 16; e++) amax = fmaxf(amax, fabsf(v[e]));
+      amax = fmaxf(amax, __shfl_xor_sync(0xffffffffu, amax, 1));
+      const float d = __fdiv_rn(amax, 127.f);
+      const float id = amax != 0.f ? __fdiv_rn(127.f, amax) : 0.f;
+      int q[16];
+      int sum = 0;
+#pragma unroll
+      for (int e = 0; e < 16; e++) { q[e] = __float2int_rn(__fmul_rn(v[e], id)); sum += q[e]; }
+      sum += __shfl_xor_sync(0xffffffffu, sum, 1);
+      if (valid > 0) {
+        *(uint4*)(qs + base) = make_uint4(pack4(q), pack4(q + 4), pack4(q + 8), pack4(q + 12));
+        if ((lane & 1) == 0) *(float2*)(dd + (base >> 4)) = make_float2(d, __fmul_rn(d, (float)sum));
+      }
     } else if (act == ACT_F16) {
       uint16_t* h = (uint16_t*)smem;
 #pragma unroll
@@ -539,8 +560,42 @@ __device__ __forceinline__ float dot_q80(const DevMat& w, int row, const ActView
   return group_hsum8(acc);
 }
 
+// Q4_1 / Q5_1 with a Q8_1 activation (ggml.c:2770-2803, 3234-3259): unsigned nibbles (Q5_1: the fifth bit ORed in as 0x10, value
+// 0..31), lane l the integer sum of elements 4l..4l+3 (bytes_from_nibbles_32 + mul_sum_us8_pairs_float), acc = fma(d_w*d_y, sum,
+// acc) per block; the mins enter through the scalar chain summs += m_w * s_y in block order, which the reference binary fuses
+// (vfmadd231ss), and the result is hsum_float_8(acc) + summs.  Every lane of the row's group runs the same summs chain.
+template <bool Q5>
+__device__ __forceinline__ float dot_q1(const DevMat& w, int row, const ActView& a, int l) {
+  const int nb = w.nb;
+  const uint8_t* qrow = w.qs + (size_t)row * nb * 16 + (l & 3) * 4;
+  const uint32_t* hrow = (const uint32_t*)w.qh + (size_t)row * nb;
+  const uint16_t* drow = w.d + (size_t)row * nb;
+  const uint16_t* mrow = w.mn + (size_t)row * nb;
+  const int shift = (l >> 2) * 4;
+  float acc = 0.f, summs = 0.f;
+#pragma unroll 8
+  for (int b = 0; b < nb; b++) {
+    const uint32_t q = (uint32_t)__ldg((const int*)(qrow + (size_t)b * 16));
+    const float dw = h2f(__ldg(drow + b));
+    const float mw = h2f(__ldg(mrow + b));
+    const int aw = *(const int*)(a.qs + b * 32 + l * 4);
+    const float2 ds = *(const float2*)(a.d + 2 * b);
+    uint32_t bx = (q >> shift) & 0x0f0f0f0fu;
+    if (Q5) bx |= ((((__ldg(hrow + b) >> (4 * l)) & 0xfu) * 0x00204081u) & 0x01010101u) << 4;   // bit k of the 4 -> 0x10 in byte k
+    acc = __fmaf_rn(__fmul_rn(dw, ds.x), (float)__dp4a((int)bx, aw, 0), acc);
+    summs = __fmaf_rn(mw, ds.y, summs);
+  }
+  return __fadd_rn(group_hsum8(acc), summs);
+}
+
 __device__ __forceinline__ float dot_legacy(const DevMat& w, int row, const ActView& a, int l) {
-  return w.type == GT_Q4_0 ? dot_q40(w, row, a, l) : (w.type == GT_Q5_0 ? dot_q50(w, row, a, l) : dot_q80(w, row, a, l));
+  switch (w.type) {
+    case GT_Q4_0: return dot_q40(w, row, a, l);
+    case GT_Q5_0: return dot_q50(w, row, a, l);
+    case GT_Q4_1: return dot_q1<false>(w, row, a, l);
+    case GT_Q5_1: return dot_q1<true>(w, row, a, l);
+    default: return dot_q80(w, row, a, l);
+  }
 }
 
 // GGML_F32x8_REDUCE over a warp that plays 4 accumulators x 8 lanes (lane = 8*j + l): (0+2),(1+3) -> (0+1) -> lo128+hi128 ->
@@ -595,7 +650,7 @@ __device__ __forceinline__ void store_epilogue(const MVSeg& sg, const MVParams& 
 __host__ __device__ inline int rows_per_unit(int type) { return (type == GT_F16 || type == GT_F32) ? 1 : MV_ROWS; }
 
 // ---------------------------------------------------------------------------------------------
-// Q4_0 / Q8_0 / F16 / F32 weights.  Persistent: one CTA per SM, warp tasks strided over all warps of the grid.
+// Q4_0 / Q5_0 / Q8_0 / Q4_1 / Q5_1 / F16 / F32 weights.  Persistent: one CTA per SM, warp tasks strided over all warps of the grid.
 static __global__ void __launch_bounds__(MV_THREADS, 1) k_matvec(const __grid_constant__ MVParams p) {
   extern __shared__ __align__(16) uint8_t smem[];
   __shared__ double red[3 * MV_WARPS];

@@ -57,11 +57,15 @@ size_t raw_row_bytes(int type, int K) {
   switch (type) {
     case GT_F32: return (size_t)K * 4; case GT_F16: return (size_t)K * 2;
     case GT_Q4_0: return (size_t)K / 32 * 18; case GT_Q5_0: return (size_t)K / 32 * 22; case GT_Q8_0: return (size_t)K / 32 * 34;
+    case GT_Q4_1: return (size_t)K / 32 * 20; case GT_Q5_1: return (size_t)K / 32 * 24;
     case GT_Q4_K: return (size_t)K / 256 * 144; case GT_Q5_K: return (size_t)K / 256 * 176; case GT_Q6_K: return (size_t)K / 256 * 210;
   }
   throw std::runtime_error("unsupported ggml type " + std::to_string(type));
 }
-int block_elems(int type) { return type_is_kquant(type) ? 256 : (type == GT_Q4_0 || type == GT_Q5_0 || type == GT_Q8_0) ? 32 : 1; }
+int block_elems(int type) {
+  if (type_is_kquant(type)) return 256;
+  return (type == GT_Q4_0 || type == GT_Q5_0 || type == GT_Q8_0 || type == GT_Q4_1 || type == GT_Q5_1) ? 32 : 1;
+}
 
 struct OwnedMat {
   DevMat m;
@@ -86,13 +90,13 @@ void upload(OwnedMat& o, int type, const void* blocks, int K, int M) {
     return;
   }
   const PlaneSizes ps = plane_sizes(type, M, o.m.nb, bytes);
-  uint16_t* pl[3] = {nullptr, nullptr, nullptr};
-  const size_t sz[3] = {ps.qs, ps.qh, ps.d};
-  for (int i = 0; i < 3; i++)
+  uint16_t* pl[4] = {nullptr, nullptr, nullptr, nullptr};
+  const size_t sz[4] = {ps.qs, ps.qh, ps.d, ps.mn};
+  for (int i = 0; i < 4; i++)
     if (sz[i]) { OPS_CUDA(cudaMalloc((void**)&pl[i], sz[i])); o.bufs.push_back(pl[i]); }
-  k_repack<<<(int)std::min<size_t>((bytes / 2 + 255) / 256, 4096), 256>>>(type, raw.as<uint16_t>(), bytes / 2, pl[0], pl[1], pl[2]);
+  k_repack<<<(int)std::min<size_t>((bytes / 2 + 255) / 256, 4096), 256>>>(type, raw.as<uint16_t>(), bytes / 2, pl[0], pl[1], pl[2], pl[3]);
   OPS_CUDA(cudaDeviceSynchronize());
-  o.m.qs = (const uint8_t*)pl[0]; o.m.qh = (const uint8_t*)pl[1]; o.m.d = pl[2];
+  o.m.qs = (const uint8_t*)pl[0]; o.m.qh = (const uint8_t*)pl[1]; o.m.d = pl[2]; o.m.mn = pl[3];
 }
 
 int sm_count() {
@@ -279,6 +283,20 @@ int ctb_quantize_row_q8_0(const float* x, void* y, int k) {
       const uint16_t h = __half_as_ushort(__float2half_rn(d[b]));   // d[b] is already fp16-representable
       memcpy(out + (size_t)b * 34, &h, 2);
       memcpy(out + (size_t)b * 34 + 2, dump.data() + (size_t)b * 32, 32);
+    }
+  });
+}
+
+int ctb_quantize_row_q8_1(const float* x, void* y, int k) {
+  return guarded("ctb_quantize_row_q8_1", [&] {
+    if (k % 32) throw std::runtime_error("k must be a multiple of 32");
+    std::vector<uint8_t> dump;
+    stage_to_host(x, nullptr, nullptr, nullptr, NORM_NONE, 0.f, k, ACT_Q8_1, dump);
+    const size_t off = ((size_t)k + 15) & ~(size_t)15;
+    uint8_t* out = (uint8_t*)y;   // block_q8_1: float d; float s; int8 qs[32]  (ggml.c:928-932)
+    for (int b = 0; b < k / 32; b++) {
+      memcpy(out + (size_t)b * 40, dump.data() + off + (size_t)b * 8, 8);
+      memcpy(out + (size_t)b * 40 + 8, dump.data() + (size_t)b * 32, 32);
     }
   });
 }

@@ -76,6 +76,7 @@ EXTRA_PROTOTYPES = {
     "ctb_mul_mat": (C.c_int, [C.c_int, _P, _P, _P, C.c_int, C.c_int, C.c_int]),
     "ctb_quantize_row_q8_K": (C.c_int, [_P, _P, C.c_int]),
     "ctb_quantize_row_q8_0": (C.c_int, [_P, _P, C.c_int]),
+    "ctb_quantize_row_q8_1": (C.c_int, [_P, _P, C.c_int]),
     "ctb_norm": (C.c_int, [C.c_int, _P, _P, _P, _P, C.c_int, C.c_float]),
     "ctb_norm_path": (C.c_int, [C.c_int, C.c_int, _P, _P, _P, _P, C.c_int, C.c_float]),
     "ctb_rope": (C.c_int, [_P, C.c_int, C.c_int, C.c_int, C.c_int, C.c_float, C.c_float]),

@@ -118,12 +118,14 @@ int ctb_sample(const float* logits, int n_vocab, const int* last_tokens, int n_l
                float repetition_penalty, int seed);
 
 /* Op-level mirrors (host pointers in, host pointers out; return 0 on success).  ggml type ids: 0 F32, 1 F16,
- * 2 Q4_0, 8 Q8_0, 12 Q4_K, 13 Q5_K, 14 Q6_K (models/ggml/ggml.h enum ggml_type). */
+ * 2 Q4_0, 3 Q4_1, 6 Q5_0, 7 Q5_1, 8 Q8_0, 12 Q4_K, 13 Q5_K, 14 Q6_K (models/ggml/ggml.h enum ggml_type). */
 /* ggml_mul_mat for quantized src0 (ggml.c:11031-11245): dst[n*M+m] = dot(W row m, quantize(x col n)). */
 int ctb_mul_mat(int type, const void* w_blocks, const float* x, float* dst, int K, int M, int N);
 /* quantize_row_q8_K (k_quants.c:1191-1241) / quantize_row_q8_0 (ggml.c:1232-1268): reference block bytes out. */
 int ctb_quantize_row_q8_K(const float* x, void* y, int k);
 int ctb_quantize_row_q8_0(const float* x, void* y, int k);
+/* quantize_row_q8_1 (ggml.c:1420-1481, the activation of Q4_1 / Q5_1 weights): block_q8_1 bytes {float d, float s, int8 qs[32]}. */
+int ctb_quantize_row_q8_1(const float* x, void* y, int k);
 /* ggml_rms_norm + ggml_mul (mode 1) or ggml_norm + ggml_mul + ggml_add (mode 2) (ggml.c:10674-10720, 10605-10654). */
 int ctb_norm(int mode, const float* x, const float* w, const float* b, float* y, int n, float eps);
 /* The same norm (mode 1 or 2) through one of the kernels that normalise a mat-vec's input:
