@@ -105,13 +105,25 @@ static __global__ void k_embed(const EmbedParams em) {
 // KV cache layouts (ours; the reference keeps K [n_ctx][n_embd_gqa] and V transposed [n_embd_gqa][n_ctx], llama.cpp:2323-2335).
 // Both are permuted so that the GPU lane that plays lane L of the reference's 4x8-lane f16 dot (ggml_vec_dot_f16,
 // ggml.c:2392-2426: lane L accumulates elements 32i+L in order i) finds ITS elements contiguous:
-//   K: [n_kv][n_ctx][hd]        head-major (a head's rows of positions 0..T-1 are one contiguous run: one bulk copy brings a
-//                               stretch of them into shared memory); element e of a row is stored at (e & 31) * (hd/32) + (e >> 5)
+//   K: [n_kv][n_ctx][k_stride]  head-major (a head's rows of positions 0..T-1 are one contiguous run: one bulk copy brings a
+//                               stretch of them into shared memory).  The first np = hd & ~31 elements of a row (the dot's SIMD
+//                               part) are lane-major: element e < np at (e & 31) * (np/32) + (e >> 5).  The tail np .. hd-1
+//                               (added one by one in double) follows in element order.  The row stride k_stride is hd rounded up
+//                               to 8 halves, so that every row and every run of rows is 16-byte aligned for bulk copies and
+//                               16-byte loads (hd 64 / 128: stride hd, no tail).
 //   V: [n_kv][hd][ctx_pad]      (channel-major like the reference) position t at (t & ~255) + (t & 31) * 8 + ((t >> 5) & 7)
 __host__ __device__ inline int kv_ctx_pad(int n_ctx) { return (n_ctx + 255) & ~255; }
-__host__ __device__ inline size_t k_row(int kv_head, int pos, int n_ctx, int hd) { return ((size_t)kv_head * n_ctx + pos) * hd; }   // element offset of a K row
+__host__ __device__ inline int k_stride(int hd) { return (hd + 7) & ~7; }
+// (GEN = false: the caller's hd is 64 or 128, where the stride is hd and there is no tail — the same values in fewer operations)
+template <bool GEN = true>
+__host__ __device__ inline size_t k_row(int kv_head, int pos, int n_ctx, int hd) { return ((size_t)kv_head * n_ctx + pos) * (GEN ? k_stride(hd) : hd); }   // element offset of a K row
 __host__ __device__ inline size_t v_chan(int kv_head, int c, int n_ctx, int hd) { return ((size_t)kv_head * hd + c) * kv_ctx_pad(n_ctx); }   // ... of a V channel
-__host__ __device__ inline int k_perm(int e, int hd) { return (e & 31) * (hd >> 5) + (e >> 5); }
+template <bool GEN = true>
+__host__ __device__ inline int k_perm(int e, int hd) {
+  if (!GEN) return (e & 31) * (hd >> 5) + (e >> 5);
+  const int np = hd & ~31;
+  return e < np ? (e & 31) * (np >> 5) + (e >> 5) : e;
+}
 __host__ __device__ inline int v_perm(int t) { return (t & ~255) + (t & 31) * 8 + ((t >> 5) & 7); }
 
 // The (cos, sin) table [n_pos][hd/2] every RoPE kernel reads: the reference's theta recurrence with the same libm calls
@@ -152,13 +164,14 @@ __device__ __forceinline__ void rope_head_pair(const float* x, int i, int hd, in
 }
 
 // the same, rounded to f16 and stored at the pair's K-permuted places of a row, and of a second row when one is given
+template <bool GEN = true>
 __device__ __forceinline__ void rope_k_pair(const float* x, int i, int hd, int neox, float2 cs, uint16_t* row, uint16_t* row2 = nullptr) {
   int i0, i1;
   float o0, o1;
   rope_head_pair(x, i, hd, neox, cs, i0, i1, o0, o1);
   const uint16_t h0 = f2h(o0), h1 = f2h(o1);
-  row[k_perm(i0, hd)] = h0; row[k_perm(i1, hd)] = h1;
-  if (row2) { row2[k_perm(i0, hd)] = h0; row2[k_perm(i1, hd)] = h1; }
+  row[k_perm<GEN>(i0, hd)] = h0; row[k_perm<GEN>(i1, hd)] = h1;
+  if (row2) { row2[k_perm<GEN>(i0, hd)] = h0; row2[k_perm<GEN>(i1, hd)] = h1; }
 }
 
 // ------------------------------------------------------------------------------------------- attn
@@ -170,14 +183,15 @@ __device__ __forceinline__ void rope_k_pair(const float* x, int i, int hd, int n
 //   pb_attn_warp_task  the batched prefill kernel, one warp per task (prefill.cuh)
 // The pieces:
 //   attn_stage    RoPE on q and k (the reference's cos/sin recurrence), q -> f16; decode: k, v -> f16 and the cache  (llama.cpp:2303-2335)
-//   attn_scores   KQ = ggml_vec_dot_f16(hd, K row, f16(q)) — lane L: fma over elements 32i+L in order, then the 4x8 reduce;
-//                 KQ *= kq_scale
+//   attn_scores   KQ = ggml_vec_dot_f16(hd, K row, f16(q)) — lane L: fma over elements 32i+L (i < hd/32) in order, then the
+//                 4x8 reduce, then elements hd & ~31 .. hd-1 added one by one in double (ggml.c:2392-2426); KQ *= kq_scale
 //   attn_softmax  causal soft_max: max, fp16 exp table, fp64 sum (exact), * (float)(1/sum), P -> f16   (ggml.c:12047-12069)
 //   attn_vp       KQV = ggml_vec_dot_f16(n_total, V^T row, f16(P)): the first n_total & ~31 positions through the 32 lanes, the
 //                 rest added one by one in double — n_total = n_past + N of the eval call the token belongs to (that is the row
 //                 length the reference's mul_mat sees, llama.cpp:2373-2385), so results match the reference for the same
 //                 batch_size chunking.
-// head_dim is 64 or 128 (the engine and the op-level entry points refuse others).
+// head_dim is any even size from 32 to 256 (attn_head_dim_ok; the engine and the op-level entry points refuse others).  A task
+// covers ATTN_CH output channels; the last channel group of a head holds hd % ATTN_CH of them when hd is not a multiple.
 struct AttnParams {
   const float* q;        // [N][q_stride] raw projections (NOT yet rotated)
   const float* k;        // [N][kv_stride]
@@ -194,21 +208,24 @@ struct AttnParams {
 
 constexpr int ATTN_THREADS = 512;
 constexpr int ATTN_CH = 32;   // output channels per CTA
+__host__ __device__ inline int attn_groups(int hd) { return (hd + ATTN_CH - 1) / ATTN_CH; }   // channel groups (tasks) of a head
 
 // Scratch of one task, carved from base:
 //   sc  [cp] f32 scores, then exp values         p16 [cp] f16 probabilities, V-permuted order
-//   q16 [hd] f16 rotated query, K-permuted order
-//   cur (decode): k16 [hd] f16 rotated key of this position (K-permuted order), v16 [hd] f16 value of this position
+//   q16 [k_stride] f16 rotated query, K-permuted order
+//   cur (decode): k16 [k_stride] f16 rotated key of this position (K-permuted order), v16 [hd] f16 value of this position
+// (q16 and k16 are laid out like a K row, so they stay 16-byte aligned)
 struct AttnScratch { float* sc; uint16_t *p16, *q16, *k16, *v16; size_t bytes; };
+template <bool GEN = true>
 __host__ __device__ inline AttnScratch attn_scratch(uint8_t* base, int n_ctx, int hd, bool cur) {
-  const size_t cp = kv_ctx_pad(n_ctx), end_q = cp * 6 + (size_t)hd * 2;
+  const size_t cp = kv_ctx_pad(n_ctx), ks = GEN ? k_stride(hd) : hd, end_q = cp * 6 + ks * 2;
   AttnScratch s;
   s.sc = (float*)base;
   s.p16 = (uint16_t*)(base + cp * 4);
   s.q16 = s.p16 + cp;
-  s.k16 = cur ? s.q16 + hd : nullptr;
-  s.v16 = cur ? s.k16 + hd : nullptr;
-  s.bytes = cur ? end_q + (size_t)hd * 4 : end_q;
+  s.k16 = cur ? s.q16 + ks : nullptr;
+  s.v16 = cur ? s.k16 + ks : nullptr;
+  s.bytes = cur ? end_q + ks * 2 + (size_t)hd * 2 : end_q;
   return s;
 }
 // shared memory of k_attn and of the step kernel's attention phases (the ATTN_CH floats past the scratch are unused; they
@@ -259,18 +276,18 @@ __device__ __forceinline__ float2 attn_cs0(const AttnParams& p, int pos) {
 // RoPE + f16 of query token n's q for head h into the scratch; with s.k16 (decode) also its k and v.  Then the first query
 // head of the KV group writes this position's K row (task cg == 0) and V (every task its ATTN_CH channels) to the cache;
 // the task itself takes them from k16 / v16, so there is no ordering hazard.
-template <int NT>
+template <int NT, bool GEN>
 __device__ __forceinline__ void attn_stage(const AttnParams& p, const AttnScratch& s, int n, int h, int cg, int pos, float2 cs0) {
   const int hd = p.hd, tid = attn_tid<NT>(), group = p.n_head / p.n_kv, kvh = h / group;
   const bool kv_writer = (h % group) == 0;
   const float* qv = p.q + (size_t)n * p.q_stride + (size_t)h * hd;
   const float* kv = p.k + (size_t)n * p.kv_stride + (size_t)kvh * hd;
   const float* vv = p.v + (size_t)n * p.kv_stride + (size_t)kvh * hd;
-  uint16_t* kd = (kv_writer && cg == 0) ? p.kc + k_row(kvh, pos, p.n_ctx, hd) : nullptr;
+  uint16_t* kd = (kv_writer && cg == 0) ? p.kc + k_row<GEN>(kvh, pos, p.n_ctx, hd) : nullptr;
   for (int i = tid; i < hd / 2; i += NT) {
     const float2 cs = i == tid ? cs0 : p.rope[(size_t)pos * (hd / 2) + i];
-    rope_k_pair(qv, i, hd, p.neox, cs, s.q16);
-    if (s.k16) rope_k_pair(kv, i, hd, p.neox, cs, s.k16, kd);
+    rope_k_pair<GEN>(qv, i, hd, p.neox, cs, s.q16);
+    if (s.k16) rope_k_pair<GEN>(kv, i, hd, p.neox, cs, s.k16, kd);
   }
   if (s.k16) {
     for (int c = tid; c < hd; c += NT) {
@@ -281,59 +298,131 @@ __device__ __forceinline__ void attn_stage(const AttnParams& p, const AttnScratc
   }
 }
 
-// this lane's PER = hd/32 f16 elements of a K-permuted row (hd 64: in .x)
+// this lane's PER = hd/32 f16 elements of a K-permuted row, two to a word (PER 2: one word).  Every load is aligned: a row
+// starts 16-byte aligned and the lane's elements start at 2 * PER * lane bytes.
 template <int PER>
-__device__ __forceinline__ uint2 attn_klane(const uint16_t* row) {
-  const int lane = threadIdx.x & 31;
-  if constexpr (PER == 4) return *(const uint2*)(row + lane * 4);
-  else return make_uint2(*(const uint32_t*)(row + lane * 2), 0u);
+struct KLane { uint32_t w[(PER + 1) / 2]; };
+template <int PER>
+__device__ __forceinline__ KLane<PER> attn_klane(const uint16_t* row) {
+  const uint16_t* p = row + (threadIdx.x & 31) * PER;
+  KLane<PER> k;
+  if constexpr (PER == 8) {
+    const uint4 v = *(const uint4*)p;
+    k.w[0] = v.x; k.w[1] = v.y; k.w[2] = v.z; k.w[3] = v.w;
+  } else if constexpr (PER == 4) {
+    const uint2 v = *(const uint2*)p;
+    k.w[0] = v.x; k.w[1] = v.y;
+  } else if constexpr (PER % 2 == 0) {
+#pragma unroll
+    for (int i = 0; i < PER / 2; i++) k.w[i] = ((const uint32_t*)p)[i];
+  } else {
+#pragma unroll
+    for (int i = 0; i < PER / 2; i++) k.w[i] = (uint32_t)p[2 * i] | ((uint32_t)p[2 * i + 1] << 16);
+    k.w[PER / 2] = p[PER - 1];
+  }
+  return k;
 }
-// ... of the rows t0 .. t0+7 of a run of n rows at `rows` (row stride hd, clamped to the last row); row `skip` is left 0
 template <int PER>
-__device__ __forceinline__ void attn_k8(uint2 (&kk)[8], const uint16_t* rows, int t0, int n, int skip) {
+__device__ __forceinline__ uint16_t klane_elem(const KLane<PER>& k, int e) { return (uint16_t)((k.w[e >> 1] >> ((e & 1) * 16)) & 0xffff); }
+// ... of the rows t0 .. t0+7 of a run of n rows at `rows` (row stride `stride`, clamped to the last row); row `skip` is left 0
+template <int PER>
+__device__ __forceinline__ void attn_k8(KLane<PER> (&kk)[8], const uint16_t* rows, int stride, int t0, int n, int skip) {
 #pragma unroll
   for (int i = 0; i < 8; i++) {
     const int t = min(t0 + i, n - 1);
-    kk[i] = t == skip ? make_uint2(0u, 0u) : attn_klane<PER>(rows + (size_t)t * (PER * 32));
+    kk[i] = t == skip ? KLane<PER>{} : attn_klane<PER>(rows + (size_t)t * stride);
   }
 }
 
-// Scores of a run of n K rows at `rows` (row stride hd) into sc[0..n).  The warp takes the groups of 8 rows t0 = t_first,
-// t_first + t_step, ...; the 8 loads of a group are issued before the first is used (the loop is latency-bound otherwise).
-// Row cur_t (-1: none) comes from `cur` instead of `rows`.  pre, when given, is the first group as attn_k8(.., skip = cur_t)
-// loaded it, early.
-template <int PER>
-__device__ __forceinline__ void attn_scores_per(const uint16_t* rows, int n, int t_first, int t_step, const uint16_t* q16, float kq_scale, float* sc,
-                                                int cur_t, const uint16_t* cur, const uint2 (*pre)[8]) {
+// Scores of a run of n K rows at `rows` (row stride k_stride(hd)) into sc[0..n).  The warp takes the groups of 8 rows t0 =
+// t_first, t_first + t_step, ...; the 8 loads of a group are issued before the first is used (the loop is latency-bound
+// otherwise).  Row cur_t (-1: none) comes from `cur` instead of `rows`.  pre, when given, is the first group as
+// attn_k8(.., skip = cur_t) loaded it, early.  TAIL: hd may not be 32 * PER; the row's elements 32 * PER .. hd-1 (<= 30 of
+// them, the element-ordered tail of the K layout) are added after the lane reduction one by one in double, in element order
+// (ggml.c:2415-2418): lane l forms the fp32 product of element 32 * PER + l and the warp adds them in lane order via shuffles.
+template <int PER, bool TAIL>
+__device__ __forceinline__ void attn_scores_per(const uint16_t* rows, int hd, int n, int t_first, int t_step, const uint16_t* q16, float kq_scale, float* sc,
+                                                int cur_t, const uint16_t* cur, const KLane<PER> (*pre)[8]) {
+  constexpr int NP = PER * 32;
+  constexpr int R = PER > 4 ? 4 : 8;   // rows loaded ahead: a group of 8 in two halves when a lane's share is wider than 8 bytes (registers)
   const int lane = threadIdx.x & 31;
-  const uint2 qq = attn_klane<PER>(q16);
-  const float q[4] = {h2f((uint16_t)(qq.x & 0xffff)), h2f((uint16_t)(qq.x >> 16)), h2f((uint16_t)(qq.y & 0xffff)), h2f((uint16_t)(qq.y >> 16))};
+  const int stride = TAIL ? k_stride(hd) : NP, tail = TAIL ? hd - NP : 0;
+  const KLane<PER> qq = attn_klane<PER>(q16);
+  float q[PER];
+#pragma unroll
+  for (int e = 0; e < PER; e++) q[e] = h2f(klane_elem(qq, e));
+  const float qt = (TAIL && lane < tail) ? h2f(q16[NP + lane]) : 0.f;
   for (int t0 = t_first; t0 < n; t0 += t_step) {
-    uint2 kk[8];
-    if (pre && t0 == t_first) {
 #pragma unroll
-      for (int i = 0; i < 8; i++) kk[i] = (*pre)[i];
-    } else {
-      attn_k8<PER>(kk, rows, t0, n, cur_t);
-    }
+    for (int r0 = 0; r0 < 8; r0 += R) {
+      KLane<PER> kk[R];
+      uint16_t kt[R];
+      if (pre && t0 == t_first) {
 #pragma unroll
-    for (int i = 0; i < 8; i++)
-      if (min(t0 + i, n - 1) == cur_t) kk[i] = attn_klane<PER>(cur);
+        for (int i = 0; i < R; i++) kk[i] = (*pre)[r0 + i];
+      } else {
 #pragma unroll
-    for (int i = 0; i < 8; i++) {
-      const uint32_t w[2] = {kk[i].x, kk[i].y};
-      float s = 0.f;
+        for (int i = 0; i < R; i++) {
+          const int t = min(t0 + r0 + i, n - 1);
+          kk[i] = t == cur_t ? KLane<PER>{} : attn_klane<PER>(rows + (size_t)t * stride);
+        }
+      }
+      if constexpr (TAIL) {
 #pragma unroll
-      for (int e = 0; e < PER; e++) s = __fmaf_rn(h2f((uint16_t)((w[e >> 1] >> ((e & 1) * 16)) & 0xffff)), q[e], s);
-      s = attn_reduce_f32x8(s);
-      if (lane == 0 && t0 + i < n) sc[t0 + i] = __fmul_rn(s, kq_scale);
+        for (int i = 0; i < R; i++) {
+          const int t = min(t0 + r0 + i, n - 1);
+          kt[i] = lane < tail ? (t == cur_t ? cur : rows + (size_t)t * stride)[NP + lane] : (uint16_t)0;
+        }
+      }
+#pragma unroll
+      for (int i = 0; i < R; i++)
+        if (min(t0 + r0 + i, n - 1) == cur_t) kk[i] = attn_klane<PER>(cur);
+#pragma unroll
+      for (int i = 0; i < R; i++) {
+        float s = 0.f;
+#pragma unroll
+        for (int e = 0; e < PER; e++) s = __fmaf_rn(h2f(klane_elem(kk[i], e)), q[e], s);
+        s = attn_reduce_f32x8(s);
+        if constexpr (TAIL) {
+          const float term = __fmul_rn(h2f(kt[i]), qt);
+          double sumf = (double)s;
+          for (int l = 0; l < tail; l++) sumf += (double)__shfl_sync(0xffffffffu, term, l);
+          s = (float)sumf;
+        }
+        if (lane == 0 && t0 + r0 + i < n) sc[t0 + r0 + i] = __fmul_rn(s, kq_scale);
+      }
     }
   }
 }
+// Head sizes 64 / 128 (attn_fast_hd) have kernels of their own; every other size runs in a separate kernel instantiation
+// (k_attn<true>, k_step<.., true>) or one out-of-line call (k_pstep), GEN = true below, which keeps its registers out of
+// the hot paths of the 64 / 128 kernels.
+// F(PER, TAIL) called with the instantiation of head size hd: GEN = false, hd 64 / 128, no tail; GEN = true, any other size,
+// with the tail loop (empty when hd is a multiple of 32)
+#define ATTN_PER_DISPATCH(GEN, hd, F)                             \
+  do {                                                            \
+    if constexpr (!(GEN)) {                                       \
+      if ((hd) == 128) F(4, false);                               \
+      else F(2, false);                                           \
+    } else {                                                      \
+      switch ((hd) >> 5) {                                        \
+        case 1: F(1, true); break;                                \
+        case 2: F(2, true); break;                                \
+        case 3: F(3, true); break;                                \
+        case 4: F(4, true); break;                                \
+        case 5: F(5, true); break;                                \
+        case 6: F(6, true); break;                                \
+        case 7: F(7, true); break;                                \
+        default: F(8, true); break;                               \
+      }                                                           \
+    }                                                             \
+  } while (0)
+template <bool GEN>
 __device__ __forceinline__ void attn_scores(int hd, const uint16_t* rows, int n, int t_first, int t_step, const uint16_t* q16, float kq_scale, float* sc,
-                                            int cur_t = -1, const uint16_t* cur = nullptr, const uint2 (*pre)[8] = nullptr) {
-  if (hd == 128) attn_scores_per<4>(rows, n, t_first, t_step, q16, kq_scale, sc, cur_t, cur, pre);
-  else attn_scores_per<2>(rows, n, t_first, t_step, q16, kq_scale, sc, cur_t, cur, pre);
+                                            int cur_t = -1, const uint16_t* cur = nullptr) {
+#define ATTN_SCORES_F(PER, TAIL) attn_scores_per<PER, TAIL>(rows, hd, n, t_first, t_step, q16, kq_scale, sc, cur_t, cur, nullptr)
+  ATTN_PER_DISPATCH(GEN, hd, ATTN_SCORES_F);
+#undef ATTN_SCORES_F
 }
 
 // soft_max of sc[0..T) (ggml.c:12047-12069) -> p16 in V-permuted order, zero up to the end of the last 256-position chunk.
@@ -414,55 +503,74 @@ __device__ __forceinline__ float attn_vp(const uint16_t* vrow, const uint16_t* p
 
 // RoPE + KV-cache store + attention for one query token n, one head h and one group cg of ATTN_CH output channels, by NT
 // threads with barrier BAR, K / V read from global memory.  Every task of a head recomputes that head's scores (K rows come
-// from L2); the channel groups split the V·P work, which gives n_head * hd/32 tasks per token instead of n_head.
+// from L2); the channel groups split the V·P work, which gives n_head * ceil(hd/32) tasks per token instead of n_head.
 // PDLWAIT = true: a kernel of its own, q/k/v come from the previous kernel (griddepcontrol.wait after the prefetches).
 // PDLWAIT = false: a phase of the persistent step kernel (stream.cuh); the caller has already synchronised with the producers.
-template <int NT, int BAR, bool PDLWAIT>
-__device__ __forceinline__ void attn_body(const AttnParams& p, uint8_t* smem, const int h, const int n, const int cg, const int* st) {
+template <int NT, int BAR, bool PDLWAIT, int PER, bool TAIL>
+__device__ __forceinline__ void attn_body_per(const AttnParams& p, uint8_t* smem, const int h, const int n, const int cg, const AttnPos& a,
+                                              float* red_f, double* red_d) {
   constexpr int NW = NT / 32;
-  __shared__ float red_f[NW];
-  __shared__ double red_d[NW];
   // Everything up to pdl_wait() reads only what earlier steps left behind (device state, RoPE table, cached K/V rows of
   // older positions): it overlaps the tail of the QKV kernel.  q/k/v of this token are read after the wait.
-  const AttnPos a = attn_pos(p, st);
-  if (a.T == 0) return;
-  const int hd = p.hd, kvh = h / (p.n_head / p.n_kv);
+  const int hd = p.hd, kvh = h / (p.n_head / p.n_kv), nch = TAIL ? min(ATTN_CH, hd - cg * ATTN_CH) : ATTN_CH;
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const AttnScratch s = attn_scratch(smem, p.n_ctx, hd, true);
-  const uint16_t* krows = p.kc + k_row(kvh, 0, p.n_ctx, hd);
+  const AttnScratch s = attn_scratch<TAIL>(smem, p.n_ctx, hd, true);
+  const uint16_t* krows = p.kc + k_row<TAIL>(kvh, 0, p.n_ctx, hd);
   constexpr int CPW = (ATTN_CH + NW - 1) / NW;          // V channels per warp (the last round may be partial)
   uint4 vpre[CPW][2];                                   // this warp's V rows, first two 256-position chunks
-  uint2 kpre[8];                                        // this warp's first 8 K rows
+  constexpr bool KPRE = PER <= 4;                       // (a wider share would hold 8 x 16 bytes of registers across the staging)
+  KLane<PER> kpre[8];                                   // this warp's first 8 K rows
 #pragma unroll
   for (int j = 0; j < CPW; j++)
 #pragma unroll
     for (int ch = 0; ch < 2; ch++)
-      vpre[j][ch] = (ch * 256 < a.lim && warp + j * NW < ATTN_CH) ? *(const uint4*)(p.vc + v_chan(kvh, cg * ATTN_CH + warp + j * NW, p.n_ctx, hd) + ch * 256 + lane * 8) : make_uint4(0, 0, 0, 0);
-  if (hd == 128) attn_k8<4>(kpre, krows, warp * 8, a.T, a.pos);
-  else attn_k8<2>(kpre, krows, warp * 8, a.T, a.pos);
+      vpre[j][ch] = (ch * 256 < a.lim && warp + j * NW < nch) ? *(const uint4*)(p.vc + v_chan(kvh, cg * ATTN_CH + warp + j * NW, p.n_ctx, hd) + ch * 256 + lane * 8) : make_uint4(0, 0, 0, 0);
+  if constexpr (KPRE) attn_k8<PER>(kpre, krows, TAIL ? k_stride(hd) : PER * 32, warp * 8, a.T, a.pos);
   const float2 cs0 = attn_cs0<NT>(p, a.pos);
   if (PDLWAIT) pdl_wait();
 
-  attn_stage<NT>(p, s, n, h, cg, a.pos, cs0);
+  attn_stage<NT, TAIL>(p, s, n, h, cg, a.pos, cs0);
   attn_bar<BAR, NT>();
-  attn_scores(hd, krows, a.T, warp * 8, NW * 8, s.q16, p.kq_scale, s.sc, a.pos, s.k16, &kpre);
+  attn_scores_per<PER, TAIL>(krows, hd, a.T, warp * 8, NW * 8, s.q16, p.kq_scale, s.sc, a.pos, s.k16, KPRE ? &kpre : nullptr);
   attn_bar<BAR, NT>();
   attn_softmax<NT, BAR>(s.sc, s.p16, a.T, p.exp_tab, red_f, red_d);
 #pragma unroll
   for (int j = 0; j < CPW; j++) {
     const int cc = warp + j * NW;
-    if (cc >= ATTN_CH) break;
+    if (cc >= nch) break;
     const int c = cg * ATTN_CH + cc;
     const float o = attn_vp(p.vc + v_chan(kvh, c, p.n_ctx, hd), s.p16, a, a.pos, s.v16[c], vpre[j]);
     if (lane == 0) p.out[(size_t)n * p.n_head * hd + (size_t)h * hd + c] = o;
   }
 }
+// attn_body's reduction slots: one set per CTA size, shared by both GEN forms (a kernel's static shared memory stays as it was)
+template <int NT>
+__device__ __forceinline__ void attn_body_red(float*& red_f, double*& red_d) {
+  __shared__ float rf[NT / 32];
+  __shared__ double rd[NT / 32];
+  red_f = rf;
+  red_d = rd;
+}
+template <int NT, int BAR, bool PDLWAIT, bool GEN>
+__device__ __forceinline__ void attn_body(const AttnParams& p, uint8_t* smem, const int h, const int n, const int cg, const int* st) {
+  float* red_f;
+  double* red_d;
+  attn_body_red<NT>(red_f, red_d);
+  const AttnPos a = attn_pos(p, st);
+  if (a.T == 0) return;
+#define ATTN_BODY_F(PER, TAIL) attn_body_per<NT, BAR, PDLWAIT, PER, TAIL>(p, smem, h, n, cg, a, red_f, red_d)
+  ATTN_PER_DISPATCH(GEN, p.hd, ATTN_BODY_F);
+#undef ATTN_BODY_F
+}
 
+template <bool GEN>
 static __global__ void __launch_bounds__(ATTN_THREADS) k_attn(const AttnParams p) {
   extern __shared__ __align__(16) uint8_t smem[];
   pdl_trigger();
-  attn_body<ATTN_THREADS, 0, true>(p, smem, blockIdx.x, blockIdx.y, blockIdx.z, p.state);
+  attn_body<ATTN_THREADS, 0, true, GEN>(p, smem, blockIdx.x, blockIdx.y, blockIdx.z, p.state);
 }
+// the k_attn of head size hd
+inline void (*attn_kernel(int hd))(const AttnParams) { return attn_fast_hd(hd) ? k_attn<false> : k_attn<true>; }
 
 // ----------------------------------------------------------------------------------------- argmax
 // Greedy pick over logits[0, n) by the first NT threads (named barrier BAR): the largest value, the lowest id among equal ones.

@@ -113,4 +113,10 @@ __device__ __forceinline__ float warp_max(float v) {
   return v;
 }
 
+// head sizes the attention kernels take (attention.cuh): even, because RoPE rotates pairs; 32 .. 256, so that a lane's share
+// of the f16 dot's SIMD part is 1 .. 8 elements
+__host__ __device__ inline bool attn_head_dim_ok(int hd) { return hd >= 32 && hd <= 256 && hd % 2 == 0; }
+// ... of which 64 and 128 run in the kernels' own inline paths (the others in separate instantiations, attention.cuh)
+__host__ __device__ inline bool attn_fast_hd(int hd) { return hd == 64 || hd == 128; }
+
 }  // namespace ctb

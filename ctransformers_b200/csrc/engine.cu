@@ -96,7 +96,7 @@ size_t engine_arena_bytes(const GGUFFile& g, const HParams& hp) {
     if (t.ne[1] > 0) total += align_up(t.nbytes / (size_t)t.ne[1] * ST_ROWS, 256);   // K-quants: rows padded to whole 16-row tiles
   }
   total += UP_CHUNK * UP_BUFS + 256;                                            // device staging of the upload pipeline
-  const size_t kv = (size_t)hp.n_layer * (hp.n_ctx + 256) * hp.n_embd_gqa() * 2;
+  const size_t kv = (size_t)hp.n_layer * (hp.n_ctx + 256) * hp.n_head_kv * k_stride(hp.head_dim()) * 2;   // K rows padded to 8 halves
   total += 2 * align_up(kv, 256);
   total += 3 * align_up(65536 * 2, 256);
   total += align_up((size_t)hp.n_ctx * (hp.head_dim() / 2) * 8, 256);
@@ -365,7 +365,7 @@ void Engine::init(const GGUFFile& g) {
   }
   // ---- KV cache + workspace
   const size_t gqa_l = (size_t)nkv_ * hp_.head_dim(), qw_l = (size_t)nh_ * hp_.head_dim();   // this rank's K/V and Q widths
-  const size_t kv = (size_t)hp_.n_layer * hp_.n_ctx * gqa_l;
+  const size_t kv = (size_t)hp_.n_layer * hp_.n_ctx * nkv_ * k_stride(hp_.head_dim());   // K rows padded to 8 halves (attention.cuh)
   const size_t vv = (size_t)hp_.n_layer * kv_ctx_pad(hp_.n_ctx) * gqa_l;
   kc_ = (uint16_t*)alloc(kv * 2);
   vc_ = (uint16_t*)alloc(vv * 2);
@@ -406,7 +406,7 @@ void Engine::init(const GGUFFile& g) {
   }
   CTB_CUDA(cudaEventCreateWithFlags(&ev_pick_, cudaEventDisableTiming));
   CTB_CUDA(matvec_set_smem_limit(MV_SMEM_LIMIT));
-  CTB_CUDA(cudaFuncSetAttribute(k_attn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)attn_smem_bytes(hp_.n_ctx, hp_.head_dim())));
+  CTB_CUDA(cudaFuncSetAttribute(attn_kernel(hp_.head_dim()), cudaFuncAttributeMaxDynamicSharedMemorySize, (int)attn_smem_bytes(hp_.n_ctx, hp_.head_dim())));
   if (tp_.world > 1) tp_setup_peer();
   build_ops();
   if (tp_peer_)
@@ -568,7 +568,7 @@ void Engine::build_ops() {
   float* y = xb_;
   for (int il = 0; il < hp_.n_layer; il++) {
     const LayerW& L = layers_[il];
-    uint16_t* kc = kc_ + (size_t)il * hp_.n_ctx * gqa;
+    uint16_t* kc = kc_ + (size_t)il * hp_.n_ctx * n_kv * k_stride(hd);
     uint16_t* vc = vc_ + (size_t)il * gqa * kv_ctx_pad(hp_.n_ctx);
     AttnParams ap{};
     ap.kc = kc; ap.vc = vc; ap.out = attn_; ap.exp_tab = exp_tab_; ap.state = d_state_; ap.kq_scale = kq_scale;
@@ -688,7 +688,7 @@ void Engine::build_ops() {
   for (const StepOp& op : ops_) any_stream |= op.ph.kind == PH_MATVEC && op.stream;
   std::vector<Phase> phs;
   for (const StepOp& op : ops_) if (op.ph.kind != PH_XCHG && (op.ph.kind != PH_MATVEC || op.stream)) phs.push_back(op.ph);
-  const StepLaunch sl = step_launch_shape(phs.data(), (int)phs.size(), sm_count_, max_dyn_smem(k_step<true>));
+  const StepLaunch sl = step_launch_shape(phs.data(), (int)phs.size(), sm_count_, max_dyn_smem(k_step<true, false>));
   step_grid_ = sl.grid; step_slots_ = sl.n_slots; step_smem_ = sl.smem;
   if (const char* e = getenv("CTB_ST_SLOTS")) {   // A/B knob: fewer ring slots = less prefetch in flight
     const int want = atoi(e);
@@ -721,7 +721,7 @@ void Engine::upload_prog(Phase* dst, int* dst_bounds, const std::vector<StepOp>&
 void Engine::enqueue_ops(const std::vector<StepOp>& ops, const Phase* d_prog, const int* d_bounds, int n) {
   launches_per_step_ = 0;
   StepLaunch step_shape_;
-  step_shape_.grid = step_grid_; step_shape_.n_slots = step_slots_; step_shape_.smem = step_smem_;
+  step_shape_.grid = step_grid_; step_shape_.n_slots = step_slots_; step_shape_.smem = step_smem_; step_shape_.gen = !attn_fast_hd(hp_.head_dim());
   auto capable = [&](const StepOp& op) { return op.ph.kind != PH_XCHG && (op.ph.kind != PH_MATVEC || op.stream); };
   int i = 0;
   while (i < n) {
@@ -744,7 +744,7 @@ void Engine::enqueue_ops(const std::vector<StepOp>& ops, const Phase* d_prog, co
         mark(3);
         break;
       case PH_ATTN:
-        CTB_CUDA(launch_kernel(k_attn, dim3(nh_, 1, hp_.head_dim() / ATTN_CH), dim3(ATTN_THREADS), attn_smem_bytes(hp_.n_ctx, hp_.head_dim()), stream_, pdl_, op.ph.at));
+        CTB_CUDA(launch_kernel(attn_kernel(hp_.head_dim()), dim3(nh_, 1, attn_groups(hp_.head_dim())), dim3(ATTN_THREADS), attn_smem_bytes(hp_.n_ctx, hp_.head_dim()), stream_, pdl_, op.ph.at));
         launches_per_step_++;
         mark(1);
         break;
@@ -866,7 +866,7 @@ long Engine::trace_step(int token, int n_past, unsigned long long* out, long cap
   CTB_CUDA(cudaMalloc(&buf, (size_t)n * step_grid_ * 64));
   CTB_CUDA(cudaMemset(buf, 0, (size_t)n * step_grid_ * 64));
   StepLaunch L;
-  L.grid = step_grid_; L.n_slots = step_slots_; L.smem = step_smem_;
+  L.grid = step_grid_; L.n_slots = step_slots_; L.smem = step_smem_; L.gen = !attn_fast_hd(hp_.head_dim());
   if (h_state_cap_ < 1) { h_state_cap_ = 512; CTB_CUDA(cudaMallocHost(&h_state_, (size_t)h_state_cap_ * 16)); }
   for (int rep = 0; rep < 3; rep++) {   // the last (warm) run is the one read back
     h_state_[0] = token; h_state_[1] = n_past; h_state_[2] = 0; h_state_[3] = n_past + 1;

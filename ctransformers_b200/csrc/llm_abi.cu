@@ -76,7 +76,7 @@ static HParams read_hparams(const GGUFFile& g, const std::string& arch, int n_ct
   hp.n_ctx = n_ctx_req > 0 ? n_ctx_req : 512;   // llama_context_default_params().n_ctx (llama.cpp:5281)
   if (hp.n_head_kv <= 0 || hp.n_head % hp.n_head_kv) throw std::runtime_error("invalid kv head count");
   const int hd = hp.head_dim();
-  if (hd != 64 && hd != 128) throw std::runtime_error("unsupported head size " + std::to_string(hd) + " (the CUDA path handles 64 and 128)");
+  if (!attn_head_dim_ok(hd)) throw std::runtime_error("unsupported head size " + std::to_string(hd) + " (the CUDA path handles even sizes from 32 to 256)");
   return hp;
 }
 
@@ -106,6 +106,7 @@ static LLM* create_llm(const char* model_path, const char* model_type, const ctr
     else if (const char* lr = getenv("LOCAL_RANK")) device = atoi(lr) % ndev;
     TPShard tp;
     if (world > 1) {
+      if (!attn_fast_hd(llm->hp.head_dim())) throw std::runtime_error("tensor parallel: head size " + std::to_string(llm->hp.head_dim()) + " (this mode takes 64 and 128)");
       if (!unique_id) throw std::runtime_error("tensor parallel: no communicator id");
       tp = tp_shard(llm->hp.n_embd, llm->hp.n_head, llm->hp.n_head_kv, llm->hp.n_ff, rank, world);
       if (cudaSetDevice(device) != cudaSuccess) throw std::runtime_error("cudaSetDevice failed");

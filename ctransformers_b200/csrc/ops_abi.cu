@@ -115,7 +115,7 @@ unsigned* sync_words() {
 // a program of phases through the persistent step kernel, exactly as the engine launches it
 void run_phases(std::vector<Phase> phs) {
   unsigned* d_sync = sync_words();
-  const StepLaunch L = step_launch_shape(phs.data(), (int)phs.size(), sm_count(), max_dyn_smem(k_step<true>));
+  const StepLaunch L = step_launch_shape(phs.data(), (int)phs.size(), sm_count(), max_dyn_smem(k_step<true, false>));
   const std::vector<int> hb = step_bounds(phs.data(), (int)phs.size(), L.grid);
   DevBuf dbounds(hb.size() * 4);
   OPS_CUDA(cudaMemcpy(dbounds.p, hb.data(), hb.size() * 4, cudaMemcpyHostToDevice));
@@ -212,7 +212,7 @@ void stage_to_host(const float* x, const float* w, const float* b, float* y_norm
 void kv_to_device(const uint16_t* kref, const uint16_t* vref, int v_ld, int n_pos, int n_kv, int hd, int n_ctx, std::vector<uint16_t>& kp,
                   std::vector<uint16_t>& vp) {
   const int cp = kv_ctx_pad(n_ctx);
-  kp.assign((size_t)n_ctx * n_kv * hd, 0);
+  kp.assign((size_t)n_ctx * n_kv * k_stride(hd), 0);
   vp.assign((size_t)n_kv * hd * cp, 0);
   for (int t = 0; t < n_pos; t++)
     for (int kh = 0; kh < n_kv; kh++)
@@ -353,7 +353,7 @@ int ctb_rope(float* x, int n_heads, int head_dim, int pos, int mode, float freq_
 int ctb_attention(const float* q, const uint16_t* kcache, const uint16_t* vcache, float* out, int n_head, int n_kv, int head_dim, int T,
                   int n_total, float kq_scale) {
   return guarded("ctb_attention", [&] {
-    if (head_dim != 64 && head_dim != 128) throw std::runtime_error("head_dim must be 64 or 128");
+    if (!attn_head_dim_ok(head_dim)) throw std::runtime_error("head_dim must be even, from 32 to 256");
     if (n_total < T) n_total = T;
     const size_t nq = (size_t)n_head * head_dim;
     std::vector<uint16_t> kp, vp;
@@ -382,8 +382,8 @@ int ctb_attention(const float* q, const uint16_t* kcache, const uint16_t* vcache
     ap.out = dout.as<float>(); ap.exp_tab = tables().ex; ap.rope = dtab.as<float2>(); ap.state = dst.as<int>(); ap.kq_scale = kq_scale;
     ap.n_head = n_head; ap.n_kv = n_kv; ap.hd = head_dim; ap.n_ctx = n_total; ap.q_stride = (int)nq; ap.kv_stride = n_kv * head_dim; ap.neox = 0;
     const size_t smem = attn_smem_bytes(n_total, head_dim);
-    OPS_CUDA(cudaFuncSetAttribute(k_attn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)std::max<size_t>(smem, 48 * 1024)));
-    k_attn<<<dim3(n_head, 1, head_dim / ATTN_CH), ATTN_THREADS, smem>>>(ap);
+    OPS_CUDA(cudaFuncSetAttribute(attn_kernel(head_dim), cudaFuncAttributeMaxDynamicSharedMemorySize, (int)std::max<size_t>(smem, 48 * 1024)));
+    attn_kernel(head_dim)<<<dim3(n_head, 1, attn_groups(head_dim)), ATTN_THREADS, smem>>>(ap);
     OPS_CUDA(cudaGetLastError());
     OPS_CUDA(cudaMemcpy(out, dout.p, nq * 4, cudaMemcpyDeviceToHost));
   });
@@ -395,7 +395,7 @@ int ctb_attention_path(int path, const float* q, const float* k_new, const float
   return guarded("ctb_attention_path", [&] {
     const int hd = head_dim;
     if (path < 0 || path > 3) throw std::runtime_error("unknown attention path " + std::to_string(path));
-    if (hd != 64 && hd != 128) throw std::runtime_error("head_dim must be 64 or 128");
+    if (!attn_head_dim_ok(hd)) throw std::runtime_error("head_dim must be even, from 32 to 256");
     if (n_head < 1 || n_kv < 1 || n_head % n_kv) throw std::runtime_error("n_head must be a multiple of n_kv");
     if (n_tok < 1 || pos0 < 0 || pos0 + n_tok > n_ctx) throw std::runtime_error("the tokens' positions must lie inside the context");
     for (int i = 0; i < n_tok; i++)
@@ -443,16 +443,16 @@ int ctb_attention_path(int path, const float* q, const float* k_new, const float
       if (path == 1) {
         Phase ph{};
         ph.kind = PH_ATTN; ph.q6 = 1; ph.at = ap;
-        const StepLaunch L = step_launch_shape(&ph, 1, sm_count(), max_dyn_smem(k_step<true>));
+        const StepLaunch L = step_launch_shape(&ph, 1, sm_count(), max_dyn_smem(k_step<true, false>));
         if (!st_attn_ring_ok(n_ctx, L.n_slots)) throw std::runtime_error("the step kernel's ring cannot carry K / V at this n_ctx");
       }
       const size_t smem = attn_smem_bytes(n_ctx, hd);
-      if (path == 0) OPS_CUDA(cudaFuncSetAttribute(k_attn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)std::max<size_t>(smem, 48 * 1024)));
+      if (path == 0) OPS_CUDA(cudaFuncSetAttribute(attn_kernel(hd), cudaFuncAttributeMaxDynamicSharedMemorySize, (int)std::max<size_t>(smem, 48 * 1024)));
       for (int i = 0; i < n_tok; i++) {
         AttnParams a = ap;
         a.q += (size_t)i * nq; a.k += (size_t)i * nkv; a.v += (size_t)i * nkv; a.out += (size_t)i * nq; a.state += (size_t)i * 4;
         if (path == 0) {
-          k_attn<<<dim3(n_head, 1, hd / ATTN_CH), ATTN_THREADS, smem>>>(a);
+          attn_kernel(hd)<<<dim3(n_head, 1, attn_groups(hd)), ATTN_THREADS, smem>>>(a);
           OPS_CUDA(cudaGetLastError());
         } else {
           Phase ph{};
@@ -480,7 +480,7 @@ int ctb_prefill_mul_mat(int nseg, const int* types, const void* const* w_blocks,
     if ((norm_mode != NORM_NONE && !norm_w) || (norm_mode == NORM_LAYER && !norm_b)) throw std::runtime_error("RMSNorm needs norm_w, LayerNorm norm_w and norm_b");
     if (norm_mode == NORM_NONE) norm_w = nullptr;   // the prologue applies whatever weight and bias it is given: only the mode's own
     if (norm_mode != NORM_LAYER) norm_b = nullptr;
-    if (head_dim != 64 && head_dim != 128) throw std::runtime_error("head_dim must be 64 or 128");
+    if (!attn_head_dim_ok(head_dim)) throw std::runtime_error("head_dim must be even, from 32 to 256");
     if (n_ctx < 1) throw std::runtime_error("n_ctx must be at least 1");
     int off[MV_MAX_SEG + 1] = {0};
     for (int s = 0; s < nseg; s++) {

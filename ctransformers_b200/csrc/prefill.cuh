@@ -367,14 +367,15 @@ __device__ __forceinline__ void pb_kv_phase(const PPhase& ph, int n_tok) {
 // batch before any task starts.
 __host__ __device__ inline size_t pb_attn_warp_bytes(int n_ctx, int hd) { return (attn_scratch(nullptr, n_ctx, hd, false).bytes + 15) & ~(size_t)15; }
 
+template <bool GEN>
 __device__ __forceinline__ void pb_attn_warp_task(const AttnParams& p, const int* st, int tok, int h, uint8_t* wsm) {
   const AttnPos a = attn_pos(p, st);
   if (a.T == 0) return;
   const int hd = p.hd, kvh = h / (p.n_head / p.n_kv), lane = threadIdx.x & 31;
-  const AttnScratch s = attn_scratch(wsm, p.n_ctx, hd, false);
-  attn_stage<32>(p, s, tok, h, 0, a.pos, attn_cs0<32>(p, a.pos));
+  const AttnScratch s = attn_scratch<GEN>(wsm, p.n_ctx, hd, false);
+  attn_stage<32, GEN>(p, s, tok, h, 0, a.pos, attn_cs0<32>(p, a.pos));
   __syncwarp();
-  attn_scores(hd, p.kc + k_row(kvh, 0, p.n_ctx, hd), a.T, 0, 8, s.q16, p.kq_scale, s.sc);
+  attn_scores<GEN>(hd, p.kc + k_row<GEN>(kvh, 0, p.n_ctx, hd), a.T, 0, 8, s.q16, p.kq_scale, s.sc);
   __syncwarp();
   attn_softmax<32, 0>(s.sc, s.p16, a.T, p.exp_tab, nullptr, nullptr);
   float* orow = p.out + (size_t)tok * p.n_head * hd + (size_t)h * hd;
@@ -384,6 +385,19 @@ __device__ __forceinline__ void pb_attn_warp_task(const AttnParams& p, const int
   }
   __syncwarp();
 }
+
+// the ATTN phase of one CTA's warp: hd 64 / 128 inline, other head sizes in one out-of-line call
+template <bool GEN>
+__device__ __forceinline__ void pb_attn_phase(const PPhase& ph, int n_tok, uint8_t* work) {
+  const int warp = threadIdx.x >> 5;
+  const int n_tasks = n_tok * ph.at.n_head;
+  uint8_t* wsm = work + (size_t)warp * pb_attn_warp_bytes(ph.at.n_ctx, ph.at.hd);
+  for (int task = blockIdx.x * PB_W + warp; task < n_tasks; task += (int)gridDim.x * PB_W) {
+    const int tok = task / ph.at.n_head;
+    pb_attn_warp_task<GEN>(ph.at, ph.state + tok * 4, tok, task % ph.at.n_head, wsm);
+  }
+}
+static __device__ __noinline__ void pb_attn_phase_gen(const PPhase& ph, int n_tok, uint8_t* work) { pb_attn_phase<true>(ph, n_tok, work); }
 
 static __global__ void __launch_bounds__(PB_THREADS, 1) k_pstep(const __grid_constant__ PStepArgs args) {
   extern __shared__ __align__(16) uint8_t smem[];
@@ -432,12 +446,8 @@ static __global__ void __launch_bounds__(PB_THREADS, 1) k_pstep(const __grid_con
     } else if (ph.kind == PP_KV) {
       pb_kv_phase(ph, n_tok);
     } else if (ph.kind == PP_ATTN) {
-      const int n_tasks = n_tok * ph.at.n_head;
-      uint8_t* wsm = work + (size_t)warp * pb_attn_warp_bytes(ph.at.n_ctx, ph.at.hd);
-      for (int task = blockIdx.x * PB_W + warp; task < n_tasks; task += (int)G * PB_W) {
-        const int tok = task / ph.at.n_head;
-        pb_attn_warp_task(ph.at, ph.state + tok * 4, tok, task % ph.at.n_head, wsm);
-      }
+      if (attn_fast_hd(ph.at.hd)) pb_attn_phase<false>(ph, n_tok, work);
+      else pb_attn_phase_gen(ph, n_tok, work);
     } else if (ph.kind == PP_EMBED) {
       for (int tok = blockIdx.x; tok < n_tok; tok += G) embed_row(ph.em, ph.state[tok * 4], ph.em.out + (size_t)tok * ph.em.K, threadIdx.x, PB_NT);
     }

@@ -619,8 +619,10 @@ __device__ __forceinline__ StItem st_item(const MVParams& p, int seg, int type, 
 // one was written by earlier launches), so they travel through the SAME ring as the weights: the producer queues them between
 // the QKV mat-vec's items and the output projection's, and by the time the grid barrier after QKV opens they sit in shared
 // memory.  What is left on the critical path is one L2 round trip for q/k/v, one for the exp table, and arithmetic.
-//   K item  up to rows_per_item consecutive cached rows of the task's KV head (head-major cache: one contiguous bulk copy)
-//   V item  cv of the task's ATTN_CH channels, nchv 256-position chunks each (one bulk copy per channel)
+//   K item  up to rows_per_item consecutive cached rows of the task's KV head (head-major cache: one contiguous bulk copy;
+//           rows_per_item = ST_SLOT / the padded row's bytes, e.g. 36 rows at hd 128, 44 at hd 100)
+//   V item  cv of the task's channels, nchv 256-position chunks each (one bulk copy per channel).  A head's last channel
+//           group may hold fewer than ATTN_CH channels, and then fewer items (attn_ring_nv).
 struct AttnRingV { int nchv, cv, n_v; };   // V items of a task over T > 0 positions (the host asks for T = n_ctx)
 __host__ __device__ inline AttnRingV attn_ring_v(int T) {
   AttnRingV v;
@@ -630,21 +632,27 @@ __host__ __device__ inline AttnRingV attn_ring_v(int T) {
   return v;
 }
 struct AttnRing : AttnPos, AttnRingV { int n_k, rpi; };
+template <bool GEN>
 __device__ __forceinline__ AttnRing attn_ring_geom(const AttnParams& p) {
   AttnRing g;
   static_cast<AttnPos&>(g) = attn_pos(p, p.state);
-  g.rpi = ST_SLOT / (p.hd * 2);
+  g.rpi = ST_SLOT / ((GEN ? k_stride(p.hd) : p.hd) * 2);
   if (g.T == 0) { g.n_k = 0; g.n_v = 0; g.cv = 1; g.nchv = 0; return g; }
   static_cast<AttnRingV&>(g) = attn_ring_v(g.T);
   g.n_k = (g.pos + g.rpi - 1) / g.rpi;
   return g;
 }
+// channels of channel group cg of a head, and the V items they take (g.n_v for a whole group)
+__device__ __forceinline__ int attn_group_ch(int hd, int cg) { return min(ATTN_CH, hd - cg * ATTN_CH); }
+template <bool GEN>
+__device__ __forceinline__ int attn_ring_nv(const AttnRing& g, int hd, int cg) { return GEN && g.n_v > 0 ? (attn_group_ch(hd, cg) + g.cv - 1) / g.cv : g.n_v; }
 
 // producer side of one attention phase (whole warp: lane i issues item i of a task's K run / V groups)
+template <bool GEN>
 __device__ __forceinline__ void st_attn_produce(const AttnParams& p, uint8_t* ring, uint64_t* full_bar, uint64_t* empty_bar, uint32_t S, uint32_t& seq) {
   const int lane = threadIdx.x & 31;
-  const AttnRing g = attn_ring_geom(p);
-  const int n_cg = p.hd / ATTN_CH, n_tasks = p.n_head * n_cg, group = p.n_head / p.n_kv;
+  const AttnRing g = attn_ring_geom<GEN>(p);
+  const int n_cg = GEN ? attn_groups(p.hd) : p.hd / ATTN_CH, n_tasks = p.n_head * n_cg, group = p.n_head / p.n_kv, row_bytes = (GEN ? k_stride(p.hd) : p.hd) * 2;
   for (int task = blockIdx.x; task < n_tasks; task += gridDim.x) {
     const int h = task / n_cg, cg = task % n_cg, kvh = h / group;
     const int step = min(32, ST_W * (int)S);   // lanes of one batch never share a slot (see st_producer)
@@ -655,33 +663,36 @@ __device__ __forceinline__ void st_attn_produce(const AttnParams& p, uint8_t* ri
         const RingPos rp = st_ring(n, S);
         const int rows = min(g.rpi, g.pos - i * g.rpi);
         mbar_wait(&empty_bar[rp.slot], rp.parity ^ 1u, W_FREE_K_SLOT, (int)n);
-        mbar_expect_tx(&full_bar[rp.slot], (uint32_t)(rows * p.hd * 2));
-        bulk_g2s(ring + (size_t)rp.slot * ST_SLOT, p.kc + k_row(kvh, i * g.rpi, p.n_ctx, p.hd), (uint32_t)(rows * p.hd * 2), &full_bar[rp.slot]);
+        mbar_expect_tx(&full_bar[rp.slot], (uint32_t)(rows * row_bytes));
+        bulk_g2s(ring + (size_t)rp.slot * ST_SLOT, p.kc + k_row<GEN>(kvh, i * g.rpi, p.n_ctx, p.hd), (uint32_t)(rows * row_bytes), &full_bar[rp.slot]);
       }
       __syncwarp();
     }
     seq += (uint32_t)g.n_k;
-    for (int iv = lane; iv < g.n_v; iv += 32) {   // n_v <= 32 / cv <= S is checked on the host (st_attn_ring_ok)
+    const int n_v = attn_ring_nv<GEN>(g, p.hd, cg), ch_g = GEN ? attn_group_ch(p.hd, cg) : ATTN_CH;
+    for (int iv = lane; iv < n_v; iv += 32) {   // n_v <= 32 / cv <= S is checked on the host (st_attn_ring_ok)
       const uint32_t n = seq + (uint32_t)iv;
       const RingPos rp = st_ring(n, S);
-      const int nch = min(g.cv, ATTN_CH - iv * g.cv);
+      const int nch = min(g.cv, ch_g - iv * g.cv);
       const uint32_t bytes = (uint32_t)(g.nchv * 512);
       mbar_wait(&empty_bar[rp.slot], rp.parity ^ 1u, W_FREE_V_SLOT, (int)n);
       mbar_expect_tx(&full_bar[rp.slot], bytes * nch);
       for (int q = 0; q < nch; q++)
-        bulk_g2s(ring + (size_t)rp.slot * ST_SLOT + (size_t)q * bytes, p.vc + v_chan(kvh, cg * ATTN_CH + iv * g.cv + q, p.n_ctx, p.hd), bytes, &full_bar[rp.slot]);
+        bulk_g2s(ring + (size_t)rp.slot * ST_SLOT + (size_t)q * bytes, p.vc + v_chan(kvh, cg * ATTN_CH + iv * g.cv + q, p.n_ctx, p.hd), bytes,
+                 &full_bar[rp.slot]);
     }
     __syncwarp();
-    seq += (uint32_t)g.n_v;
+    seq += (uint32_t)n_v;
   }
 }
 
 // consumer side: one (head, channel group) task, K / V of the older positions read from the ring, this position's from k16 / v16
+template <bool GEN>
 __device__ __forceinline__ void st_attn_task(const AttnParams& p, uint8_t* smem, const uint8_t* ring, uint64_t* full_bar, uint64_t* empty_bar, uint32_t S, uint32_t seq0,
                                              const AttnRing& g, int h, int cg, float* red_f, double* red_d) {
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const AttnScratch s = attn_scratch(smem, p.n_ctx, p.hd, true);
-  attn_stage<ST_NT>(p, s, 0, h, cg, g.pos, attn_cs0<ST_NT>(p, g.pos));
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, nch = GEN ? attn_group_ch(p.hd, cg) : ATTN_CH;
+  const AttnScratch s = attn_scratch<GEN>(smem, p.n_ctx, p.hd, true);
+  attn_stage<ST_NT, GEN>(p, s, 0, h, cg, g.pos, attn_cs0<ST_NT>(p, g.pos));
   bar_sync<ST_BAR, ST_NT>();
   // ---- scores: K item i = ring item seq0 + i belongs to warp (seq0 + i) % ST_W (which also frees its slot)
   for (int i = (int)(((uint32_t)warp + ST_W - seq0 % ST_W) % ST_W); i < g.n_k; i += ST_W) {
@@ -689,15 +700,15 @@ __device__ __forceinline__ void st_attn_task(const AttnParams& p, uint8_t* smem,
     const RingPos rp = st_ring(n, S);
     const int r0 = i * g.rpi;
     mbar_wait(&full_bar[rp.slot], rp.parity, W_K_ITEM, (int)n);
-    attn_scores(p.hd, (const uint16_t*)(ring + (size_t)rp.slot * ST_SLOT), min(g.rpi, g.pos - r0), 0, 8, s.q16, p.kq_scale, s.sc + r0);
+    attn_scores<GEN>(p.hd, (const uint16_t*)(ring + (size_t)rp.slot * ST_SLOT), min(g.rpi, g.pos - r0), 0, 8, s.q16, p.kq_scale, s.sc + r0);
     __syncwarp();
     if (lane == 0) mbar_arrive(&empty_bar[rp.slot]);
   }
-  if (warp == (int)((seq0 + (uint32_t)g.n_k) % ST_W)) attn_scores(p.hd, s.k16, 1, 0, 8, s.q16, p.kq_scale, s.sc + g.pos);   // the current position
+  if (warp == (int)((seq0 + (uint32_t)g.n_k) % ST_W)) attn_scores<GEN>(p.hd, s.k16, 1, 0, 8, s.q16, p.kq_scale, s.sc + g.pos);   // the current position
   bar_sync<ST_BAR, ST_NT>();
   attn_softmax<ST_NT, ST_BAR>(s.sc, s.p16, g.T, p.exp_tab, red_f, red_d);
   // ---- V·P for this task's channels
-  for (int cc = warp; cc < ATTN_CH; cc += ST_W) {
+  for (int cc = warp; cc < nch; cc += ST_W) {
     const int c = cg * ATTN_CH + cc;
     const uint32_t n = seq0 + (uint32_t)(g.n_k + cc / g.cv);
     const RingPos rp = st_ring(n, S);
@@ -707,16 +718,43 @@ __device__ __forceinline__ void st_attn_task(const AttnParams& p, uint8_t* smem,
     if (lane == 0) p.out[(size_t)h * p.hd + c] = o;
   }
   bar_sync<ST_BAR, ST_NT>();
-  if (threadIdx.x < g.n_v) {
+  if ((int)threadIdx.x < attn_ring_nv<GEN>(g, p.hd, cg)) {
     const uint32_t n = seq0 + (uint32_t)(g.n_k + threadIdx.x);
     mbar_arrive(&empty_bar[st_ring(n, S).slot]);
   }
+}
+
+// The consumers' side of an attention phase: tasks (head, channel group) blockIdx.x, + gridDim.x, ...; K / V through the ring
+// (ph.q6) or from global memory.  hd 64 / 128 inline (GEN = false), other head sizes in one out-of-line call.
+template <bool GEN>
+__device__ __forceinline__ void st_attn_phase(const Phase& ph, uint8_t* act_smem, uint8_t* ring, uint64_t* full_bar, uint64_t* empty_bar, int n_slots,
+                                              uint32_t& seq, float* pick_v, double* red) {
+  const int n_cg = GEN ? attn_groups(ph.at.hd) : ph.at.hd / ATTN_CH, n_tasks = ph.at.n_head * n_cg, G = (int)gridDim.x;
+  if (ph.q6) {
+    const AttnRing ag = attn_ring_geom<GEN>(ph.at);
+    for (int task = blockIdx.x; task < n_tasks; task += G) {
+      if (task != (int)blockIdx.x) bar_sync<ST_BAR, ST_NT>();
+      if (ag.T > 0) st_attn_task<GEN>(ph.at, act_smem, ring, full_bar, empty_bar, (uint32_t)(n_slots / ST_W), seq, ag, task / n_cg, task % n_cg, pick_v, red);
+      seq += (uint32_t)(ag.n_k + attn_ring_nv<GEN>(ag, ph.at.hd, task % n_cg));
+    }
+  } else {
+    for (int task = blockIdx.x; task < n_tasks; task += G) {
+      if (task != (int)blockIdx.x) bar_sync<ST_BAR, ST_NT>();
+      attn_body<ST_NT, ST_BAR, false, GEN>(ph.at, act_smem, task / n_cg, 0, task % n_cg, ph.at.state);
+    }
+  }
+}
+static __device__ __noinline__ uint32_t st_attn_phase_gen(const Phase& ph, uint8_t* act_smem, uint8_t* ring, uint64_t* full_bar, uint64_t* empty_bar, int n_slots,
+                                                   uint32_t seq, float* pick_v, double* red) {
+  st_attn_phase<true>(ph, act_smem, ring, full_bar, empty_bar, n_slots, seq, pick_v, red);
+  return seq;
 }
 
 // Producer warp: the same enumeration as the consumers, one bulk copy per item, as far ahead as the ring allows.  The weight
 // copies read with an L2 evict-first policy: a weight line is dead once its ring copy has read it (the next read is a step
 // later, 4 GB of stream away), so the stream's lines go first and the step's live data (KV cache, activation vectors, exp
 // table) stays in L2.  K / V items keep the default policy.
+template <bool XC, bool GEN>
 __device__ __forceinline__ void st_producer(const StepArgs& args, uint8_t* ring, uint64_t* full_bar, uint64_t* empty_bar) {
   const int lane = threadIdx.x & 31;
   const uint32_t S = (uint32_t)(args.n_slots / ST_W);   // ring depth per consumer warp
@@ -725,7 +763,10 @@ __device__ __forceinline__ void st_producer(const StepArgs& args, uint8_t* ring,
   for (int ip = 0; ip < args.n_phases; ip++) {
     const Phase* ph = args.prog + ip;
     if (ph->kind == PH_ATTN) {
-      if (ph->q6) st_attn_produce(ph->at, ring, full_bar, empty_bar, S, seq);
+      if (ph->q6) {
+        if (GEN) st_attn_produce<true>(ph->at, ring, full_bar, empty_bar, S, seq);
+        else st_attn_produce<false>(ph->at, ring, full_bar, empty_bar, S, seq);
+      }
       continue;
     }
     if (ph->kind != PH_MATVEC) continue;
@@ -850,7 +891,10 @@ __device__ __forceinline__ void grid_rearm(unsigned* sync, bool set_xc = false, 
   }
 }
 
-template <bool XC>
+// GEN: the program's attention phases have a head size other than 64 / 128 (attn_fast_hd); they run in one out-of-line call,
+// and the kernels of the other models (GEN = false) have no trace of them.  The tensor-sharded mode takes heads of 64 / 128
+// only, so there is no exchange kernel with GEN.
+template <bool XC, bool GEN>
 static __global__ void __launch_bounds__(ST_THREADS, 1) k_step(const __grid_constant__ StepArgs args) {
   extern __shared__ __align__(16) uint8_t smem[];
   __shared__ __align__(8) uint64_t full_bar[ST_MAX_SLOTS];
@@ -869,7 +913,7 @@ static __global__ void __launch_bounds__(ST_THREADS, 1) k_step(const __grid_cons
   pdl_trigger();
   pdl_wait();           // (the producer reads device state too: the position decides how many K / V items an attention phase has)
   if (warp == ST_W) {
-    st_producer(args, ring, full_bar, empty_bar);
+    st_producer<XC, GEN>(args, ring, full_bar, empty_bar);
     return;
   }
   const unsigned G = gridDim.x;
@@ -916,20 +960,8 @@ static __global__ void __launch_bounds__(ST_THREADS, 1) k_step(const __grid_cons
       // (the tile bounds were written by threads 0/1 above; the barriers inside the activation staging order them)
       st_matvec_phase<XC>(ph, np, ring, act_smem, red, full_bar, empty_bar, mailbox, flags, (uint32_t)(args.n_slots / ST_W), seq, &tb_s[ip & 1][0], tr, xc_base);
     } else if (ph.kind == PH_ATTN) {
-      const int n_cg = ph.at.hd / ATTN_CH, n_tasks = ph.at.n_head * n_cg;
-      if (ph.q6) {
-        const AttnRing ag = attn_ring_geom(ph.at);
-        for (int task = blockIdx.x; task < n_tasks; task += G) {
-          if (task != (int)blockIdx.x) bar_sync<ST_BAR, ST_NT>();
-          if (ag.T > 0) st_attn_task(ph.at, act_smem, ring, full_bar, empty_bar, (uint32_t)(args.n_slots / ST_W), seq, ag, task / n_cg, task % n_cg, pick_v, red);
-          seq += (uint32_t)(ag.n_k + ag.n_v);
-        }
-      } else {
-        for (int task = blockIdx.x; task < n_tasks; task += G) {
-          if (task != (int)blockIdx.x) bar_sync<ST_BAR, ST_NT>();
-          attn_body<ST_NT, ST_BAR, false>(ph.at, act_smem, task / n_cg, 0, task % n_cg, ph.at.state);
-        }
-      }
+      if (GEN) seq = st_attn_phase_gen(ph, act_smem, ring, full_bar, empty_bar, args.n_slots, seq, pick_v, red);
+      else st_attn_phase<false>(ph, act_smem, ring, full_bar, empty_bar, args.n_slots, seq, pick_v, red);
     } else if (ph.kind == PH_EMBED) {
       if (blockIdx.x == 0) embed_row(ph.em, ph.em.tokens[0], ph.em.out, threadIdx.x, ST_NT);
     } else if (ph.kind == PH_PICK) {
@@ -946,7 +978,7 @@ static __global__ void __launch_bounds__(ST_THREADS, 1) k_step(const __grid_cons
 
 // ---------------------------------------------------------------------------------------------
 // Host side
-struct StepLaunch { int grid; int n_slots; size_t smem; };
+struct StepLaunch { int grid; int n_slots; size_t smem; bool gen = false; /* k_step<.., true>: see k_step */ };
 
 // shared-memory budget: ring slots fill what the largest activation image of the program leaves
 inline StepLaunch step_launch_shape(const Phase* phases, int n, int n_sm, size_t max_dyn_smem, size_t extra_act = 0) {
@@ -955,9 +987,12 @@ inline StepLaunch step_launch_shape(const Phase* phases, int n, int n_sm, size_t
     if (phases[i].kind == PH_MATVEC) act = std::max(act, st_act_bytes(phases[i].mv.K, phases[i].q6 != 0));
     if (phases[i].kind == PH_ATTN) act = std::max(act, attn_smem_bytes(phases[i].at.n_ctx, phases[i].at.hd));
   }
+  bool gen = false;
+  for (int i = 0; i < n; i++) gen |= phases[i].kind == PH_ATTN && !attn_fast_hd(phases[i].at.hd);
   act = (act + 127) & ~(size_t)127;
   StepLaunch L;
   L.grid = n_sm;
+  L.gen = gen;
   if (act + (size_t)ST_W * ST_SLOT > max_dyn_smem) { L.n_slots = 0; L.smem = 0; return L; }
   L.n_slots = ST_W * (int)std::min<size_t>(ST_MAX_DEPTH, (max_dyn_smem - act) / ((size_t)ST_W * ST_SLOT));   // whole sub-rings only
   L.smem = (size_t)L.n_slots * ST_SLOT + act;
@@ -999,15 +1034,16 @@ inline Phase matvec_phase(const MVParams& p) {
 // point the kernels' watchdog at 4 ints of host-mapped memory (each translation unit has its own copy of the symbol)
 static inline cudaError_t st_set_debug_words(int* dev_ptr) { return cudaMemcpyToSymbol(g_st_dbg, &dev_ptr, sizeof(int*)); }
 static inline cudaError_t step_set_smem_limit(size_t bytes) {
-  const cudaError_t e = cudaFuncSetAttribute(k_step<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes);
-  return e != cudaSuccess ? e : cudaFuncSetAttribute(k_step<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes);
+  cudaError_t e = cudaFuncSetAttribute(k_step<false, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes);
+  if (e == cudaSuccess) e = cudaFuncSetAttribute(k_step<false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes);
+  return e != cudaSuccess ? e : cudaFuncSetAttribute(k_step<true, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes);
 }
 
 static inline cudaError_t launch_step(const StepLaunch& L, cudaStream_t st, const Phase* d_prog, const int* d_bounds, int n_phases, unsigned* d_sync, bool pdl = false,
                                       unsigned long long* trace = nullptr, bool xchg = false) {
   StepArgs a;
   a.prog = d_prog; a.bounds = d_bounds; a.n_phases = n_phases; a.n_slots = L.n_slots; a.sync = d_sync; a.trace = trace;
-  return launch_kernel(xchg ? k_step<true> : k_step<false>, dim3(L.grid), dim3(ST_THREADS), L.smem, st, pdl, a);
+  return launch_kernel(xchg ? k_step<true, false> : (L.gen ? k_step<false, true> : k_step<false, false>), dim3(L.grid), dim3(ST_THREADS), L.smem, st, pdl, a);
 }
 
 }  // namespace ctb

@@ -214,6 +214,9 @@ class LlamaShape:
 
 LLAMA2_7B = LlamaShape()
 LLAMA2_13B = LlamaShape(n_embd=5120, n_head=40, n_head_kv=40, n_ff=13824, n_layer=40)
+# OpenLLaMA-3B and the models fine-tuned from it (the reference's MODEL_3B, 26 layers): heads of 100.  n_embd 3200 is not a
+# multiple of 256, so the reference quantizer writes such files in the legacy types only.
+OPENLLAMA_3B = LlamaShape(n_vocab=32000, n_embd=3200, n_head=32, n_head_kv=32, n_ff=8640, n_layer=26, n_ctx_train=2048)
 
 
 @dataclass
