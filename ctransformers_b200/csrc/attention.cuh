@@ -22,7 +22,18 @@ __device__ __forceinline__ void k4_scale_min(int j, const uint8_t* q, int& sc, i
   else { sc = (q[j + 4] & 0xF) | ((q[j - 4] >> 6) << 4); m = (q[j + 4] >> 4) | ((q[j] >> 6) << 4); }
 }
 
+// Q3 = false: the callers in the kernels of models without Q3_K tensors, which then carry none of its code (see k_step)
+template <bool Q3 = true>
 __device__ __forceinline__ float dequant_elem(int type, const uint8_t* row, int e) {
+  if (Q3 && type == GT_Q3_K) {   // dequantize_row_q3_K (k_quants.c:575-623): block = hmask[32], qs[64], scales[12], d; dl = d·(sc - 32), then dl·q
+    const uint8_t* blk = row + (size_t)(e >> 8) * 110;
+    const int r = e & 255, n = r >> 7, j = (r & 127) >> 5, l = r & 31, is = 8 * n + 2 * j + (l >> 4);
+    const int w = is >> 2, b = is & 3;   // scale word w of the unpacked 16 (k_quants.c:594-598), byte b
+    const int lo = w & 1 ? blk[100 + b] : blk[96 + b];
+    const int sc = ((w < 2 ? lo : lo >> 4) & 0xF) | (((blk[104 + b] >> (2 * w)) & 3) << 4);
+    const int q = ((blk[32 + 32 * n + l] >> (2 * j)) & 3) - ((blk[l] >> (4 * n + j)) & 1 ? 0 : 4);
+    return __fmul_rn(__fmul_rn(h2f((uint16_t)(blk[108] | (blk[109] << 8))), (float)(sc - 32)), (float)q);
+  }
   switch (type) {
     case GT_F32: return ((const float*)row)[e];
     case GT_F16: return h2f(((const uint16_t*)row)[e]);
@@ -91,9 +102,10 @@ __device__ __forceinline__ float dequant_elem(int type, const uint8_t* row, int 
 struct EmbedParams { const uint8_t* table; size_t row_bytes; const int* tokens; float* out; int type, K, n_vocab; };
 
 // the embedding row of token id `tok` (clamped to the vocabulary) into out[K], by threads tid, tid + nt, ...
+template <bool Q3 = true>
 __device__ __forceinline__ void embed_row(const EmbedParams& em, int tok, float* out, int tid, int nt) {
   const uint8_t* row = em.table + (size_t)min(max(tok, 0), em.n_vocab - 1) * em.row_bytes;
-  for (int e = tid; e < em.K; e += nt) out[e] = dequant_elem(em.type, row, e);
+  for (int e = tid; e < em.K; e += nt) out[e] = dequant_elem<Q3>(em.type, row, e);
 }
 
 // grid = N tokens; out[n][K]

@@ -2,8 +2,8 @@
 //
 // Weights are NOT kept in GGUF's array-of-blocks form.  At load time every 2-D weight is repacked,
 // byte for byte (same total size, so the HBM roofline denominator is unchanged):
-//   K-quants (Q4_K / Q5_K / Q6_K): the STREAM layout of stream.cuh — 16-row tiles, block-major, every (tile, block) a
-//   contiguous 16-byte-aligned piece of 16 x {144,176,210} bytes that one cp.async.bulk moves into shared memory and whose
+//   K-quants (Q3_K / Q4_K / Q5_K / Q6_K): the STREAM layout of stream.cuh — 16-row tiles, block-major, every (tile, block) a
+//   contiguous 16-byte-aligned piece of 16 x {110,144,176,210} bytes that one cp.async.bulk moves into shared memory and whose
 //   interior is ordered for conflict-free 16-byte shared-memory loads of the mma.sync operand fragments.
 //   Other types: per-tensor planes so that every lane of a warp issues 16-byte-aligned, fully coalesced loads no
 //   matter how odd the source block size is (Q4_0 = 18 B, Q8_0 = 34 B):
@@ -28,7 +28,7 @@
 
 namespace ctb {
 
-enum : int { GT_F32 = 0, GT_F16 = 1, GT_Q4_0 = 2, GT_Q4_1 = 3, GT_Q5_0 = 6, GT_Q5_1 = 7, GT_Q8_0 = 8, GT_Q4_K = 12, GT_Q5_K = 13, GT_Q6_K = 14 };
+enum : int { GT_F32 = 0, GT_F16 = 1, GT_Q4_0 = 2, GT_Q4_1 = 3, GT_Q5_0 = 6, GT_Q5_1 = 7, GT_Q8_0 = 8, GT_Q3_K = 11, GT_Q4_K = 12, GT_Q5_K = 13, GT_Q6_K = 14 };
 
 struct DevMat {
   int type = -1;
@@ -43,7 +43,7 @@ struct DevMat {
   size_t bytes = 0;     // total bytes of all planes (= GGUF tensor bytes)
 };
 
-__host__ __device__ inline bool type_is_kquant(int t) { return t == GT_Q4_K || t == GT_Q5_K || t == GT_Q6_K; }
+__host__ __device__ inline bool type_is_kquant(int t) { return t == GT_Q3_K || t == GT_Q4_K || t == GT_Q5_K || t == GT_Q6_K; }
 // activation format each weight type is multiplied with (reference: type_traits vec_dot_type, ggml.c:1638-1808)
 enum : int { ACT_Q8_K = 0, ACT_Q8_0 = 1, ACT_F16 = 2, ACT_F32 = 3, ACT_Q8_1 = 4 };
 __host__ __device__ inline int act_format_for(int t) {

@@ -73,6 +73,7 @@ struct PrefillState {
   float* x_final = nullptr;         // batched buffer that holds the last layer's output rows
   int n_slots = 0;
   size_t smem = 0;
+  bool q3 = false;                  // the program holds Q3_K matrices (k_pstep<true>)
   bool ok = false, tried = false;
   ~PrefillState() {
     for (void* b : bufs) cudaFree(b);
@@ -85,7 +86,7 @@ constexpr size_t UP_CHUNK = (size_t)32 << 20;   // upload pipeline: chunk bytes 
 constexpr int UP_BUFS = 3;
 
 static bool supported_matrix_type(uint32_t t) {
-  return t == T_F32 || t == T_F16 || t == T_Q4_0 || t == T_Q4_1 || t == T_Q5_0 || t == T_Q5_1 || t == T_Q8_0 || t == T_Q4_K || t == T_Q5_K ||
+  return t == T_F32 || t == T_F16 || t == T_Q4_0 || t == T_Q4_1 || t == T_Q5_0 || t == T_Q5_1 || t == T_Q8_0 || t == T_Q3_K || t == T_Q4_K || t == T_Q5_K ||
          t == T_Q6_K;
 }
 
@@ -688,8 +689,8 @@ void Engine::build_ops() {
   for (const StepOp& op : ops_) any_stream |= op.ph.kind == PH_MATVEC && op.stream;
   std::vector<Phase> phs;
   for (const StepOp& op : ops_) if (op.ph.kind != PH_XCHG && (op.ph.kind != PH_MATVEC || op.stream)) phs.push_back(op.ph);
-  const StepLaunch sl = step_launch_shape(phs.data(), (int)phs.size(), sm_count_, max_dyn_smem(k_step<true, false>));
-  step_grid_ = sl.grid; step_slots_ = sl.n_slots; step_smem_ = sl.smem;
+  const StepLaunch sl = step_launch_shape(phs.data(), (int)phs.size(), sm_count_, max_dyn_smem(k_step<true, false, false>));
+  step_grid_ = sl.grid; step_slots_ = sl.n_slots; step_smem_ = sl.smem; step_q3_ = sl.q3;
   if (const char* e = getenv("CTB_ST_SLOTS")) {   // A/B knob: fewer ring slots = less prefetch in flight
     const int want = atoi(e);
     if (want >= ST_W && want < step_slots_ && want % ST_W == 0) { step_smem_ -= (size_t)(step_slots_ - want) * ST_SLOT; step_slots_ = want; }
@@ -722,6 +723,7 @@ void Engine::enqueue_ops(const std::vector<StepOp>& ops, const Phase* d_prog, co
   launches_per_step_ = 0;
   StepLaunch step_shape_;
   step_shape_.grid = step_grid_; step_shape_.n_slots = step_slots_; step_shape_.smem = step_smem_; step_shape_.gen = !attn_fast_hd(hp_.head_dim());
+  step_shape_.q3 = step_q3_;
   auto capable = [&](const StepOp& op) { return op.ph.kind != PH_XCHG && (op.ph.kind != PH_MATVEC || op.stream); };
   int i = 0;
   while (i < n) {
@@ -866,7 +868,7 @@ long Engine::trace_step(int token, int n_past, unsigned long long* out, long cap
   CTB_CUDA(cudaMalloc(&buf, (size_t)n * step_grid_ * 64));
   CTB_CUDA(cudaMemset(buf, 0, (size_t)n * step_grid_ * 64));
   StepLaunch L;
-  L.grid = step_grid_; L.n_slots = step_slots_; L.smem = step_smem_; L.gen = !attn_fast_hd(hp_.head_dim());
+  L.grid = step_grid_; L.n_slots = step_slots_; L.smem = step_smem_; L.gen = !attn_fast_hd(hp_.head_dim()); L.q3 = step_q3_;
   if (h_state_cap_ < 1) { h_state_cap_ = 512; CTB_CUDA(cudaMallocHost(&h_state_, (size_t)h_state_cap_ * 16)); }
   for (int rep = 0; rep < 3; rep++) {   // the last (warm) run is the one read back
     h_state_[0] = token; h_state_[1] = n_past; h_state_[2] = 0; h_state_[3] = n_past + 1;
@@ -1162,6 +1164,7 @@ bool Engine::ensure_prefill() {
   int ld;
   P.x_final = bat(ops_[n_body_].ph.mv.x, ld);
   P.n_phases = (int)prog.size();
+  P.q3 = pstep_q3(prog);
   P.d_prog = (PPhase*)dalloc((prog.size() + 1) * sizeof(PPhase));
   CTB_CUDA(cudaMemcpy(P.d_prog, prog.data(), prog.size() * sizeof(PPhase), cudaMemcpyHostToDevice));
   if (!pstep_shape(pb_work_bytes(K_max, hp_.n_ctx, hp_.head_dim()), P.n_slots, P.smem)) return false;
@@ -1182,7 +1185,7 @@ void Engine::prefill_batch(const int* tokens, const int* pos, const int* n_total
   }
   st[PB_T * 4] = n;
   CTB_CUDA(cudaMemcpyAsync(P.d_state, st, (PB_T * 4 + 4) * 4, cudaMemcpyHostToDevice, stream_));
-  CTB_CUDA(launch_pstep(step_grid_, P.n_slots, P.smem, stream_, P.d_prog, P.n_phases, d_sync_));
+  CTB_CUDA(launch_pstep(step_grid_, P.n_slots, P.smem, stream_, P.d_prog, P.n_phases, d_sync_, P.q3));
   prefill_launches_++;
   if (last) {
     const StepOp& head = ops_[n_body_];

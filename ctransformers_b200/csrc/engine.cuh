@@ -164,6 +164,7 @@ class Engine {
   int step_grid_ = 0, step_slots_ = 0;   // launch shape of the step kernel: CTAs, ring slots,
   size_t step_smem_ = 0;                 // dynamic shared memory
   bool fused_ = true;            // CTB_STEP_FUSE=0: one kernel per op
+  bool step_q3_ = false;         // some mat-vec phase holds a Q3_K matrix: the k_step<.., .., true> build
   bool ring_attn_ = false;       // the step kernel's attention phases take cached K / V through the ring (st_attn_ring_ok)
   void build_ops();
   void push_matvec(struct MVParams& p, int kind);

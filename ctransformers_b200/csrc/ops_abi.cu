@@ -58,6 +58,7 @@ size_t raw_row_bytes(int type, int K) {
     case GT_F32: return (size_t)K * 4; case GT_F16: return (size_t)K * 2;
     case GT_Q4_0: return (size_t)K / 32 * 18; case GT_Q5_0: return (size_t)K / 32 * 22; case GT_Q8_0: return (size_t)K / 32 * 34;
     case GT_Q4_1: return (size_t)K / 32 * 20; case GT_Q5_1: return (size_t)K / 32 * 24;
+    case GT_Q3_K: return (size_t)K / 256 * 110;
     case GT_Q4_K: return (size_t)K / 256 * 144; case GT_Q5_K: return (size_t)K / 256 * 176; case GT_Q6_K: return (size_t)K / 256 * 210;
   }
   throw std::runtime_error("unsupported ggml type " + std::to_string(type));
@@ -115,7 +116,7 @@ unsigned* sync_words() {
 // a program of phases through the persistent step kernel, exactly as the engine launches it
 void run_phases(std::vector<Phase> phs) {
   unsigned* d_sync = sync_words();
-  const StepLaunch L = step_launch_shape(phs.data(), (int)phs.size(), sm_count(), max_dyn_smem(k_step<true, false>));
+  const StepLaunch L = step_launch_shape(phs.data(), (int)phs.size(), sm_count(), max_dyn_smem(k_step<true, false, false>));
   const std::vector<int> hb = step_bounds(phs.data(), (int)phs.size(), L.grid);
   DevBuf dbounds(hb.size() * 4);
   OPS_CUDA(cudaMemcpy(dbounds.p, hb.data(), hb.size() * 4, cudaMemcpyHostToDevice));
@@ -443,7 +444,7 @@ int ctb_attention_path(int path, const float* q, const float* k_new, const float
       if (path == 1) {
         Phase ph{};
         ph.kind = PH_ATTN; ph.q6 = 1; ph.at = ap;
-        const StepLaunch L = step_launch_shape(&ph, 1, sm_count(), max_dyn_smem(k_step<true, false>));
+        const StepLaunch L = step_launch_shape(&ph, 1, sm_count(), max_dyn_smem(k_step<true, false, false>));
         if (!st_attn_ring_ok(n_ctx, L.n_slots)) throw std::runtime_error("the step kernel's ring cannot carry K / V at this n_ctx");
       }
       const size_t smem = attn_smem_bytes(n_ctx, hd);
@@ -545,7 +546,7 @@ int ctb_prefill_mul_mat(int nseg, const int* types, const void* const* w_blocks,
       if (x2) OPS_CUDA(cudaMemcpy(dx2.p, x2 + (size_t)b * K, (size_t)n * K * 4, cudaMemcpyHostToDevice));
       if (res) OPS_CUDA(cudaMemcpy(dres.p, res + (size_t)b * W, (size_t)n * W * 4, cudaMemcpyHostToDevice));
       if (res2) OPS_CUDA(cudaMemcpy(dres2.p, res2 + (size_t)b * W, (size_t)n * W * 4, cudaMemcpyHostToDevice));
-      OPS_CUDA(launch_pstep(sm_count(), slots, smem, 0, dprog.as<PPhase>(), (int)prog.size(), sync_words()));
+      OPS_CUDA(launch_pstep(sm_count(), slots, smem, 0, dprog.as<PPhase>(), (int)prog.size(), sync_words(), pstep_q3(prog)));
       OPS_CUDA(cudaDeviceSynchronize());
       OPS_CUDA(cudaMemcpy(out + (size_t)b * W, dout.p, (size_t)n * W * 4, cudaMemcpyDeviceToHost));
     }
@@ -598,7 +599,7 @@ int ctb_matvec_partition(const int* types, const int* rows, int nseg, int K, int
     max_items = std::max(max_items, items);
   }
   meta[0] = n_sm; meta[1] = ST_SLOT; meta[2] = ST_MAXT; meta[3] = ts.ntiles; meta[4] = ST_W; meta[5] = ST_ROWS; meta[6] = (int)max_items;
-  meta[7] = st_chunk_blocks(GT_Q4_K) | (st_chunk_blocks(GT_Q5_K) << 8) | (st_chunk_blocks(GT_Q6_K) << 16);
+  meta[7] = st_chunk_blocks(GT_Q4_K) | (st_chunk_blocks(GT_Q5_K) << 8) | (st_chunk_blocks(GT_Q6_K) << 16) | (st_chunk_blocks(GT_Q3_K) << 24);
   return 0;
 }
 

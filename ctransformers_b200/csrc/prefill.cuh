@@ -4,11 +4,11 @@
 // every activation column on its own).
 //
 // The exact formulation.  Per (weight row, token, 256-block) the reference's AVX2 kernels need the eight int32 lane values
-//     sumi[l] = Σ_s scale_s · Σ_{e<4} w[32s + 4l + e] · q8[32s + 4l + e]        (k_quants.c:2651-2714, 3174-3262, 3794-3872)
+//     sumi[l] = Σ_s scale_s · Σ_{e<4} w[32s + 4l + e] · q8[32s + 4l + e]        (k_quants.c:1950-2052, 2651-2714, 3174-3262, 3794-3872)
 // i.e. for a FIXED lane l a contraction over 32 (s, e) pairs — exactly the K = 32 of mma.sync.m16n8k32 — if the scale can
-// ride on the weight operand.  w·scale does not fit a byte (15·63, 31·63, (q6-32)·int8), so it is split into two exact
-// digits:  Q4_K / Q5_K: scale = 8·hi + lo (hi, lo <= 7; w·7 <= 217 fits u8)  →  sumi = D(w·lo) + 8·D(w·hi)
-//          Q6_K:        v = (q6-32)·scale, v = 128·(v >> 7) + (v & 127)       →  sumi = D(v & 127) + 128·D(v >> 7)
+// ride on the weight operand.  w·scale does not fit a byte (15·63, 31·63, (q6-32)·int8, (q3-4)·(-32)), so it is split into two
+// exact digits:  Q4_K / Q5_K: scale = 8·hi + lo (hi, lo <= 7; w·7 <= 217 fits u8)  →  sumi = D(w·lo) + 8·D(w·hi)
+//                Q6_K / Q3_K: v = (q-32)·scale or (q-4)·(sc-32), v = 128·(v >> 7) + (v & 127)  →  sumi = D(v & 127) + 128·D(v >> 7)
 // Two dense mma per (16 rows x 8 tokens x lane l x block): A = digits of 16 rows x 32 (s,e), B = int8 activations of 8 tokens,
 // D = exact int32.  The fp32 part is the reference's: one fmadd per block into the lane accumulator, blocks in order,
 // hsum_float_8 at the end (+ the mins accumulators) — the same instructions as stream.cuh, so the bits agree.
@@ -142,6 +142,42 @@ __device__ __forceinline__ void pb_block(const uint8_t* blk, int b, const uint8_
         Ahi[li][i] = q * shi[rr][hs];
       }
     }
+  } else if (TYPE == GT_Q3_K) {   // v = (q3 - 4)·(sc - 32) in [-124, 128], split as Q6_K's
+    const uint32_t* sp = (const uint32_t*)(blk + 1536);
+    dw[0] = h2f(((const uint16_t*)(blk + 1728))[g]);
+    dw[1] = h2f(((const uint16_t*)(blk + 1728))[8 + g]);
+    const int par = lp >> 1;   // both lanes l = 2lp + li lie in the same 16-weight half of each group
+    int sc[2][2];              // [rr][hs]: the six-bit scale of sub-block 2·grp + par, grp = t + 4hs (k_quants.c:1968-1974)
+#pragma unroll
+    for (int rr = 0; rr < 2; rr++) {
+      const uint32_t* h = sp + 3 * (rr * 8 + g);
+      const uint32_t a0 = h[0], a1 = h[1], a2 = h[2];
+      const uint32_t lo = (t >> 1) ? a1 : a0;   // sub-blocks 2t + par (word t >> 1) and 8 + 2t + par (word 2 + (t >> 1))
+      const int byte = 2 * (t & 1) + par, sh = 8 * byte;
+      sc[rr][0] = (int)(((lo >> sh) & 0x0fu) | (((a2 >> (sh + 2 * (t >> 1))) & 0x03u) << 4)) - 32;
+      sc[rr][1] = (int)(((lo >> (sh + 4)) & 0x0fu) | (((a2 >> (sh + 4 + 2 * (t >> 1))) & 0x03u) << 4)) - 32;
+    }
+#pragma unroll
+    for (int li = 0; li < 2; li++) {
+      const int l = 2 * lp + li;
+#pragma unroll
+      for (int i = 0; i < 4; i++) {
+        const int rr = i & 1, hs = i >> 1, grp = t + 4 * hs;   // qs word hs, bits 2t; hmask bit grp
+        const int e0 = (((l >> 2) * 2 + rr) * 32 + g * 4 + (l & 3));
+        const uint32_t qw = *(const uint32_t*)(blk + e0 * 8 + hs * 4);
+        const uint32_t hm = *(const uint32_t*)(blk + 1024 + e0 * 4);
+        const uint32_t u = ((qw >> (2 * t)) & 0x03030303u) | (((hm >> grp) & 0x01010101u) << 2);
+        const int scale = sc[rr][hs];
+        uint32_t lo = 0u, hi = 0u;
+#pragma unroll
+        for (int e = 0; e < 4; e++) {
+          const int v = ((int)((u >> (8 * e)) & 0xffu) - 4) * scale;
+          lo |= (uint32_t)(v & 127) << (8 * e);
+          hi |= (uint32_t)((v >> 7) & 0xff) << (8 * e);
+        }
+        Alo[li][i] = lo; Ahi[li][i] = hi;
+      }
+    }
   } else {   // Q6_K: v = (q6 - 32)·scale split into v >> 7 (signed) and v & 127
     const int4 s0 = ((const int4*)(blk + 3072))[g], s1 = ((const int4*)(blk + 3072))[8 + g];
     dw[0] = h2f(((const uint16_t*)(blk + 3328))[g]);
@@ -186,7 +222,7 @@ __device__ __forceinline__ void pb_block(const uint8_t* blk, int b, const uint8_
     for (int li = 0; li < 2; li++) {
       const uint32_t b0 = li ? bw.z : bw.x, b1 = li ? bw.w : bw.y;
       int Dl[4], Dh[4];
-      if (TYPE == GT_Q6_K) {
+      if (TYPE == GT_Q6_K || TYPE == GT_Q3_K) {
         mma_s8s8(Dl, Alo[li][0], Alo[li][1], Alo[li][2], Alo[li][3], b0, b1);
         mma_s8s8(Dh, Ahi[li][0], Ahi[li][1], Ahi[li][2], Ahi[li][3], b0, b1);
       } else {
@@ -195,7 +231,7 @@ __device__ __forceinline__ void pb_block(const uint8_t* blk, int b, const uint8_
       }
 #pragma unroll
       for (int r = 0; r < 4; r++) {
-        const int sumi = Dl[r] + (TYPE == GT_Q6_K ? 128 : 8) * Dh[r];
+        const int sumi = Dl[r] + (TYPE == GT_Q6_K || TYPE == GT_Q3_K ? 128 : 8) * Dh[r];
         st.acc[tg][li][r] = __fmaf_rn(dd[r], (float)sumi, st.acc[tg][li][r]);
       }
     }
@@ -265,6 +301,7 @@ __device__ __forceinline__ void pb_finish(const PBState& st, float* xch, int typ
 
 // ---------------------------------------------------------------------------------------------
 // Ring addressing: every team owns PB_TEAMS-strided slots of the ring (ring_pos in stream.cuh); cnt[t] counts team t's items.
+template <bool Q3>
 __device__ __forceinline__ void pb_producer(const PStepArgs& args, uint8_t* ring, uint64_t* full_bar, uint64_t* empty_bar) {
   const int lane = threadIdx.x & 31;
   const uint32_t D = (uint32_t)(args.n_slots / PB_TEAMS);
@@ -276,12 +313,12 @@ __device__ __forceinline__ void pb_producer(const PStepArgs& args, uint8_t* ring
     if (ph->kind != PP_GEMM) continue;
     const MVParams& p = ph->mv;
     TileSpace ts;
-    ts.init(p);
+    ts.init<Q3>(p);
     const int T0 = ts.boundary(blockIdx.x, gridDim.x), T1 = ts.boundary(blockIdx.x + 1, gridDim.x);
     const int nb = p.K >> 8;
     for (int w0 = T0; w0 < T1; w0 += PB_TEAMS) {
       const int ntw = min(PB_TEAMS, T1 - w0);
-      const TileInfo ti = tile_info(ts, p, w0 + lane, nb, lane < ntw);
+      const TileInfo ti = tile_info<Q3>(ts, p, w0 + lane, nb, lane < ntw);
       for (int kc = 0;; kc++) {
         const unsigned mask = __ballot_sync(0xffffffffu, kc < ti.nch);
         if (!mask) break;
@@ -291,7 +328,7 @@ __device__ __forceinline__ void pb_producer(const PStepArgs& args, uint8_t* ring
           const int seg = __shfl_sync(0xffffffffu, ti.seg, j), til = __shfl_sync(0xffffffffu, ti.til, j), type = __shfl_sync(0xffffffffu, ti.type, j);
           if (lane == 0) {
             const RingPos rp = ring_pos(cnt[j], (uint32_t)j, PB_TEAMS, D);
-            const StItem it = st_item(p, seg, type, til, kc, nb);
+            const StItem it = st_item<Q3>(p, seg, type, til, kc, nb);
             mbar_wait(&empty_bar[rp.slot], rp.parity ^ 1u, W_PF_FREE_SLOT, (int)cnt[j]);
             mbar_expect_tx(&full_bar[rp.slot], it.bytes);
             bulk_g2s(ring + (size_t)rp.slot * ST_SLOT, it.src, it.bytes, &full_bar[rp.slot]);
@@ -303,18 +340,19 @@ __device__ __forceinline__ void pb_producer(const PStepArgs& args, uint8_t* ring
   }
 }
 
+template <bool Q3>
 __device__ __forceinline__ void pb_gemm_phase(const PPhase& ph, int n_tok, uint8_t* ring, float* xch_all, uint64_t* full_bar, uint64_t* empty_bar, uint32_t D, uint32_t& cnt) {
   const MVParams& p = ph.mv;
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, team = warp >> 2, lp = warp & 3;
   float* xch = xch_all + (size_t)team * (PB_XCH / 4);
   TileSpace ts;
-  ts.init(p);
+  ts.init<Q3>(p);
   const int T0 = ts.boundary(blockIdx.x, gridDim.x), T1 = ts.boundary(blockIdx.x + 1, gridDim.x);
   const int nb = p.K >> 8;
 #pragma unroll 1
   for (int w0 = T0; w0 < T1; w0 += PB_TEAMS) {
     const int ntw = min(PB_TEAMS, T1 - w0);
-    const TileInfo ti = tile_info(ts, p, w0 + lane, nb, lane < ntw);
+    const TileInfo ti = tile_info<Q3>(ts, p, w0 + lane, nb, lane < ntw);
     const int my_seg = __shfl_sync(0xffffffffu, ti.seg, team), my_til = __shfl_sync(0xffffffffu, ti.til, team), my_type = __shfl_sync(0xffffffffu, ti.type, team);
     PBState st;
 #pragma unroll
@@ -327,12 +365,13 @@ __device__ __forceinline__ void pb_gemm_phase(const PPhase& ph, int n_tok, uint8
       if (!mask) break;
       if ((mask >> team) & 1u) {
         const RingPos rp = ring_pos(cnt, (uint32_t)team, PB_TEAMS, D);
-        const int kb = st_chunk_blocks(my_type);
+        const int kb = st_chunk_blocks<Q3>(my_type);
         const int b0 = kc * kb, nblk = min(kb, nb - b0);
         const uint8_t* sp = ring + (size_t)rp.slot * ST_SLOT;
         mbar_wait(&full_bar[rp.slot], rp.parity, W_PF_WEIGHT_ITEM, (int)cnt);
         if (my_type == GT_Q4_K) pb_chunk<GT_Q4_K>(sp, nblk, b0, ph.qbuf, nb, lane, lp, (n_tok + 7) >> 3, st);
         else if (my_type == GT_Q6_K) pb_chunk<GT_Q6_K>(sp, nblk, b0, ph.qbuf, nb, lane, lp, (n_tok + 7) >> 3, st);
+        else if (Q3 && my_type == GT_Q3_K) pb_chunk<GT_Q3_K>(sp, nblk, b0, ph.qbuf, nb, lane, lp, (n_tok + 7) >> 3, st);
         else pb_chunk<GT_Q5_K>(sp, nblk, b0, ph.qbuf, nb, lane, lp, (n_tok + 7) >> 3, st);
         __syncwarp();
         if (lane == 0) mbar_arrive(&empty_bar[rp.slot]);   // 4 arrivals (the team's warps) free the slot
@@ -397,8 +436,13 @@ __device__ __forceinline__ void pb_attn_phase(const PPhase& ph, int n_tok, uint8
     pb_attn_warp_task<GEN>(ph.at, ph.state + tok * 4, tok, task % ph.at.n_head, wsm);
   }
 }
+// (one copy per kernel build, Q3: ptxas fits an out-of-line function's registers to all its callers at once)
+template <bool Q3>
 static __device__ __noinline__ void pb_attn_phase_gen(const PPhase& ph, int n_tok, uint8_t* work) { pb_attn_phase<true>(ph, n_tok, work); }
 
+// Q3: the build for programs that hold Q3_K matrices or a Q3_K embedding table.  The build without it compiles to the same
+// instructions as before Q3_K was added; with the Q3_K code inlined into the one kernel, ptxas spilled more there (DESIGN.md §6).
+template <bool Q3>
 static __global__ void __launch_bounds__(PB_THREADS, 1) k_pstep(const __grid_constant__ PStepArgs args) {
   extern __shared__ __align__(16) uint8_t smem[];
   __shared__ __align__(8) uint64_t full_bar[ST_MAX_SLOTS];
@@ -410,7 +454,7 @@ static __global__ void __launch_bounds__(PB_THREADS, 1) k_pstep(const __grid_con
   uint8_t* work = smem + (size_t)args.n_slots * ST_SLOT;   // activation image (QUANT) / team exchange buffers (GEMM) / attention scratch
   ring_init(full_bar, empty_bar, args.n_slots, 4);
   if (warp == PB_W) {
-    pb_producer(args, ring, full_bar, empty_bar);
+    pb_producer<Q3>(args, ring, full_bar, empty_bar);
     return;
   }
   const unsigned G = gridDim.x;
@@ -432,7 +476,7 @@ static __global__ void __launch_bounds__(PB_THREADS, 1) k_pstep(const __grid_con
     bar_sync<PB_BAR, PB_NT>();
     const int n_tok = min(PB_T, ph.state[PB_T * 4]);
     if (ph.kind == PP_GEMM) {
-      pb_gemm_phase(ph, n_tok, ring, (float*)work, full_bar, empty_bar, (uint32_t)(args.n_slots / PB_TEAMS), seq);
+      pb_gemm_phase<Q3>(ph, n_tok, ring, (float*)work, full_bar, empty_bar, (uint32_t)(args.n_slots / PB_TEAMS), seq);
     } else if (ph.kind == PP_QUANT) {
       for (int tok = blockIdx.x; tok < n_tok; tok += G) {
         MVParams q = ph.mv;
@@ -447,9 +491,9 @@ static __global__ void __launch_bounds__(PB_THREADS, 1) k_pstep(const __grid_con
       pb_kv_phase(ph, n_tok);
     } else if (ph.kind == PP_ATTN) {
       if (attn_fast_hd(ph.at.hd)) pb_attn_phase<false>(ph, n_tok, work);
-      else pb_attn_phase_gen(ph, n_tok, work);
+      else pb_attn_phase_gen<Q3>(ph, n_tok, work);
     } else if (ph.kind == PP_EMBED) {
-      for (int tok = blockIdx.x; tok < n_tok; tok += G) embed_row(ph.em, ph.state[tok * 4], ph.em.out + (size_t)tok * ph.em.K, threadIdx.x, PB_NT);
+      for (int tok = blockIdx.x; tok < n_tok; tok += G) embed_row<Q3>(ph.em, ph.state[tok * 4], ph.em.out + (size_t)tok * ph.em.K, threadIdx.x, PB_NT);
     }
   }
   bar_sync<PB_BAR, PB_NT>();
@@ -466,7 +510,7 @@ inline size_t pb_work_bytes(int K_max, int n_ctx, int hd) {
 // launch shape of k_pstep around `work` bytes of scratch: whole per-team sub-rings in what shared memory has left.  false
 // when fewer than 4 slots fit (the attention scratch of a long context): the caller then has no batched prefill.
 inline bool pstep_shape(size_t work, int& n_slots, size_t& smem) {
-  const size_t room = max_dyn_smem(k_pstep);
+  const size_t room = std::min(max_dyn_smem(k_pstep<false>), max_dyn_smem(k_pstep<true>));
   if (work + 4 * (size_t)ST_SLOT > room) return false;
   n_slots = (int)std::min<size_t>(ST_MAX_SLOTS, (room - work) / ST_SLOT) / PB_TEAMS * PB_TEAMS;
   smem = (size_t)n_slots * ST_SLOT + work;
@@ -492,11 +536,25 @@ inline void pb_matvec_phases(const MVParams& m, uint8_t* qbuf, const int* state,
   }
   ph.kind = PP_GEMM; prog.push_back(ph);
 }
-static inline cudaError_t pstep_set_smem_limit(size_t bytes) { return cudaFuncSetAttribute(k_pstep, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes); }
-static inline cudaError_t launch_pstep(int grid, int n_slots, size_t smem, cudaStream_t st, const PPhase* d_prog, int n_phases, unsigned* d_sync) {
+static inline cudaError_t pstep_set_smem_limit(size_t bytes) {
+  const cudaError_t e = cudaFuncSetAttribute(k_pstep<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes);
+  return e != cudaSuccess ? e : cudaFuncSetAttribute(k_pstep<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes);
+}
+// does a program hold Q3_K matrices or a Q3_K embedding table (then it runs on k_pstep<true>)?
+inline bool pstep_q3(const std::vector<PPhase>& prog) {
+  for (const PPhase& ph : prog) {
+    if (ph.kind == PP_EMBED && ph.em.type == GT_Q3_K) return true;
+    if (ph.kind == PP_GEMM)
+      for (int s = 0; s < ph.mv.nseg; s++)
+        if (ph.mv.seg[s].w.type == GT_Q3_K) return true;
+  }
+  return false;
+}
+static inline cudaError_t launch_pstep(int grid, int n_slots, size_t smem, cudaStream_t st, const PPhase* d_prog, int n_phases, unsigned* d_sync, bool q3 = false) {
   PStepArgs a;
   a.prog = d_prog; a.n_phases = n_phases; a.n_slots = n_slots; a.sync = d_sync;
-  k_pstep<<<grid, PB_THREADS, smem, st>>>(a);
+  if (q3) k_pstep<true><<<grid, PB_THREADS, smem, st>>>(a);
+  else k_pstep<false><<<grid, PB_THREADS, smem, st>>>(a);
   return cudaGetLastError();
 }
 

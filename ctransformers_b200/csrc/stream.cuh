@@ -3,8 +3,8 @@
 // stream that never stops at them.
 //
 // Replaces, bit-exactly, what ggml_graph_compute does per token for a Llama / Falcon graph (llama.cpp:2162-2798, 2835-2981):
-//   ggml_compute_forward_mul_mat over Q4_K / Q5_K / Q6_K weights with Q8_K activations   ggml.c:11031-11245
-//   ggml_vec_dot_q4_K_q8_K / q5_K / q6_K, AVX2 variants                                  k_quants.c:2651-2714, 3174-3262, 3794-3872
+//   ggml_compute_forward_mul_mat over Q3_K / Q4_K / Q5_K / Q6_K weights with Q8_K activations   ggml.c:11031-11245
+//   ggml_vec_dot_q3_K_q8_K / q4_K / q5_K / q6_K, AVX2 variants              k_quants.c:1950-2052, 2651-2714, 3174-3262, 3794-3872
 //   norm + quantize prologue and residual / SiLU / GELU epilogue                         matvec.cuh (shared with k_matvec)
 //   RoPE, KV store, K·q, softmax, V·p                                                    attention.cuh (attn_body, or st_attn_task below)
 //
@@ -14,7 +14,7 @@
 //                   activations, so the copies for the next phases are already in flight (or landed) while the consumers
 //                   still wait at a grid barrier, stage an activation vector or run attention, until the ring is full
 //                   (one ring is about 8 us of HBM time on an H100; DESIGN.md §5.2 has what the boundaries cost).
-//   work item       (16-row tile, chunk of 3-4 consecutive 256-weight blocks): 16 x {144,176,210} bytes per block, contiguous
+//   work item       (16-row tile, chunk of 2-5 consecutive 256-weight blocks): 16 x {110,144,176,210} bytes per block, contiguous
 //                   in the STREAM layout written at load time (k_repack_stream).  Items are numbered in one sequence that both
 //                   sides enumerate identically; item n belongs to consumer warp n % ST_W and lives in one of that warp's slots.
 //   consumer warp   per block: the 8 (sub-block) x 8 (AVX lane) 4-element integer dots of 16 rows come from 8 tensor-core
@@ -40,7 +40,7 @@ namespace ctb {
 constexpr int ST_W = CTB_ST_WARPS;      // consumer warps
 constexpr int ST_NT = ST_W * 32;        // consumer threads (threads 0 .. ST_NT-1)
 constexpr int ST_THREADS = ST_NT + 32;  // + the producer warp
-constexpr int ST_SLOT = 9216;           // ring slot: holds 4 Q4_K / 3 Q5_K / 2 Q6_K blocks of a 16-row tile
+constexpr int ST_SLOT = 9216;           // ring slot: holds 5 Q3_K / 4 Q4_K / 3 Q5_K / 2 Q6_K blocks of a 16-row tile
 #ifndef CTB_ST_DEPTH
 #define CTB_ST_DEPTH 2
 #endif
@@ -51,6 +51,9 @@ constexpr int ST_ROWS = 16;
 constexpr int ST_BAR = 1;               // named barrier of the consumer warps
 constexpr int ST_STATE = 6;             // floats of fold state per thread: 4 AVX-lane accumulators + up to 2 mins accumulators
 
+#ifndef CTB_CHUNK_Q3
+#define CTB_CHUNK_Q3 5
+#endif
 #ifndef CTB_CHUNK_Q4
 #define CTB_CHUNK_Q4 4
 #endif
@@ -60,22 +63,30 @@ constexpr int ST_STATE = 6;             // floats of fold state per thread: 4 AV
 #ifndef CTB_CHUNK_Q6
 #define CTB_CHUNK_Q6 2
 #endif
-// Per K-quant type: bytes of one row's 256-weight block, blocks per work item (one ring slot), mins accumulators of the fold
+// Per K-quant type: bytes of one row's 256-weight block, blocks per work item (one ring slot), mins accumulators of the fold.
+// Q3 = false: the kernels of programs without Q3_K matrices, whose arithmetic then has no trace of it (see k_step).
 struct StType { int rb, kb, nm; };
+template <bool Q3 = true>
 __host__ __device__ constexpr StType st_type(int type) {
-  return type == GT_Q4_K ? StType{144, CTB_CHUNK_Q4, 2} : (type == GT_Q5_K ? StType{176, CTB_CHUNK_Q5, 1} : StType{210, CTB_CHUNK_Q6, 0});
+  return Q3 && type == GT_Q3_K ? StType{110, CTB_CHUNK_Q3, 0}
+                               : (type == GT_Q4_K ? StType{144, CTB_CHUNK_Q4, 2} : (type == GT_Q5_K ? StType{176, CTB_CHUNK_Q5, 1} : StType{210, CTB_CHUNK_Q6, 0}));
 }
 template <int TYPE> struct StTraits {
   static constexpr int KB = st_type(TYPE).kb, BB = ST_ROWS * st_type(TYPE).rb, NM = st_type(TYPE).nm;
   static_assert(KB * BB <= ST_SLOT, "a work item must fit one ring slot");
 };
 __host__ __device__ inline int st_row_block_bytes(int type) { return st_type(type).rb; }
-__host__ __device__ inline int st_block_bytes(int type) { return ST_ROWS * st_type(type).rb; }   // 2304 / 2816 / 3360
-__host__ __device__ inline int st_chunk_blocks(int type) { return st_type(type).kb; }
-__host__ __device__ inline int st_tile_cost(int type) { return st_type(type).rb / 2; }
+template <bool Q3 = true>
+__host__ __device__ inline int st_block_bytes(int type) { return ST_ROWS * st_type<Q3>(type).rb; }   // 1760 / 2304 / 2816 / 3360
+template <bool Q3 = true>
+__host__ __device__ inline int st_chunk_blocks(int type) { return st_type<Q3>(type).kb; }
+template <bool Q3 = true>
+__host__ __device__ inline int st_tile_cost(int type) { return st_type<Q3>(type).rb / 2; }
 // work items of a row of nb blocks (constant divisors)
+template <bool Q3 = true>
 __host__ __device__ inline int st_chunks(int type, int nb) {
-  constexpr int K4 = StTraits<GT_Q4_K>::KB, K5 = StTraits<GT_Q5_K>::KB, K6 = StTraits<GT_Q6_K>::KB;
+  constexpr int K3 = StTraits<GT_Q3_K>::KB, K4 = StTraits<GT_Q4_K>::KB, K5 = StTraits<GT_Q5_K>::KB, K6 = StTraits<GT_Q6_K>::KB;
+  if (Q3 && type == GT_Q3_K) return (nb + K3 - 1) / K3;
   return type == GT_Q4_K ? (nb + K4 - 1) / K4 : (type == GT_Q5_K ? (nb + K5 - 1) / K5 : (nb + K6 - 1) / K6);
 }
 __host__ __device__ inline size_t st_matrix_bytes(int type, int M, int nb) { return (size_t)((M + ST_ROWS - 1) / ST_ROWS) * nb * st_block_bytes(type); }
@@ -88,8 +99,21 @@ __host__ __device__ inline size_t st_matrix_bytes(int type, int M, int nb) { ret
 //   Q5_K  [0,2048)    as Q4_K;  [2048,2560) 4 B at ((h*2+rr)*32 + lane)*4: qh word l;  [2560,2816) headers      (k_quants.h:98-104)
 //   Q6_K  [0,2048)    16 B: ql words (half 0, v 0) (0,1) (1,0) (1,1) of AVX lane l;  [2048,3072) 8 B at ((h*2+rr)*32 + lane)*8: qh
 //         words of halves 0, 1;  [3072,3328) 16 int8 scales per row;  [3328,3360) fp16 d per row                (k_quants.h:112-117)
+//   Q3_K  [0,1024)    8 B at ((h*2+rr)*32 + lane)*8: qs words of halves 0, 1 of AVX lane l;  [1024,1536) 4 B at ((h*2+rr)*32 +
+//         lane)*4: hmask word l;  [1536,1728) the 12 scale bytes per row;  [1728,1760) fp16 d per row         (k_quants.h:55-61)
 // A warp-wide 16-byte load of one (h, rr) plane touches 512 consecutive bytes: conflict-free.  Rows >= M are zero blocks.
 __device__ __forceinline__ void st_decode(int type, int o, int& rl, int& src) {
+  if (type == GT_Q3_K) {   // raw block: hmask[32] qs[64] scales[12] d
+    if (o < 1536) {
+      const bool qs = o < 1024;
+      const int r = qs ? o : o - 1024, q = qs ? r >> 3 : r >> 2, hr = q >> 5, lane = q & 31, h = hr >> 1, rr = hr & 1, g = lane >> 2, t = lane & 3;
+      rl = rr * 8 + g;
+      src = (qs ? 32 + ((r >> 2) & 1) * 32 : 0) + 4 * (t + 4 * h) + (r & 3);
+      return;
+    }
+    if (o < 1728) { const int r = o - 1536; rl = r / 12; src = 96 + r % 12; return; }
+    rl = (o - 1728) >> 1; src = 108; return;
+  }
   const int q4 = (type == GT_Q6_K) ? 0 : (type == GT_Q5_K ? 48 : 16);   // raw offset of the 128 nibble bytes
   if (o < 2048) {
     const int q = o >> 4, hr = q >> 5, lane = q & 31, h = hr >> 1, rr = hr & 1, g = lane >> 2, t = lane & 3, l = t + 4 * h;
@@ -194,8 +218,9 @@ __device__ __forceinline__ void mma_u8s8(int (&d)[4], uint32_t a0, uint32_t a1, 
 // ---------------------------------------------------------------------------------------------
 // Activation vector in shared memory: the Q8_K image written by stage_activation (qs lane-major per block, d, bsums) plus
 //   pairs  per block 4 words: (bsums[4k]+bsums[4k+1]) | (bsums[4k+2]+bsums[4k+3]) << 16 — the operands of the Q4_K / Q5_K mins terms
-//   cneg   Q6_K phases: per block [t][group][c] int32 = -32 · Σ of the 4 activations of AVX lane l = 2t+c of 32-weight group
-//          `group`: the accumulator input that turns u·q8 into (u-32)·q8 (the AVX2 kernel subtracts maddubs(32, q8), k_quants.c:3829-3843)
+//   cneg   Q6_K / Q3_K phases: per block [t][group][c] int32 = -32 · Σ of the 4 activations of AVX lane l = 2t+c of 32-weight group
+//          `group`: the accumulator input that turns u·q8 into (u-32)·q8 (the AVX2 kernel subtracts maddubs(32, q8), k_quants.c:3829-3843);
+//          Q3_K takes cneg / 8, which turns u·q8 into (u-4)·q8
 struct StAct {
   const int8_t* qs;
   const float* d;
@@ -255,7 +280,7 @@ __device__ __forceinline__ int scale_fold8(int d0, int d1, int d2, int d3, int d
 
 // What one block contributes to this thread's share of the 16 rows: p[rr*2+c] = (float) of int32 lane l = 2t+c of row g+8rr;
 // dd[rr] = y.d·d; mins: Q4_K pm[rr] = mins lane k = t of row g+8rr (ddm[rr] = -y.d·dmin); Q5_K pm[0] = the scalar mins term of
-// row g+8(t&1) (ddm[0]); Q6_K none.
+// row g+8(t&1) (ddm[0]); Q3_K / Q6_K none.
 struct Terms { float p[4]; float pm[2]; float dd[2]; float ddm[2]; };
 
 __device__ __forceinline__ void load_b_operands(const StAct& a, int b, int g, int t, uint32_t (&bA)[8], uint32_t (&bB)[8]) {
@@ -411,6 +436,57 @@ __device__ __forceinline__ void block_terms<GT_Q6_K>(const uint8_t* blk, int b, 
   }
 }
 
+// k_quants.c:1950-2052.  The weight u = q3l | (hbit << 2) in [0, 7] is the u8 operand; the reference's value is u - 4, and the
+// -4 rides in as the accumulator input: -4 · Σ of the lane's 4 activations = cneg / 8 (exact: cneg is a multiple of 32).  Every
+// D fits int16 (|u - 4| <= 4, 4 products of |q8| <= 128), as scale_fold8 needs.
+template <>
+__device__ __forceinline__ void block_terms<GT_Q3_K>(const uint8_t* blk, int b, const StAct& a, int lane, Terms& r) {
+  const int g = lane >> 2, t = lane & 3;
+  const int2* qp = (const int2*)blk;
+  const uint32_t* hp = (const uint32_t*)(blk + 1024);
+  const int2 QS[4] = {qp[lane], qp[32 + lane], qp[64 + lane], qp[96 + lane]};   // index h*2+rr; words of halves 0, 1
+  const uint32_t HM[4] = {hp[lane], hp[32 + lane], hp[64 + lane], hp[96 + lane]};
+  const uint32_t* sp = (const uint32_t*)(blk + 1536);
+  const uint32_t sa[2][3] = {{sp[3 * g], sp[3 * g + 1], sp[3 * g + 2]}, {sp[3 * (8 + g)], sp[3 * (8 + g) + 1], sp[3 * (8 + g) + 2]}};
+  const uint16_t d0 = ((const uint16_t*)(blk + 1728))[g], d1 = ((const uint16_t*)(blk + 1728))[8 + g];
+  uint32_t bA[8], bB[8];
+  load_b_operands(a, b, g, t, bA, bB);
+  const int4* cp = (const int4*)(a.cneg + (b * 4 + t) * 16);   // [group][c] for this thread's two columns
+  const int4 cn[4] = {cp[0], cp[1], cp[2], cp[3]};
+  const int C[8][2] = {{cn[0].x, cn[0].y}, {cn[0].z, cn[0].w}, {cn[1].x, cn[1].y}, {cn[1].z, cn[1].w}, {cn[2].x, cn[2].y}, {cn[2].z, cn[2].w}, {cn[3].x, cn[3].y}, {cn[3].z, cn[3].w}};
+  int D[8][4];
+#pragma unroll
+  for (int grp = 0; grp < 8; grp++) {   // 32-weight group grp = 4j + k: bits 2k of qs word j, bit grp of the hmask byte
+    uint32_t u[4];
+#pragma unroll
+    for (int i = 0; i < 4; i++) {
+      const uint32_t q = (uint32_t)(grp < 4 ? QS[i].x : QS[i].y);
+      u[i] = ((q >> (2 * (grp & 3))) & 0x03030303u) | (((HM[i] >> grp) & 0x01010101u) << 2);
+    }
+    mma_u8s8(D[grp], u[0], u[1], u[2], u[3], bA[grp], bB[grp], C[grp][0] >> 3, C[grp][1] >> 3);
+  }
+  const float yd = a.d[b];
+  const int par = t >> 1;   // this thread's columns 2t, 2t+1 are AVX lanes of the first (par 0) or second (par 1) 16 weights of each group
+#pragma unroll
+  for (int rr = 0; rr < 2; rr++) {
+    // the 16 six-bit scales (k_quants.c:1968-1974), minus 32 per byte: word w holds sub-blocks 4w .. 4w+3
+    const uint32_t a0 = sa[rr][0], a1 = sa[rr][1], a2 = sa[rr][2];
+    const uint32_t w0 = __vsub4((a0 & 0x0f0f0f0fu) | ((a2 & 0x03030303u) << 4), 0x20202020u);
+    const uint32_t w1 = __vsub4((a1 & 0x0f0f0f0fu) | (((a2 >> 2) & 0x03030303u) << 4), 0x20202020u);
+    const uint32_t w2 = __vsub4(((a0 >> 4) & 0x0f0f0f0fu) | (((a2 >> 4) & 0x03030303u) << 4), 0x20202020u);
+    const uint32_t w3 = __vsub4(((a1 >> 4) & 0x0f0f0f0fu) | (((a2 >> 6) & 0x03030303u) << 4), 0x20202020u);
+    // scale of (group grp, par) = sub-block 2grp + par: S0 = groups 0..3, S1 = groups 4..7, as 4 signed bytes
+    const uint32_t sel = par ? 0x7531u : 0x6420u;
+    const uint32_t S0 = __byte_perm(w0, w1, sel), S1 = __byte_perm(w2, w3, sel);
+#pragma unroll
+    for (int c = 0; c < 2; c++) {
+      const int i = rr * 2 + c;
+      r.p[i] = (float)scale_fold8(D[0][i], D[1][i], D[2][i], D[3][i], D[4][i], D[5][i], D[6][i], D[7][i], S0, S1);
+    }
+    r.dd[rr] = __fmul_rn(yd, h2f(rr ? d1 : d0));
+  }
+}
+
 // One work item: blocks [b0, b0 + nblk) of the 16-row tile whose pieces lie in `slot`.  Integer work first (the slot is
 // released as soon as the last weight word has been read), then the ordered fp32 fold: state in from the mailbox unless this
 // is the tile's first chunk, blocks folded in order, state out unless it is the last chunk — then hsum_float_8 and the epilogue.
@@ -445,7 +521,7 @@ __device__ __forceinline__ void run_item(const uint8_t* slot, uint64_t* empty_ba
 #pragma unroll
   for (int i = 0; i < KB; i++) {
     if (i < nblk) {   // (a skipped block must not touch the accumulators: fma(0, 0, -0.0f) would flip a sign bit)
-      // one fmadd per block and AVX lane, blocks in order (k_quants.c:2706, 3253, 3864); mins: 2699-2701 (Q4_K), 3199-3201 (Q5_K)
+      // one fmadd per block and AVX lane, blocks in order (k_quants.c:2048, 2706, 3253, 3864); mins: 2699-2701 (Q4_K), 3199-3201 (Q5_K)
 #pragma unroll
       for (int q = 0; q < 4; q++) acc[q] = __fmaf_rn(tr[i].dd[q >> 1], tr[i].p[q], acc[q]);
 #pragma unroll
@@ -505,12 +581,13 @@ __device__ __forceinline__ void run_item(const uint8_t* slot, uint64_t* empty_ba
 struct TileSpace {
   int tiles[MV_MAX_SEG], cost[MV_MAX_SEG], nseg, ntiles;
   long total;   // Σ tiles·cost
+  template <bool Q3 = true>
   __host__ __device__ __forceinline__ void init(const MVParams& p) {
     nseg = p.nseg; ntiles = 0; total = 0;
 #pragma unroll
     for (int s = 0; s < MV_MAX_SEG; s++) {
       tiles[s] = s < p.nseg ? (p.seg[s].w.M + ST_ROWS - 1) / ST_ROWS : 0;
-      cost[s] = s < p.nseg ? st_tile_cost(p.seg[s].w.type) : 1;
+      cost[s] = s < p.nseg ? st_tile_cost<Q3>(p.seg[s].w.type) : 1;
       ntiles += tiles[s]; total += (long)tiles[s] * cost[s];
     }
   }
@@ -560,7 +637,7 @@ struct XchgParams {
 struct PickParams { const float* logits; int* state; int* out_tokens; int n; };
 struct alignas(16) Phase {
   int kind;
-  int q6;           // PH_MATVEC: some matrix of the phase is Q6_K (the activation staging then also builds cneg)
+  int q6;           // PH_MATVEC: some matrix of the phase is Q6_K or Q3_K (the activation staging then also builds cneg)
                     // PH_ATTN: 1 = cached K / V travel through the ring (st_attn_ring_ok), 0 = read from global memory (attn_body)
   MVParams mv;      // PH_MATVEC
   AttnParams at;    // PH_ATTN
@@ -592,6 +669,7 @@ __device__ __forceinline__ unsigned ld_acquire_u32(const unsigned* p) {
 
 // what lane j knows about tile T0 + j of this CTA's range
 struct TileInfo { int seg, til, nch, type; };
+template <bool Q3>
 __device__ __forceinline__ TileInfo tile_info(const TileSpace& ts, const MVParams& p, int tile, int nb, bool valid) {
   TileInfo ti;
   ti.seg = 0; ti.til = 0; ti.nch = 0; ti.type = GT_Q4_K;
@@ -600,15 +678,16 @@ __device__ __forceinline__ TileInfo tile_info(const TileSpace& ts, const MVParam
     ti.seg = ts.locate(tl);
     ti.til = tl;
     ti.type = ti.seg == 0 ? p.seg[0].w.type : (ti.seg == 1 ? p.seg[1].w.type : p.seg[2].w.type);
-    ti.nch = st_chunks(ti.type, nb);
+    ti.nch = st_chunks<Q3>(ti.type, nb);
   }
   return ti;
 }
 
 // source and bytes of work item (chunk kc of tile til) of segment seg, whose type is `type`
 struct StItem { const uint8_t* src; uint32_t bytes; };
+template <bool Q3>
 __device__ __forceinline__ StItem st_item(const MVParams& p, int seg, int type, int til, int kc, int nb) {
-  const int kb = st_chunk_blocks(type), bb = st_block_bytes(type);
+  const int kb = st_chunk_blocks<Q3>(type), bb = st_block_bytes<Q3>(type);
   const int nblk = min(kb, nb - kc * kb);
   const uint8_t* base = seg == 0 ? p.seg[0].w.st : (seg == 1 ? p.seg[1].w.st : p.seg[2].w.st);
   return {base + ((size_t)til * nb + (size_t)kc * kb) * bb, (uint32_t)(nblk * bb)};
@@ -744,6 +823,8 @@ __device__ __forceinline__ void st_attn_phase(const Phase& ph, uint8_t* act_smem
     }
   }
 }
+// (one copy per kernel build, Q3: ptxas fits an out-of-line function's registers to all its callers at once)
+template <bool Q3>
 static __device__ __noinline__ uint32_t st_attn_phase_gen(const Phase& ph, uint8_t* act_smem, uint8_t* ring, uint64_t* full_bar, uint64_t* empty_bar, int n_slots,
                                                    uint32_t seq, float* pick_v, double* red) {
   st_attn_phase<true>(ph, act_smem, ring, full_bar, empty_bar, n_slots, seq, pick_v, red);
@@ -754,7 +835,7 @@ static __device__ __noinline__ uint32_t st_attn_phase_gen(const Phase& ph, uint8
 // copies read with an L2 evict-first policy: a weight line is dead once its ring copy has read it (the next read is a step
 // later, 4 GB of stream away), so the stream's lines go first and the step's live data (KV cache, activation vectors, exp
 // table) stays in L2.  K / V items keep the default policy.
-template <bool XC, bool GEN>
+template <bool XC, bool GEN, bool Q3>
 __device__ __forceinline__ void st_producer(const StepArgs& args, uint8_t* ring, uint64_t* full_bar, uint64_t* empty_bar) {
   const int lane = threadIdx.x & 31;
   const uint32_t S = (uint32_t)(args.n_slots / ST_W);   // ring depth per consumer warp
@@ -772,13 +853,13 @@ __device__ __forceinline__ void st_producer(const StepArgs& args, uint8_t* ring,
     if (ph->kind != PH_MATVEC) continue;
     const MVParams& p = ph->mv;
     TileSpace ts;
-    ts.init(p);
+    ts.init<Q3>(p);
     const int* bnd = args.bounds + (size_t)ip * (gridDim.x + 1) + blockIdx.x;
     const int T0 = __ldg(bnd), T1 = __ldg(bnd + 1);
     const int nb = p.K >> 8;
     for (int w0 = T0; w0 < T1; w0 += ST_MAXT) {
       const int ntw = min(ST_MAXT, T1 - w0);
-      const TileInfo ti = tile_info(ts, p, w0 + lane, nb, lane < ntw);
+      const TileInfo ti = tile_info<Q3>(ts, p, w0 + lane, nb, lane < ntw);
       for (int kc = 0;; kc++) {
         const unsigned mask = __ballot_sync(0xffffffffu, kc < ti.nch);
         if (!mask) break;
@@ -791,7 +872,7 @@ __device__ __forceinline__ void st_producer(const StepArgs& args, uint8_t* ring,
           if (((mask >> lane) & 1u) && rank >= base && rank < base + ST_W * (int)S) {
             const uint32_t n = seq + (uint32_t)rank;
             const RingPos rp = st_ring(n, S);
-            const StItem it = st_item(p, ti.seg, ti.type, ti.til, kc, nb);
+            const StItem it = st_item<Q3>(p, ti.seg, ti.type, ti.til, kc, nb);
             mbar_wait(&empty_bar[rp.slot], rp.parity ^ 1u, W_FREE_WEIGHT_SLOT, (int)n);
             mbar_expect_tx(&full_bar[rp.slot], it.bytes);
             bulk_g2s_hint(ring + (size_t)rp.slot * ST_SLOT, it.src, it.bytes, &full_bar[rp.slot], weight_pol);
@@ -807,8 +888,8 @@ __device__ __forceinline__ void st_producer(const StepArgs& args, uint8_t* ring,
 
 // Consumer side of one mat-vec phase.  `seq` is the running item number (identical in every warp and in the producer).
 // XC: the build of the kernel that can exchange partial vectors between ranks (tensor-parallel mode); the single-GPU build
-// carries none of that code.
-template <bool XC>
+// carries none of that code.  Q3: the build for programs that hold Q3_K matrices (the others carry none of its code).
+template <bool XC, bool Q3>
 __device__ __forceinline__ void st_matvec_phase(const Phase& ph, const NormPre& np, uint8_t* ring, uint8_t* act_smem, double* red, uint64_t* full_bar, uint64_t* empty_bar,
                                                 float (*mailbox)[ST_STATE * 32], int* flags, uint32_t S, uint32_t& seq, const int* tb, unsigned long long* tr,
                                                 unsigned xc_base) {
@@ -822,7 +903,7 @@ __device__ __forceinline__ void st_matvec_phase(const Phase& ph, const NormPre& 
   if (tr && threadIdx.x == 0) tr[1] = globaltimer_ns();
   bool first_item = tr != nullptr && threadIdx.x == 0;
   TileSpace ts;
-  ts.init(p);
+  ts.init<Q3>(p);
   const int nb = p.K >> 8;
   const int T0 = tb[0], T1 = tb[1];
 #pragma unroll 1
@@ -833,7 +914,7 @@ __device__ __forceinline__ void st_matvec_phase(const Phase& ph, const NormPre& 
       bar_sync<ST_BAR, ST_NT>();
     }
     const int ntw = min(ST_MAXT, T1 - w0);
-    const TileInfo ti = tile_info(ts, p, w0 + lane, nb, lane < ntw);
+    const TileInfo ti = tile_info<Q3>(ts, p, w0 + lane, nb, lane < ntw);
 #pragma unroll 1
     for (int kc = 0;; kc++) {
       const unsigned mask = __ballot_sync(0xffffffffu, kc < ti.nch);
@@ -848,7 +929,7 @@ __device__ __forceinline__ void st_matvec_phase(const Phase& ph, const NormPre& 
         const int nch = __shfl_sync(0xffffffffu, ti.nch, j);
         const uint32_t n = seq + (uint32_t)r;
         const RingPos rp = st_ring(n, S);
-        const int kb = st_chunk_blocks(type);
+        const int kb = st_chunk_blocks<Q3>(type);
         const int b0 = kc * kb, nblk = min(kb, nb - b0);
         const MVSeg& sg = p.seg[seg];
         const uint8_t* sp = ring + (size_t)rp.slot * ST_SLOT;
@@ -859,6 +940,7 @@ __device__ __forceinline__ void st_matvec_phase(const Phase& ph, const NormPre& 
         const bool last = kc == nch - 1;
         if (type == GT_Q4_K) run_item<GT_Q4_K, XC>(sp, &empty_bar[rp.slot], nblk, b0, kc, last, a, lane, mail, flag, sg, p, til * ST_ROWS);
         else if (type == GT_Q6_K) run_item<GT_Q6_K, XC>(sp, &empty_bar[rp.slot], nblk, b0, kc, last, a, lane, mail, flag, sg, p, til * ST_ROWS);
+        else if (Q3 && type == GT_Q3_K) run_item<GT_Q3_K, XC>(sp, &empty_bar[rp.slot], nblk, b0, kc, last, a, lane, mail, flag, sg, p, til * ST_ROWS);
         else run_item<GT_Q5_K, XC>(sp, &empty_bar[rp.slot], nblk, b0, kc, last, a, lane, mail, flag, sg, p, til * ST_ROWS);
       }
       seq += (uint32_t)cnt;
@@ -893,8 +975,10 @@ __device__ __forceinline__ void grid_rearm(unsigned* sync, bool set_xc = false, 
 
 // GEN: the program's attention phases have a head size other than 64 / 128 (attn_fast_hd); they run in one out-of-line call,
 // and the kernels of the other models (GEN = false) have no trace of them.  The tensor-sharded mode takes heads of 64 / 128
-// only, so there is no exchange kernel with GEN.
-template <bool XC, bool GEN>
+// only, so there is no exchange kernel with GEN.  Q3: some phase of the program holds a Q3_K matrix or embedding table.  The
+// builds without it compile to the same instructions as before Q3_K was added; with the Q3_K code inlined into every build,
+// ptxas spilled more in the builds of the other models (DESIGN.md §6).
+template <bool XC, bool GEN, bool Q3>
 static __global__ void __launch_bounds__(ST_THREADS, 1) k_step(const __grid_constant__ StepArgs args) {
   extern __shared__ __align__(16) uint8_t smem[];
   __shared__ __align__(8) uint64_t full_bar[ST_MAX_SLOTS];
@@ -913,7 +997,7 @@ static __global__ void __launch_bounds__(ST_THREADS, 1) k_step(const __grid_cons
   pdl_trigger();
   pdl_wait();           // (the producer reads device state too: the position decides how many K / V items an attention phase has)
   if (warp == ST_W) {
-    st_producer<XC, GEN>(args, ring, full_bar, empty_bar);
+    st_producer<XC, GEN, Q3>(args, ring, full_bar, empty_bar);
     return;
   }
   const unsigned G = gridDim.x;
@@ -958,12 +1042,12 @@ static __global__ void __launch_bounds__(ST_THREADS, 1) k_step(const __grid_cons
     if (XC && ph.kind == PH_MATVEC && ph.xc.role == 1) xc_done++;
     if (ph.kind == PH_MATVEC) {
       // (the tile bounds were written by threads 0/1 above; the barriers inside the activation staging order them)
-      st_matvec_phase<XC>(ph, np, ring, act_smem, red, full_bar, empty_bar, mailbox, flags, (uint32_t)(args.n_slots / ST_W), seq, &tb_s[ip & 1][0], tr, xc_base);
+      st_matvec_phase<XC, Q3>(ph, np, ring, act_smem, red, full_bar, empty_bar, mailbox, flags, (uint32_t)(args.n_slots / ST_W), seq, &tb_s[ip & 1][0], tr, xc_base);
     } else if (ph.kind == PH_ATTN) {
-      if (GEN) seq = st_attn_phase_gen(ph, act_smem, ring, full_bar, empty_bar, args.n_slots, seq, pick_v, red);
+      if (GEN) seq = st_attn_phase_gen<Q3>(ph, act_smem, ring, full_bar, empty_bar, args.n_slots, seq, pick_v, red);
       else st_attn_phase<false>(ph, act_smem, ring, full_bar, empty_bar, args.n_slots, seq, pick_v, red);
     } else if (ph.kind == PH_EMBED) {
-      if (blockIdx.x == 0) embed_row(ph.em, ph.em.tokens[0], ph.em.out, threadIdx.x, ST_NT);
+      if (blockIdx.x == 0) embed_row<Q3>(ph.em, ph.em.tokens[0], ph.em.out, threadIdx.x, ST_NT);
     } else if (ph.kind == PH_PICK) {
       if (blockIdx.x == 0) st_pick_phase(ph.pk, pick_v, pick_i);
     }
@@ -978,7 +1062,7 @@ static __global__ void __launch_bounds__(ST_THREADS, 1) k_step(const __grid_cons
 
 // ---------------------------------------------------------------------------------------------
 // Host side
-struct StepLaunch { int grid; int n_slots; size_t smem; bool gen = false; /* k_step<.., true>: see k_step */ };
+struct StepLaunch { int grid; int n_slots; size_t smem; bool gen = false, q3 = false; /* k_step<.., GEN, Q3>: see k_step */ };
 
 // shared-memory budget: ring slots fill what the largest activation image of the program leaves
 inline StepLaunch step_launch_shape(const Phase* phases, int n, int n_sm, size_t max_dyn_smem, size_t extra_act = 0) {
@@ -987,12 +1071,18 @@ inline StepLaunch step_launch_shape(const Phase* phases, int n, int n_sm, size_t
     if (phases[i].kind == PH_MATVEC) act = std::max(act, st_act_bytes(phases[i].mv.K, phases[i].q6 != 0));
     if (phases[i].kind == PH_ATTN) act = std::max(act, attn_smem_bytes(phases[i].at.n_ctx, phases[i].at.hd));
   }
-  bool gen = false;
-  for (int i = 0; i < n; i++) gen |= phases[i].kind == PH_ATTN && !attn_fast_hd(phases[i].at.hd);
+  bool gen = false, q3 = false;
+  for (int i = 0; i < n; i++) {
+    gen |= phases[i].kind == PH_ATTN && !attn_fast_hd(phases[i].at.hd);
+    if (phases[i].kind == PH_MATVEC)
+      for (int s = 0; s < phases[i].mv.nseg; s++) q3 |= phases[i].mv.seg[s].w.type == GT_Q3_K;
+    q3 |= phases[i].kind == PH_EMBED && phases[i].em.type == GT_Q3_K;
+  }
   act = (act + 127) & ~(size_t)127;
   StepLaunch L;
   L.grid = n_sm;
   L.gen = gen;
+  L.q3 = q3;
   if (act + (size_t)ST_W * ST_SLOT > max_dyn_smem) { L.n_slots = 0; L.smem = 0; return L; }
   L.n_slots = ST_W * (int)std::min<size_t>(ST_MAX_DEPTH, (max_dyn_smem - act) / ((size_t)ST_W * ST_SLOT));   // whole sub-rings only
   L.smem = (size_t)L.n_slots * ST_SLOT + act;
@@ -1027,23 +1117,29 @@ inline Phase matvec_phase(const MVParams& p) {
   ph.kind = PH_MATVEC;
   ph.mv = p;
   ph.mv.act = ACT_Q8_K;
-  for (int s = 0; s < p.nseg; s++) ph.q6 |= p.seg[s].w.type == GT_Q6_K;
+  for (int s = 0; s < p.nseg; s++) ph.q6 |= p.seg[s].w.type == GT_Q6_K || p.seg[s].w.type == GT_Q3_K;
   return ph;
 }
 
 // point the kernels' watchdog at 4 ints of host-mapped memory (each translation unit has its own copy of the symbol)
 static inline cudaError_t st_set_debug_words(int* dev_ptr) { return cudaMemcpyToSymbol(g_st_dbg, &dev_ptr, sizeof(int*)); }
 static inline cudaError_t step_set_smem_limit(size_t bytes) {
-  cudaError_t e = cudaFuncSetAttribute(k_step<false, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes);
-  if (e == cudaSuccess) e = cudaFuncSetAttribute(k_step<false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes);
-  return e != cudaSuccess ? e : cudaFuncSetAttribute(k_step<true, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes);
+  void (*const kernels[])(StepArgs) = {k_step<false, false, false>, k_step<false, true, false>, k_step<true, false, false>,
+                                        k_step<false, false, true>, k_step<false, true, true>, k_step<true, false, true>};
+  for (auto k : kernels) {
+    const cudaError_t e = cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes);
+    if (e != cudaSuccess) return e;
+  }
+  return cudaSuccess;
 }
 
 static inline cudaError_t launch_step(const StepLaunch& L, cudaStream_t st, const Phase* d_prog, const int* d_bounds, int n_phases, unsigned* d_sync, bool pdl = false,
                                       unsigned long long* trace = nullptr, bool xchg = false) {
   StepArgs a;
   a.prog = d_prog; a.bounds = d_bounds; a.n_phases = n_phases; a.n_slots = L.n_slots; a.sync = d_sync; a.trace = trace;
-  return launch_kernel(xchg ? k_step<true, false> : (L.gen ? k_step<false, true> : k_step<false, false>), dim3(L.grid), dim3(ST_THREADS), L.smem, st, pdl, a);
+  auto kernel = L.q3 ? (xchg ? k_step<true, false, true> : (L.gen ? k_step<false, true, true> : k_step<false, false, true>))
+                     : (xchg ? k_step<true, false, false> : (L.gen ? k_step<false, true, false> : k_step<false, false, false>));
+  return launch_kernel(kernel, dim3(L.grid), dim3(ST_THREADS), L.smem, st, pdl, a);
 }
 
 }  // namespace ctb

@@ -118,7 +118,7 @@ int ctb_sample(const float* logits, int n_vocab, const int* last_tokens, int n_l
                float repetition_penalty, int seed);
 
 /* Op-level mirrors (host pointers in, host pointers out; return 0 on success).  ggml type ids: 0 F32, 1 F16,
- * 2 Q4_0, 3 Q4_1, 6 Q5_0, 7 Q5_1, 8 Q8_0, 12 Q4_K, 13 Q5_K, 14 Q6_K (models/ggml/ggml.h enum ggml_type). */
+ * 2 Q4_0, 3 Q4_1, 6 Q5_0, 7 Q5_1, 8 Q8_0, 11 Q3_K, 12 Q4_K, 13 Q5_K, 14 Q6_K (models/ggml/ggml.h enum ggml_type). */
 /* ggml_mul_mat for quantized src0 (ggml.c:11031-11245): dst[n*M+m] = dot(W row m, quantize(x col n)). */
 int ctb_mul_mat(int type, const void* w_blocks, const float* x, float* dst, int K, int M, int N);
 /* quantize_row_q8_K (k_quants.c:1191-1241) / quantize_row_q8_0 (ggml.c:1232-1268): reference block bytes out. */
@@ -166,12 +166,12 @@ int ctb_attention_path(int path, const float* q, const float* k_new, const float
  *   input  row i of x [n_tok][K]; x2 non-null: x * x2 (ggml_mul, the down projection's silu(gate) * up); norm_mode 1 RMSNorm * w,
  *          2 LayerNorm * w + b (norm_w / norm_b [K], eps; a mode ignores what it does not use), 0 none (required with x2); then
  *          quantize_row_q8_K
- *   rows   nseg (1..3) K-quant matrices (types[s] 12 Q4_K, 13 Q5_K, 14 Q6_K; w_blocks[s]: rows[s] rows of K weights in the
+ *   rows   nseg (1..3) K-quant matrices (types[s] 11 Q3_K, 12 Q4_K, 13 Q5_K, 14 Q6_K; w_blocks[s]: rows[s] rows of K weights in the
  *          reference's block layout) whose outputs sit side by side: out [n_tok][W], W = rows[0] + .. + rows[nseg-1]
  *   epi[s] 0 STORE v, 1 ADD v + res, 3 ADD2 (v + res) + res2, 2 GELU / 4 SILU: the fp16 table of v (ggml.c:3600-3632);
  *          res / res2 [n_tok][W] in out's layout, read only by the segments that add them
  * *n_slots (if non-null) gets the ring slots used.  0 on success, -1 (with a message on stderr) for what the kernel cannot take: a
- * type other than Q4_K / Q5_K / Q6_K, K not a multiple of 256, more than 3 segments, n_tok < 1, or an n_ctx whose attention
+ * type other than Q3_K / Q4_K / Q5_K / Q6_K, K not a multiple of 256, more than 3 segments, n_tok < 1, or an n_ctx whose attention
  * scratch leaves no ring (the engine then has no batched prefill). */
 int ctb_prefill_mul_mat(int nseg, const int* types, const void* const* w_blocks, const int* rows, int K, int n_tok, const float* x,
                         const float* x2, int norm_mode, const float* norm_w, const float* norm_b, float eps, const int* epi,
@@ -182,7 +182,7 @@ int ctb_ffn_gate(int type, const void* w1_blocks, const void* w3_blocks, const f
 /* How a K-quant mat-vec phase over nseg matrices (types[], rows[], all K wide) is cut up on a GPU with n_sm SMs — pure host
  * arithmetic, no device needed: first_tile[0..grid] = first 16-row tile of each CTA (byte-balanced), meta = {grid, ring slot
  * bytes, tiles alive per CTA (mailboxes), tiles, consumer warps per CTA, rows per tile, work items of the largest CTA,
- * blocks per work item as Q4_K | Q5_K << 8 | Q6_K << 16}.  0 on success. */
+ * blocks per work item as Q4_K | Q5_K << 8 | Q6_K << 16 | Q3_K << 24}.  0 on success. */
 int ctb_matvec_partition(const int* types, const int* rows, int nseg, int K, int n_sm, int* first_tile, int* meta);
 
 int ctb_get_row(int type, const void* table_blocks, int K, int n_rows, int row, float* out);
