@@ -75,12 +75,26 @@ struct PrefillState {
   size_t smem = 0;
   bool q3 = false;                  // the program holds Q3_K matrices (k_pstep<true>)
   bool ok = false, tried = false;
+  // multi-sequence mode (HParams::n_seq > 1): the same program on slot-addressed state (k_pstep<.., true>), plus the output head
+  PPhase* d_mprog = nullptr;
+  int n_mphases = 0;
+  bool mq3 = false;
+  int* d_mstate = nullptr;          // PB_STATE_MS ints
+  int* h_mstate = nullptr;          // pinned, PF_RING launches deep
+  int mh_next = 0;
+  bool mhead = false;               // K-quant head: its QUANT + GEMM phases end the launch, every token's row in logits_b / embd_b
+  float *logits_b = nullptr, *embd_b = nullptr;
+  float *d_mlogits = nullptr, *d_membd = nullptr;   // [n_seq][n_vocab], [n_seq][n_embd]: each slot's last results
+  int* d_mpick = nullptr;                           // [n_seq][2]: k_argmax of each slot's logits
+  long m_launches = 0;
   ~PrefillState() {
     for (void* b : bufs) cudaFree(b);
     if (h_state) cudaFreeHost(h_state);
+    if (h_mstate) cudaFreeHost(h_mstate);
   }
 };
 constexpr int PF_RING = 64;
+static_assert(MULTI_LAUNCH_TOKENS == PB_T, "multi_pack cuts launches of PB_T tokens");
 
 constexpr size_t UP_CHUNK = (size_t)32 << 20;   // upload pipeline: chunk bytes and buffers in flight
 constexpr int UP_BUFS = 3;
@@ -98,7 +112,7 @@ size_t engine_arena_bytes(const GGUFFile& g, const HParams& hp) {
   }
   total += UP_CHUNK * UP_BUFS + 256;                                            // device staging of the upload pipeline
   const size_t kv = (size_t)hp.n_layer * (hp.n_ctx + 256) * hp.n_head_kv * k_stride(hp.head_dim()) * 2;   // K rows padded to 8 halves
-  total += 2 * align_up(kv, 256);
+  total += 2 * align_up(kv * hp.n_seq, 256);
   total += 3 * align_up(65536 * 2, 256);
   total += align_up((size_t)hp.n_ctx * (hp.head_dim() / 2) * 8, 256);
   const size_t qkv = (size_t)hp.n_embd + 2 * (size_t)hp.n_embd_gqa();
@@ -368,10 +382,10 @@ void Engine::init(const GGUFFile& g) {
   const size_t gqa_l = (size_t)nkv_ * hp_.head_dim(), qw_l = (size_t)nh_ * hp_.head_dim();   // this rank's K/V and Q widths
   const size_t kv = (size_t)hp_.n_layer * hp_.n_ctx * nkv_ * k_stride(hp_.head_dim());   // K rows padded to 8 halves (attention.cuh)
   const size_t vv = (size_t)hp_.n_layer * kv_ctx_pad(hp_.n_ctx) * gqa_l;
-  kc_ = (uint16_t*)alloc(kv * 2);
-  vc_ = (uint16_t*)alloc(vv * 2);
-  CTB_CUDA(cudaMemset(kc_, 0, kv * 2));
-  CTB_CUDA(cudaMemset(vc_, 0, vv * 2));
+  kc_ = (uint16_t*)alloc(kv * 2 * hp_.n_seq);   // [slot][layer]...: slot 0 is the single-sequence cache
+  vc_ = (uint16_t*)alloc(vv * 2 * hp_.n_seq);
+  CTB_CUDA(cudaMemset(kc_, 0, kv * 2 * hp_.n_seq));
+  CTB_CUDA(cudaMemset(vc_, 0, vv * 2 * hp_.n_seq));
   const size_t qkv = qw_l + 2 * gqa_l;
   d_state_ = (int*)alloc(64);
   xa_ = (float*)alloc(hp_.n_embd * 4); xb_ = (float*)alloc(hp_.n_embd * 4);
@@ -1106,7 +1120,7 @@ void Engine::eval_list(const int* tokens, const int* pos, const int* n_total, in
 }
 
 bool Engine::ensure_prefill() {
-  if (!prefill_on_ || tp_.world > 1) return false;
+  if ((!prefill_on_ && hp_.n_seq == 1) || tp_.world > 1) return false;   // (multi-sequence evals have no other path)
   if (pf_ && pf_->tried) return pf_->ok;
   if (!pf_) pf_ = new PrefillState();
   PrefillState& P = *pf_;
@@ -1167,6 +1181,28 @@ bool Engine::ensure_prefill() {
   P.q3 = pstep_q3(prog);
   P.d_prog = (PPhase*)dalloc((prog.size() + 1) * sizeof(PPhase));
   CTB_CUDA(cudaMemcpy(P.d_prog, prog.data(), prog.size() * sizeof(PPhase), cudaMemcpyHostToDevice));
+  if (hp_.n_seq > 1) {
+    P.d_mstate = (int*)dalloc(PB_STATE_MS * 4);
+    CTB_CUDA(cudaMallocHost(&P.h_mstate, (size_t)PF_RING * PB_STATE_MS * 4));
+    std::vector<PPhase> mprog = prog;
+    for (PPhase& ph : mprog) { ph.state = P.d_mstate; ph.at.state = P.d_mstate; }
+    const StepOp& head = ops_[n_body_];
+    P.mhead = head.stream;
+    if (P.mhead) {   // the final norm (written as every token's embeddings) and the output matrix over every token of the launch
+      add(d_logits_, hp_.n_vocab); add(d_embd_, n_embd);
+      pb_matvec_phases(head.ph.mv, (uint8_t*)dalloc(pb_qbuf_bytes(head.ph.mv.K)), P.d_mstate, bat, mprog);
+      P.logits_b = bat(d_logits_, ld);
+      P.embd_b = bat(d_embd_, ld);
+      mprog[mprog.size() - 2].mv.norm_out = P.embd_b;
+    }
+    P.n_mphases = (int)mprog.size();
+    P.mq3 = pstep_q3(mprog);
+    P.d_mprog = (PPhase*)dalloc((mprog.size() + 1) * sizeof(PPhase));
+    CTB_CUDA(cudaMemcpy(P.d_mprog, mprog.data(), mprog.size() * sizeof(PPhase), cudaMemcpyHostToDevice));
+    P.d_mlogits = (float*)dalloc((size_t)hp_.n_seq * hp_.n_vocab * 4);
+    P.d_membd = (float*)dalloc((size_t)hp_.n_seq * n_embd * 4);
+    P.d_mpick = (int*)dalloc((size_t)hp_.n_seq * 8);
+  }
   if (!pstep_shape(pb_work_bytes(K_max, hp_.n_ctx, hp_.head_dim()), P.n_slots, P.smem)) return false;
   CTB_CUDA(pstep_set_smem_limit(P.smem));
   P.ok = true;
@@ -1187,18 +1223,103 @@ void Engine::prefill_batch(const int* tokens, const int* pos, const int* n_total
   CTB_CUDA(cudaMemcpyAsync(P.d_state, st, (PB_T * 4 + 4) * 4, cudaMemcpyHostToDevice, stream_));
   CTB_CUDA(launch_pstep(step_grid_, P.n_slots, P.smem, stream_, P.d_prog, P.n_phases, d_sync_, P.q3));
   prefill_launches_++;
-  if (last) {
-    const StepOp& head = ops_[n_body_];
-    CTB_CUDA(cudaMemcpyAsync(const_cast<float*>(head.ph.mv.x), P.x_final + (size_t)(n - 1) * hp_.n_embd, (size_t)hp_.n_embd * 4, cudaMemcpyDeviceToDevice, stream_));
-    const bool keep = fused_;
-    fused_ = false;                                    // just this one op, the way the un-fused schedule launches it
-    std::vector<StepOp> one(1, head);
-    const long keepl = launches_per_step_;
-    try { enqueue_ops(one, d_prog_ + n_body_, d_bounds_ + (size_t)n_body_ * (sm_count_ + 1), 1); } catch (...) { fused_ = keep; throw; }
-    fused_ = keep;
-    launches_per_step_ = keepl;
-  }
+  if (last) head_from(P.x_final + (size_t)(n - 1) * hp_.n_embd);
 }
+
+void Engine::head_from(const float* row) {
+  const StepOp& head = ops_[n_body_];
+  CTB_CUDA(cudaMemcpyAsync(const_cast<float*>(head.ph.mv.x), row, (size_t)hp_.n_embd * 4, cudaMemcpyDeviceToDevice, stream_));
+  const bool keep = fused_;
+  fused_ = false;                                    // just this one op, the way the un-fused schedule launches it
+  std::vector<StepOp> one(1, head);
+  const long keepl = launches_per_step_;
+  try { enqueue_ops(one, d_prog_ + n_body_, d_bounds_ + (size_t)n_body_ * (sm_count_ + 1), 1); } catch (...) { fused_ = keep; throw; }
+  fused_ = keep;
+  launches_per_step_ = keepl;
+}
+
+// ---- multi-sequence mode
+std::string Engine::multi_refusal() {
+  if (tp_.world > 1) return "the tensor-sharded mode";
+  for (int i = 0; i < n_body_; i++)
+    if (ops_[i].ph.kind == PH_MATVEC && !ops_[i].stream) return "layer matrices that are not K-quants (Q3_K / Q4_K / Q5_K / Q6_K)";
+  DeviceGuard dev_guard(device_);
+  if (!ensure_prefill() || !pf_->d_mprog) return "a context of " + std::to_string(hp_.n_ctx) + " (the batched kernel's attention scratch does not fit in shared memory)";
+  return "";
+}
+
+void Engine::multi_eval(const std::vector<MultiTok>& toks, const std::vector<int>& starts) {
+  DeviceGuard dev_guard(device_);
+  if (hp_.n_seq < 2 || !ensure_prefill() || !pf_->d_mprog) throw std::runtime_error("this engine has no multi-sequence path");
+  PrefillState& P = *pf_;
+  const int hd = hp_.head_dim(), n_embd = hp_.n_embd, n_vocab = hp_.n_vocab;
+  const size_t kslot = (size_t)hp_.n_layer * hp_.n_ctx * nkv_ * k_stride(hd), vslot = (size_t)hp_.n_layer * kv_ctx_pad(hp_.n_ctx) * nkv_ * hd;
+  if (kslot > 0xffffffffu || vslot > 0xffffffffu) throw std::runtime_error("multi-sequence: a slot's KV region is too large");
+  CTB_CUDA(cudaEventRecord(ev0_, stream_));
+  for (size_t l = 0; l + 1 < starts.size(); l++) {
+    const int a = starts[l], n = starts[l + 1] - a;
+    if (n < 1 || n > PB_T) throw std::runtime_error("multi-sequence: bad launch size");
+    if (P.mh_next % PF_RING == PF_RING - 1) CTB_CUDA(cudaStreamSynchronize(stream_));   // pinned state ring
+    int* st = P.h_mstate + (size_t)(P.mh_next++ % PF_RING) * PB_STATE_MS;
+    for (int i = 0; i < PB_T; i++) {
+      const MultiTok& t = toks[a + std::min(i, n - 1)];
+      st[i * 4] = t.token; st[i * 4 + 1] = t.pos; st[i * 4 + 2] = 0; st[i * 4 + 3] = t.n_total;
+      st[PB_S + i] = t.slot;
+    }
+    st[PB_T * 4] = n; st[PB_T * 4 + 1] = (int)(unsigned)kslot; st[PB_T * 4 + 2] = (int)(unsigned)vslot; st[PB_T * 4 + 3] = 0;
+    CTB_CUDA(cudaMemcpyAsync(P.d_mstate, st, PB_STATE_MS * 4, cudaMemcpyHostToDevice, stream_));
+    CTB_CUDA(launch_pstep(step_grid_, P.n_slots, P.smem, stream_, P.d_mprog, P.n_mphases, d_sync_, P.mq3, true));
+    P.m_launches++;
+    for (int r = 0; r < n; r++) {
+      const MultiTok& t = toks[a + r];
+      if (!t.last) continue;   // (its logits, if the launch computed them, are dropped)
+      float* lg = P.d_mlogits + (size_t)t.slot * n_vocab;
+      float* em = P.d_membd + (size_t)t.slot * n_embd;
+      const float* lsrc = d_logits_;
+      const float* esrc = d_embd_;
+      if (P.mhead) {
+        lsrc = P.logits_b + (size_t)r * n_vocab;
+        esrc = P.embd_b + (size_t)r * n_embd;
+      } else {
+        head_from(P.x_final + (size_t)r * n_embd);   // a head that is not a K-quant: k_matvec, one row at a time
+      }
+      CTB_CUDA(cudaMemcpyAsync(lg, lsrc, (size_t)n_vocab * 4, cudaMemcpyDeviceToDevice, stream_));
+      CTB_CUDA(cudaMemcpyAsync(em, esrc, (size_t)n_embd * 4, cudaMemcpyDeviceToDevice, stream_));
+      k_argmax<<<1, ARGMAX_THREADS, 0, stream_>>>(lg, n_vocab, P.d_mpick + 2 * t.slot);
+      CTB_CUDA(cudaGetLastError());
+    }
+  }
+  CTB_CUDA(cudaEventRecord(ev1_, stream_));
+  CTB_CUDA(cudaEventSynchronize(ev1_));
+  float ms = 0;
+  cudaEventElapsedTime(&ms, ev0_, ev1_);
+  stats.last_eval_ms = ms;
+}
+
+void Engine::multi_fetch(int slot, float* logits, float* embd) {
+  DeviceGuard dev_guard(device_);
+  PrefillState& P = *pf_;
+  CTB_CUDA(cudaMemcpyAsync(logits, P.d_mlogits + (size_t)slot * hp_.n_vocab, (size_t)hp_.n_vocab * 4, cudaMemcpyDeviceToHost, stream_));
+  CTB_CUDA(cudaMemcpyAsync(embd, P.d_membd + (size_t)slot * hp_.n_embd, (size_t)hp_.n_embd * 4, cudaMemcpyDeviceToHost, stream_));
+  CTB_CUDA(cudaStreamSynchronize(stream_));
+}
+
+void Engine::multi_pick(int slot, int* out2) {
+  DeviceGuard dev_guard(device_);
+  CTB_CUDA(cudaMemcpyAsync(out2, pf_->d_mpick + 2 * slot, 8, cudaMemcpyDeviceToHost, stream_));
+  CTB_CUDA(cudaStreamSynchronize(stream_));
+}
+
+void Engine::multi_reset(int slot) {
+  DeviceGuard dev_guard(device_);
+  const int hd = hp_.head_dim();
+  const size_t kslot = (size_t)hp_.n_layer * hp_.n_ctx * nkv_ * k_stride(hd), vslot = (size_t)hp_.n_layer * kv_ctx_pad(hp_.n_ctx) * nkv_ * hd;
+  CTB_CUDA(cudaMemsetAsync(kc_ + (size_t)slot * kslot, 0, kslot * 2, stream_));
+  CTB_CUDA(cudaMemsetAsync(vc_ + (size_t)slot * vslot, 0, vslot * 2, stream_));
+  CTB_CUDA(cudaStreamSynchronize(stream_));
+}
+
+long Engine::multi_launches() const { return pf_ ? pf_->m_launches : 0; }
 
 double Engine::decode_greedy(int first_token, int n_past, int n_steps, int* out_tokens) {
   if (n_steps <= 0) return 0.0;

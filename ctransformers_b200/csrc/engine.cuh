@@ -35,6 +35,7 @@ struct HParams {
   int n_vocab = 0, n_ctx_train = 0, n_embd = 0, n_ff = 0, n_head = 0, n_head_kv = 0, n_layer = 0, n_rot = 0;
   float eps = 1e-5f, rope_base = 10000.f, rope_scale = 1.f;
   int n_ctx = 512;
+  int n_seq = 1;   // sequence slots of the KV cache (multi-sequence mode); slot 0 has the single-sequence layout
   int head_dim() const { return n_embd / n_head; }
   int n_embd_gqa() const { return head_dim() * n_head_kv; }
 };
@@ -51,6 +52,11 @@ struct StepOp;   // engine.cu: one op of the per-token schedule
 struct MVParams;
 struct Uploader;
 struct PrefillState;
+
+// One token of a multi-sequence eval (multi_pack in llm_abi.cu): its slot, id, position, the row length n_total of its eval
+// chunk, and whether its slot's eval ends with it (then its logits are kept).
+struct MultiTok { int slot, token, pos, n_total; bool last; };
+constexpr int MULTI_LAUNCH_TOKENS = 32;   // tokens of one batched launch (prefill.cuh PB_T)
 
 struct EvalStats { double last_eval_ms = 0; long launches = 0; size_t weight_bytes_per_token = 0; long spec_hits = 0; double load_ms = 0; size_t load_bytes = 0; };
 
@@ -74,6 +80,15 @@ class Engine {
   double time_matvec_only(int reps, long* launches, unsigned mask = 0);
   int profile_step(int token, int n_past, double ms_by_kind[4], int count_by_kind[4]);
   long trace_step(int token, int n_past, unsigned long long* out, long cap_words);
+  // Multi-sequence mode (hp.n_seq > 1): every slot has its own KV region.  multi_refusal: why the model cannot run it, "" when
+  // it can.  multi_eval: tokens [starts[i], starts[i+1]) of toks share batched launch i (a slot's tokens within one launch at
+  // consecutive positions); afterwards each slot whose eval ended holds its logits, embeddings and greedy pick on the device.
+  std::string multi_refusal();
+  void multi_eval(const std::vector<MultiTok>& toks, const std::vector<int>& starts);
+  void multi_fetch(int slot, float* logits, float* embd);   // host copies of the slot's last results
+  void multi_pick(int slot, int* out2);                     // {arg-max (lowest id), logits equal to the maximum}
+  void multi_reset(int slot);                               // zero the slot's KV region: a reused slot is a fresh one
+  long multi_launches() const;
   // Which implementations the evals run (include/ctransformers_b200.h ctb_llm_paths): entries written, or -needed.
   int paths(int* out, int cap);
 
@@ -187,6 +202,7 @@ class Engine {
   bool ensure_prefill();
   void prefill_batch(const int* tokens, const int* pos, const int* n_total, int n, bool last);
   void decode_one(int token, int pos, int n_total, bool with_logits);
+  void head_from(const float* row);   // the output head (un-fused, as the single-token schedule launches it) on one hidden row
   void finish_eval(int next_pos, bool hit);
   enum : int { MVK_QKV = 0, MVK_WO = 1, MVK_UP = 2, MVK_DOWN = 3, MVK_OUT = 4 };   // which projection a mat-vec launch is
   bool profiling_ = false;

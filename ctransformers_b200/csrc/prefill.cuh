@@ -50,6 +50,11 @@ struct alignas(16) PPhase {
   EmbedParams em;         // EMBED: out row stride = K
   const int* state;       // [PB_T][4]: {token, position, step, n_total} per token; state[PB_T*4] = valid tokens of this launch
 };
+// Multi-sequence launches (the MS builds of k_pstep): the KV cache holds one region per sequence slot, and state[PB_S + i] is
+// token i's slot.  state[PB_T*4 + 1] / [PB_T*4 + 2]: halves between the slots' K / V regions.
+constexpr int PB_S = PB_T * 4 + 4;
+constexpr int PB_STATE_MS = PB_S + PB_T;   // ints of a multi-sequence launch's state
+__device__ __forceinline__ size_t pb_slot_off(const int* state, int tok, int which) { return (size_t)state[PB_S + tok] * (unsigned)state[PB_T * 4 + 1 + which]; }
 
 struct PStepArgs {
   const PPhase* prog;
@@ -385,7 +390,8 @@ __device__ __forceinline__ void pb_gemm_phase(const PPhase& ph, int n_tok, uint8
   }
 }
 
-// RoPE of K + fp16 store of K and V of every valid token (attn_stage's cache writes, for the whole batch)
+// RoPE of K + fp16 store of K and V of every valid token (attn_stage's cache writes, for the whole batch); MS: into its slot's region
+template <bool MS>
 __device__ __forceinline__ void pb_kv_phase(const PPhase& ph, int n_tok) {
   const AttnParams& a = ph.at;
   const int half = a.hd / 2, per_tok = a.n_kv * half, total = n_tok * per_tok;
@@ -393,9 +399,17 @@ __device__ __forceinline__ void pb_kv_phase(const PPhase& ph, int n_tok) {
     const int tok = idx / per_tok, r = idx % per_tok, kh = r / half, i = r % half;
     const int pos = ph.state[tok * 4 + 1];
     if (pos >= a.n_ctx) continue;
-    rope_k_pair(a.k + (size_t)tok * a.kv_stride + (size_t)kh * a.hd, i, a.hd, a.neox, a.rope[(size_t)pos * half + i], a.kc + k_row(kh, pos, a.n_ctx, a.hd));
-    const float* vsrc = a.v + (size_t)tok * a.kv_stride + (size_t)kh * a.hd;
-    for (int c = 2 * i; c < 2 * i + 2; c++) a.vc[v_chan(kh, c, a.n_ctx, a.hd) + v_perm(pos)] = f2h(__ldcg(vsrc + c));
+    if constexpr (MS) {
+      uint16_t* kc = a.kc + pb_slot_off(ph.state, tok, 0);
+      uint16_t* vc = a.vc + pb_slot_off(ph.state, tok, 1);
+      rope_k_pair(a.k + (size_t)tok * a.kv_stride + (size_t)kh * a.hd, i, a.hd, a.neox, a.rope[(size_t)pos * half + i], kc + k_row(kh, pos, a.n_ctx, a.hd));
+      const float* vsrc = a.v + (size_t)tok * a.kv_stride + (size_t)kh * a.hd;
+      for (int c = 2 * i; c < 2 * i + 2; c++) vc[v_chan(kh, c, a.n_ctx, a.hd) + v_perm(pos)] = f2h(__ldcg(vsrc + c));
+    } else {   // (kept as it was: one expression for both builds changes the instructions ptxas emits for this one)
+      rope_k_pair(a.k + (size_t)tok * a.kv_stride + (size_t)kh * a.hd, i, a.hd, a.neox, a.rope[(size_t)pos * half + i], a.kc + k_row(kh, pos, a.n_ctx, a.hd));
+      const float* vsrc = a.v + (size_t)tok * a.kv_stride + (size_t)kh * a.hd;
+      for (int c = 2 * i; c < 2 * i + 2; c++) a.vc[v_chan(kh, c, a.n_ctx, a.hd) + v_perm(pos)] = f2h(__ldcg(vsrc + c));
+    }
   }
 }
 
@@ -425,24 +439,35 @@ __device__ __forceinline__ void pb_attn_warp_task(const AttnParams& p, const int
   __syncwarp();
 }
 
-// the ATTN phase of one CTA's warp: hd 64 / 128 inline, other head sizes in one out-of-line call
-template <bool GEN>
+// the ATTN phase of one CTA's warp: hd 64 / 128 inline, other head sizes in one out-of-line call; MS: each token reads its
+// slot's region of the cache
+template <bool GEN, bool MS>
 __device__ __forceinline__ void pb_attn_phase(const PPhase& ph, int n_tok, uint8_t* work) {
   const int warp = threadIdx.x >> 5;
   const int n_tasks = n_tok * ph.at.n_head;
   uint8_t* wsm = work + (size_t)warp * pb_attn_warp_bytes(ph.at.n_ctx, ph.at.hd);
   for (int task = blockIdx.x * PB_W + warp; task < n_tasks; task += (int)gridDim.x * PB_W) {
     const int tok = task / ph.at.n_head;
-    pb_attn_warp_task<GEN>(ph.at, ph.state + tok * 4, tok, task % ph.at.n_head, wsm);
+    if constexpr (MS) {
+      AttnParams p = ph.at;
+      p.kc += pb_slot_off(ph.state, tok, 0);
+      p.vc += pb_slot_off(ph.state, tok, 1);
+      pb_attn_warp_task<GEN>(p, ph.state + tok * 4, tok, task % ph.at.n_head, wsm);
+    } else {
+      pb_attn_warp_task<GEN>(ph.at, ph.state + tok * 4, tok, task % ph.at.n_head, wsm);
+    }
   }
 }
-// (one copy per kernel build, Q3: ptxas fits an out-of-line function's registers to all its callers at once)
-template <bool Q3>
-static __device__ __noinline__ void pb_attn_phase_gen(const PPhase& ph, int n_tok, uint8_t* work) { pb_attn_phase<true>(ph, n_tok, work); }
+// (one copy per kernel build, Q3 / MS: ptxas fits an out-of-line function's registers to all its callers at once)
+template <bool Q3, bool MS>
+static __device__ __noinline__ void pb_attn_phase_gen(const PPhase& ph, int n_tok, uint8_t* work) { pb_attn_phase<true, MS>(ph, n_tok, work); }
 
 // Q3: the build for programs that hold Q3_K matrices or a Q3_K embedding table.  The build without it compiles to the same
 // instructions as before Q3_K was added; with the Q3_K code inlined into the one kernel, ptxas spilled more there (DESIGN.md §6).
-template <bool Q3>
+// MS: the build for multi-sequence launches (a KV slot per token, PB_S), kept apart for the same reason: the single-sequence
+// builds compile to the same instructions as before it was added.  A QUANT phase with norm_out set (the output head's) also
+// writes every token's normalised row there, norm_out + token * K (the embeddings).
+template <bool Q3, bool MS = false>
 static __global__ void __launch_bounds__(PB_THREADS, 1) k_pstep(const __grid_constant__ PStepArgs args) {
   extern __shared__ __align__(16) uint8_t smem[];
   __shared__ __align__(8) uint64_t full_bar[ST_MAX_SLOTS];
@@ -482,16 +507,20 @@ static __global__ void __launch_bounds__(PB_THREADS, 1) k_pstep(const __grid_con
         MVParams q = ph.mv;
         q.x = ph.mv.x + (size_t)tok * ph.x_ld;
         if (q.x2) q.x2 = ph.mv.x2 + (size_t)tok * ph.x2_ld;
+        if constexpr (MS) {
+          if (q.norm_out) q.norm_out = ph.mv.norm_out + (size_t)tok * q.K;
+        }
         NormPre np;
         preload_norm(np, q);
-        stage_activation<PB_NT, PB_BAR>(q, np, ACT_Q8_K, work, red, false);
+        if constexpr (MS) stage_activation<PB_NT, PB_BAR>(q, np, ACT_Q8_K, work, red, q.norm_out != nullptr);
+        else stage_activation<PB_NT, PB_BAR>(q, np, ACT_Q8_K, work, red, false);
         pb_quant_store<PB_NT, PB_BAR>(work, q.K, tok, ph.qbuf);
       }
     } else if (ph.kind == PP_KV) {
-      pb_kv_phase(ph, n_tok);
+      pb_kv_phase<MS>(ph, n_tok);
     } else if (ph.kind == PP_ATTN) {
-      if (attn_fast_hd(ph.at.hd)) pb_attn_phase<false>(ph, n_tok, work);
-      else pb_attn_phase_gen<Q3>(ph, n_tok, work);
+      if (attn_fast_hd(ph.at.hd)) pb_attn_phase<false, MS>(ph, n_tok, work);
+      else pb_attn_phase_gen<Q3, MS>(ph, n_tok, work);
     } else if (ph.kind == PP_EMBED) {
       for (int tok = blockIdx.x; tok < n_tok; tok += G) embed_row<Q3>(ph.em, ph.state[tok * 4], ph.em.out + (size_t)tok * ph.em.K, threadIdx.x, PB_NT);
     }
@@ -510,7 +539,8 @@ inline size_t pb_work_bytes(int K_max, int n_ctx, int hd) {
 // launch shape of k_pstep around `work` bytes of scratch: whole per-team sub-rings in what shared memory has left.  false
 // when fewer than 4 slots fit (the attention scratch of a long context): the caller then has no batched prefill.
 inline bool pstep_shape(size_t work, int& n_slots, size_t& smem) {
-  const size_t room = std::min(max_dyn_smem(k_pstep<false>), max_dyn_smem(k_pstep<true>));
+  const size_t room = std::min(std::min(max_dyn_smem(k_pstep<false>), max_dyn_smem(k_pstep<true>)),
+                               std::min(max_dyn_smem(k_pstep<false, true>), max_dyn_smem(k_pstep<true, true>)));
   if (work + 4 * (size_t)ST_SLOT > room) return false;
   n_slots = (int)std::min<size_t>(ST_MAX_SLOTS, (room - work) / ST_SLOT) / PB_TEAMS * PB_TEAMS;
   smem = (size_t)n_slots * ST_SLOT + work;
@@ -537,8 +567,11 @@ inline void pb_matvec_phases(const MVParams& m, uint8_t* qbuf, const int* state,
   ph.kind = PP_GEMM; prog.push_back(ph);
 }
 static inline cudaError_t pstep_set_smem_limit(size_t bytes) {
-  const cudaError_t e = cudaFuncSetAttribute(k_pstep<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes);
-  return e != cudaSuccess ? e : cudaFuncSetAttribute(k_pstep<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes);
+  for (auto k : {k_pstep<false>, k_pstep<true>, k_pstep<false, true>, k_pstep<true, true>}) {
+    const cudaError_t e = cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes);
+    if (e != cudaSuccess) return e;
+  }
+  return cudaSuccess;
 }
 // does a program hold Q3_K matrices or a Q3_K embedding table (then it runs on k_pstep<true>)?
 inline bool pstep_q3(const std::vector<PPhase>& prog) {
@@ -550,10 +583,14 @@ inline bool pstep_q3(const std::vector<PPhase>& prog) {
   }
   return false;
 }
-static inline cudaError_t launch_pstep(int grid, int n_slots, size_t smem, cudaStream_t st, const PPhase* d_prog, int n_phases, unsigned* d_sync, bool q3 = false) {
+static inline cudaError_t launch_pstep(int grid, int n_slots, size_t smem, cudaStream_t st, const PPhase* d_prog, int n_phases, unsigned* d_sync, bool q3 = false,
+                                       bool ms = false) {
   PStepArgs a;
   a.prog = d_prog; a.n_phases = n_phases; a.n_slots = n_slots; a.sync = d_sync;
-  if (q3) k_pstep<true><<<grid, PB_THREADS, smem, st>>>(a);
+  if (ms) {
+    if (q3) k_pstep<true, true><<<grid, PB_THREADS, smem, st>>>(a);
+    else k_pstep<false, true><<<grid, PB_THREADS, smem, st>>>(a);
+  } else if (q3) k_pstep<true><<<grid, PB_THREADS, smem, st>>>(a);
   else k_pstep<false><<<grid, PB_THREADS, smem, st>>>(a);
   return cudaGetLastError();
 }

@@ -95,6 +95,18 @@ EXTRA_PROTOTYPES = {
     "ctb_vocab_tokenize": (C.c_int, [_P, C.c_char_p, C.c_bool, _IP, C.c_int]),
     "ctb_vocab_piece": (C.c_int, [_P, C.c_int, C.c_char_p, C.c_int]),
     "ctb_sample": (C.c_int, [_FP, C.c_int, _IP, C.c_int, C.c_int, C.c_float, C.c_float, C.c_float, C.c_int]),
+    "ctb_multi_create": (_P, [C.c_char_p, C.c_char_p, ConfigStruct, C.c_int]),
+    "ctb_multi_delete": (None, [_P]),
+    "ctb_multi_info": (C.c_int, [_P, _IP]),
+    "ctb_multi_eval": (C.c_bool, [_P, C.c_int, _IP, _IP, _IP, _IP, C.c_int]),
+    "ctb_multi_logits": (_FP, [_P, C.c_int]),
+    "ctb_multi_embeddings": (_FP, [_P, C.c_int]),
+    "ctb_multi_greedy": (C.c_int, [_P, C.c_int, _IP, _IP]),
+    "ctb_multi_sample": (C.c_int, [_P, C.c_int, _IP, C.c_int, C.c_int, C.c_float, C.c_float, C.c_float, C.c_int]),
+    "ctb_multi_reset": (C.c_int, [_P, C.c_int]),
+    "ctb_multi_launches": (C.c_long, [_P]),
+    "ctb_multi_last_eval_ms": (C.c_double, [_P]),
+    "ctb_multi_pack": (C.c_int, [C.c_int, _IP, _IP, _IP, C.c_int, C.c_int, _IP, C.c_int]),
 }
 
 

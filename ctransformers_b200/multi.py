@@ -1,0 +1,141 @@
+"""Many independent sequences on one GPU (include/ctransformers_b200.h ctb_multi_*): every slot behaves like its own LLM with the
+same config, bit for bit, while the slots listed in one eval share batched launches — one pass over the weights per launch of
+up to 32 tokens instead of one per token of every sequence."""
+from ctypes import c_int
+from pathlib import Path
+from typing import Dict, List, Optional, Sequence
+
+from .lib import load_library
+from .llm import Config, Vector, _pick, is_gguf
+
+
+class MultiLLM:
+    def __init__(self, model_path: str, model_type: Optional[str] = None, *, n_slots: int, config: Optional[Config] = None,
+                 lib: Optional[str] = None):
+        self._config = config or Config()
+        self._m, self._lib = None, None
+        if not Path(model_path).is_file():
+            raise ValueError(f"Model path '{model_path}' doesn't exist.")
+        if not model_type:
+            if not is_gguf(model_path):
+                raise ValueError("Unable to detect model type. Please specify a model type.")
+            model_type = "gguf"
+        self._lib = load_library(lib)
+        self._m = self._lib.ctb_multi_create(model_path.encode(), model_type.encode(), self._config.to_struct(), n_slots)
+        if self._m is None:
+            raise RuntimeError(f"Failed to create a {n_slots}-slot MultiLLM from '{model_path}'.")
+        info = (c_int * 6)()
+        self._lib.ctb_multi_info(self._m, info)
+        self.n_slots, self.vocab_size, self.n_embd, self.context_length, self.eos_token_id, self.bos_token_id = list(info)
+        self._context: List[List[int]] = [[] for _ in range(self.n_slots)]
+
+    config = property(lambda self: self._config)
+
+    def context(self, slot: int) -> List[int]:
+        """The tokens slot `slot` has evaluated since it was created or reset (LLM._context of that slot)."""
+        return self._context[self._slot(slot)]
+
+    def _slot(self, slot: int) -> int:
+        if not 0 <= slot < self.n_slots:
+            raise IndexError(f"slot {slot} is out of range (0 .. {self.n_slots - 1})")
+        return slot
+
+    def eval(self, tokens_by_slot: Dict[int, Sequence[int]], *, batch_size: Optional[int] = None) -> None:
+        """Each listed slot evaluates its tokens after its own history (n_past = its context length), chunked by batch_size as
+        LLM.eval chunks; all of them share batched launches."""
+        bs = _pick(batch_size, self._config.batch_size)
+        slots = [self._slot(s) for s in tokens_by_slot]
+        off, flat = [0], []
+        for s in slots:
+            flat.extend(tokens_by_slot[s])
+            off.append(len(flat))
+        n = len(slots)
+        arr = (c_int * max(len(flat), 1))(*flat)
+        past = [len(self._context[s]) for s in slots]
+        if not self._lib.ctb_multi_eval(self._m, n, (c_int * max(n, 1))(*slots), (c_int * (n + 1))(*off), arr, (c_int * max(n, 1))(*past), bs):
+            raise RuntimeError("Failed to evaluate tokens.")
+        for s in slots:
+            self._context[s].extend(tokens_by_slot[s])
+
+    def logits(self, slot: int) -> List[float]:
+        p = self._lib.ctb_multi_logits(self._m, self._slot(slot))
+        return Vector(p, self.vocab_size if p else 0)
+
+    def embeddings(self, slot: int) -> List[float]:
+        p = self._lib.ctb_multi_embeddings(self._m, self._slot(slot))
+        return Vector(p, self.n_embd if p else 0)
+
+    def greedy(self, slots: Sequence[int]) -> List[int]:
+        """The greedy picks of these slots (what sample(top_k=1, repetition_penalty=1.0) returns), computed on the device."""
+        slots = [self._slot(s) for s in slots]
+        out = (c_int * max(len(slots), 1))()
+        if self._lib.ctb_multi_greedy(self._m, len(slots), (c_int * max(len(slots), 1))(*slots), out) != 0:
+            raise RuntimeError("No logits to pick from: every slot must have been evaluated.")
+        return list(out[: len(slots)])
+
+    def sample(self, slot: int, *, top_k=None, top_p=None, temperature=None, repetition_penalty=None, last_n_tokens=None, seed=None) -> int:
+        """LLM.sample on this slot: the same defaults, its own last_n_tokens window."""
+        cfg = self._config
+        ctx = self._context[self._slot(slot)]
+        last_n = _pick(last_n_tokens, cfg.last_n_tokens)
+        if last_n < 0:
+            last_n = self.context_length
+        recent = ctx[-last_n:]
+        t = self._lib.ctb_multi_sample(self._m, slot, (c_int * max(len(recent), 1))(*recent), len(recent), _pick(top_k, cfg.top_k),
+                                       _pick(top_p, cfg.top_p), _pick(temperature, cfg.temperature),
+                                       _pick(repetition_penalty, cfg.repetition_penalty), _pick(seed, cfg.seed))
+        if t < 0:
+            raise RuntimeError(f"Slot {slot} has no logits to sample from.")
+        return t
+
+    def reset(self, slot: int) -> None:
+        """The slot starts over, as a fresh LLM."""
+        self._lib.ctb_multi_reset(self._m, self._slot(slot))
+        self._context[slot] = []
+
+    def launches(self) -> int:
+        return self._lib.ctb_multi_launches(self._m)
+
+    def last_eval_ms(self) -> float:
+        return self._lib.ctb_multi_last_eval_ms(self._m)
+
+    def generate_many(self, prompts: Sequence[Sequence[int]], max_new_tokens: int, *, batch_size: Optional[int] = None,
+                      **sampling) -> List[List[int]]:
+        """Generates for every prompt, up to n_slots at once: a sequence ends at EOS (not included) or after max_new_tokens, and
+        its slot takes the next waiting prompt, whose prompt tokens then share launches with the other slots' decode tokens.
+        Each result equals LLM.generate of that prompt on a fresh LLM with the same sampling arguments."""
+        results: List[Optional[List[int]]] = [None] * len(prompts)
+        waiting = list(range(len(prompts)))[::-1]
+        owner: Dict[int, int] = {}        # slot -> prompt index
+        pending: Dict[int, List[int]] = {}
+        for slot in range(self.n_slots):
+            if not waiting:
+                break
+            self.reset(slot)
+            i = waiting.pop()
+            owner[slot], pending[slot], results[i] = i, list(prompts[i]), []
+        while owner:
+            self.eval(pending, batch_size=batch_size)
+            pending = {}
+            for slot in sorted(owner):
+                i = owner[slot]
+                tok = self.sample(slot, **sampling)
+                if tok == self.eos_token_id or max_new_tokens <= 0:
+                    done = True
+                else:
+                    results[i].append(tok)
+                    done = len(results[i]) >= max_new_tokens
+                    pending[slot] = [tok]
+                if done:
+                    pending.pop(slot, None)
+                    del owner[slot]
+                    if waiting:
+                        self.reset(slot)
+                        j = waiting.pop()
+                        owner[slot], pending[slot], results[j] = j, list(prompts[j]), []
+        return results
+
+    def __del__(self):
+        if self.__dict__.get("_m") is not None and self.__dict__.get("_lib") is not None:
+            self._lib.ctb_multi_delete(self._m)
+            self._m = None

@@ -187,6 +187,34 @@ int ctb_matvec_partition(const int* types, const int* rows, int nseg, int K, int
 
 int ctb_get_row(int type, const void* table_blocks, int K, int n_rows, int row, float* out);
 
+/* Multi-sequence decoding: one handle owns n_slots sequence slots, each of which behaves like a fresh single-sequence LLM with
+ * the same config, and every eval's slots share batched launches (one pass over the weights per launch of up to 32 tokens).
+ * After every eval a slot's logits, embeddings, greedy pick and sampler draws are bit-identical to what a single-sequence LLM
+ * returns for that slot's own call history.  The KV cache holds one region per slot ([slot][layer][kv_head][pos][k_stride]).
+ * Runs models whose layer matrices are all K-quants at contexts where the batched kernel fits (not at 4096 and above); create
+ * returns NULL (+ stderr) otherwise, without a CUDA device, in a process that holds a tensor-sharded rank, and when the n_slots
+ * KV regions do not fit (the message gives the bytes needed). */
+typedef struct ctb_multi ctb_multi;
+ctb_multi* ctb_multi_create(const char* model_path, const char* model_type, const ctransformers_config config, int n_slots);
+void ctb_multi_delete(ctb_multi* m);
+int ctb_multi_info(ctb_multi* m, int* out6);   /* {n_slots, n_vocab, n_embd, context length, eos id, bos id}; returns 6 */
+/* slot slots[i] evaluates tokens[off[i] .. off[i+1]) at n_past[i], chunked by batch_size as ctransformers_llm_batch_eval
+ * chunks; all listed slots (each at most once) share launches.  false (+ stderr) on error. */
+bool ctb_multi_eval(ctb_multi* m, int n, const int* slots, const int* off, const int* tokens, const int* n_past, int batch_size);
+const float* ctb_multi_logits(ctb_multi* m, int slot);       /* n_vocab floats of the slot's last eval; NULL before one */
+const float* ctb_multi_embeddings(ctb_multi* m, int slot);   /* n_embd floats */
+/* greedy picks (= sample with top_k 1, no penalty) of n slots from the device arg-max; 0, or -1 (+ stderr) on error */
+int ctb_multi_greedy(ctb_multi* m, int n, const int* slots, int* out);
+/* = ctransformers_llm_sample on that slot's logits (RNG reseeded per call); -1 on error */
+int ctb_multi_sample(ctb_multi* m, int slot, const int* last_tokens, int n_last, int top_k, float top_p, float temperature,
+                     float repetition_penalty, int seed);
+int ctb_multi_reset(ctb_multi* m, int slot);    /* the slot starts over; 0, or -1 when out of range */
+long ctb_multi_launches(ctb_multi* m);           /* batched launches so far */
+double ctb_multi_last_eval_ms(ctb_multi* m);     /* CUDA-event time of the last eval */
+/* Host only: the token list ctb_multi_eval makes of these arguments, out[i] = {slot, position, n_total, launch, last of its
+ * slot's eval} (5 ints per token).  Returns the token count, or -count when cap is smaller. */
+int ctb_multi_pack(int n, const int* slots, const int* off, const int* n_past, int batch_size, int n_ctx, int* out, int cap);
+
 #ifdef __cplusplus
 }
 #endif
