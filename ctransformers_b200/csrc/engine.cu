@@ -453,6 +453,9 @@ void Engine::release() {
   h_dbg_ = nullptr;
   if (h_sample_) cudaFreeHost(h_sample_);
   h_sample_ = nullptr;
+  if (h_stage_) cudaFreeHost(h_stage_);
+  h_stage_ = nullptr;
+  stage_cap_ = 0;
   if (ev_pick_) cudaEventDestroy(ev_pick_);
   if (ev_sample_) cudaEventDestroy(ev_sample_);
   ev_sample_ = nullptr;
@@ -1320,6 +1323,148 @@ void Engine::multi_reset(int slot) {
 }
 
 long Engine::multi_launches() const { return pf_ ? pf_->m_launches : 0; }
+
+// ---- sequence states
+void Engine::kv_slot_elems(size_t& k, size_t& v) const {
+  const int hd = hp_.head_dim();
+  k = (size_t)hp_.n_layer * hp_.n_ctx * nkv_ * k_stride(hd);
+  v = (size_t)hp_.n_layer * kv_ctx_pad(hp_.n_ctx) * nkv_ * hd;
+}
+
+float* Engine::results_of(int slot, float** embd) {
+  if (hp_.n_seq == 1) {
+    *embd = d_embd_keep_;
+    return d_logits_keep_;
+  }
+  if (!pf_ || !pf_->d_mlogits) throw std::runtime_error("this engine has no multi-sequence path");
+  *embd = pf_->d_membd + (size_t)slot * hp_.n_embd;
+  return pf_->d_mlogits + (size_t)slot * hp_.n_vocab;
+}
+
+uint8_t* Engine::stage(size_t bytes) {
+  if (bytes > stage_cap_) {
+    if (h_stage_) CTB_CUDA(cudaFreeHost(h_stage_));
+    h_stage_ = nullptr;
+    stage_cap_ = 0;
+    CTB_CUDA(cudaMallocHost(&h_stage_, bytes));
+    stage_cap_ = bytes;
+  }
+  return h_stage_;
+}
+
+int Engine::state_k_stride() const { return k_stride(hp_.head_dim()); }
+
+// V rows hold position t at v_perm(t), a permutation within each block of 256 positions: a state keeps whole blocks,
+// n_pad = n_past rounded up to 256 entries per channel, in the cache's order.
+static int v_pad(int n_past) { return (n_past + 255) & ~255; }
+
+// The entries of positions n_past .. n_pad - 1 of every V row are zero in a state, whatever the slot held there (a longer
+// history, or the look-ahead step's row at n_past).
+static void zero_v_tail(uint16_t* v, size_t rows, int n_past) {
+  const int n_pad = v_pad(n_past);
+  for (size_t r = 0; r < rows; r++)
+    for (int t = n_past; t < n_pad; t++) v[r * n_pad + v_perm(t)] = 0;
+}
+
+size_t Engine::state_bytes(int n_past, bool results) const {
+  const int hd = hp_.head_dim();
+  return (size_t)hp_.n_layer * nkv_ * ((size_t)n_past * k_stride(hd) + (size_t)v_pad(n_past) * hd) * 2 +
+         (results ? ((size_t)hp_.n_vocab + hp_.n_embd) * 4 : 0);
+}
+
+// K: one 2-D copy of n_layer * n_kv rows (a head's positions are contiguous); V: one of n_layer * n_kv * hd rows (a channel's
+// positions are one run of whole 256-blocks).  The host side is the contiguous pinned staging buffer.
+void Engine::state_save(int slot, int n_past, bool results, void* out) {
+  DeviceGuard dev_guard(device_);
+  const int hd = hp_.head_dim(), ks = k_stride(hd);
+  size_t kslot, vslot;
+  kv_slot_elems(kslot, vslot);
+  const size_t rows = (size_t)hp_.n_layer * nkv_, kb = rows * n_past * ks * 2, vb = rows * hd * v_pad(n_past) * 2;
+  uint8_t* h = stage(std::max<size_t>(state_bytes(n_past, results), 1));
+  if (n_past > 0) {
+    CTB_CUDA(cudaMemcpy2DAsync(h, (size_t)n_past * ks * 2, kc_ + slot * kslot, (size_t)hp_.n_ctx * ks * 2, (size_t)n_past * ks * 2, rows,
+                               cudaMemcpyDeviceToHost, stream_));
+    CTB_CUDA(cudaMemcpy2DAsync(h + kb, (size_t)v_pad(n_past) * 2, vc_ + slot * vslot, (size_t)kv_ctx_pad(hp_.n_ctx) * 2, (size_t)v_pad(n_past) * 2,
+                               rows * hd, cudaMemcpyDeviceToHost, stream_));
+  }
+  if (results) {
+    float* em;
+    const float* lg = results_of(slot, &em);
+    CTB_CUDA(cudaMemcpyAsync(h + kb + vb, lg, (size_t)hp_.n_vocab * 4, cudaMemcpyDeviceToHost, stream_));
+    CTB_CUDA(cudaMemcpyAsync(h + kb + vb + (size_t)hp_.n_vocab * 4, em, (size_t)hp_.n_embd * 4, cudaMemcpyDeviceToHost, stream_));
+  }
+  CTB_CUDA(cudaStreamSynchronize(stream_));
+  zero_v_tail((uint16_t*)(h + kb), rows * hd, n_past);
+  memcpy(out, h, state_bytes(n_past, results));
+}
+
+void Engine::state_load(int slot, int n_past, bool results, const void* in, int last_token) {
+  DeviceGuard dev_guard(device_);
+  const int hd = hp_.head_dim(), ks = k_stride(hd);
+  size_t kslot, vslot;
+  kv_slot_elems(kslot, vslot);
+  const size_t rows = (size_t)hp_.n_layer * nkv_, kb = rows * n_past * ks * 2, vb = rows * hd * v_pad(n_past) * 2;
+  float* em = nullptr;
+  float* lg = results ? results_of(slot, &em) : nullptr;
+  uint8_t* h = stage(std::max<size_t>(state_bytes(n_past, results), 1));
+  memcpy(h, in, state_bytes(n_past, results));
+  zero_v_tail((uint16_t*)(h + kb), rows * hd, n_past);
+  if (hp_.n_seq == 1) {   // a look-ahead step may still be in the stream: it runs before the copies below
+    spec_pending_ = false; spec_deferred_ = false; spec_pos_ = -1; spec_streak_ = 0;
+  }
+  CTB_CUDA(cudaMemsetAsync(kc_ + slot * kslot, 0, kslot * 2, stream_));
+  CTB_CUDA(cudaMemsetAsync(vc_ + slot * vslot, 0, vslot * 2, stream_));
+  if (n_past > 0) {
+    CTB_CUDA(cudaMemcpy2DAsync(kc_ + slot * kslot, (size_t)hp_.n_ctx * ks * 2, h, (size_t)n_past * ks * 2, (size_t)n_past * ks * 2, rows,
+                               cudaMemcpyHostToDevice, stream_));
+    CTB_CUDA(cudaMemcpy2DAsync(vc_ + slot * vslot, (size_t)kv_ctx_pad(hp_.n_ctx) * 2, h + kb, (size_t)v_pad(n_past) * 2, (size_t)v_pad(n_past) * 2,
+                               rows * hd, cudaMemcpyHostToDevice, stream_));
+  }
+  if (results) {
+    CTB_CUDA(cudaMemcpyAsync(lg, h + kb + vb, (size_t)hp_.n_vocab * 4, cudaMemcpyHostToDevice, stream_));
+    CTB_CUDA(cudaMemcpyAsync(em, h + kb + vb + (size_t)hp_.n_vocab * 4, (size_t)hp_.n_embd * 4, cudaMemcpyHostToDevice, stream_));
+    if (hp_.n_seq > 1) {
+      k_argmax<<<1, ARGMAX_THREADS, 0, stream_>>>(lg, hp_.n_vocab, pf_->d_mpick + 2 * slot);
+      CTB_CUDA(cudaGetLastError());
+    }
+  }
+  if (hp_.n_seq == 1) {
+    kv_high_ = n_past;
+    host_fresh_ = false;
+    if (results && n_past > 0) {
+      // as finish_eval leaves an eval of these tokens: the step state at the last token, its results in d_logits_ / d_embd_
+      // too, and the greedy pick of the look-ahead (after_eval), whose step then resumes once the caller decodes greedily
+      CTB_CUDA(cudaMemcpyAsync(d_logits_, lg, (size_t)hp_.n_vocab * 4, cudaMemcpyDeviceToDevice, stream_));
+      CTB_CUDA(cudaMemcpyAsync(d_embd_, em, (size_t)hp_.n_embd * 4, cudaMemcpyDeviceToDevice, stream_));
+      if (h_state_cap_ < 1) { h_state_cap_ = 512; CTB_CUDA(cudaMallocHost(&h_state_, (size_t)h_state_cap_ * 16)); }
+      int* st = h_state_ + (size_t)(h_state_next_ % h_state_cap_) * 4;
+      h_state_next_++;
+      st[0] = last_token; st[1] = n_past - 1; st[2] = 0; st[3] = n_past;
+      CTB_CUDA(cudaMemcpyAsync(d_state_, st, 16, cudaMemcpyHostToDevice, stream_));
+      after_eval(n_past);
+    }
+  }
+  CTB_CUDA(cudaStreamSynchronize(stream_));
+}
+
+void Engine::state_fork(int src, const int* dsts, int n) {
+  DeviceGuard dev_guard(device_);
+  size_t kslot, vslot;
+  kv_slot_elems(kslot, vslot);
+  float* sem;
+  const float* slg = results_of(src, &sem);
+  for (int i = 0; i < n; i++) {
+    const int d = dsts[i];
+    float* dem;
+    float* dlg = results_of(d, &dem);
+    CTB_CUDA(cudaMemcpyAsync(kc_ + d * kslot, kc_ + src * kslot, kslot * 2, cudaMemcpyDeviceToDevice, stream_));
+    CTB_CUDA(cudaMemcpyAsync(vc_ + d * vslot, vc_ + src * vslot, vslot * 2, cudaMemcpyDeviceToDevice, stream_));
+    CTB_CUDA(cudaMemcpyAsync(dlg, slg, (size_t)hp_.n_vocab * 4, cudaMemcpyDeviceToDevice, stream_));
+    CTB_CUDA(cudaMemcpyAsync(dem, sem, (size_t)hp_.n_embd * 4, cudaMemcpyDeviceToDevice, stream_));
+    CTB_CUDA(cudaMemcpyAsync(pf_->d_mpick + 2 * d, pf_->d_mpick + 2 * src, 8, cudaMemcpyDeviceToDevice, stream_));
+  }
+  CTB_CUDA(cudaStreamSynchronize(stream_));
+}
 
 double Engine::decode_greedy(int first_token, int n_past, int n_steps, int* out_tokens) {
   if (n_steps <= 0) return 0.0;

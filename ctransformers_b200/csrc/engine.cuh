@@ -89,6 +89,17 @@ class Engine {
   void multi_pick(int slot, int* out2);                     // {arg-max (lowest id), logits equal to the maximum}
   void multi_reset(int slot);                               // zero the slot's KV region: a reused slot is a fresh one
   long multi_launches() const;
+  // Sequence states (include/ctransformers_b200.h ctb_state_header): the slot's K / V at positions [0, n_past) as
+  // K [layer][kv_head][pos][k_stride] then V [layer][kv_channel][pos], fp16, then with `results` its last logits and embeddings
+  // (a multi-sequence slot's rows, or the single-sequence eval's kept results).  Every copy is stream-ordered on the engine
+  // stream, behind whatever is already in it (a look-ahead step writes position n_past, which a state does not hold).
+  size_t state_bytes(int n_past, bool results) const;
+  int state_k_stride() const;   // halves of a K row
+  void state_save(int slot, int n_past, bool results, void* out);
+  // Also zeroes the slot's positions from n_past on, so the slot equals a fresh one that evaluated those tokens.  A
+  // single-sequence engine drops its look-ahead and starts over from this state as after an eval ending with last_token.
+  void state_load(int slot, int n_past, bool results, const void* in, int last_token);
+  void state_fork(int src, const int* dsts, int n);   // multi-sequence: slot src's whole KV region and last results into each dst
   // Which implementations the evals run (include/ctransformers_b200.h ctb_llm_paths): entries written, or -needed.
   int paths(int* out, int cap);
 
@@ -210,6 +221,12 @@ class Engine {
   std::vector<cudaEvent_t> prof_ev_;
   std::vector<int> prof_kind_;
   void mark(int kind);
+  // sequence states
+  uint8_t* h_stage_ = nullptr;   // pinned staging of state_save / state_load, grown on demand
+  size_t stage_cap_ = 0;
+  uint8_t* stage(size_t bytes);
+  void kv_slot_elems(size_t& k, size_t& v) const;   // halves of one slot's K and V regions
+  float* results_of(int slot, float** embd);        // where the slot's last logits / embeddings live on the device
 };
 
 size_t engine_arena_bytes(const GGUFFile& g, const HParams& hp);

@@ -128,6 +128,17 @@ class GGUFFile {
     return v->s;
   }
 
+  // bytes of one element of a numeric value type (0: not one)
+  static size_t scalar_size(uint32_t t) {
+    switch (t) {
+      case 0: case 1: case 7: return 1;   // u8 i8 bool
+      case 2: case 3: return 2;           // u16 i16
+      case 4: case 5: case 6: return 4;   // u32 i32 f32
+      case 10: case 11: case 12: return 8;  // u64 i64 f64
+    }
+    return 0;
+  }
+
  private:
   int fd_ = -1;
   const uint8_t* base_ = nullptr;
@@ -143,15 +154,6 @@ class GGUFFile {
     std::string s((const char*)base_ + pos_, (size_t)n);
     pos_ += n;
     return s;
-  }
-  static size_t scalar_size(uint32_t t) {
-    switch (t) {
-      case 0: case 1: case 7: return 1;   // u8 i8 bool
-      case 2: case 3: return 2;           // u16 i16
-      case 4: case 5: case 6: return 4;   // u32 i32 f32
-      case 10: case 11: case 12: return 8;  // u64 i64 f64
-    }
-    return 0;
   }
   void rd_scalar(uint32_t t, GGUFValue& v) {
     switch (t) {

@@ -48,6 +48,7 @@ struct LLM {
   std::mt19937 rng;
   bool has_logits = false;
   long gpu_samples = 0;   // sample() calls answered by the device-side penalty + top-k
+  uint64_t fingerprint = 0;   // of the model file, computed on first use (model_fingerprint)
 };
 
 static bool file_is_gguf(const char* path) {
@@ -126,6 +127,117 @@ static std::vector<int> multi_pack(int n, const int* slots, const int* off, cons
   }
   if ((int)toks.size() > starts.back()) starts.push_back((int)toks.size());
   return starts;
+}
+
+// ---- sequence states (include/ctransformers_b200.h ctb_state_header)
+static void fnv(uint64_t& h, const void* p, size_t n) {
+  const uint8_t* b = (const uint8_t*)p;
+  for (size_t i = 0; i < n; i++) { h ^= b[i]; h *= 0x100000001b3ull; }
+}
+static void fnv_str(uint64_t& h, const std::string& s) {
+  const uint64_t n = s.size();
+  fnv(h, &n, 8);
+  fnv(h, s.data(), s.size());
+}
+
+// FNV-1a over the metadata, the tensor table and the first 4 KiB of every tensor's data: two files of the same shape differ in
+// their weights, and reading every weight would cost as much as loading the model.
+static uint64_t model_fingerprint(LLM& L) {
+  if (L.fingerprint) return L.fingerprint;
+  const GGUFFile& g = *L.file;
+  uint64_t h = 0xcbf29ce484222325ull;
+  fnv(h, &g.version, 4);
+  for (const auto& [key, v] : g.kv) {
+    fnv_str(h, key);
+    fnv(h, &v.type, 4); fnv(h, &v.u, 8); fnv(h, &v.f, 8); fnv_str(h, v.s);
+    fnv(h, &v.arr_type, 4); fnv(h, &v.arr_n, 8);
+    if (v.arr_data) fnv(h, v.arr_data, GGUFFile::scalar_size(v.arr_type) * v.arr_n);
+    for (const std::string& s : v.arr_str) fnv_str(h, s);
+  }
+  for (const GGUFTensor& t : g.tensors) {
+    fnv_str(h, t.name);
+    fnv(h, &t.n_dims, 4); fnv(h, t.ne, sizeof(t.ne)); fnv(h, &t.type, 4); fnv(h, &t.offset, 8);
+    fnv(h, t.data, (size_t)std::min<uint64_t>(t.nbytes, 4096));
+  }
+  return L.fingerprint = h ? h : 1;
+}
+
+static ctb_state_header state_header(LLM& L, int n_tokens, bool results) {
+  ctb_state_header s{};
+  s.magic = CTB_STATE_MAGIC;
+  s.version = CTB_STATE_VERSION;
+  s.n_layer = L.hp.n_layer; s.n_head_kv = L.hp.n_head_kv; s.head_dim = L.hp.head_dim(); s.k_stride = L.engine->state_k_stride();
+  s.n_embd = L.hp.n_embd; s.n_vocab = L.hp.n_vocab;
+  s.n_tokens = n_tokens;
+  s.has_results = results ? 1 : 0;
+  s.fingerprint = model_fingerprint(L);
+  return s;
+}
+
+static uint64_t state_size(const ctb_state_header& s) {
+  const uint64_t n = (uint64_t)s.n_tokens, n_pad = (n + 255) & ~255ull, rows = (uint64_t)s.n_layer * s.n_head_kv;
+  return sizeof(ctb_state_header) + 4 * n + rows * (n * s.k_stride + n_pad * s.head_dim) * 2 +
+         (s.has_results ? ((uint64_t)s.n_vocab + s.n_embd) * 4 : 0);
+}
+
+// Why buf cannot be a state ("" when it can); s gets its header.  The bounds keep state_size within 64 bits.
+static std::string state_check(const void* buf, size_t size, ctb_state_header& s) {
+  if (!buf || size < sizeof(s)) return "a state has at least a " + std::to_string(sizeof(s)) + "-byte header; this one has " + std::to_string(size) + " bytes";
+  memcpy(&s, buf, sizeof(s));
+  if (s.magic != CTB_STATE_MAGIC) return "not a sequence state (bad magic)";
+  if (s.version != CTB_STATE_VERSION) return "state version " + std::to_string(s.version) + " (this library reads version " + std::to_string(CTB_STATE_VERSION) + ")";
+  auto in = [](int32_t v, int32_t lo, int32_t hi) { return v >= lo && v <= hi; };
+  if (!in(s.n_layer, 1, 4096) || !in(s.n_head_kv, 1, 4096) || !in(s.head_dim, 1, 4096) || !in(s.k_stride, s.head_dim, 4096) ||
+      !in(s.n_embd, 1, 1 << 24) || !in(s.n_vocab, 1, 1 << 24) || !in(s.n_tokens, 0, 1 << 24) || !in(s.has_results, 0, 1))
+    return "the state's header is malformed";
+  if (state_size(s) != size)
+    return "the state's size (" + std::to_string(size) + " bytes) disagrees with its header (" + std::to_string(state_size(s)) + " bytes)";
+  return "";
+}
+
+static size_t state_size_for(LLM& L, int n_tokens) {
+  if (n_tokens < 0 || n_tokens > L.hp.n_ctx) return 0;
+  return (size_t)state_size(state_header(L, n_tokens, n_tokens > 0));
+}
+
+static void save_state(LLM& L, int slot, const int* tokens, int n_tokens, bool results, void* buf, size_t cap) {
+  if (n_tokens < 0 || n_tokens > L.hp.n_ctx)
+    throw std::runtime_error(std::to_string(n_tokens) + " tokens: a state holds 0 .. " + std::to_string(L.hp.n_ctx) + " (the context length)");
+  if (n_tokens > 0 && !tokens) throw std::runtime_error("no tokens");
+  const ctb_state_header s = state_header(L, n_tokens, results && n_tokens > 0);
+  const uint64_t need = state_size(s);
+  if (!buf || cap < need) throw std::runtime_error("the state needs " + std::to_string(need) + " bytes; the buffer has " + std::to_string(cap));
+  uint8_t* p = (uint8_t*)buf;
+  memcpy(p, &s, sizeof(s));
+  memcpy(p + sizeof(s), tokens, (size_t)n_tokens * 4);
+  L.engine->state_save(slot, n_tokens, s.has_results, p + sizeof(s) + (size_t)n_tokens * 4);
+}
+
+// Checks everything before the first device copy: a refused state leaves the slot as it was.  Returns the header.
+static ctb_state_header restore_state(LLM& L, int slot, const void* buf, size_t size) {
+  ctb_state_header s;
+  std::string why = state_check(buf, size, s);
+  const ctb_state_header want = state_header(L, 0, false);
+  if (why.empty() && (s.n_layer != want.n_layer || s.n_head_kv != want.n_head_kv || s.head_dim != want.head_dim || s.k_stride != want.k_stride ||
+                      s.n_embd != want.n_embd || s.n_vocab != want.n_vocab))
+    why = "the state is of a model of another shape";
+  if (why.empty() && s.fingerprint != want.fingerprint) why = "the state is of another model file";
+  if (why.empty() && s.n_tokens > L.hp.n_ctx)
+    why = "the state holds " + std::to_string(s.n_tokens) + " positions; the context length is " + std::to_string(L.hp.n_ctx);
+  const uint8_t* p = (const uint8_t*)buf + sizeof(s);
+  int last = 0;
+  for (int i = 0; why.empty() && i < s.n_tokens; i++) {
+    memcpy(&last, p + (size_t)i * 4, 4);
+    if (last < 0 || last >= L.hp.n_vocab) why = "the state holds a token id out of range";
+  }
+  if (!why.empty()) throw std::invalid_argument(why);
+  L.engine->state_load(slot, s.n_tokens, s.has_results, p + (size_t)s.n_tokens * 4, last);
+  return s;
+}
+
+static int state_error(const char* what, const std::exception& e) {
+  fprintf(stderr, "ctransformers-b200: %s: %s\n", what, e.what());
+  return -1;
 }
 
 extern "C" {
@@ -352,6 +464,44 @@ double ctb_llm_time_matvec_kinds(LLM* llm, int reps, long* launches, unsigned ki
   }
 }
 
+int ctb_state_info(const void* buf, size_t size, ctb_state_header* out) {
+  ctb_state_header s;
+  const std::string why = state_check(buf, size, s);
+  if (!why.empty()) {
+    fprintf(stderr, "ctransformers-b200: %s\n", why.c_str());
+    return -1;
+  }
+  if (out) *out = s;
+  return 0;
+}
+
+static void llm_states_ok(LLM* llm) {
+  if (llm->comm) throw std::runtime_error("the tensor-sharded mode has no sequence states");
+}
+
+size_t ctb_llm_state_size(LLM* llm, int n_tokens) {
+  try {
+    llm_states_ok(llm);
+    return state_size_for(*llm, n_tokens);
+  } catch (...) { return 0; }
+}
+
+int ctb_llm_save_state(LLM* llm, const int* tokens, int n_tokens, void* buf, size_t cap) {
+  try {
+    llm_states_ok(llm);
+    save_state(*llm, 0, tokens, n_tokens, llm->has_logits, buf, cap);
+    return 0;
+  } catch (const std::exception& e) { return state_error("cannot save the state", e); }
+}
+
+int ctb_llm_load_state(LLM* llm, const void* buf, size_t size) {
+  try {
+    llm_states_ok(llm);
+    llm->has_logits = restore_state(*llm, 0, buf, size).has_results != 0;
+    return 0;
+  } catch (const std::exception& e) { return state_error("cannot load the state", e); }
+}
+
 // ---- host-only logic (no GPU needed): tokenizer / detokenizer / sampler on their own
 struct ctb_vocab { std::unique_ptr<GGUFFile> file; Vocab vocab; };
 
@@ -541,6 +691,48 @@ int ctb_multi_reset(ctb_multi* m, int slot) {
     fprintf(stderr, "ctransformers-b200: multi-sequence reset failed: %s\n", e.what());
     return -1;
   }
+}
+
+size_t ctb_multi_state_size(ctb_multi* m, int n_tokens) {
+  try { return state_size_for(*m->llm, n_tokens); } catch (...) { return 0; }
+}
+
+int ctb_multi_save(ctb_multi* m, int slot, const int* tokens, int n_tokens, void* buf, size_t cap) {
+  try {
+    if (!multi_slot_ok(m, slot)) return -1;
+    save_state(*m->llm, slot, tokens, n_tokens, m->has[slot] != 0, buf, cap);
+    return 0;
+  } catch (const std::exception& e) { return state_error("cannot save the state", e); }
+}
+
+int ctb_multi_restore(ctb_multi* m, int slot, const void* buf, size_t size) {
+  try {
+    if (!multi_slot_ok(m, slot)) return -1;
+    m->has[slot] = restore_state(*m->llm, slot, buf, size).has_results != 0;
+    m->fresh[slot] = 0;
+    return 0;
+  } catch (const std::exception& e) { return state_error("cannot restore the state", e); }
+}
+
+int ctb_multi_fork(ctb_multi* m, int src, int n, const int* dsts) {
+  try {
+    if (!multi_slot_ok(m, src)) return -1;
+    for (int i = 0; i < n; i++) {
+      if (!multi_slot_ok(m, dsts[i])) return -1;
+      if (dsts[i] == src) throw std::invalid_argument("slot " + std::to_string(src) + " cannot be forked into itself");
+    }
+    m->llm->engine->state_fork(src, dsts, n);
+    for (int i = 0; i < n; i++) {
+      const int d = dsts[i];
+      m->has[d] = m->has[src];
+      m->fresh[d] = m->fresh[src];
+      if (m->fresh[src]) {
+        m->logits[d] = m->logits[src];
+        m->embd[d] = m->embd[src];
+      }
+    }
+    return 0;
+  } catch (const std::exception& e) { return state_error("cannot fork the slot", e); }
 }
 
 long ctb_multi_launches(ctb_multi* m) { return m->llm->engine->multi_launches(); }

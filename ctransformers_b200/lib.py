@@ -107,7 +107,22 @@ EXTRA_PROTOTYPES = {
     "ctb_multi_launches": (C.c_long, [_P]),
     "ctb_multi_last_eval_ms": (C.c_double, [_P]),
     "ctb_multi_pack": (C.c_int, [C.c_int, _IP, _IP, _IP, C.c_int, C.c_int, _IP, C.c_int]),
+    "ctb_state_info": (C.c_int, [_P, C.c_size_t, _P]),
+    "ctb_llm_state_size": (C.c_size_t, [_P, C.c_int]),
+    "ctb_llm_save_state": (C.c_int, [_P, _IP, C.c_int, _P, C.c_size_t]),
+    "ctb_llm_load_state": (C.c_int, [_P, _P, C.c_size_t]),
+    "ctb_multi_state_size": (C.c_size_t, [_P, C.c_int]),
+    "ctb_multi_save": (C.c_int, [_P, C.c_int, _IP, C.c_int, _P, C.c_size_t]),
+    "ctb_multi_restore": (C.c_int, [_P, C.c_int, _P, C.c_size_t]),
+    "ctb_multi_fork": (C.c_int, [_P, C.c_int, C.c_int, _IP]),
 }
+
+
+class StateHeader(C.Structure):
+    """ctb_state_header (include/ctransformers_b200.h): the header of a sequence state."""
+    _fields_ = [("magic", C.c_uint32), ("version", C.c_uint32), ("n_layer", C.c_int32), ("n_head_kv", C.c_int32), ("head_dim", C.c_int32),
+                ("k_stride", C.c_int32), ("n_embd", C.c_int32), ("n_vocab", C.c_int32), ("n_tokens", C.c_int32), ("has_results", C.c_int32),
+                ("fingerprint", C.c_uint64)]
 
 
 def load_library(path: Optional[str] = None):

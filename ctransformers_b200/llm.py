@@ -13,7 +13,9 @@ from functools import partial
 from pathlib import Path
 from typing import Generator, List, Optional, Sequence, Union
 
+from . import state
 from .lib import ConfigStruct, load_library
+from .state import SequenceState
 
 import logging
 
@@ -191,6 +193,15 @@ class LLM:
         return self.ctransformers_llm_sample(arr, len(recent), _pick(top_k, cfg.top_k), _pick(top_p, cfg.top_p),
                                              _pick(temperature, cfg.temperature), _pick(repetition_penalty, cfg.repetition_penalty),
                                              _pick(seed, cfg.seed))
+
+    def save_state(self) -> SequenceState:
+        """What this LLM has evaluated (its tokens, K / V cache and last results), for load_state here or in any LLM or MultiLLM
+        of the same model file."""
+        return state.save(partial(self._lib.ctb_llm_state_size, self._llm), partial(self._lib.ctb_llm_save_state, self._llm), self._context)
+
+    def load_state(self, saved: SequenceState) -> None:
+        """Continues from a saved state exactly as if its tokens had just been evaluated here."""
+        self._context = state.restore(self._lib, saved, partial(self._lib.ctb_llm_load_state, self._llm))
 
     def reset(self) -> None:
         warnings.warn("`LLM.reset()` method is deprecated since 0.2.27. Please use high-level API.")

@@ -3,10 +3,13 @@ same config, bit for bit, while the slots listed in one eval share batched launc
 up to 32 tokens instead of one per token of every sequence."""
 from ctypes import c_int
 from pathlib import Path
-from typing import Dict, List, Optional, Sequence
+from functools import partial
+from typing import Dict, List, Optional, Sequence, Tuple
 
 from .lib import load_library
+from . import state
 from .llm import Config, Vector, _pick, is_gguf
+from .state import SequenceState
 
 
 class MultiLLM:
@@ -99,41 +102,79 @@ class MultiLLM:
     def last_eval_ms(self) -> float:
         return self._lib.ctb_multi_last_eval_ms(self._m)
 
-    def generate_many(self, prompts: Sequence[Sequence[int]], max_new_tokens: int, *, batch_size: Optional[int] = None,
-                      **sampling) -> List[List[int]]:
+    def fork(self, src: int, dsts: Sequence[int]) -> None:
+        """Each slot in dsts becomes a copy of slot src, device to device: its KV cache, last results and tokens."""
+        src, dsts = self._slot(src), [self._slot(d) for d in dsts]
+        if src in dsts:
+            raise ValueError(f"slot {src} cannot be forked into itself")
+        if self._lib.ctb_multi_fork(self._m, src, len(dsts), (c_int * max(len(dsts), 1))(*dsts)) != 0:
+            raise RuntimeError(f"Failed to fork slot {src}.")
+        for d in dsts:
+            self._context[d] = list(self._context[src])
+
+    def save(self, slot: int) -> SequenceState:
+        """What slot `slot` has evaluated, for restore into any slot here, another MultiLLM or an LLM of the same model file."""
+        slot = self._slot(slot)
+        return state.save(partial(self._lib.ctb_multi_state_size, self._m), partial(self._lib.ctb_multi_save, self._m, slot),
+                          self._context[slot])
+
+    def restore(self, slot: int, saved: SequenceState) -> None:
+        """The slot continues from a saved state exactly as if it had just evaluated the state's tokens."""
+        slot = self._slot(slot)
+        self._context[slot] = state.restore(self._lib, saved, partial(self._lib.ctb_multi_restore, self._m, slot))
+
+    def generate_many(self, prompts: Sequence[Sequence[int]], max_new_tokens: int, *, n: int = 1, seeds: Optional[Sequence[int]] = None,
+                      batch_size: Optional[int] = None, **sampling) -> list:
         """Generates for every prompt, up to n_slots at once: a sequence ends at EOS (not included) or after max_new_tokens, and
         its slot takes the next waiting prompt, whose prompt tokens then share launches with the other slots' decode tokens.
-        Each result equals LLM.generate of that prompt on a fresh LLM with the same sampling arguments."""
-        results: List[Optional[List[int]]] = [None] * len(prompts)
+        Each result equals LLM.generate of that prompt on a fresh LLM with the same sampling arguments.
+
+        n > 1 draws n samples of every prompt: the prompt is evaluated once, in one slot, which is then forked into n - 1 more;
+        sample j draws with seed seeds[j] (required: equal seeds draw equal samples).  The result of a prompt is then the list
+        of its n samples, sample j equal to LLM.generate(prompt, seed=seeds[j], ...) on a fresh LLM."""
+        if not 1 <= n <= self.n_slots:
+            raise ValueError(f"n = {n}: each prompt's samples need a slot each, and there are {self.n_slots}")
+        if (n > 1 or seeds is not None) and (seeds is None or len(seeds) != n):
+            raise ValueError(f"n = {n} samples per prompt need n seeds (equal seeds draw equal samples)")
+        results: List[List[Optional[List[int]]]] = [[None] * n for _ in prompts]
         waiting = list(range(len(prompts)))[::-1]
-        owner: Dict[int, int] = {}        # slot -> prompt index
+        owner: Dict[int, Tuple[int, int]] = {}   # slot -> (prompt index, sample index)
         pending: Dict[int, List[int]] = {}
-        for slot in range(self.n_slots):
-            if not waiting:
-                break
-            self.reset(slot)
-            i = waiting.pop()
-            owner[slot], pending[slot], results[i] = i, list(prompts[i]), []
+        forks: Dict[int, List[int]] = {}          # slot evaluating a prompt -> the slots it is forked into after that eval
+        free = list(range(self.n_slots))
+
+        def admit():
+            while waiting and len(free) >= n:
+                i, group = waiting.pop(), free[:n]
+                del free[:n]
+                self.reset(group[0])
+                pending[group[0]], forks[group[0]] = list(prompts[i]), group[1:]
+                for j, s in enumerate(group):
+                    owner[s], results[i][j] = (i, j), []
+
+        admit()
         while owner:
             self.eval(pending, batch_size=batch_size)
             pending = {}
+            for s, dsts in forks.items():
+                if dsts:
+                    self.fork(s, dsts)
+            forks = {}
             for slot in sorted(owner):
-                i = owner[slot]
-                tok = self.sample(slot, **sampling)
+                i, j = owner[slot]
+                tok = self.sample(slot, **(sampling if seeds is None else {**sampling, "seed": seeds[j]}))
                 if tok == self.eos_token_id or max_new_tokens <= 0:
                     done = True
                 else:
-                    results[i].append(tok)
-                    done = len(results[i]) >= max_new_tokens
+                    results[i][j].append(tok)
+                    done = len(results[i][j]) >= max_new_tokens
                     pending[slot] = [tok]
                 if done:
                     pending.pop(slot, None)
                     del owner[slot]
-                    if waiting:
-                        self.reset(slot)
-                        j = waiting.pop()
-                        owner[slot], pending[slot], results[j] = j, list(prompts[j]), []
-        return results
+                    free.append(slot)
+                    admit()
+        return results if n > 1 else [r[0] for r in results]
 
     def __del__(self):
         if self.__dict__.get("_m") is not None and self.__dict__.get("_lib") is not None:

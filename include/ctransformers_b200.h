@@ -215,6 +215,46 @@ double ctb_multi_last_eval_ms(ctb_multi* m);     /* CUDA-event time of the last 
  * slot's eval} (5 ints per token).  Returns the token count, or -count when cap is smaller. */
 int ctb_multi_pack(int n, const int* slots, const int* off, const int* n_past, int batch_size, int n_ctx, int* out, int cap);
 
+/* Sequence states: what a sequence has evaluated, as one self-describing blob that moves between slots of a handle, between
+ * handles of the same file whatever their context lengths and slot counts, and between LLM and ctb_multi.  Little-endian:
+ *   ctb_state_header
+ *   int32  tokens[n_tokens]                                 n_past = n_tokens
+ *   fp16   K[n_layer][n_head_kv][n_past][k_stride]          rotated K rows as the cache holds them (k_stride = head_dim rounded up
+ *                                                           to a multiple of 8: the first head_dim & ~31 channels lane-major, the
+ *                                                           rest in order, then zeros)
+ *   fp16   V[n_layer][n_head_kv * head_dim][n_pad]          V transposed, one row of positions per channel, in whole blocks of
+ *                                                           256 (n_pad = n_past rounded up to 256) permuted as the cache holds
+ *                                                           them: position t at (t & ~255) + (t & 31) * 8 + ((t >> 5) & 7);
+ *                                                           the entries of positions n_past .. n_pad - 1 are zero
+ *   float  logits[n_vocab], embeddings[n_embd]              only when has_results: the last eval's
+ * The fingerprint hashes (64-bit FNV-1a) the GGUF metadata, the tensor table and the first 4 KiB of every tensor's data, so a
+ * state of another file is refused even when the shapes agree.  A restore zeroes the positions from n_past on, so the slot equals
+ * a fresh one that evaluated the tokens; it needs n_past <= the context length.  Refusals (bad magic or version, a size that
+ * disagrees with the header, another model, n_past above the context) return -1 with the reason on stderr and leave the slot or
+ * LLM as it was.  The tensor-sharded mode has no states. */
+#define CTB_STATE_MAGIC 0x53425443u /* "CTBS" */
+#define CTB_STATE_VERSION 1u
+typedef struct ctb_state_header {
+  uint32_t magic, version;
+  int32_t n_layer, n_head_kv, head_dim, k_stride, n_embd, n_vocab;
+  int32_t n_tokens;    /* n_past */
+  int32_t has_results; /* 0 or 1 */
+  uint64_t fingerprint;
+} ctb_state_header;
+/* Host only: checks a blob's header and that size is exactly what it describes; 0 and *out filled, or -1 (+ stderr). */
+int ctb_state_info(const void* buf, size_t size, ctb_state_header* out);
+size_t ctb_llm_state_size(LLM* llm, int n_tokens);                 /* bytes of the state after these tokens; 0 on error */
+/* the LLM's state after it has evaluated tokens[0 .. n_tokens) (its n_past); 0, or -1 (+ stderr), e.g. when cap is smaller */
+int ctb_llm_save_state(LLM* llm, const int* tokens, int n_tokens, void* buf, size_t cap);
+/* After a load, sample and batch_eval behave as after an ordinary eval of the state's tokens, the greedy look-ahead included. */
+int ctb_llm_load_state(LLM* llm, const void* buf, size_t size);
+size_t ctb_multi_state_size(ctb_multi* m, int n_tokens);
+int ctb_multi_save(ctb_multi* m, int slot, const int* tokens, int n_tokens, void* buf, size_t cap);
+int ctb_multi_restore(ctb_multi* m, int slot, const void* buf, size_t size);
+/* Device to device: each of slots dsts[0 .. n) becomes a byte-identical copy of slot src (its whole KV region, last results and
+ * greedy pick), stream-ordered.  src must not be among dsts.  0, or -1 (+ stderr). */
+int ctb_multi_fork(ctb_multi* m, int src, int n, const int* dsts);
+
 #ifdef __cplusplus
 }
 #endif
