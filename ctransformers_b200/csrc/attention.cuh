@@ -585,8 +585,10 @@ static __global__ void __launch_bounds__(ATTN_THREADS) k_attn(const AttnParams p
 inline void (*attn_kernel(int hd))(const AttnParams) { return attn_fast_hd(hd) ? k_attn<false> : k_attn<true>; }
 
 // ----------------------------------------------------------------------------------------- argmax
-// Greedy pick over logits[0, n) by the first NT threads (named barrier BAR): the largest value, the lowest id among equal ones.
-// Thread 0 ends with the result in best / idx.  CG: the logits were written earlier in the same kernel (read them from L2).
+// Greedy pick over logits[0, n) by the first NT threads (named barrier BAR): the reference's top_k = 1, a scan that starts at
+// element 0 and moves on strictly greater values only.  That is the largest value, the lowest id among equal ones; NaNs never
+// win, and id 0 stays picked when nothing exceeds -inf or when logits[0] is NaN.  Thread 0 ends with the result in best / idx.
+// CG: the logits were written earlier in the same kernel (read them from L2).
 template <int NT, int BAR, bool CG>
 __device__ __forceinline__ void block_argmax(const float* logits, int n, float* bv /* [NT / 32] smem */, int* bi /* [NT / 32] smem */, float& best, int& idx) {
   best = -INFINITY;
@@ -604,9 +606,12 @@ __device__ __forceinline__ void block_argmax(const float* logits, int n, float* 
   }
   if ((threadIdx.x & 31) == 0) { bv[threadIdx.x >> 5] = best; bi[threadIdx.x >> 5] = idx; }
   bar_sync<BAR, NT>();
-  if (threadIdx.x == 0)
+  if (threadIdx.x == 0) {
     for (int w = 1; w < NT / 32; w++)
       if (bv[w] > best || (bv[w] == best && bi[w] < idx)) { best = bv[w]; idx = bi[w]; }
+    const float x0 = CG ? __ldcg(logits) : logits[0];
+    if (idx == 0x7fffffff || x0 != x0) { best = x0; idx = 0; }   // nothing above -inf, or a NaN at 0 that no value is greater than
+  }
 }
 
 // the decode state {token, position, step, n_total} after a greedy pick: the pick is the next token (and goes to
@@ -620,7 +625,8 @@ __device__ __forceinline__ void advance_state(int* state, int* out_tokens, int p
 }
 
 constexpr int ARGMAX_THREADS = 1024;
-// single block; writes the id of the largest logit (lowest id on ties) to out[0] and the number of logits equal to it to out[1]
+// single block; writes the greedy pick of block_argmax to out[0] and the number of logits equal to the picked one to out[1] (0 when
+// it is a NaN)
 static __global__ void k_argmax(const float* logits, int n, int* out) {
   __shared__ float bv[ARGMAX_THREADS / 32];
   __shared__ int bi[ARGMAX_THREADS / 32];

@@ -1037,7 +1037,7 @@ std::vector<float> Engine::logits_copy() {
 }
 
 int Engine::topk_candidates(const int* last, int n_last, float penalty, int k, int* ids, float* logits) {
-  if (n_last > SG_MAX_LAST || k < 1 || k > SG_MAX_OUT / 2) return -1;
+  if (!sg_accepts(n_last, k)) return -1;
   DeviceGuard dev_guard(device_);
   if (!d_sample_) {
     d_sample_ = (SampleGpuOut*)alloc(sizeof(SampleGpuOut));
@@ -1049,16 +1049,13 @@ int Engine::topk_candidates(const int* last, int n_last, float penalty, int k, i
   int* h_last = (int*)(h_sample_ + 1);
   for (int i = 0; i < n_last; i++) h_last[i] = last[i];
   if (n_last > 0) CTB_CUDA(cudaMemcpyAsync(d_last_, h_last, (size_t)n_last * 4, cudaMemcpyHostToDevice, stream_));
-  k_sample_topk<<<1, SG_THREADS, 0, stream_>>>(d_logits_keep_, hp_.n_vocab, d_last_, n_last, penalty, std::min(k, hp_.n_vocab), d_sample_);
+  sg_launch(d_logits_keep_, hp_.n_vocab, d_last_, n_last, penalty, k, d_sample_, stream_);
   CTB_CUDA(cudaGetLastError());
   CTB_CUDA(cudaMemcpyAsync(h_sample_, d_sample_, sizeof(SampleGpuOut), cudaMemcpyDeviceToHost, stream_));
   CTB_CUDA(cudaEventRecord(ev_sample_, stream_));
   launch_deferred_spec();                          // the look-ahead step runs while the host finishes the draw
   CTB_CUDA(cudaEventSynchronize(ev_sample_));
-  const int n = h_sample_->count;
-  if (n < 0 || n > SG_MAX_OUT) return -1;
-  for (int i = 0; i < n; i++) { ids[i] = h_sample_->id[i]; logits[i] = h_sample_->logit[i]; }
-  return n;
+  return sg_take(*h_sample_, ids, logits);
 }
 
 void Engine::finish_eval(int next_pos, bool hit) {

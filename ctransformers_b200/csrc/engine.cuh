@@ -111,7 +111,7 @@ class Engine {
   bool lazy_logits() const { return !eager_; }
   std::vector<float> logits_copy();   // this eval's logits without switching the engine to eager host views
   // Device half of the sampler (sample_gpu.cuh): candidates >= the k-th largest penalised logit.  Returns their count, or -1
-  // when the device path does not apply (window too long, k too large).
+  // when the device path does not apply (window too long, k too large, a NaN among the logits, more than SG_MAX_OUT candidates).
   int topk_candidates(const int* last, int n_last, float penalty, int k, int* ids, float* logits);
   // The last eval's greedy pick when the engine has it and it is unambiguous (a unique maximum), else -1.
   int greedy_pick();

@@ -4,6 +4,7 @@
 #include <cmath>
 #include <cstdio>
 #include <cstring>
+#include <ctime>
 #include <functional>
 #include <memory>
 #include <stdexcept>
@@ -15,6 +16,8 @@
 #include "matvec.cuh"
 #include "prefill.cuh"
 #include "repack.cuh"
+#include "sample_gpu.cuh"
+#include "sampler.hpp"
 #include "stream.cuh"
 #include "tables.hpp"
 
@@ -228,6 +231,25 @@ void kv_from_device(const std::vector<uint16_t>& kp, const std::vector<uint16_t>
       for (int e = 0; e < hd; e++) kref[((size_t)t * n_kv + kh) * hd + e] = kp[k_row(kh, t, n_ctx, hd) + k_perm(e, hd)];
   for (int ch = 0; ch < n_kv * hd; ch++)
     for (int t = 0; t < n_ctx; t++) vref[(size_t)ch * n_ctx + t] = vp[(size_t)ch * cp + v_perm(t)];
+}
+
+// k_argmax over n device logits, as Engine::after_eval launches it: {pick, logits equal to the picked one}
+void argmax_on_device(const float* d_logits, int n, int* pick2) {
+  DevBuf dout(8);
+  k_argmax<<<1, ARGMAX_THREADS>>>(d_logits, n, dout.as<int>());
+  OPS_CUDA(cudaGetLastError());
+  OPS_CUDA(cudaMemcpy(pick2, dout.p, 8, cudaMemcpyDeviceToHost));
+}
+
+// k_sample_topk over n device logits, as Engine::topk_candidates launches it
+SampleGpuOut topk_on_device(const float* d_logits, int n, const int* last, int n_last, float penalty, int k) {
+  DevBuf dlast((size_t)std::max(n_last, 1) * 4), dout(sizeof(SampleGpuOut));
+  if (n_last > 0) OPS_CUDA(cudaMemcpy(dlast.p, last, (size_t)n_last * 4, cudaMemcpyHostToDevice));
+  sg_launch(d_logits, n, dlast.as<int>(), n_last, penalty, k, dout.as<SampleGpuOut>(), 0);
+  OPS_CUDA(cudaGetLastError());
+  SampleGpuOut o;
+  OPS_CUDA(cudaMemcpy(&o, dout.p, sizeof(o), cudaMemcpyDeviceToHost));
+  return o;
 }
 
 }  // namespace
@@ -615,6 +637,72 @@ int ctb_get_row(int type, const void* table_blocks, int K, int n_rows, int row, 
     OPS_CUDA(cudaGetLastError());
     OPS_CUDA(cudaMemcpy(out, dout.p, (size_t)K * 4, cudaMemcpyDeviceToHost));
   });
+}
+
+int ctb_argmax_path(int path, const float* logits, int n, int* out) {
+  return guarded("ctb_argmax_path", [&] {
+    if (path < 0 || path > 1) throw std::runtime_error("unknown argmax path " + std::to_string(path));
+    if (n < 1) throw std::runtime_error("no logits");
+    DevBuf dlog((size_t)n * 4);
+    OPS_CUDA(cudaMemcpy(dlog.p, logits, (size_t)n * 4, cudaMemcpyHostToDevice));
+    if (path == 0) {
+      argmax_on_device(dlog.as<float>(), n, out);
+      return;
+    }
+    // one PH_PICK phase of the step kernel on the decode state out[0..4], as the last phase of the engine's step program
+    const int step = out[2];
+    if (step < 0 || step >= (1 << 20)) throw std::runtime_error("step out of range");
+    DevBuf dstate(5 * 4), dtok((size_t)(step + 1) * 4);
+    OPS_CUDA(cudaMemcpy(dstate.p, out, 5 * 4, cudaMemcpyHostToDevice));
+    OPS_CUDA(cudaMemset(dtok.p, 0xff, (size_t)(step + 1) * 4));
+    Phase ph{};
+    ph.kind = PH_PICK;
+    ph.pk.logits = dlog.as<float>(); ph.pk.state = dstate.as<int>(); ph.pk.out_tokens = dtok.as<int>(); ph.pk.n = n;
+    run_phases({ph});
+    OPS_CUDA(cudaMemcpy(out, dstate.p, 5 * 4, cudaMemcpyDeviceToHost));
+    OPS_CUDA(cudaMemcpy(out + 5, dtok.as<int>() + step, 4, cudaMemcpyDeviceToHost));
+  });
+}
+
+int ctb_sample_topk(const float* logits, int n, const int* last_tokens, int n_last, float repetition_penalty, int k, int* ids, float* lg) {
+  int count = -1;
+  const int rc = guarded("ctb_sample_topk", [&] {
+    if (n < 1 || !sg_accepts(n_last, k)) throw std::runtime_error("n < 1, or a window or k the device sampler does not take");
+    DevBuf dlog((size_t)n * 4);
+    OPS_CUDA(cudaMemcpy(dlog.p, logits, (size_t)n * 4, cudaMemcpyHostToDevice));
+    const SampleGpuOut o = topk_on_device(dlog.as<float>(), n, last_tokens, n_last, repetition_penalty, k);
+    if (o.nan) { count = -2; return; }
+    count = o.count;
+    for (int i = 0; i < std::min(o.count, SG_MAX_OUT); i++) { ids[i] = o.id[i]; lg[i] = o.logit[i]; }
+  });
+  return rc == 0 ? count : -1;
+}
+
+int ctb_sample_device(const float* logits, int n, const int* last_tokens, int n_last, int top_k, float top_p, float temperature,
+                      float repetition_penalty, int seed, int* used_device) {
+  int tok = -1;
+  const int rc = guarded("ctb_sample_device", [&] {
+    if (n < 1) throw std::runtime_error("no logits");
+    if (seed < 0) seed = (int)time(nullptr);
+    std::mt19937 rng((unsigned)seed);
+    DevBuf dlog((size_t)n * 4);
+    OPS_CUDA(cudaMemcpy(dlog.p, logits, (size_t)n * 4, cudaMemcpyHostToDevice));
+    bool dev = false;
+    tok = sample_lazy(
+        n, last_tokens, n_last, top_k, top_p, temperature, repetition_penalty, rng, dev,
+        [&] {
+          int pk[2];
+          argmax_on_device(dlog.as<float>(), n, pk);
+          return pk[1] == 1 ? pk[0] : -1;   // the rule of Engine::greedy_pick
+        },
+        [&](const int* last, int nl, float pen, int k, int* i, float* l) {
+          if (!sg_accepts(nl, k)) return -1;
+          return sg_take(topk_on_device(dlog.as<float>(), n, last, nl, pen, k), i, l);
+        },
+        [&] { return std::vector<float>(logits, logits + n); });
+    *used_device = dev ? 1 : 0;
+  });
+  return rc == 0 ? tok : -1;
 }
 
 }  // extern "C"

@@ -85,4 +85,32 @@ inline bool device_candidates_usable(const int* ids, const float* logits, int co
   return true;
 }
 
+// The sampler chain for logits that are still on the device (ctransformers_llm_sample before anybody asked for a host view):
+// penalty + top-k run on the device and only the candidates come back; the host finishes with the same code as sample_token.
+//   pick()                                   the device's greedy pick when it is the only largest logit, else < 0
+//   topk(last, n_last, penalty, k, ids, lg)  the device candidates (Engine::topk_candidates): their count, < 0 when the device
+//                                            cannot answer
+//   all()                                    the full logits on the host, as a std::vector<float>
+// used_device: whether the device answered (false: the host sampler ran on all()).
+template <class Pick, class TopK, class All>
+int sample_lazy(int n_vocab, const int* last, int n_last, int top_k, float top_p, float temperature, float penalty, std::mt19937& rng,
+                bool& used_device, Pick&& pick, TopK&& topk, All&& all) {
+  used_device = true;
+  if (top_k == 1 && (penalty == 1.0f || n_last <= 0)) {
+    // greedy: one candidate survives top-k, so top-p / temperature / the draw cannot change it (llama.cpp:3832-3857, 4215-4240).
+    // Equal maxima fall through (std::partial_sort's choice among equals is the reference's).
+    const int p = pick();
+    if (p >= 0) return p;
+  }
+  int ids[256];
+  float lg[256];
+  const int count = topk(last, n_last, penalty, top_k, ids, lg);
+  std::vector<Candidate> c;
+  if (count > 0 && device_candidates_usable(ids, lg, count, top_k, n_vocab, c)) return sample_candidates(c, top_k, top_p, temperature, rng);
+  // ambiguous cut (equal logits, NaN): the reference's own sort over all candidates decides — host path on a private copy
+  used_device = false;
+  const std::vector<float> v = all();
+  return sample_token(v.data(), n_vocab, last, n_last, top_k, top_p, temperature, penalty, rng);
+}
+
 }  // namespace ctb

@@ -89,6 +89,9 @@ EXTRA_PROTOTYPES = {
     "ctb_ffn_gate": (C.c_int, [C.c_int, _P, _P, _P, _P, C.c_int, C.c_int]),
     "ctb_matvec_partition": (C.c_int, [_IP, _IP, C.c_int, C.c_int, C.c_int, _IP, _IP]),
     "ctb_get_row": (C.c_int, [C.c_int, _P, C.c_int, C.c_int, C.c_int, _P]),
+    "ctb_argmax_path": (C.c_int, [C.c_int, _P, C.c_int, _IP]),
+    "ctb_sample_topk": (C.c_int, [_P, C.c_int, _IP, C.c_int, C.c_float, C.c_int, _IP, _P]),
+    "ctb_sample_device": (C.c_int, [_P, C.c_int, _IP, C.c_int, C.c_int, C.c_float, C.c_float, C.c_float, C.c_int, _IP]),
     "ctb_vocab_load": (_P, [C.c_char_p]),
     "ctb_vocab_free": (None, [_P]),
     "ctb_vocab_size": (C.c_int, [_P]),

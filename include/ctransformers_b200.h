@@ -187,6 +187,25 @@ int ctb_matvec_partition(const int* types, const int* rows, int nseg, int K, int
 
 int ctb_get_row(int type, const void* table_blocks, int K, int n_rows, int row, float* out);
 
+/* The greedy pick of n logits, the reference's top_k = 1 (std::partial_sort of one element: the first largest value; id 0 when
+ * nothing exceeds -inf or logits[0] is NaN), through one of the engine's two implementations:
+ *   path 0  k_argmax (the look-ahead pick, the un-fused PICK op, each multi-sequence slot's pick): out = {pick, number of logits
+ *           equal to the picked one}
+ *   path 1  the PH_PICK phase of the persistent step kernel (ctb_llm_decode_greedy's token feedback): out[0..4] is the decode
+ *           state {token, position, step, n_total, pick} in and out, advanced as after a greedy step; out[5] = out_tokens[step]
+ * 0 on success, -1 (with a message on stderr) for an unknown path or n < 1. */
+int ctb_argmax_path(int path, const float* logits, int n, int* out);
+/* The device half of the sampler (k_sample_topk), launched as Engine::topk_candidates launches it: the repetition penalty
+ * (llama.cpp:4025-4055) over the ids in last_tokens, then every id whose penalised logit is >= the min(k, n)-th largest.  Returns
+ * their count (ids / lg get at most 256 of them, in no particular order), -2 when some penalised logit is NaN, -1 for what the
+ * kernel does not take (n_last > 256, k < 1, k > 128, n < 1). */
+int ctb_sample_topk(const float* logits, int n, const int* last_tokens, int n_last, float repetition_penalty, int k, int* ids, float* lg);
+/* ctransformers_llm_sample's chain for logits that live on the device, on an uploaded copy of logits: the greedy shortcut on a
+ * unique k_argmax pick, else the device top-k when its cut is unambiguous, else the host sampler on all logits.  Returns the
+ * token (the one ctb_sample draws with the same arguments), -1 on error; *used_device = 1 when the device answered. */
+int ctb_sample_device(const float* logits, int n, const int* last_tokens, int n_last, int top_k, float top_p, float temperature,
+                      float repetition_penalty, int seed, int* used_device);
+
 /* Multi-sequence decoding: one handle owns n_slots sequence slots, each of which behaves like a fresh single-sequence LLM with
  * the same config, and every eval's slots share batched launches (one pass over the weights per launch of up to 32 tokens).
  * After every eval a slot's logits, embeddings, greedy pick and sampler draws are bit-identical to what a single-sequence LLM
