@@ -12,6 +12,7 @@
 #include "prefill.cuh"
 #include "repack.cuh"
 #include "sample_gpu.cuh"
+#include "score_gpu.cuh"
 #include "stream.cuh"
 #include "tables.hpp"
 #include "tp_nccl.hpp"
@@ -87,6 +88,11 @@ struct PrefillState {
   float *d_mlogits = nullptr, *d_membd = nullptr;   // [n_seq][n_vocab], [n_seq][n_embd]: each slot's last results
   int* d_mpick = nullptr;                           // [n_seq][2]: k_argmax of each slot's logits
   long m_launches = 0;
+  // rows of every token (RowSink), single sequence: the single-sequence program followed by a K-quant head's QUANT + GEMM phases,
+  // every token's logits row of a launch in Engine::d_rows_ (built on first use)
+  PPhase* d_rprog = nullptr;
+  int n_rphases = 0;
+  bool rq3 = false, rtried = false;
   ~PrefillState() {
     for (void* b : bufs) cudaFree(b);
     if (h_state) cudaFreeHost(h_state);
@@ -456,6 +462,10 @@ void Engine::release() {
   if (h_stage_) cudaFreeHost(h_stage_);
   h_stage_ = nullptr;
   stage_cap_ = 0;
+  if (d_rows_) cudaFree(d_rows_);
+  if (d_score_) cudaFree(d_score_);
+  if (h_score_) cudaFreeHost(h_score_);
+  d_rows_ = nullptr; d_score_ = h_score_ = nullptr; score_cap_ = 0;
   if (ev_pick_) cudaEventDestroy(ev_pick_);
   if (ev_sample_) cudaEventDestroy(ev_sample_);
   ev_sample_ = nullptr;
@@ -1076,9 +1086,122 @@ void Engine::finish_eval(int next_pos, bool hit) {
   stats.spec_hits += hit ? 1 : 0;
 }
 
-void Engine::eval_list(const int* tokens, const int* pos, const int* n_total, int n) {
+// ---- rows of every token (RowSink)
+void Engine::rows_begin(const RowSink* rows, int n) {
+  sink_ = nullptr; rows_pending_ = 0; rows_done_ = 0; rows_n_ = n;
+  if (!rows) return;
+  if (tp_.world > 1) throw std::runtime_error("the tensor-sharded mode keeps no per-token rows");
+  if (!d_rows_) CTB_CUDA(cudaMalloc(&d_rows_, (size_t)PB_T * hp_.n_vocab * 4));
+  if (rows->targets) {
+    if (n > score_cap_) {
+      if (d_score_) CTB_CUDA(cudaFree(d_score_));
+      if (h_score_) CTB_CUDA(cudaFreeHost(h_score_));
+      d_score_ = h_score_ = nullptr; score_cap_ = 0;
+      const int cap = std::max(n, 1024);
+      CTB_CUDA(cudaMalloc(&d_score_, (size_t)cap * 16));
+      CTB_CUDA(cudaMallocHost(&h_score_, (size_t)cap * 16));
+      score_cap_ = cap;
+    }
+    d_lp_ = (double*)d_score_; d_tgt_ = (int*)(d_score_ + (size_t)score_cap_ * 8); d_gr_ = d_tgt_ + score_cap_;
+    memcpy(h_score_ + (size_t)score_cap_ * 8, rows->targets, (size_t)n * 4);
+    CTB_CUDA(cudaMemcpyAsync(d_tgt_, h_score_ + (size_t)score_cap_ * 8, (size_t)n * 4, cudaMemcpyHostToDevice, stream_));
+  }
+  sink_ = rows;
+}
+
+void Engine::rows_take(const float* src, int m) {
+  if (rows_done_ + m > rows_n_) throw std::runtime_error("rows: more rows than tokens");
+  const size_t nv = (size_t)hp_.n_vocab;
+  if (sink_->host) {
+    CTB_CUDA(cudaMemcpyAsync(sink_->host + (size_t)rows_done_ * nv, src, (size_t)m * nv * 4, cudaMemcpyDeviceToHost, stream_));
+  } else {
+    rl_launch(src, m, hp_.n_vocab, d_tgt_ + rows_done_, d_lp_ + rows_done_, d_gr_ + rows_done_, stream_);
+    CTB_CUDA(cudaGetLastError());
+  }
+  rows_done_ += m;
+}
+
+void Engine::rows_push(const float* row) {
+  CTB_CUDA(cudaMemcpyAsync(d_rows_ + (size_t)rows_pending_ * hp_.n_vocab, row, (size_t)hp_.n_vocab * 4, cudaMemcpyDeviceToDevice, stream_));
+  if (++rows_pending_ == PB_T) rows_drain();
+}
+
+void Engine::rows_drain() {
+  if (!sink_ || !rows_pending_) return;
+  const int m = rows_pending_;
+  rows_pending_ = 0;
+  rows_take(d_rows_, m);
+}
+
+void Engine::rows_finish() {
+  if (!sink_) return;
+  rows_drain();
+  if (rows_done_ != rows_n_) throw std::runtime_error("rows: " + std::to_string(rows_done_) + " rows for " + std::to_string(rows_n_) + " tokens");
+  if (sink_->targets) {
+    CTB_CUDA(cudaMemcpyAsync(h_score_, d_lp_, (size_t)rows_n_ * 8, cudaMemcpyDeviceToHost, stream_));
+    CTB_CUDA(cudaMemcpyAsync(h_score_ + (size_t)score_cap_ * 12, d_gr_, (size_t)rows_n_ * 4, cudaMemcpyDeviceToHost, stream_));
+  }
+}
+
+void Engine::rows_end() {
+  if (sink_ && sink_->targets) {
+    if (sink_->logprob) memcpy(sink_->logprob, h_score_, (size_t)rows_n_ * 8);
+    if (sink_->greedy) memcpy(sink_->greedy, h_score_ + (size_t)score_cap_ * 12, (size_t)rows_n_ * 4);
+  }
+  sink_ = nullptr;
+}
+
+void Engine::score_kept(int target, double* logprob, int* greedy) {
+  DeviceGuard dev_guard(device_);
+  RowSink s;
+  s.targets = &target; s.logprob = logprob; s.greedy = greedy;
+  struct Release { Engine* e; ~Release() { e->sink_ = nullptr; } } release{this};
+  rows_begin(&s, 1);
+  rows_take(d_logits_keep_, 1);
+  rows_finish();
+  CTB_CUDA(cudaStreamSynchronize(stream_));
+  rows_end();
+}
+
+// The single-sequence program followed by the output head's QUANT + GEMM phases, built the way ensure_prefill ends the
+// multi-sequence program: the head runs over every token of the launch and leaves its rows in d_rows_.  The embeddings stay the
+// last token's (head_from).  False for a head that is not a K-quant: its rows then come from head_from, one row at a time.
+bool Engine::ensure_rows_prog() {
+  PrefillState& P = *pf_;
+  if (P.rtried) return P.d_rprog != nullptr;
+  P.rtried = true;
+  const StepOp& head = ops_[n_body_];
+  if (!head.stream) return false;
+  std::vector<PPhase> rprog(P.n_phases);
+  CTB_CUDA(cudaMemcpy(rprog.data(), P.d_prog, rprog.size() * sizeof(PPhase), cudaMemcpyDeviceToHost));
+  const float* hx = head.ph.mv.x;
+  auto bat = [&](const float* p, int& ld) -> float* {
+    if (!p) { ld = 0; return nullptr; }
+    if (p == hx) { ld = hp_.n_embd; return P.x_final; }
+    if (p == d_logits_) { ld = hp_.n_vocab; return d_rows_; }
+    throw std::runtime_error("rows: pointer outside the output head's buffers");
+  };
+  auto dalloc = [&](size_t bytes) {
+    void* p = nullptr;
+    CTB_CUDA(cudaMalloc(&p, bytes));
+    P.bufs.push_back(p);
+    CTB_CUDA(cudaMemset(p, 0, bytes));
+    return p;
+  };
+  pb_matvec_phases(head.ph.mv, (uint8_t*)dalloc(pb_qbuf_bytes(head.ph.mv.K)), P.d_state, bat, rprog);
+  P.n_rphases = (int)rprog.size();
+  P.rq3 = pstep_q3(rprog);
+  PPhase* d = (PPhase*)dalloc((rprog.size() + 1) * sizeof(PPhase));
+  CTB_CUDA(cudaMemcpy(d, rprog.data(), rprog.size() * sizeof(PPhase), cudaMemcpyHostToDevice));
+  P.d_rprog = d;
+  return true;
+}
+
+void Engine::eval_list(const int* tokens, const int* pos, const int* n_total, int n, const RowSink* rows) {
   if (n <= 0) return;
   DeviceGuard dev_guard(device_);
+  struct Release { Engine* e; ~Release() { e->sink_ = nullptr; } } release{this};   // a failed eval leaves no sink behind
+  rows_begin(rows, n);
   if (h_state_cap_ < 1) { h_state_cap_ = 512; CTB_CUDA(cudaMallocHost(&h_state_, (size_t)h_state_cap_ * 16)); }
   bool hit = false;
   if (spec_pos_ >= 0) {
@@ -1105,18 +1228,23 @@ void Engine::eval_list(const int* tokens, const int* pos, const int* n_total, in
       if (j - i >= prefill_min_ && pos[i] < hp_.n_ctx && ensure_prefill()) {
         for (int b = i; b < j; b += PB_T) {
           const int m = std::min(PB_T, j - b);
-          prefill_batch(tokens + b, pos + b, n_total + b, m, b + m == n);
+          prefill_batch(tokens + b, pos + b, n_total + b, m, b + m == n, sink_ != nullptr);
         }
       } else {
         for (int k = i; k < j; k++) {
-          decode_one(tokens[k], pos[k], n_total[k], k == n - 1);
+          decode_one(tokens[k], pos[k], n_total[k], k == n - 1 || sink_);   // (the full step's body is the same as the short one's)
+          if (sink_) rows_push(d_logits_);
           if ((k - i) % 128 == 127) CTB_CUDA(cudaStreamSynchronize(stream_));   // keeps the pinned state ring from wrapping under the GPU
         }
       }
       i = j;
     }
+  } else if (sink_) {
+    rows_push(d_logits_);   // the look-ahead step (graph_full_) computed this token's row
   }   // else: the step for this token at this position is already in the stream
+  rows_finish();
   finish_eval(pos[n - 1] + 1, hit);
+  rows_end();
 }
 
 bool Engine::ensure_prefill() {
@@ -1211,8 +1339,11 @@ bool Engine::ensure_prefill() {
 
 // n <= PB_T tokens at consecutive positions through all layers in one launch; `last`: the list ends here, so the head
 // mat-vec (logits + final-norm hidden state of the last token) follows on the single-token kernel.
-void Engine::prefill_batch(const int* tokens, const int* pos, const int* n_total, int n, bool last) {
+// rows: every token's logits row goes to the sink (RowSink), from the launch itself (ensure_rows_prog) or from head_from per row.
+void Engine::prefill_batch(const int* tokens, const int* pos, const int* n_total, int n, bool last, bool rows) {
   PrefillState& P = *pf_;
+  const bool rp = rows && ensure_rows_prog();
+  if (rp) rows_drain();   // the launch writes d_rows_
   if (P.h_next % PF_RING == PF_RING - 1) CTB_CUDA(cudaStreamSynchronize(stream_));   // pinned state ring
   int* st = P.h_state + (size_t)(P.h_next++ % PF_RING) * (PB_T * 4 + 4);
   for (int i = 0; i < PB_T; i++) {
@@ -1221,8 +1352,18 @@ void Engine::prefill_batch(const int* tokens, const int* pos, const int* n_total
   }
   st[PB_T * 4] = n;
   CTB_CUDA(cudaMemcpyAsync(P.d_state, st, (PB_T * 4 + 4) * 4, cudaMemcpyHostToDevice, stream_));
-  CTB_CUDA(launch_pstep(step_grid_, P.n_slots, P.smem, stream_, P.d_prog, P.n_phases, d_sync_, P.q3));
+  if (rp) CTB_CUDA(launch_pstep(step_grid_, P.n_slots, P.smem, stream_, P.d_rprog, P.n_rphases, d_sync_, P.rq3));
+  else CTB_CUDA(launch_pstep(step_grid_, P.n_slots, P.smem, stream_, P.d_prog, P.n_phases, d_sync_, P.q3));
   prefill_launches_++;
+  if (rp) {
+    rows_pending_ = n;
+    rows_drain();
+  } else if (rows) {
+    for (int r = 0; r < n; r++) {
+      head_from(P.x_final + (size_t)r * hp_.n_embd);
+      rows_push(d_logits_);
+    }
+  }
   if (last) head_from(P.x_final + (size_t)(n - 1) * hp_.n_embd);
 }
 
@@ -1248,10 +1389,12 @@ std::string Engine::multi_refusal() {
   return "";
 }
 
-void Engine::multi_eval(const std::vector<MultiTok>& toks, const std::vector<int>& starts) {
+void Engine::multi_eval(const std::vector<MultiTok>& toks, const std::vector<int>& starts, const RowSink* rows) {
   DeviceGuard dev_guard(device_);
   if (hp_.n_seq < 2 || !ensure_prefill() || !pf_->d_mprog) throw std::runtime_error("this engine has no multi-sequence path");
   PrefillState& P = *pf_;
+  struct Release { Engine* e; ~Release() { e->sink_ = nullptr; } } release{this};
+  rows_begin(rows, (int)toks.size());
   const int hd = hp_.head_dim(), n_embd = hp_.n_embd, n_vocab = hp_.n_vocab;
   const size_t kslot = (size_t)hp_.n_layer * hp_.n_ctx * nkv_ * k_stride(hd), vslot = (size_t)hp_.n_layer * kv_ctx_pad(hp_.n_ctx) * nkv_ * hd;
   if (kslot > 0xffffffffu || vslot > 0xffffffffu) throw std::runtime_error("multi-sequence: a slot's KV region is too large");
@@ -1270,9 +1413,10 @@ void Engine::multi_eval(const std::vector<MultiTok>& toks, const std::vector<int
     CTB_CUDA(cudaMemcpyAsync(P.d_mstate, st, PB_STATE_MS * 4, cudaMemcpyHostToDevice, stream_));
     CTB_CUDA(launch_pstep(step_grid_, P.n_slots, P.smem, stream_, P.d_mprog, P.n_mphases, d_sync_, P.mq3, true));
     P.m_launches++;
+    if (sink_ && P.mhead) rows_take(P.logits_b, n);   // every token's row of the launch
     for (int r = 0; r < n; r++) {
       const MultiTok& t = toks[a + r];
-      if (!t.last) continue;   // (its logits, if the launch computed them, are dropped)
+      if (!t.last && !(sink_ && !P.mhead)) continue;   // (its logits, if the launch computed them, are dropped)
       float* lg = P.d_mlogits + (size_t)t.slot * n_vocab;
       float* em = P.d_membd + (size_t)t.slot * n_embd;
       const float* lsrc = d_logits_;
@@ -1282,15 +1426,19 @@ void Engine::multi_eval(const std::vector<MultiTok>& toks, const std::vector<int
         esrc = P.embd_b + (size_t)r * n_embd;
       } else {
         head_from(P.x_final + (size_t)r * n_embd);   // a head that is not a K-quant: k_matvec, one row at a time
+        if (sink_) rows_push(d_logits_);
       }
+      if (!t.last) continue;
       CTB_CUDA(cudaMemcpyAsync(lg, lsrc, (size_t)n_vocab * 4, cudaMemcpyDeviceToDevice, stream_));
       CTB_CUDA(cudaMemcpyAsync(em, esrc, (size_t)n_embd * 4, cudaMemcpyDeviceToDevice, stream_));
       k_argmax<<<1, ARGMAX_THREADS, 0, stream_>>>(lg, n_vocab, P.d_mpick + 2 * t.slot);
       CTB_CUDA(cudaGetLastError());
     }
   }
+  rows_finish();
   CTB_CUDA(cudaEventRecord(ev1_, stream_));
   CTB_CUDA(cudaEventSynchronize(ev1_));
+  rows_end();
   float ms = 0;
   cudaEventElapsedTime(&ms, ev0_, ev1_);
   stats.last_eval_ms = ms;

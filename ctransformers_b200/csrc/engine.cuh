@@ -58,6 +58,16 @@ struct PrefillState;
 struct MultiTok { int slot, token, pos, n_total; bool last; };
 constexpr int MULTI_LAUNCH_TOKENS = 32;   // tokens of one batched launch (prefill.cuh PB_T)
 
+// Where an eval's per-token logits rows go (the reference's logits_all, llama.cpp:2949-2960): every evaluated token's row, in
+// call order, either copied to host[i * n_vocab] or reduced on the device by k_row_logprob (score_gpu.cuh) against
+// targets[i] into logprob[i] / greedy[i].  Exactly one of host / targets is set.
+struct RowSink {
+  float* host = nullptr;
+  const int* targets = nullptr;
+  double* logprob = nullptr;
+  int* greedy = nullptr;
+};
+
 struct EvalStats { double last_eval_ms = 0; long launches = 0; size_t weight_bytes_per_token = 0; long spec_hits = 0; double load_ms = 0; size_t load_bytes = 0; };
 
 class Engine {
@@ -71,7 +81,10 @@ class Engine {
   void eval(const int* tokens, int n, int n_past);
   // Evaluate a token list with explicit per-token position and n_total (= n_past + N of the reference eval call the token
   // belongs to, llm.h:40-54): consecutive positions go through the batched prefill kernel, PB_T tokens per launch.
-  void eval_list(const int* tokens, const int* pos, const int* n_total, int n);
+  // rows: also keep every token's logits row (RowSink); logits() / embeddings() / the greedy look-ahead come out the same.
+  void eval_list(const int* tokens, const int* pos, const int* n_total, int n, const RowSink* rows = nullptr);
+  // k_row_logprob on the last eval's kept logits (what logits() holds) against one target
+  void score_kept(int target, double* logprob, int* greedy);
   // n_steps greedy decode steps entirely on the device stream (token feedback through k_argmax);
   // out_tokens[n_steps] receives the picked ids.  Returns device-timed milliseconds for the steps.
   double decode_greedy(int first_token, int n_past, int n_steps, int* out_tokens);
@@ -84,7 +97,8 @@ class Engine {
   // it can.  multi_eval: tokens [starts[i], starts[i+1]) of toks share batched launch i (a slot's tokens within one launch at
   // consecutive positions); afterwards each slot whose eval ended holds its logits, embeddings and greedy pick on the device.
   std::string multi_refusal();
-  void multi_eval(const std::vector<MultiTok>& toks, const std::vector<int>& starts);
+  // rows: the row of every listed token, in the order of toks
+  void multi_eval(const std::vector<MultiTok>& toks, const std::vector<int>& starts, const RowSink* rows = nullptr);
   void multi_fetch(int slot, float* logits, float* embd);   // host copies of the slot's last results
   void multi_pick(int slot, int* out2);                     // {arg-max (lowest id), logits equal to the maximum}
   void multi_reset(int slot);                               // zero the slot's KV region: a reused slot is a fresh one
@@ -211,7 +225,23 @@ class Engine {
   long prefill_launches_ = 0;    // k_pstep launches so far
   long single_steps_ = 0;        // tokens of batch_eval that went through the single-token step
   bool ensure_prefill();
-  void prefill_batch(const int* tokens, const int* pos, const int* n_total, int n, bool last);
+  void prefill_batch(const int* tokens, const int* pos, const int* n_total, int n, bool last, bool rows = false);
+  // rows of an eval (RowSink), allocated on first use outside the arena: d_rows_ holds up to PB_T rows on their way out
+  const RowSink* sink_ = nullptr;
+  float* d_rows_ = nullptr;
+  int rows_pending_ = 0, rows_done_ = 0;
+  int rows_n_ = 0;
+  uint8_t *d_score_ = nullptr, *h_score_ = nullptr;   // [cap] doubles logprob, [cap] ints target, [cap] ints greedy; device and pinned
+  int score_cap_ = 0;
+  double* d_lp_ = nullptr;
+  int *d_tgt_ = nullptr, *d_gr_ = nullptr;
+  void rows_begin(const RowSink* rows, int n);
+  void rows_finish();                        // enqueue the scores' copy to the host (before finish_eval's event)
+  void rows_take(const float* src, int m);   // m rows at src (n_vocab apart) leave for the sink
+  void rows_push(const float* row);          // one row through d_rows_
+  void rows_drain();
+  void rows_end();                           // after the stream is synchronised: the scores to the caller; the sink is released
+  bool ensure_rows_prog();
   void decode_one(int token, int pos, int n_total, bool with_logits);
   void head_from(const float* row);   // the output head (un-fused, as the single-token schedule launches it) on one hidden row
   void finish_eval(int next_pos, bool hit);

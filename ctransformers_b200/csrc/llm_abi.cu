@@ -490,6 +490,73 @@ int ctb_llm_load_state(LLM* llm, const void* buf, size_t size) {
   } catch (const std::exception& e) { return state_error("cannot load the state", e); }
 }
 
+// ---- rows of every token (the reference's logits_all) and their scores
+static void check_tokens(const int* tokens, int n, int n_vocab) {
+  if (n > 0 && !tokens) throw std::invalid_argument("no tokens");
+  for (int i = 0; i < n; i++)
+    if (tokens[i] < 0 || tokens[i] >= n_vocab) throw std::invalid_argument("token id out of range");
+}
+
+// targets: -1 (no target) or a token id
+static void check_targets(const int* targets, int n, int n_vocab) {
+  if (n > 0 && !targets) throw std::invalid_argument("no targets");
+  for (int i = 0; i < n; i++)
+    if (targets[i] < -1 || targets[i] >= n_vocab)
+      throw std::invalid_argument("target " + std::to_string(targets[i]) + " of token " + std::to_string(i) + " is out of range (-1 .. " + std::to_string(n_vocab - 1) + ")");
+}
+
+static void llm_rows_ok(LLM* llm) {
+  if (llm->comm) throw std::invalid_argument("the tensor-sharded mode keeps no per-token rows");
+}
+
+// ctransformers_llm_batch_eval with a RowSink: everything is checked before the first launch, so a refusal leaves the handle as it was
+static int llm_eval_rows(LLM* llm, const int* tokens, int n_tokens, int n_past, int batch_size, const RowSink& sink, const char* what) {
+  try {
+    llm_rows_ok(llm);
+    check_tokens(tokens, n_tokens, llm->hp.n_vocab);
+    if (sink.targets) check_targets(sink.targets, n_tokens, llm->hp.n_vocab);
+    else if (n_tokens > 0 && !sink.host) throw std::invalid_argument("no memory for the rows");
+    if (n_tokens <= 0) return 0;
+    std::vector<int> pos(n_tokens), nt(n_tokens);
+    eval_positions(n_tokens, n_past, batch_size, llm->hp.n_ctx, pos.data(), nt.data());
+    llm->engine->eval_list(tokens, pos.data(), nt.data(), n_tokens, &sink);
+    llm->has_logits = true;
+    return 0;
+  } catch (const std::exception& e) {
+    fprintf(stderr, "ctransformers-b200: %s failed: %s\n", what, e.what());
+    return -1;
+  } catch (...) { return -1; }
+}
+
+int ctb_llm_batch_eval_rows(LLM* llm, const int* tokens, int n_tokens, int n_past, int batch_size, float* rows) {
+  RowSink s;
+  s.host = rows;
+  return llm_eval_rows(llm, tokens, n_tokens, n_past, batch_size, s, "eval with rows");
+}
+
+int ctb_llm_batch_eval_scored(LLM* llm, const int* tokens, int n_tokens, int n_past, int batch_size, const int* targets, double* logprob, int* greedy) {
+  RowSink s;
+  s.targets = targets; s.logprob = logprob; s.greedy = greedy;
+  if (n_tokens > 0 && (!logprob || !greedy)) {
+    fprintf(stderr, "ctransformers-b200: scored eval failed: no memory for the scores\n");
+    return -1;
+  }
+  return llm_eval_rows(llm, tokens, n_tokens, n_past, batch_size, s, "scored eval");
+}
+
+int ctb_llm_score_last(LLM* llm, int target, double* logprob, int* greedy) {
+  try {
+    llm_rows_ok(llm);
+    if (!llm->has_logits) throw std::invalid_argument("nothing has been evaluated");
+    check_targets(&target, 1, llm->hp.n_vocab);
+    llm->engine->score_kept(target, logprob, greedy);
+    return 0;
+  } catch (const std::exception& e) {
+    fprintf(stderr, "ctransformers-b200: scoring the last logits failed: %s\n", e.what());
+    return -1;
+  } catch (...) { return -1; }
+}
+
 // ---- host-only logic (no GPU needed): tokenizer / detokenizer / sampler on their own
 struct ctb_vocab { std::unique_ptr<GGUFFile> file; Vocab vocab; };
 
@@ -624,6 +691,50 @@ bool ctb_multi_eval(ctb_multi* m, int n, const int* slots, const int* off, const
     fprintf(stderr, "ctransformers-b200: multi-sequence eval failed: %s\n", e.what());
     return false;
   } catch (...) { return false; }
+}
+
+// ctb_multi_eval with a RowSink over the packed token list (call order); checked before the first launch
+static int multi_eval_rows(ctb_multi* m, int n, const int* slots, const int* off, const int* tokens, const int* n_past, int batch_size, const RowSink& sink,
+                           const char* what) {
+  try {
+    std::vector<char> seen(m->n_slots, 0);
+    for (int i = 0; i < n; i++) {
+      if (!multi_slot_ok(m, slots[i])) return -1;
+      if (seen[slots[i]]++) throw std::invalid_argument("slot " + std::to_string(slots[i]) + " is listed twice");
+    }
+    const int total = n > 0 ? off[n] - off[0] : 0;
+    check_tokens(tokens ? tokens + (n > 0 ? off[0] : 0) : nullptr, total, m->llm->hp.n_vocab);
+    if (sink.targets) check_targets(sink.targets, total, m->llm->hp.n_vocab);
+    else if (total > 0 && !sink.host) throw std::invalid_argument("no memory for the rows");
+    std::vector<MultiTok> toks;
+    const std::vector<int> starts = multi_pack(n, slots, off, tokens, n_past, batch_size, m->llm->hp.n_ctx, toks);
+    if (toks.empty()) return 0;
+    for (int i = 0; i < n; i++) m->fresh[slots[i]] = 0;
+    m->llm->engine->multi_eval(toks, starts, &sink);
+    for (int i = 0; i < n; i++)
+      if (off[i + 1] > off[i]) m->has[slots[i]] = 1;
+    return 0;
+  } catch (const std::exception& e) {
+    fprintf(stderr, "ctransformers-b200: %s failed: %s\n", what, e.what());
+    return -1;
+  } catch (...) { return -1; }
+}
+
+int ctb_multi_eval_rows(ctb_multi* m, int n, const int* slots, const int* off, const int* tokens, const int* n_past, int batch_size, float* rows) {
+  RowSink s;
+  s.host = rows;
+  return multi_eval_rows(m, n, slots, off, tokens, n_past, batch_size, s, "multi-sequence eval with rows");
+}
+
+int ctb_multi_eval_scored(ctb_multi* m, int n, const int* slots, const int* off, const int* tokens, const int* n_past, int batch_size, const int* targets,
+                          double* logprob, int* greedy) {
+  RowSink s;
+  s.targets = targets; s.logprob = logprob; s.greedy = greedy;
+  if (n > 0 && off[n] > off[0] && (!logprob || !greedy)) {
+    fprintf(stderr, "ctransformers-b200: multi-sequence scored eval failed: no memory for the scores\n");
+    return -1;
+  }
+  return multi_eval_rows(m, n, slots, off, tokens, n_past, batch_size, s, "multi-sequence scored eval");
 }
 
 const float* ctb_multi_logits(ctb_multi* m, int slot) {

@@ -18,6 +18,7 @@
 #include "repack.cuh"
 #include "sample_gpu.cuh"
 #include "sampler.hpp"
+#include "score_gpu.cuh"
 #include "stream.cuh"
 #include "tables.hpp"
 
@@ -703,6 +704,21 @@ int ctb_sample_device(const float* logits, int n, const int* last_tokens, int n_
     *used_device = dev ? 1 : 0;
   });
   return rc == 0 ? tok : -1;
+}
+
+int ctb_row_logprob(const float* rows, int n_rows, int n_vocab, const int* targets, double* logprob, int* greedy) {
+  return guarded("ctb_row_logprob", [&] {
+    if (n_rows < 1 || n_vocab < 1) throw std::runtime_error("no rows");
+    for (int r = 0; r < n_rows; r++)
+      if (targets[r] < -1 || targets[r] >= n_vocab) throw std::runtime_error("target " + std::to_string(targets[r]) + " of row " + std::to_string(r) + " is out of range");
+    DevBuf drows((size_t)n_rows * n_vocab * 4), dt((size_t)n_rows * 4), dlp((size_t)n_rows * 8), dg((size_t)n_rows * 4);
+    OPS_CUDA(cudaMemcpy(drows.p, rows, (size_t)n_rows * n_vocab * 4, cudaMemcpyHostToDevice));
+    OPS_CUDA(cudaMemcpy(dt.p, targets, (size_t)n_rows * 4, cudaMemcpyHostToDevice));
+    rl_launch(drows.as<float>(), n_rows, n_vocab, dt.as<int>(), dlp.as<double>(), dg.as<int>(), 0);
+    OPS_CUDA(cudaGetLastError());
+    OPS_CUDA(cudaMemcpy(logprob, dlp.p, (size_t)n_rows * 8, cudaMemcpyDeviceToHost));
+    OPS_CUDA(cudaMemcpy(greedy, dg.p, (size_t)n_rows * 4, cudaMemcpyDeviceToHost));
+  });
 }
 
 }  // extern "C"

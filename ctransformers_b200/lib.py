@@ -34,6 +34,7 @@ def find_library(path: Optional[str] = None) -> str:
 _P = C.c_void_p
 _IP = C.POINTER(C.c_int)
 _FP = C.POINTER(C.c_float)
+_DP = C.POINTER(C.c_double)
 
 # name -> (restype, argtypes); part 1 = the reference FFI (models/llm.cc:32-138)
 PROTOTYPES = {
@@ -118,6 +119,12 @@ EXTRA_PROTOTYPES = {
     "ctb_multi_save": (C.c_int, [_P, C.c_int, _IP, C.c_int, _P, C.c_size_t]),
     "ctb_multi_restore": (C.c_int, [_P, C.c_int, _P, C.c_size_t]),
     "ctb_multi_fork": (C.c_int, [_P, C.c_int, C.c_int, _IP]),
+    "ctb_llm_batch_eval_rows": (C.c_int, [_P, _IP, C.c_int, C.c_int, C.c_int, _FP]),
+    "ctb_llm_batch_eval_scored": (C.c_int, [_P, _IP, C.c_int, C.c_int, C.c_int, _IP, _DP, _IP]),
+    "ctb_llm_score_last": (C.c_int, [_P, C.c_int, _DP, _IP]),
+    "ctb_row_logprob": (C.c_int, [_P, C.c_int, C.c_int, _IP, _DP, _IP]),
+    "ctb_multi_eval_rows": (C.c_int, [_P, C.c_int, _IP, _IP, _IP, _IP, C.c_int, _FP]),
+    "ctb_multi_eval_scored": (C.c_int, [_P, C.c_int, _IP, _IP, _IP, _IP, C.c_int, _IP, _DP, _IP]),
 }
 
 

@@ -7,7 +7,7 @@ Same class names, method names, keyword arguments, defaults and error behaviour,
 import re
 import warnings
 from collections.abc import MutableSequence
-from ctypes import c_int
+from ctypes import POINTER, byref, c_double, c_float, c_int
 from dataclasses import dataclass, fields
 from functools import partial
 from pathlib import Path
@@ -96,7 +96,22 @@ def _split_incomplete_utf8(seq: bytes):
     return seq[:i], seq[i:]
 
 
+def _check_ids(tokens: Sequence[int], n_vocab: int, what: str, lo: int = 0) -> List[int]:
+    """tokens as a list of ints, each in [lo, n_vocab): what the library would refuse is refused here, with the culprit named."""
+    ids = [int(t) for t in tokens]
+    for i, t in enumerate(ids):
+        if not lo <= t < n_vocab:
+            raise ValueError(f"{what} {i} is {t}: out of range ({lo} .. {n_vocab - 1})")
+    return ids
+
+
+def _ints(values: Sequence[int]):
+    return (c_int * max(len(values), 1))(*values)
+
+
 class LLM:
+    all_logits = None   # eval(..., logits_all=True): the rows of that eval's tokens
+
     def __init__(self, model_path: str, model_type: Optional[str] = None, *, config: Optional[Config] = None, lib: Optional[str] = None, tp=None):
         """Loads a GGUF model onto the GPU (reference: ctransformers/llm.py:212-259).
         tp = (rank, world, unique_id_bytes) loads this process's shard of the tensor-sharded mode (ctransformers_b200/tp.py;
@@ -172,16 +187,69 @@ class LLM:
         return self.ctransformers_llm_is_eos_token(token)
 
     # ---- eval / sample (reference: llm.py:379-455)
-    def eval(self, tokens: Sequence[int], *, batch_size: Optional[int] = None, threads: Optional[int] = None) -> None:
+    def eval(self, tokens: Sequence[int], *, batch_size: Optional[int] = None, threads: Optional[int] = None, logits_all: bool = False) -> None:
+        """logits_all=True (an extension; the reference's llama.cpp has the context flag, ctransformers never sets it) also keeps
+        the logits of every evaluated token, not only the last one's: `all_logits` is then an (n, vocab_size) float32 array, row i
+        bit-identical to the reference's row for tokens[i].  Everything else comes out as from an ordinary eval."""
         cfg = self._config
         batch_size, threads = _pick(batch_size, cfg.batch_size), _pick(threads, cfg.threads)
         n_past, n = len(self._context), len(tokens)
         if n_past + n > self.context_length:
             logger.warning(f"Number of tokens ({n_past + n}) exceeded maximum context length ({self.context_length}).")
+        self.all_logits = None
+        if logits_all:
+            import numpy as np
+            ids = _check_ids(tokens, self.vocab_size, "token")
+            rows = np.empty((n, self.vocab_size), np.float32)
+            if self._lib.ctb_llm_batch_eval_rows(self._llm, _ints(ids), n, n_past, batch_size, rows.ctypes.data_as(POINTER(c_float))) != 0:
+                raise RuntimeError("Failed to evaluate tokens.")
+            self._context.extend(ids)
+            self.all_logits = rows
+            return
         arr = (c_int * n)(*tokens)
         if not self.ctransformers_llm_batch_eval(arr, n, n_past, batch_size, threads):
             raise RuntimeError("Failed to evaluate tokens.")
         self._context.extend(arr)
+
+    def score(self, tokens: Sequence[int], *, batch_size: Optional[int] = None):
+        """Evaluates tokens after the current context and scores each of them under the logits that precede it.  Returns
+        (logprob, greedy): float64 log-probabilities and bool flags "is the greedy pick" (sample(top_k=1)), one per token, reduced
+        on the GPU (csrc/score_gpu.cuh defines both, NaN and infinite logits included).  Token 0 is scored from the last logits
+        of the context; without a context nothing precedes it, and it gets NaN / False."""
+        import numpy as np
+        cfg = self._config
+        batch_size = _pick(batch_size, cfg.batch_size)
+        n_vocab = self.vocab_size
+        ids = _check_ids(tokens, n_vocab, "token")
+        n, n_past = len(ids), len(self._context)
+        logprob, greedy = np.full(n, np.nan), np.zeros(n, bool)
+        if n == 0:
+            return logprob, greedy
+        if n_past + n > self.context_length:
+            logger.warning(f"Number of tokens ({n_past + n}) exceeded maximum context length ({self.context_length}).")
+        if n_past:
+            lp0, g0 = c_double(), c_int()
+            if self._lib.ctb_llm_score_last(self._llm, ids[0], byref(lp0), byref(g0)) != 0:
+                raise RuntimeError("Failed to score the first token against the last logits.")
+            logprob[0], greedy[0] = lp0.value, bool(g0.value)
+        lp, gr = np.zeros(n, np.float64), np.zeros(n, np.int32)
+        if self._lib.ctb_llm_batch_eval_scored(self._llm, _ints(ids), n, n_past, batch_size, _ints(ids[1:] + [-1]),
+                                               lp.ctypes.data_as(POINTER(c_double)), gr.ctypes.data_as(POINTER(c_int))) != 0:
+            raise RuntimeError("Failed to evaluate tokens.")
+        self._context.extend(ids)
+        self.all_logits = None
+        logprob[1:], greedy[1:] = lp[:-1], gr[:-1] != 0
+        return logprob, greedy
+
+    def perplexity(self, tokens: Sequence[int], *, batch_size: Optional[int] = None) -> float:
+        """exp of the mean negative log-probability of the scored tokens (score: every token but a first one without context)."""
+        import numpy as np
+        had_context = bool(self._context)
+        logprob, _ = self.score(tokens, batch_size=batch_size)
+        scored = logprob if had_context else logprob[1:]
+        if len(scored) == 0:
+            raise ValueError("perplexity needs a scored token: give a context or at least two tokens")
+        return float(np.exp(-np.mean(scored)))
 
     def sample(self, *, top_k=None, top_p=None, temperature=None, repetition_penalty=None, last_n_tokens=None, seed=None) -> int:
         cfg = self._config

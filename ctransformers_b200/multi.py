@@ -1,18 +1,20 @@
 """Many independent sequences on one GPU (include/ctransformers_b200.h ctb_multi_*): every slot behaves like its own LLM with the
 same config, bit for bit, while the slots listed in one eval share batched launches — one pass over the weights per launch of
 up to 32 tokens instead of one per token of every sequence."""
-from ctypes import c_int
+from ctypes import POINTER, c_double, c_float, c_int
 from pathlib import Path
 from functools import partial
 from typing import Dict, List, Optional, Sequence, Tuple
 
 from .lib import load_library
 from . import state
-from .llm import Config, Vector, _pick, is_gguf
+from .llm import Config, Vector, _check_ids, _ints, _pick, is_gguf
 from .state import SequenceState
 
 
 class MultiLLM:
+    all_logits = None   # eval(..., logits_all=True): {slot: the rows of that slot's tokens}
+
     def __init__(self, model_path: str, model_type: Optional[str] = None, *, n_slots: int, config: Optional[Config] = None,
                  lib: Optional[str] = None):
         self._config = config or Config()
@@ -43,9 +45,21 @@ class MultiLLM:
             raise IndexError(f"slot {slot} is out of range (0 .. {self.n_slots - 1})")
         return slot
 
-    def eval(self, tokens_by_slot: Dict[int, Sequence[int]], *, batch_size: Optional[int] = None) -> None:
+    def eval(self, tokens_by_slot: Dict[int, Sequence[int]], *, batch_size: Optional[int] = None, logits_all: bool = False) -> None:
         """Each listed slot evaluates its tokens after its own history (n_past = its context length), chunked by batch_size as
-        LLM.eval chunks; all of them share batched launches."""
+        LLM.eval chunks; all of them share batched launches.  logits_all=True also keeps the logits of every evaluated token:
+        `all_logits` is then {slot: (n, vocab_size) float32 array}, each row what LLM.eval(..., logits_all=True) gives."""
+        self.all_logits = None
+        if logits_all:
+            import numpy as np
+            slots = [self._slot(s) for s in tokens_by_slot]
+            total = sum(len(tokens_by_slot[s]) for s in slots)
+            rows = np.empty((total, self.vocab_size), np.float32)
+            self._eval_call(tokens_by_slot, batch_size, self._lib.ctb_multi_eval_rows, rows.ctypes.data_as(POINTER(c_float)))
+            self.all_logits, at = {}, 0
+            for s in slots:
+                self.all_logits[s], at = rows[at:at + len(tokens_by_slot[s])], at + len(tokens_by_slot[s])
+            return
         bs = _pick(batch_size, self._config.batch_size)
         slots = [self._slot(s) for s in tokens_by_slot]
         off, flat = [0], []
@@ -59,6 +73,55 @@ class MultiLLM:
             raise RuntimeError("Failed to evaluate tokens.")
         for s in slots:
             self._context[s].extend(tokens_by_slot[s])
+
+    def _eval_call(self, tokens_by_slot, batch_size, fn, *out) -> None:
+        """One ctb_multi_eval_rows / ctb_multi_eval_scored call: the slots' lists concatenated in dict order."""
+        bs = _pick(batch_size, self._config.batch_size)
+        slots = [self._slot(s) for s in tokens_by_slot]
+        off, flat = [0], []
+        for s in slots:
+            flat.extend(_check_ids(tokens_by_slot[s], self.vocab_size, f"slot {s}: token"))
+            off.append(len(flat))
+        n = len(slots)
+        past = [len(self._context[s]) for s in slots]
+        if fn(self._m, n, _ints(slots), (c_int * (n + 1))(*off), _ints(flat), _ints(past), bs, *out) != 0:
+            raise RuntimeError("Failed to evaluate tokens.")
+        for s in slots:
+            self._context[s].extend(tokens_by_slot[s])
+
+    def score_many(self, requests: Sequence[Tuple[Sequence[int], Sequence[int]]], *, batch_size: Optional[int] = None) -> List[Tuple[float, bool]]:
+        """The loglikelihood requests of an evaluation harness: for each (context_tokens, continuation_tokens), the sum of the
+        continuation tokens' log-probabilities, each under the logits after the tokens before it, and whether every continuation
+        token is the greedy pick there (LLM.score defines both).  Each request runs in a fresh slot; up to n_slots requests are
+        admitted at once and share every launch.  The context must hold at least one token (BOS, say)."""
+        import numpy as np
+        reqs = []
+        for i, (ctx, cont) in enumerate(requests):
+            ctx, cont = _check_ids(ctx, self.vocab_size, f"request {i}: context token"), _check_ids(cont, self.vocab_size, f"request {i}: continuation token")
+            if not ctx or not cont:
+                raise ValueError(f"request {i}: the context and the continuation must each hold at least one token")
+            if len(ctx) + len(cont) - 1 > self.context_length:
+                raise ValueError(f"request {i}: {len(ctx) + len(cont) - 1} tokens to evaluate; the context length is {self.context_length}")
+            reqs.append((ctx, cont))
+        results: List[Tuple[float, bool]] = []
+        for first in range(0, len(reqs), self.n_slots):
+            group = reqs[first:first + self.n_slots]
+            by_slot, targets = {}, []
+            for s, (ctx, cont) in enumerate(group):
+                self.reset(s)
+                whole = ctx + cont
+                by_slot[s] = whole[:-1]   # the last token's row scores nothing
+                targets += [-1] * (len(ctx) - 1) + cont
+            lp, gr = np.zeros(len(targets), np.float64), np.zeros(len(targets), np.int32)
+            self._eval_call(by_slot, batch_size, self._lib.ctb_multi_eval_scored, _ints(targets), lp.ctypes.data_as(POINTER(c_double)),
+                            gr.ctypes.data_as(POINTER(c_int)))
+            at = 0
+            for s, (ctx, cont) in enumerate(group):
+                n = len(ctx) + len(cont) - 1
+                mine, pick = lp[at + len(ctx) - 1:at + n], gr[at + len(ctx) - 1:at + n]
+                results.append((float(np.sum(mine)), bool(np.all(pick != 0))))
+                at += n
+        return results
 
     def logits(self, slot: int) -> List[float]:
         p = self._lib.ctb_multi_logits(self._m, self._slot(slot))

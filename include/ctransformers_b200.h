@@ -274,6 +274,33 @@ int ctb_multi_restore(ctb_multi* m, int slot, const void* buf, size_t size);
  * greedy pick), stream-ordered.  src must not be among dsts.  0, or -1 (+ stderr). */
 int ctb_multi_fork(ctb_multi* m, int src, int n, const int* dsts);
 
+/* Rows of every token: the logits row of every evaluated token, not only the last one's, each bit-identical to what the
+ * reference's llama_eval returns for that token with the context flag logits_all set (llama.cpp:2949-2960), under the same
+ * batch_size chunking and n_past clamp as ctransformers_llm_batch_eval.  Otherwise an eval with rows is an ordinary eval:
+ * logits_data, embeddings_data (the last token's only, as in the reference), the greedy look-ahead and sample come out the same.
+ *
+ * ctb_llm_batch_eval_rows: ctransformers_llm_batch_eval that also writes token i's n_vocab logits to rows[i * n_vocab].
+ * ctb_llm_batch_eval_scored: the same eval, each row reduced on the device against targets[i] (-1: none) to
+ *   logprob[i] = (double)l[t] - m - log(sum_j exp((double)l[j] - m)),  m = the row's largest logit, and
+ *   greedy[i]  = 1 when targets[i] is the row's greedy pick (sample with top_k = 1: the lowest id of the largest logit), else 0;
+ *   only 12 bytes per token come back to the host.  The order of the sum and the results for rows with NaN or infinities are
+ *   those of k_row_logprob (csrc/score_gpu.cuh): NaN in the row gives NaN; +inf entries share the mass; all -inf gives NaN;
+ *   no target gives logprob 0, greedy 0.
+ * ctb_llm_score_last: that reduction of the last eval's logits (what logits_data holds) against one target.
+ * ctb_row_logprob: the same kernel on n_rows host rows (op level).
+ * ctb_multi_eval_rows / ctb_multi_eval_scored: ctb_multi_eval with every listed token's row or score, in the order of the
+ *   concatenated token lists (tokens[off[0]] first); targets is aligned with it.
+ * 0 on success, -1 (+ stderr) on failure.  A target outside -1 .. n_vocab - 1, a token id out of range, or the tensor-sharded
+ * mode (which keeps no rows) is refused before anything runs, and the handle stays usable. */
+int ctb_llm_batch_eval_rows(LLM* llm, const int* tokens, int n_tokens, int n_past, int batch_size, float* rows);
+int ctb_llm_batch_eval_scored(LLM* llm, const int* tokens, int n_tokens, int n_past, int batch_size, const int* targets, double* logprob,
+                              int* greedy);
+int ctb_llm_score_last(LLM* llm, int target, double* logprob, int* greedy);
+int ctb_row_logprob(const float* rows, int n_rows, int n_vocab, const int* targets, double* logprob, int* greedy);
+int ctb_multi_eval_rows(ctb_multi* m, int n, const int* slots, const int* off, const int* tokens, const int* n_past, int batch_size, float* rows);
+int ctb_multi_eval_scored(ctb_multi* m, int n, const int* slots, const int* off, const int* tokens, const int* n_past, int batch_size,
+                          const int* targets, double* logprob, int* greedy);
+
 #ifdef __cplusplus
 }
 #endif
