@@ -458,7 +458,8 @@ void Engine::release() {
   if (h_dbg_) cudaFreeHost(h_dbg_);
   h_dbg_ = nullptr;
   if (h_sample_) cudaFreeHost(h_sample_);
-  h_sample_ = nullptr;
+  if (d_sample_) cudaFree(d_sample_);
+  h_sample_ = d_sample_ = nullptr;
   if (h_stage_) cudaFreeHost(h_stage_);
   h_stage_ = nullptr;
   stage_cap_ = 0;
@@ -1046,26 +1047,48 @@ std::vector<float> Engine::logits_copy() {
   return v;
 }
 
+// Upload the rows' argument block, launch k_sample_topk over them and copy their results back (with every slot's greedy pick when
+// `picks`), all on the engine stream; the caller synchronises.
+void Engine::sample_enqueue(const SampleRow* rows, int R, const float* logits, size_t stride, bool picks) {
+  const int S = hp_.n_seq;
+  if (R < 0 || R > S) throw std::runtime_error("device sampler: " + std::to_string(R) + " rows for " + std::to_string(S) + " slots");
+  const size_t picks_b = (size_t)S * 8, outs_b = (size_t)S * sizeof(SampleGpuOut);
+  if (!d_sample_) {
+    const size_t bytes = picks_b + outs_b + sg_block_ints(S, S * SG_MAX_LAST) * 4;
+    CTB_CUDA(cudaMalloc(&d_sample_, bytes));
+    CTB_CUDA(cudaMallocHost(&h_sample_, bytes));
+  }
+  SampleGpuOut* d_out = (SampleGpuOut*)(d_sample_ + picks_b);
+  int* h_blk = (int*)(h_sample_ + picks_b + outs_b);
+  int* d_blk = (int*)(d_sample_ + picks_b + outs_b);
+  int n_tok = 0;
+  for (int r = 0; r < R; r++) {
+    if (!sg_accepts(rows[r].n_last, rows[r].k) || rows[r].slot < 0 || rows[r].slot >= S) throw std::runtime_error("device sampler: a row it does not take");
+    n_tok += sg_window(rows[r].n_last);
+  }
+  for (int r = 0; r < R; r++) sg_put(h_blk, R, r, rows[r].slot, rows[r].last, rows[r].n_last, rows[r].penalty, rows[r].k, hp_.n_vocab);
+  if (R > 0) {
+    CTB_CUDA(cudaMemcpyAsync(d_blk, h_blk, sg_block_ints(R, n_tok) * 4, cudaMemcpyHostToDevice, stream_));
+    sg_launch(sg_rows(d_blk, R, logits, stride, d_out), R, hp_.n_vocab, stream_);
+    CTB_CUDA(cudaGetLastError());
+  }
+  // one copy back: the picks (first in the buffer) and then the R results
+  if (picks) CTB_CUDA(cudaMemcpyAsync(d_sample_, pf_->d_mpick, picks_b, cudaMemcpyDeviceToDevice, stream_));
+  const size_t from = picks ? 0 : picks_b, to = picks_b + (size_t)R * sizeof(SampleGpuOut);
+  if (to > from) CTB_CUDA(cudaMemcpyAsync(h_sample_ + from, d_sample_ + from, to - from, cudaMemcpyDeviceToHost, stream_));
+}
+
 int Engine::topk_candidates(const int* last, int n_last, float penalty, int k, int* ids, float* logits) {
   if (!sg_accepts(n_last, k)) return -1;
   DeviceGuard dev_guard(device_);
-  if (!d_sample_) {
-    d_sample_ = (SampleGpuOut*)alloc(sizeof(SampleGpuOut));
-    d_last_ = (int*)alloc(SG_MAX_LAST * 4 + 16);
-    CTB_CUDA(cudaMallocHost(&h_sample_, sizeof(SampleGpuOut) + SG_MAX_LAST * 4));
-  }
   if (!ev_sample_) CTB_CUDA(cudaEventCreateWithFlags(&ev_sample_, cudaEventDisableTiming));
   sampler_mode_ = true;
-  int* h_last = (int*)(h_sample_ + 1);
-  for (int i = 0; i < n_last; i++) h_last[i] = last[i];
-  if (n_last > 0) CTB_CUDA(cudaMemcpyAsync(d_last_, h_last, (size_t)n_last * 4, cudaMemcpyHostToDevice, stream_));
-  sg_launch(d_logits_keep_, hp_.n_vocab, d_last_, n_last, penalty, k, d_sample_, stream_);
-  CTB_CUDA(cudaGetLastError());
-  CTB_CUDA(cudaMemcpyAsync(h_sample_, d_sample_, sizeof(SampleGpuOut), cudaMemcpyDeviceToHost, stream_));
+  const SampleRow row{0, last, n_last, penalty, k};
+  sample_enqueue(&row, 1, d_logits_keep_, 0, false);
   CTB_CUDA(cudaEventRecord(ev_sample_, stream_));
   launch_deferred_spec();                          // the look-ahead step runs while the host finishes the draw
   CTB_CUDA(cudaEventSynchronize(ev_sample_));
-  return sg_take(*h_sample_, ids, logits);
+  return sg_take(*(const SampleGpuOut*)(h_sample_ + (size_t)hp_.n_seq * 8), ids, logits);
 }
 
 void Engine::finish_eval(int next_pos, bool hit) {
@@ -1452,10 +1475,13 @@ void Engine::multi_fetch(int slot, float* logits, float* embd) {
   CTB_CUDA(cudaStreamSynchronize(stream_));
 }
 
-void Engine::multi_pick(int slot, int* out2) {
+const SampleGpuOut* Engine::multi_sample(const SampleRow* rows, int R, int* picks) {
   DeviceGuard dev_guard(device_);
-  CTB_CUDA(cudaMemcpyAsync(out2, pf_->d_mpick + 2 * slot, 8, cudaMemcpyDeviceToHost, stream_));
+  if (!pf_ || !pf_->d_mlogits) throw std::runtime_error("this engine has no multi-sequence path");
+  sample_enqueue(rows, R, pf_->d_mlogits, (size_t)hp_.n_vocab, true);
   CTB_CUDA(cudaStreamSynchronize(stream_));
+  memcpy(picks, h_sample_, (size_t)hp_.n_seq * 8);
+  return (const SampleGpuOut*)(h_sample_ + (size_t)hp_.n_seq * 8);
 }
 
 void Engine::multi_reset(int slot) {

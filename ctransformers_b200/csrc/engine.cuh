@@ -58,6 +58,10 @@ struct PrefillState;
 struct MultiTok { int slot, token, pos, n_total; bool last; };
 constexpr int MULTI_LAUNCH_TOKENS = 32;   // tokens of one batched launch (prefill.cuh PB_T)
 
+// One row of the device sampler (sample_gpu.cuh: k_sample_topk): whose logits (a multi-sequence slot; 0 on a single-sequence
+// engine), the repetition window, penalty and k.
+struct SampleRow { int slot; const int* last; int n_last; float penalty; int k; };
+
 // Where an eval's per-token logits rows go (the reference's logits_all, llama.cpp:2949-2960): every evaluated token's row, in
 // call order, either copied to host[i * n_vocab] or reduced on the device by k_row_logprob (score_gpu.cuh) against
 // targets[i] into logprob[i] / greedy[i].  Exactly one of host / targets is set.
@@ -100,7 +104,11 @@ class Engine {
   // rows: the row of every listed token, in the order of toks
   void multi_eval(const std::vector<MultiTok>& toks, const std::vector<int>& starts, const RowSink* rows = nullptr);
   void multi_fetch(int slot, float* logits, float* embd);   // host copies of the slot's last results
-  void multi_pick(int slot, int* out2);                     // {arg-max (lowest id), logits equal to the maximum}
+  // The device sampler for many slots at once, on the engine stream: one upload of the rows' argument block (pinned), one
+  // k_sample_topk launch over them (none when R = 0), one copy back of their results together with every slot's greedy pick
+  // (picks[2 * slot] = {arg-max (lowest id), logits equal to the maximum}), one synchronise.  Returns the R results (row r's
+  // at [r]), valid until the next call.
+  const struct SampleGpuOut* multi_sample(const SampleRow* rows, int R, int* picks);
   void multi_reset(int slot);                               // zero the slot's KV region: a reused slot is a fresh one
   long multi_launches() const;
   // Sequence states (include/ctransformers_b200.h ctb_state_header): the slot's K / V at positions [0, n_past) as
@@ -215,9 +223,10 @@ class Engine {
   bool eager_ = false;           // host logits / embeddings are refreshed by every eval
   bool host_fresh_ = true;
   void host_views();
-  struct SampleGpuOut* d_sample_ = nullptr;
-  struct SampleGpuOut* h_sample_ = nullptr;
-  int* d_last_ = nullptr;
+  // the device sampler's buffers, allocated on first use outside the arena for n_seq rows, the same layout on the device and
+  // in pinned memory: every slot's greedy pick (int[n_seq][2]), the results (SampleGpuOut[n_seq]), the argument block
+  uint8_t *d_sample_ = nullptr, *h_sample_ = nullptr;
+  void sample_enqueue(const SampleRow* rows, int R, const float* logits, size_t stride, bool picks);
   // batched prefill (prefill.cuh): built on first use
   struct PrefillState* pf_ = nullptr;
   bool prefill_on_ = true;       // CTB_NO_PREFILL=1: prompts run through the single-token kernel

@@ -22,6 +22,7 @@
 #include "../../include/ctransformers_b200.h"
 #include "engine.cuh"
 #include "gguf.hpp"
+#include "sample_gpu.cuh"
 #include "sampler.hpp"
 #include "tp_nccl.hpp"
 #include "vocab.hpp"
@@ -593,6 +594,7 @@ struct ctb_multi {
   int n_slots = 0;
   std::vector<std::vector<float>> logits, embd;   // host copies, fetched on request
   std::vector<char> has, fresh;                   // the slot has results / its host copies are current
+  long device_samples = 0;                        // draws answered on the device (LLM::gpu_samples of every slot)
 };
 
 static bool multi_slot_ok(ctb_multi* m, int slot) {
@@ -744,39 +746,73 @@ const float* ctb_multi_embeddings(ctb_multi* m, int slot) {
   try { return multi_fetch(m, slot) ? m->embd[slot].data() : nullptr; } catch (...) { return nullptr; }
 }
 
-// The greedy pick of a slot (what sample with top_k = 1 and no repetition penalty returns): the device's arg-max when it is the
-// only largest logit, else the host sampler on the slot's logits (std::partial_sort's choice among equals is the reference's).
-static int multi_greedy_one(ctb_multi* m, int slot) {
-  if (!multi_slot_ok(m, slot) || !m->has[slot]) return -1;
-  int pk[2];
-  m->llm->engine->multi_pick(slot, pk);
-  if (pk[1] == 1) return pk[0];
-  multi_fetch(m, slot);
-  std::mt19937 rng(0);
-  return sample_token(m->logits[slot].data(), m->llm->hp.n_vocab, nullptr, 0, 1, 1.0f, 1.0f, 1.0f, rng);
-}
-
-int ctb_multi_greedy(ctb_multi* m, int n, const int* slots, int* out) {
+// ctransformers_llm_sample on each listed slot, its draws in list order: slot slots[i] with the window last_tokens[last_off[i] ..
+// last_off[i + 1]) and the i-th settings.  Everything is checked before the first draw; then every slot goes through
+// sample_lazy, the chain an LLM runs on logits that are still on the device.  Its device half runs for all slots at once
+// (Engine::multi_sample): one k_sample_topk launch over the slots that need a cut and that the kernel takes, one copy back of
+// those results and of every slot's greedy pick.  Greedy slots need no cut: their pick answers, and where it cannot (equal
+// maxima, NaN) a cut of 1 cannot either.  What the device cannot answer goes to the host sampler on that slot's logits.
+int ctb_multi_sample_many(ctb_multi* m, int n, const int* slots, const int* last_off, const int* last_tokens, const int* top_k, const float* top_p,
+                          const float* temperature, const float* repetition_penalty, const int* seed, int* out) {
   try {
-    for (int i = 0; i < n; i++)
-      if ((out[i] = multi_greedy_one(m, slots[i])) < 0) return -1;
+    if (n < 0) throw std::invalid_argument("a negative slot count");
+    if (n > 0 && (!slots || !last_off || !top_k || !top_p || !temperature || !repetition_penalty || !seed || !out))
+      throw std::invalid_argument("a missing argument array");
+    std::vector<char> seen(m->n_slots, 0);
+    for (int i = 0; i < n; i++) {
+      if (!multi_slot_ok(m, slots[i])) return -1;
+      if (seen[slots[i]]++) throw std::invalid_argument("slot " + std::to_string(slots[i]) + " is listed twice");
+      if (!m->has[slots[i]]) throw std::invalid_argument("slot " + std::to_string(slots[i]) + " has no logits to sample from");
+      if (last_off[i] < 0 || last_off[i + 1] < last_off[i]) throw std::invalid_argument("the window offsets of slot " + std::to_string(slots[i]) + " are not ascending");
+    }
+    if (n > 0 && last_off[n] > last_off[0] && !last_tokens) throw std::invalid_argument("no window tokens");
+    std::vector<SampleRow> rows;
+    std::vector<int> row_of(n, -1);
+    for (int i = 0; i < n; i++) {
+      const int nl = last_off[i + 1] - last_off[i];
+      if (sample_is_greedy(top_k[i], repetition_penalty[i], nl) || !sg_accepts(nl, top_k[i])) continue;
+      row_of[i] = (int)rows.size();
+      rows.push_back(SampleRow{slots[i], last_tokens + last_off[i], nl, repetition_penalty[i], top_k[i]});
+    }
+    std::vector<int> picks((size_t)2 * m->n_slots);
+    Engine& e = *m->llm->engine;
+    const SampleGpuOut* res = e.multi_sample(rows.data(), (int)rows.size(), picks.data());
+    for (int i = 0; i < n; i++) {
+      const int slot = slots[i];
+      m->llm->rng.seed((unsigned)(seed[i] < 0 ? (int)time(nullptr) : seed[i]));
+      bool used_device = false;
+      out[i] = sample_lazy(
+          m->llm->hp.n_vocab, last_tokens ? last_tokens + last_off[i] : nullptr, last_off[i + 1] - last_off[i], top_k[i], top_p[i], temperature[i],
+          repetition_penalty[i], m->llm->rng, used_device, [&] { return picks[2 * slot + 1] == 1 ? picks[2 * slot] : -1; },
+          [&](const int*, int, float, int, int* ids, float* lg) { return row_of[i] < 0 ? -1 : sg_take(res[row_of[i]], ids, lg); },
+          [&] {
+            multi_fetch(m, slot);
+            return m->logits[slot];
+          });
+      if (used_device) m->device_samples++;
+    }
     return 0;
   } catch (const std::exception& e) {
-    fprintf(stderr, "ctransformers-b200: multi-sequence greedy pick failed: %s\n", e.what());
+    fprintf(stderr, "ctransformers-b200: multi-sequence sampling failed: %s\n", e.what());
     return -1;
   } catch (...) { return -1; }
 }
 
+long ctb_multi_device_samples(ctb_multi* m) { return m->device_samples; }
+
+// the greedy pick of each slot: sample with top_k 1, top_p 1, temperature 1, no penalty
+int ctb_multi_greedy(ctb_multi* m, int n, const int* slots, int* out) {
+  if (n < 0) return -1;
+  const std::vector<int> off(n + 1, 0), k(n, 1), seed(n, 0);
+  const std::vector<float> one(n, 1.0f);
+  return ctb_multi_sample_many(m, n, slots, off.data(), nullptr, k.data(), one.data(), one.data(), one.data(), seed.data(), out);
+}
+
 int ctb_multi_sample(ctb_multi* m, int slot, const int* last_tokens, int n_last, int top_k, float top_p, float temperature, float repetition_penalty,
                      int seed) {
-  try {
-    if (!multi_slot_ok(m, slot) || !m->has[slot]) return -1;
-    if (top_k == 1 && (repetition_penalty == 1.0f || n_last <= 0)) return multi_greedy_one(m, slot);
-    if (seed < 0) seed = (int)time(nullptr);
-    m->llm->rng.seed((unsigned)seed);
-    multi_fetch(m, slot);
-    return sample_token(m->logits[slot].data(), m->llm->hp.n_vocab, last_tokens, n_last, top_k, top_p, temperature, repetition_penalty, m->llm->rng);
-  } catch (...) { return -1; }
+  const int off[2] = {0, std::max(n_last, 0)};
+  int tok = -1;
+  return ctb_multi_sample_many(m, 1, &slot, off, last_tokens, &top_k, &top_p, &temperature, &repetition_penalty, &seed, &tok) == 0 ? tok : -1;
 }
 
 int ctb_multi_reset(ctb_multi* m, int slot) {

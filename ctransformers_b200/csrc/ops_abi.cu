@@ -242,15 +242,40 @@ void argmax_on_device(const float* d_logits, int n, int* pick2) {
   OPS_CUDA(cudaMemcpy(pick2, dout.p, 8, cudaMemcpyDeviceToHost));
 }
 
-// k_sample_topk over n device logits, as Engine::topk_candidates launches it
-SampleGpuOut topk_on_device(const float* d_logits, int n, const int* last, int n_last, float penalty, int k) {
-  DevBuf dlast((size_t)std::max(n_last, 1) * 4), dout(sizeof(SampleGpuOut));
-  if (n_last > 0) OPS_CUDA(cudaMemcpy(dlast.p, last, (size_t)n_last * 4, cudaMemcpyHostToDevice));
-  sg_launch(d_logits, n, dlast.as<int>(), n_last, penalty, k, dout.as<SampleGpuOut>(), 0);
+// k_sample_topk over rows rows[0 ..) of a [rows][n] device buffer in one launch, as Engine::multi_sample launches it: result i is
+// row q = rows[i]'s, with its window last_tokens[last_off[q] .. last_off[q + 1]), penalty[q] and k[q]
+std::vector<SampleGpuOut> topk_rows_on_device(const float* d_logits, int n, const std::vector<int>& rows, const int* last_off, const int* last_tokens,
+                                              const float* penalty, const int* k) {
+  const int R = (int)rows.size();
+  std::vector<SampleGpuOut> o(R);
+  if (R == 0) return o;
+  int n_tok = 0;
+  for (int q : rows) n_tok += sg_window(last_off[q + 1] - last_off[q]);
+  std::vector<int> blk(sg_block_ints(R, n_tok));
+  for (int r = 0; r < R; r++) {
+    const int q = rows[r];
+    sg_put(blk.data(), R, r, q, last_tokens + last_off[q], last_off[q + 1] - last_off[q], penalty[q], k[q], n);
+  }
+  DevBuf dblk(blk.size() * 4), dout((size_t)R * sizeof(SampleGpuOut));
+  OPS_CUDA(cudaMemcpy(dblk.p, blk.data(), blk.size() * 4, cudaMemcpyHostToDevice));
+  sg_launch(sg_rows(dblk.as<int>(), R, d_logits, (size_t)n, dout.as<SampleGpuOut>()), R, n, 0);
   OPS_CUDA(cudaGetLastError());
-  SampleGpuOut o;
-  OPS_CUDA(cudaMemcpy(&o, dout.p, sizeof(o), cudaMemcpyDeviceToHost));
+  OPS_CUDA(cudaMemcpy(o.data(), dout.p, (size_t)R * sizeof(SampleGpuOut), cudaMemcpyDeviceToHost));
   return o;
+}
+
+// k_sample_topk over n device logits, as Engine::topk_candidates launches it: one row
+SampleGpuOut topk_on_device(const float* d_logits, int n, const int* last, int n_last, float penalty, int k) {
+  const int off[2] = {0, sg_window(n_last)};
+  return topk_rows_on_device(d_logits, n, {0}, off, last, &penalty, &k)[0];
+}
+
+// n_rows rows of n logits each, with their windows last_off[0 .. n_rows] into last_tokens: checked, then uploaded
+void check_rows(int n_rows, int n, const int* last_off, const int* last_tokens) {
+  if (n_rows < 1 || n < 1) throw std::runtime_error("no rows, or rows of no logits");
+  for (int r = 0; r < n_rows; r++)
+    if (last_off[r] < 0 || last_off[r + 1] < last_off[r]) throw std::runtime_error("window offsets that are not ascending");
+  if (last_off[n_rows] > last_off[0] && !last_tokens) throw std::runtime_error("no window tokens");
 }
 
 }  // namespace
@@ -704,6 +729,59 @@ int ctb_sample_device(const float* logits, int n, const int* last_tokens, int n_
     *used_device = dev ? 1 : 0;
   });
   return rc == 0 ? tok : -1;
+}
+
+int ctb_sample_topk_rows(const float* logits, int n_rows, int n, const int* last_off, const int* last_tokens, const float* repetition_penalty,
+                         const int* k, int* count, int* ids, float* lg) {
+  return guarded("ctb_sample_topk_rows", [&] {
+    check_rows(n_rows, n, last_off, last_tokens);
+    std::vector<int> rows;
+    for (int r = 0; r < n_rows; r++) {
+      count[r] = -1;
+      if (sg_accepts(last_off[r + 1] - last_off[r], k[r])) rows.push_back(r);
+    }
+    DevBuf dlog((size_t)n_rows * n * 4);
+    OPS_CUDA(cudaMemcpy(dlog.p, logits, (size_t)n_rows * n * 4, cudaMemcpyHostToDevice));
+    const std::vector<SampleGpuOut> o = topk_rows_on_device(dlog.as<float>(), n, rows, last_off, last_tokens, repetition_penalty, k);
+    for (size_t i = 0; i < rows.size(); i++) {
+      const int r = rows[i];
+      count[r] = o[i].nan ? -2 : o[i].count;
+      for (int j = 0; !o[i].nan && j < std::min(o[i].count, SG_MAX_OUT); j++) {
+        ids[(size_t)r * SG_MAX_OUT + j] = o[i].id[j];
+        lg[(size_t)r * SG_MAX_OUT + j] = o[i].logit[j];
+      }
+    }
+  });
+}
+
+int ctb_sample_device_rows(const float* logits, int n_rows, int n, const int* last_off, const int* last_tokens, const int* top_k, const float* top_p,
+                           const float* temperature, const float* repetition_penalty, const int* seed, int* tokens, int* used_device) {
+  return guarded("ctb_sample_device_rows", [&] {
+    check_rows(n_rows, n, last_off, last_tokens);
+    DevBuf dlog((size_t)n_rows * n * 4);
+    OPS_CUDA(cudaMemcpy(dlog.p, logits, (size_t)n_rows * n * 4, cudaMemcpyHostToDevice));
+    // the device half as ctb_multi_sample_many runs it: every row's pick, one top-k launch over the rows that need a cut
+    std::vector<int> picks((size_t)2 * n_rows), rows, row_of(n_rows, -1);
+    for (int r = 0; r < n_rows; r++) {
+      argmax_on_device(dlog.as<float>() + (size_t)r * n, n, &picks[2 * r]);
+      const int nl = last_off[r + 1] - last_off[r];
+      if (sample_is_greedy(top_k[r], repetition_penalty[r], nl) || !sg_accepts(nl, top_k[r])) continue;
+      row_of[r] = (int)rows.size();
+      rows.push_back(r);
+    }
+    const std::vector<SampleGpuOut> o = topk_rows_on_device(dlog.as<float>(), n, rows, last_off, last_tokens, repetition_penalty, top_k);
+    for (int r = 0; r < n_rows; r++) {
+      std::mt19937 rng((unsigned)(seed[r] < 0 ? (int)time(nullptr) : seed[r]));
+      const float* row = logits + (size_t)r * n;
+      bool dev = false;
+      tokens[r] = sample_lazy(
+          n, last_tokens ? last_tokens + last_off[r] : nullptr, last_off[r + 1] - last_off[r], top_k[r], top_p[r], temperature[r], repetition_penalty[r],
+          rng, dev, [&] { return picks[2 * r + 1] == 1 ? picks[2 * r] : -1; },
+          [&](const int*, int, float, int, int* i, float* l) { return row_of[r] < 0 ? -1 : sg_take(o[row_of[r]], i, l); },
+          [&] { return std::vector<float>(row, row + n); });
+      used_device[r] = dev ? 1 : 0;
+    }
+  });
 }
 
 int ctb_row_logprob(const float* rows, int n_rows, int n_vocab, const int* targets, double* logprob, int* greedy) {

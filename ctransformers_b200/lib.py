@@ -93,6 +93,8 @@ EXTRA_PROTOTYPES = {
     "ctb_argmax_path": (C.c_int, [C.c_int, _P, C.c_int, _IP]),
     "ctb_sample_topk": (C.c_int, [_P, C.c_int, _IP, C.c_int, C.c_float, C.c_int, _IP, _P]),
     "ctb_sample_device": (C.c_int, [_P, C.c_int, _IP, C.c_int, C.c_int, C.c_float, C.c_float, C.c_float, C.c_int, _IP]),
+    "ctb_sample_topk_rows": (C.c_int, [_P, C.c_int, C.c_int, _IP, _IP, _FP, _IP, _IP, _IP, _FP]),
+    "ctb_sample_device_rows": (C.c_int, [_P, C.c_int, C.c_int, _IP, _IP, _IP, _FP, _FP, _FP, _IP, _IP, _IP]),
     "ctb_vocab_load": (_P, [C.c_char_p]),
     "ctb_vocab_free": (None, [_P]),
     "ctb_vocab_size": (C.c_int, [_P]),
@@ -107,6 +109,8 @@ EXTRA_PROTOTYPES = {
     "ctb_multi_embeddings": (_FP, [_P, C.c_int]),
     "ctb_multi_greedy": (C.c_int, [_P, C.c_int, _IP, _IP]),
     "ctb_multi_sample": (C.c_int, [_P, C.c_int, _IP, C.c_int, C.c_int, C.c_float, C.c_float, C.c_float, C.c_int]),
+    "ctb_multi_sample_many": (C.c_int, [_P, C.c_int, _IP, _IP, _IP, _IP, _FP, _FP, _FP, _IP, _IP]),
+    "ctb_multi_device_samples": (C.c_long, [_P]),
     "ctb_multi_reset": (C.c_int, [_P, C.c_int]),
     "ctb_multi_launches": (C.c_long, [_P]),
     "ctb_multi_last_eval_ms": (C.c_double, [_P]),

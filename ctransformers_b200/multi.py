@@ -12,6 +12,16 @@ from .llm import Config, Vector, _check_ids, _ints, _pick, is_gguf
 from .state import SequenceState
 
 
+def per_slot(value, n: int, what: str) -> list:
+    """`value` for each of n slots: one value for all of them, or a sequence holding one value per slot."""
+    if isinstance(value, (str, bytes)) or not hasattr(value, "__len__"):
+        return [value] * n
+    values = list(value)
+    if len(values) != n:
+        raise ValueError(f"{what}: {len(values)} values for {n} slots")
+    return values
+
+
 class MultiLLM:
     all_logits = None   # eval(..., logits_all=True): {slot: the rows of that slot's tokens}
 
@@ -141,18 +151,34 @@ class MultiLLM:
 
     def sample(self, slot: int, *, top_k=None, top_p=None, temperature=None, repetition_penalty=None, last_n_tokens=None, seed=None) -> int:
         """LLM.sample on this slot: the same defaults, its own last_n_tokens window."""
-        cfg = self._config
-        ctx = self._context[self._slot(slot)]
-        last_n = _pick(last_n_tokens, cfg.last_n_tokens)
-        if last_n < 0:
-            last_n = self.context_length
-        recent = ctx[-last_n:]
-        t = self._lib.ctb_multi_sample(self._m, slot, (c_int * max(len(recent), 1))(*recent), len(recent), _pick(top_k, cfg.top_k),
-                                       _pick(top_p, cfg.top_p), _pick(temperature, cfg.temperature),
-                                       _pick(repetition_penalty, cfg.repetition_penalty), _pick(seed, cfg.seed))
-        if t < 0:
-            raise RuntimeError(f"Slot {slot} has no logits to sample from.")
-        return t
+        return self.sample_many([slot], top_k=top_k, top_p=top_p, temperature=temperature, repetition_penalty=repetition_penalty,
+                                last_n_tokens=last_n_tokens, seed=seed)[0]
+
+    def sample_many(self, slots: Sequence[int], *, top_k=None, top_p=None, temperature=None, repetition_penalty=None, last_n_tokens=None,
+                    seed=None) -> List[int]:
+        """sample() of every listed slot, in one call: draw i is what LLM.sample returns with the i-th settings on an LLM fed
+        slot slots[i]'s history.  Each setting is one value for every slot or a sequence with one value per slot (None: the
+        config's).  The penalty and top-k cut of all slots run in one device launch; the host finishes each draw."""
+        slots = [self._slot(s) for s in slots]
+        n, cfg = len(slots), self._config
+        args = {}
+        for name, value in (("top_k", top_k), ("top_p", top_p), ("temperature", temperature), ("repetition_penalty", repetition_penalty),
+                            ("last_n_tokens", last_n_tokens), ("seed", seed)):
+            args[name] = [_pick(v, getattr(cfg, name)) for v in per_slot(value, n, name)]
+        off, flat = [0], []
+        for s, last_n in zip(slots, args["last_n_tokens"]):
+            flat.extend(self._context[s][-(last_n if last_n >= 0 else self.context_length):])   # (last_n 0: the whole context, as LLM.sample)
+            off.append(len(flat))
+        out = (c_int * max(n, 1))()
+        floats = lambda v: (c_float * max(n, 1))(*v)
+        if self._lib.ctb_multi_sample_many(self._m, n, _ints(slots), _ints(off), _ints(flat), _ints(args["top_k"]), floats(args["top_p"]),
+                                           floats(args["temperature"]), floats(args["repetition_penalty"]), _ints(args["seed"]), out) != 0:
+            raise RuntimeError(f"Failed to sample slots {slots}: each must have logits and be listed once.")
+        return list(out[:n])
+
+    def device_samples(self) -> int:
+        """Draws so far that the device answered (the rest ran the host sampler on a slot's logits)."""
+        return self._lib.ctb_multi_device_samples(self._m)
 
     def reset(self, slot: int) -> None:
         """The slot starts over, as a fresh LLM."""
@@ -223,9 +249,10 @@ class MultiLLM:
                 if dsts:
                     self.fork(s, dsts)
             forks = {}
-            for slot in sorted(owner):
+            order = sorted(owner)
+            kw = sampling if seeds is None else {**sampling, "seed": [seeds[owner[s][1]] for s in order]}
+            for slot, tok in zip(order, self.sample_many(order, **kw)):
                 i, j = owner[slot]
-                tok = self.sample(slot, **(sampling if seeds is None else {**sampling, "seed": seeds[j]}))
                 if tok == self.eos_token_id or max_new_tokens <= 0:
                     done = True
                 else:

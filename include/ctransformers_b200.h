@@ -205,6 +205,16 @@ int ctb_sample_topk(const float* logits, int n, const int* last_tokens, int n_la
  * token (the one ctb_sample draws with the same arguments), -1 on error; *used_device = 1 when the device answered. */
 int ctb_sample_device(const float* logits, int n, const int* last_tokens, int n_last, int top_k, float top_p, float temperature,
                       float repetition_penalty, int seed, int* used_device);
+/* Both of the above on n_rows rows of n logits each (logits[r * n ..]), row r with the window last_tokens[last_off[r] ..
+ * last_off[r + 1]) and its own settings, launched as ctb_multi_sample_many launches them: one k_sample_topk launch over the rows.
+ * ctb_sample_topk_rows: count[r] as ctb_sample_topk returns it (-2 NaN, -1 for a window or k the kernel does not take: that row
+ *   is not launched), its ids / logits at ids[r * 256 ..] / lg[r * 256 ..].
+ * ctb_sample_device_rows: tokens[r] as ctb_sample_device draws it with seed[r], used_device[r] its flag.
+ * 0, or -1 (+ stderr) for no rows, n < 1 or window offsets that are not ascending. */
+int ctb_sample_topk_rows(const float* logits, int n_rows, int n, const int* last_off, const int* last_tokens, const float* repetition_penalty,
+                         const int* k, int* count, int* ids, float* lg);
+int ctb_sample_device_rows(const float* logits, int n_rows, int n, const int* last_off, const int* last_tokens, const int* top_k, const float* top_p,
+                           const float* temperature, const float* repetition_penalty, const int* seed, int* tokens, int* used_device);
 
 /* Multi-sequence decoding: one handle owns n_slots sequence slots, each of which behaves like a fresh single-sequence LLM with
  * the same config, and every eval's slots share batched launches (one pass over the weights per launch of up to 32 tokens).
@@ -224,9 +234,20 @@ const float* ctb_multi_logits(ctb_multi* m, int slot);       /* n_vocab floats o
 const float* ctb_multi_embeddings(ctb_multi* m, int slot);   /* n_embd floats */
 /* greedy picks (= sample with top_k 1, no penalty) of n slots from the device arg-max; 0, or -1 (+ stderr) on error */
 int ctb_multi_greedy(ctb_multi* m, int n, const int* slots, int* out);
-/* = ctransformers_llm_sample on that slot's logits (RNG reseeded per call); -1 on error */
+/* = ctransformers_llm_sample on that slot's logits (RNG reseeded per call); -1 (+ stderr, e.g. for a slot out of range or
+ * without logits) on error.  ctb_multi_sample_many of one slot. */
 int ctb_multi_sample(ctb_multi* m, int slot, const int* last_tokens, int n_last, int top_k, float top_p, float temperature,
                      float repetition_penalty, int seed);
+/* out[i] = ctransformers_llm_sample on slot slots[i]'s logits with the window last_tokens[last_off[i] .. last_off[i + 1]),
+ * top_k[i], top_p[i], temperature[i], repetition_penalty[i] and seed[i] (the RNG reseeded per slot, in list order; < 0: time).
+ * Each draw is the one a single-sequence LLM with that slot's history returns.  The penalty and top-k cut of every slot run in
+ * one device launch and one copy back; the host finishes each draw from its candidates, or on the slot's logits where the
+ * device cannot answer (a window over 256 tokens, top_k outside 1 .. 128, equal logits at the cut, NaN).  0, or -1 (+ stderr)
+ * for a slot out of range, listed twice or without logits, or window offsets that are not ascending: checked before the first
+ * draw, so nothing is drawn then. */
+int ctb_multi_sample_many(ctb_multi* m, int n, const int* slots, const int* last_off, const int* last_tokens, const int* top_k, const float* top_p,
+                          const float* temperature, const float* repetition_penalty, const int* seed, int* out);
+long ctb_multi_device_samples(ctb_multi* m);     /* draws of sample / sample_many / greedy answered on the device so far */
 int ctb_multi_reset(ctb_multi* m, int slot);    /* the slot starts over; 0, or -1 when out of range */
 long ctb_multi_launches(ctb_multi* m);           /* batched launches so far */
 double ctb_multi_last_eval_ms(ctb_multi* m);     /* CUDA-event time of the last eval */
