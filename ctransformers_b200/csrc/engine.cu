@@ -463,6 +463,9 @@ void Engine::release() {
   if (h_stage_) cudaFreeHost(h_stage_);
   h_stage_ = nullptr;
   stage_cap_ = 0;
+  if (d_copies_) cudaFree(d_copies_);
+  if (h_copies_) cudaFreeHost(h_copies_);
+  d_copies_ = h_copies_ = nullptr;
   if (d_rows_) cudaFree(d_rows_);
   if (d_score_) cudaFree(d_score_);
   if (h_score_) cudaFreeHost(h_score_);
@@ -1635,6 +1638,78 @@ void Engine::state_fork(int src, const int* dsts, int n) {
     CTB_CUDA(cudaMemcpyAsync(pf_->d_mpick + 2 * d, pf_->d_mpick + 2 * src, 8, cudaMemcpyDeviceToDevice, stream_));
   }
   CTB_CUDA(cudaStreamSynchronize(stream_));
+}
+
+// Beam search re-parenting.  Block (lh, c) handles layer / KV head lh of copy c: the K rows of positions [lo, hi), one contiguous
+// run of the head's positions, and for every V channel the whole 256-blocks that cover [lo, hi).  V entries are permuted within
+// 256-blocks (v_perm), so a whole block is the least that holds every position needed.  The entries below lo it also copies are
+// equal in both slots (they hold the same tokens there), and those at hi and above lie past what dst holds, so afterwards dst
+// equals src on [0, hi).  No slot is both a source and a destination, so no block reads what another writes.
+__global__ void k_kv_reparent(const KvCopy* copies, uint16_t* kc, uint16_t* vc, size_t kslot, size_t vslot, int n_ctx, int ks, int hd) {
+  const KvCopy c = copies[blockIdx.y];
+  const size_t lh = blockIdx.x;
+  const uint4* ksrc = (const uint4*)(kc + c.src * kslot + (lh * n_ctx + c.lo) * ks);
+  uint4* kdst = (uint4*)(kc + c.dst * kslot + (lh * n_ctx + c.lo) * ks);
+  const int nk = (c.hi - c.lo) * ks / 8;   // (ks is a multiple of 8 halves)
+  for (int i = threadIdx.x; i < nk; i += blockDim.x) kdst[i] = ksrc[i];
+  const size_t cp = kv_ctx_pad(n_ctx);
+  const int v0 = c.lo & ~255, nv = (((c.hi + 255) & ~255) - v0) / 8;
+  const uint16_t* vsrc = vc + c.src * vslot + lh * hd * cp + v0;
+  uint16_t* vdst = vc + c.dst * vslot + lh * hd * cp + v0;
+  for (int i = threadIdx.x; i < hd * nv; i += blockDim.x) {
+    const size_t at = (size_t)(i / nv) * cp + (size_t)(i % nv) * 8;
+    *(uint4*)(vdst + at) = *(const uint4*)(vsrc + at);
+  }
+}
+
+size_t Engine::kv_reparent(const std::vector<KvCopy>& copies) {
+  DeviceGuard dev_guard(device_);
+  if (hp_.n_seq < 2 || !pf_ || !pf_->d_mlogits) throw std::runtime_error("this engine has no multi-sequence path");
+  if (copies.empty()) return 0;
+  if ((int)copies.size() > hp_.n_seq) throw std::runtime_error("kv_reparent: more copies than slots");
+  std::vector<char> src(hp_.n_seq, 0), dst(hp_.n_seq, 0);
+  for (const KvCopy& c : copies) {
+    if (c.src < 0 || c.src >= hp_.n_seq || c.dst < 0 || c.dst >= hp_.n_seq || c.lo < 0 || c.hi < c.lo || c.hi > hp_.n_ctx)
+      throw std::runtime_error("kv_reparent: a copy out of range");
+    src[c.src] = 1;
+    if (dst[c.dst]++) throw std::runtime_error("kv_reparent: a slot is written twice");
+  }
+  for (int s = 0; s < hp_.n_seq; s++)
+    if (src[s] && dst[s]) throw std::runtime_error("kv_reparent: slot " + std::to_string(s) + " is both a source and a destination");
+  if (!d_copies_) {
+    CTB_CUDA(cudaMalloc(&d_copies_, sizeof(KvCopy) * hp_.n_seq));
+    CTB_CUDA(cudaMallocHost(&h_copies_, sizeof(KvCopy) * hp_.n_seq));
+  }
+  const int hd = hp_.head_dim(), ks = k_stride(hd);
+  size_t kslot, vslot, bytes = 0;
+  kv_slot_elems(kslot, vslot);
+  const size_t lh = (size_t)hp_.n_layer * nkv_;
+  for (const KvCopy& c : copies) bytes += lh * ((size_t)(c.hi - c.lo) * ks + (size_t)hd * (((c.hi + 255) & ~255) - (c.lo & ~255))) * 2;
+  std::copy(copies.begin(), copies.end(), h_copies_);
+  CTB_CUDA(cudaMemcpyAsync(d_copies_, h_copies_, sizeof(KvCopy) * copies.size(), cudaMemcpyHostToDevice, stream_));
+  k_kv_reparent<<<dim3((unsigned)lh, (unsigned)copies.size()), 256, 0, stream_>>>(d_copies_, kc_, vc_, kslot, vslot, hp_.n_ctx, ks, hd);
+  CTB_CUDA(cudaGetLastError());
+  for (const KvCopy& c : copies) {
+    float *sem, *dem;
+    const float* slg = results_of(c.src, &sem);
+    float* dlg = results_of(c.dst, &dem);
+    CTB_CUDA(cudaMemcpyAsync(dlg, slg, (size_t)hp_.n_vocab * 4, cudaMemcpyDeviceToDevice, stream_));
+    CTB_CUDA(cudaMemcpyAsync(dem, sem, (size_t)hp_.n_embd * 4, cudaMemcpyDeviceToDevice, stream_));
+    CTB_CUDA(cudaMemcpyAsync(pf_->d_mpick + 2 * c.dst, pf_->d_mpick + 2 * c.src, 8, cudaMemcpyDeviceToDevice, stream_));
+  }
+  CTB_CUDA(cudaStreamSynchronize(stream_));
+  return bytes;
+}
+
+const float* Engine::multi_rows(int slot0, int n) {
+  DeviceGuard dev_guard(device_);
+  if (!pf_ || !pf_->d_mlogits) throw std::runtime_error("this engine has no multi-sequence path");
+  if (slot0 < 0 || n < 0 || slot0 + n > hp_.n_seq) throw std::runtime_error("multi_rows: slots out of range");
+  const size_t b = (size_t)n * hp_.n_vocab * 4;
+  float* h = (float*)stage(std::max<size_t>(b, 1));
+  CTB_CUDA(cudaMemcpyAsync(h, pf_->d_mlogits + (size_t)slot0 * hp_.n_vocab, b, cudaMemcpyDeviceToHost, stream_));
+  CTB_CUDA(cudaStreamSynchronize(stream_));
+  return h;
 }
 
 double Engine::decode_greedy(int first_token, int n_past, int n_steps, int* out_tokens) {

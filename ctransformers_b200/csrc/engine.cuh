@@ -72,6 +72,8 @@ struct RowSink {
   int* greedy = nullptr;
 };
 
+struct KvCopy { int src, dst, lo, hi; };   // one slot-to-slot KV copy of Engine::kv_reparent
+
 struct EvalStats { double last_eval_ms = 0; long launches = 0; size_t weight_bytes_per_token = 0; long spec_hits = 0; double load_ms = 0; size_t load_bytes = 0; };
 
 class Engine {
@@ -122,6 +124,12 @@ class Engine {
   // single-sequence engine drops its look-ahead and starts over from this state as after an eval ending with last_token.
   void state_load(int slot, int n_past, bool results, const void* in, int last_token);
   void state_fork(int src, const int* dsts, int n);   // multi-sequence: slot src's whole KV region and last results into each dst
+  // Beam search re-parenting (multi-sequence): copy i gives slot dst the K rows and V entries of slot src at positions [lo, hi),
+  // for every layer and KV head, all copies in one k_kv_reparent launch; then each dst takes src's last results and greedy pick
+  // (as state_fork).  No slot may be both a source and a destination.  Returns the K / V bytes the launch moved.
+  size_t kv_reparent(const std::vector<KvCopy>& copies);
+  // the logits rows of slots [slot0, slot0 + n) in one device-to-host copy, into pinned memory valid until the next call
+  const float* multi_rows(int slot0, int n);
   // Which implementations the evals run (include/ctransformers_b200.h ctb_llm_paths): entries written, or -needed.
   int paths(int* out, int cap);
 
@@ -264,6 +272,7 @@ class Engine {
   uint8_t* h_stage_ = nullptr;   // pinned staging of state_save / state_load, grown on demand
   size_t stage_cap_ = 0;
   uint8_t* stage(size_t bytes);
+  KvCopy *d_copies_ = nullptr, *h_copies_ = nullptr;   // kv_reparent's copy list (n_seq entries), device and pinned
   void kv_slot_elems(size_t& k, size_t& v) const;   // halves of one slot's K and V regions
   float* results_of(int slot, float** embd);        // where the slot's last logits / embeddings live on the device
 };

@@ -11,6 +11,7 @@
 #include <algorithm>
 #include <atomic>
 #include <cctype>
+#include <chrono>
 #include <cstdio>
 #include <cstring>
 #include <ctime>
@@ -20,6 +21,7 @@
 #include <vector>
 
 #include "../../include/ctransformers_b200.h"
+#include "beam.hpp"
 #include "engine.cuh"
 #include "gguf.hpp"
 #include "sample_gpu.cuh"
@@ -595,6 +597,7 @@ struct ctb_multi {
   std::vector<std::vector<float>> logits, embd;   // host copies, fetched on request
   std::vector<char> has, fresh;                   // the slot has results / its host copies are current
   long device_samples = 0;                        // draws answered on the device (LLM::gpu_samples of every slot)
+  double beam_stats[8] = {0};                     // the last beam search: ctb_multi_beam_stats
 };
 
 static bool multi_slot_ok(ctb_multi* m, int slot) {
@@ -868,6 +871,269 @@ int ctb_multi_fork(ctb_multi* m, int src, int n, const int* dsts) {
     }
     return 0;
   } catch (const std::exception& e) { return state_error("cannot fork the slot", e); }
+}
+
+// ---- beam search (the reference's llama_beam_search, llama.cpp:4334-4579, driven as its examples/beam_search does)
+//
+// The reference keeps one KV cache: each step it evaluates the beams' common prefix as one chunk and shifts it off, then every
+// beam's remaining tokens as one chunk, beam after beam.  Here each live beam owns a slot, and a step evaluates every live beam's
+// newest token in one multi_eval.  What a chunk changes is the row length n_total of its V·P dots (DESIGN §2, item 4); the
+// reference's f16 dot puts the elements below n_total & ~31 in its fp32 lanes and adds the rest one by one, and the entries
+// past a token's own position are 0.  So a position p's K / V come out of one of two sums, told apart by vp_lanes(p, n_total).
+// Each slot records the (token, sum) of every position it holds; a position whose sum differs from the reference's for this
+// step is evaluated again, with every position after it.
+static bool vp_lanes(int p, int n_total) { return (n_total & ~31) >= p + 1; }
+
+struct SlotHeld { std::vector<int> tok; std::vector<char> lanes; };   // what a slot's K / V hold, per position
+
+struct BeamRun {                  // one prompt's search
+  int prompt = 0, P = 0;          // prompt index and length
+  int c = 0;                      // tokens after the prompt shifted off as the beams' common prefix
+  int iter = 0;
+  std::vector<int> slots;         // its n_beams slots
+  std::vector<BeamCand> beams, next;
+  std::vector<std::vector<int>> toks;   // beams[i]'s tokens after the prompt
+  std::vector<int> slot;                // beams[i]'s slot; -1 for an eob beam
+  std::vector<int> fin_nt;              // the reference's n_total of positions P .. P + c - 1 (their common-prefix chunk)
+};
+
+// Appends a run of one slot's tokens at consecutive positions to a multi_eval list, cut into launches of MULTI_LAUNCH_TOKENS.
+static void beam_append(std::vector<MultiTok>& toks, std::vector<int>& starts, int slot, const int* tokens, int pos0, const int* n_total, int n) {
+  for (int j = 0; j < n; j++) {
+    if ((int)toks.size() - starts.back() == MULTI_LAUNCH_TOKENS) starts.push_back((int)toks.size());
+    toks.push_back({slot, tokens[j], pos0 + j, n_total[j], j == n - 1});
+  }
+}
+
+int ctb_beam_step(int n_beams, int n_in, int n_next, const float* in_p, const unsigned char* in_eob, const float* rows, int n_vocab, int* out_parent,
+                  int* out_token, float* out_p, unsigned char* out_eob) {
+  try {
+    if (n_beams < 1 || n_beams > n_vocab) throw std::invalid_argument("n_beams must lie in 1 .. n_vocab");
+    if (n_in < 1 || n_in > n_beams || n_next < 0 || n_next > n_beams) throw std::invalid_argument("bad beam counts");
+    std::vector<BeamCand> beams(n_in), next(n_next, BeamCand{0.0f, false, -1, -1});
+    std::vector<const float*> r(n_in);
+    for (int i = 0; i < n_in; i++) {
+      beams[i] = {in_p[i], in_eob[i] != 0, -1, -1};
+      r[i] = rows + (size_t)i * n_vocab;
+    }
+    const std::vector<BeamCand> out = beam_step(n_beams, beams, next, r.data(), n_vocab);
+    for (size_t j = 0; j < out.size(); j++) {
+      out_parent[j] = out[j].parent; out_token[j] = out[j].token; out_p[j] = out[j].p; out_eob[j] = out[j].eob;
+    }
+    return (int)out.size();
+  } catch (const std::exception& e) {
+    fprintf(stderr, "ctransformers-b200: beam step failed: %s\n", e.what());
+    return -1;
+  }
+}
+
+long ctb_multi_reparent(ctb_multi* m, int n, const int* src, const int* dst, const int* lo, const int* hi) {
+  try {
+    std::vector<KvCopy> copies(n);
+    for (int i = 0; i < n; i++) {
+      if (!multi_slot_ok(m, src[i]) || !multi_slot_ok(m, dst[i])) return -1;
+      copies[i] = {src[i], dst[i], lo[i], hi[i]};
+    }
+    const size_t bytes = m->llm->engine->kv_reparent(copies);
+    for (const KvCopy& c : copies) {
+      m->has[c.dst] = m->has[c.src];
+      m->fresh[c.dst] = 0;
+    }
+    return (long)bytes;
+  } catch (const std::exception& e) { return state_error("cannot re-parent the slots", e); }
+}
+
+int ctb_multi_beam_search(ctb_multi* m, int n_prompts, const int* prompt_off, const int* prompt_tokens, int n_beams, int n_predict, int batch_size,
+                          int* out_off, int* out_tokens, float* out_p) {
+  using clk = std::chrono::steady_clock;
+  const auto ms = [](clk::time_point a, clk::time_point b) { return std::chrono::duration<double, std::milli>(b - a).count(); };
+  std::vector<char> used(m->n_slots, 0);
+  try {
+    const HParams& hp = m->llm->hp;
+    const int n_vocab = hp.n_vocab, eos = m->llm->vocab.eos;
+    if (n_prompts < 0) throw std::invalid_argument("a negative prompt count");
+    if (n_beams < 1 || n_beams > m->n_slots) throw std::invalid_argument("n_beams = " + std::to_string(n_beams) + ": each beam needs a slot, and there are " + std::to_string(m->n_slots));
+    if (n_beams > n_vocab) throw std::invalid_argument("n_beams is larger than the vocabulary");
+    if (n_predict < 0) throw std::invalid_argument("a negative n_predict");
+    for (int i = 0; i < n_prompts; i++) {
+      const int P = prompt_off[i + 1] - prompt_off[i];
+      if (P < 1) throw std::invalid_argument("prompt " + std::to_string(i) + " is empty");
+      if (P + n_predict > hp.n_ctx)
+        throw std::invalid_argument("prompt " + std::to_string(i) + ": " + std::to_string(P) + " tokens and " + std::to_string(n_predict) +
+                                    " more exceed the context length " + std::to_string(hp.n_ctx));
+      check_tokens(prompt_tokens + prompt_off[i], P, n_vocab);
+    }
+    double stats[8] = {0};   // ctb_multi_beam_stats
+    out_off[0] = 0;
+    std::vector<std::vector<int>> result(n_prompts);
+    std::vector<float> result_p(n_prompts, 1.0f);
+    Engine& e = *m->llm->engine;
+    std::vector<SlotHeld> held(m->n_slots);
+    std::vector<int> free_slots;
+    for (int s = 0; s < m->n_slots; s++) free_slots.push_back(s);
+    std::vector<BeamRun> runs;
+    int waiting = n_predict > 0 ? 0 : n_prompts;   // (n_predict 0: the reference's loop never runs; the response is empty, p 1)
+    std::vector<int> pos, nt;
+    while (!runs.empty() || waiting < n_prompts) {
+      std::vector<MultiTok> toks;
+      std::vector<int> starts(1, 0);
+      // the loop's test and the example's callback, then each live beam's tokens whose K / V differ from the reference's
+      for (size_t r = 0; r < runs.size();) {
+        BeamRun& R = runs[r];
+        const bool any_live = std::any_of(R.beams.begin(), R.beams.end(), [](const BeamCand& b) { return !b.eob; });
+        if (!(R.iter < n_predict && any_live && !R.beams[beam_top(R.beams)].eob)) {
+          const size_t top = beam_top(R.beams);   // collapse; the last callback collects the rest of the top beam's tokens
+          result[R.prompt] = R.toks[top];
+          result_p[R.prompt] = R.beams[top].p;
+          free_slots.insert(free_slots.end(), R.slots.begin(), R.slots.end());
+          runs.erase(runs.begin() + r);
+          continue;
+        }
+        const size_t nb = R.beams.size();
+        for (size_t i = 0; i < nb; i++)
+          if (!R.beams[i].eob && !R.toks[i].empty() && R.toks[i].back() == eos) {
+            R.beams[i].eob = true;
+            R.slot[i] = -1;   // an eob beam is never evaluated again: its slot is free
+          }
+        size_t cpl = R.toks[0].size() - R.c;
+        for (size_t i = 1; i < nb; i++) {
+          cpl = std::min(cpl, R.toks[i].size() - R.c);
+          for (size_t j = 0; j < cpl; j++)
+            if (R.toks[i][R.c + j] != R.toks[0][R.c + j]) { cpl = j; break; }
+        }
+        for (size_t j = 0; j < cpl; j++) R.fin_nt.push_back(R.P + R.c + (int)cpl);
+        R.c += (int)cpl;
+        for (size_t i = 0; i < nb; i++) {
+          if (R.beams[i].eob) continue;
+          const std::vector<int>& t = R.toks[i];
+          const int L = (int)t.size(), s = R.slot[i];
+          SlotHeld& h = held[s];
+          nt.resize(L);
+          for (int j = 0; j < L; j++) nt[j] = j < R.c ? R.fin_nt[j] : R.P + L;
+          int q = L - 1;   // the newest token always runs: its row is this step's
+          for (int j = 0; j < L - 1; j++)
+            if (R.P + j >= (int)h.tok.size() || h.tok[R.P + j] != t[j] || h.lanes[R.P + j] != vp_lanes(R.P + j, nt[j])) { q = j; break; }
+          h.tok.resize(R.P + q); h.lanes.resize(R.P + q);
+          for (int j = q; j < L; j++) { h.tok.push_back(t[j]); h.lanes.push_back(vp_lanes(R.P + j, nt[j])); }
+          beam_append(toks, starts, s, t.data() + q, R.P + q, nt.data() + q, L - q);
+        }
+        r++;
+      }
+      // admission: a prompt takes n_beams free slots and is evaluated, chunked as LLM::BatchEval chunks it, in the first
+      bool admitted = false;
+      while (waiting < n_prompts && (int)free_slots.size() >= n_beams) {
+        std::sort(free_slots.begin(), free_slots.end());
+        BeamRun R;
+        R.prompt = waiting++;
+        R.P = prompt_off[R.prompt + 1] - prompt_off[R.prompt];
+        R.slots.assign(free_slots.begin(), free_slots.begin() + n_beams);
+        free_slots.erase(free_slots.begin(), free_slots.begin() + n_beams);
+        for (int s : R.slots) {
+          e.multi_reset(s);
+          used[s] = 1;
+          m->has[s] = 0; m->fresh[s] = 0;
+          held[s] = SlotHeld();
+        }
+        const int* pt = prompt_tokens + prompt_off[R.prompt];
+        pos.resize(R.P); nt.resize(R.P);
+        eval_positions(R.P, 0, batch_size, hp.n_ctx, pos.data(), nt.data());
+        SlotHeld& h = held[R.slots[0]];
+        for (int j = 0; j < R.P; j++) {
+          h.tok.push_back(pt[j]);
+          h.lanes.push_back(vp_lanes(pos[j], nt[j]));
+        }
+        beam_append(toks, starts, R.slots[0], pt, 0, nt.data(), R.P);
+        R.beams.push_back(BeamCand{1.0f, false, -1, -1});
+        R.toks.emplace_back();
+        R.slot.push_back(R.slots[0]);
+        runs.push_back(std::move(R));
+        admitted = true;
+      }
+      if (runs.empty()) continue;
+      // one batched eval of every live beam's tokens (and of the prompts just admitted)
+      auto t0 = clk::now();
+      if ((int)toks.size() > starts.back()) starts.push_back((int)toks.size());
+      if (!toks.empty()) {
+        e.multi_eval(toks, starts);
+        for (const MultiTok& t : toks) { m->has[t.slot] = 1; m->fresh[t.slot] = 0; }
+      }
+      auto t1 = clk::now();
+      // their logits rows in one copy, then the reference's selection
+      int lo_s = m->n_slots, hi_s = -1;
+      for (const BeamRun& R : runs)
+        for (size_t i = 0; i < R.beams.size(); i++)
+          if (!R.beams[i].eob) { lo_s = std::min(lo_s, R.slot[i]); hi_s = std::max(hi_s, R.slot[i]); }
+      const float* rows = hi_s >= lo_s ? e.multi_rows(lo_s, hi_s - lo_s + 1) : nullptr;
+      std::vector<KvCopy> copies;
+      for (BeamRun& R : runs) {
+        std::vector<const float*> rp(R.beams.size(), nullptr);
+        for (size_t i = 0; i < R.beams.size(); i++)
+          if (!R.beams[i].eob) rp[i] = rows + (size_t)(R.slot[i] - lo_s) * n_vocab;
+        std::vector<BeamCand> nb = beam_step(n_beams, R.beams, R.next, rp.data(), n_vocab);
+        // Slots of the new beams.  A live parent's first child keeps the parent's slot; every other child takes a slot that no
+        // kept parent holds (a parent without children, an eob beam's, one not used yet).  So the copies' sources (kept slots)
+        // and destinations (the others) are disjoint, and one launch can run them all: no copy reads a slot another writes.
+        std::vector<int> slot(nb.size(), -1);
+        std::vector<std::vector<int>> nt_toks(nb.size());
+        std::vector<char> kept(m->n_slots, 0);
+        for (size_t j = 0; j < nb.size(); j++) {
+          const int pa = nb[j].parent;
+          nt_toks[j] = R.toks[pa];
+          if (nb[j].token < 0) continue;
+          nt_toks[j].push_back(nb[j].token);
+          if (!kept[R.slot[pa]]) { kept[R.slot[pa]] = 1; slot[j] = R.slot[pa]; }
+        }
+        std::vector<int> spare;
+        for (int s : R.slots)
+          if (!kept[s]) spare.push_back(s);
+        for (size_t j = 0; j < nb.size(); j++) {
+          if (nb[j].token < 0 || slot[j] >= 0) continue;
+          if (spare.empty()) throw std::logic_error("beam search: more live beams than slots");
+          const int src = R.slot[nb[j].parent], dst = spare.back();
+          spare.pop_back();
+          const SlotHeld &hs = held[src], &hd = held[dst];
+          int lo = 0;
+          while (lo < (int)std::min(hs.tok.size(), hd.tok.size()) && hs.tok[lo] == hd.tok[lo] && hs.lanes[lo] == hd.lanes[lo]) lo++;
+          copies.push_back({src, dst, lo, (int)hs.tok.size()});
+          held[dst] = hs;
+          slot[j] = dst;
+        }
+        R.next = std::move(R.beams);
+        R.beams = std::move(nb);
+        R.toks = std::move(nt_toks);
+        R.slot = std::move(slot);
+        R.iter++;
+      }
+      auto t2 = clk::now();
+      // one re-parenting launch for every prompt's copies
+      stats[4] += (double)e.kv_reparent(copies);
+      for (const KvCopy& c : copies) { m->has[c.dst] = m->has[c.src]; m->fresh[c.dst] = 0; }
+      auto t3 = clk::now();
+      stats[0] += 1; stats[1] += ms(t0, t1); stats[2] += ms(t1, t2); stats[3] += ms(t2, t3); stats[5] += (double)toks.size();
+      if (admitted) { stats[6] += 1; stats[7] += ms(t0, t1); }
+    }
+    for (int s = 0; s < m->n_slots; s++)
+      if (used[s]) ctb_multi_reset(m, s);
+    for (int i = 0; i < n_prompts; i++) {
+      out_off[i + 1] = out_off[i] + (int)result[i].size();
+      std::copy(result[i].begin(), result[i].end(), out_tokens + out_off[i]);
+      out_p[i] = result_p[i];
+    }
+    std::copy(stats, stats + 8, m->beam_stats);
+    return 0;
+  } catch (const std::exception& ex) {
+    fprintf(stderr, "ctransformers-b200: beam search failed: %s\n", ex.what());
+    try {
+      for (int s = 0; s < m->n_slots; s++)
+        if (used[s]) ctb_multi_reset(m, s);
+    } catch (...) {}
+    return -1;
+  }
+}
+
+int ctb_multi_beam_stats(ctb_multi* m, double* out8) {
+  std::copy(m->beam_stats, m->beam_stats + 8, out8);
+  return 8;
 }
 
 long ctb_multi_launches(ctb_multi* m) { return m->llm->engine->multi_launches(); }

@@ -129,6 +129,10 @@ EXTRA_PROTOTYPES = {
     "ctb_row_logprob": (C.c_int, [_P, C.c_int, C.c_int, _IP, _DP, _IP]),
     "ctb_multi_eval_rows": (C.c_int, [_P, C.c_int, _IP, _IP, _IP, _IP, C.c_int, _FP]),
     "ctb_multi_eval_scored": (C.c_int, [_P, C.c_int, _IP, _IP, _IP, _IP, C.c_int, _IP, _DP, _IP]),
+    "ctb_beam_step": (C.c_int, [C.c_int, C.c_int, C.c_int, _FP, _P, _FP, C.c_int, _IP, _IP, _FP, _P]),
+    "ctb_multi_reparent": (C.c_long, [_P, C.c_int, _IP, _IP, _IP, _IP]),
+    "ctb_multi_beam_search": (C.c_int, [_P, C.c_int, _IP, _IP, C.c_int, C.c_int, C.c_int, _IP, _IP, _FP]),
+    "ctb_multi_beam_stats": (C.c_int, [_P, _DP]),
 }
 
 

@@ -266,6 +266,54 @@ class MultiLLM:
                     admit()
         return results if n > 1 else [r[0] for r in results]
 
+    def beam_search(self, prompt_tokens: Sequence[int], n_beams: int, max_new_tokens: int, *, batch_size: Optional[int] = None) -> Tuple[List[int], float]:
+        """Beam search after the prompt, as the reference's llama_beam_search with its example's callback (a beam ends at EOS):
+        (the winning beam's tokens, an EOS included when it ends in one; its p, renormalised over the last step's beams), bit
+        for bit.  The prompt is evaluated in one slot, chunked by batch_size; the search holds n_beams slots and evaluates all
+        live beams in one batched launch per step.  It uses the lowest n_beams slots and resets them afterwards: their earlier
+        context is not kept."""
+        return self.beam_search_many([prompt_tokens], n_beams, max_new_tokens, batch_size=batch_size)[0]
+
+    def beam_search_many(self, prompts: Sequence[Sequence[int]], n_beams: int, max_new_tokens: int, *,
+                         batch_size: Optional[int] = None) -> List[Tuple[List[int], float]]:
+        """beam_search of every prompt: up to n_slots // n_beams searches at once, a prompt admitted as slots free up, the live
+        beams of all of them evaluated in the same launches.  Each result equals beam_search of that prompt alone.  The slots
+        used, the lowest n_beams * min(len(prompts), n_slots // n_beams), are reset afterwards."""
+        if not 1 <= n_beams <= min(self.n_slots, self.vocab_size):
+            raise ValueError(f"n_beams = {n_beams}: each beam needs a slot, and there are {self.n_slots}")
+        if max_new_tokens < 0:
+            raise ValueError("max_new_tokens must not be negative")
+        prompts = [_check_ids(p, self.vocab_size, f"prompt {i}: token") for i, p in enumerate(prompts)]
+        for i, p in enumerate(prompts):
+            if not p:
+                raise ValueError(f"prompt {i} is empty")
+            if len(p) + max_new_tokens > self.context_length:
+                raise ValueError(f"prompt {i}: {len(p)} tokens and {max_new_tokens} more exceed the context length {self.context_length}")
+        off, flat = [0], []
+        for p in prompts:
+            flat.extend(p)
+            off.append(len(flat))
+        n = len(prompts)
+        out_off = (c_int * (n + 1))()
+        out_tok = (c_int * max(n * max_new_tokens, 1))()
+        out_p = (c_float * max(n, 1))()
+        rc = self._lib.ctb_multi_beam_search(self._m, n, _ints(off), _ints(flat), n_beams, max_new_tokens, _pick(batch_size, self._config.batch_size),
+                                             out_off, out_tok, out_p)
+        # searches take the lowest free slots, n_beams each: these are the slots used, and the library has reset them
+        for s in range(n_beams * min(n, self.n_slots // n_beams) if max_new_tokens > 0 else 0):
+            self._context[s] = []
+        if rc != 0:
+            raise RuntimeError(f"Beam search failed (n_beams = {n_beams}); see stderr.")
+        return [(list(out_tok[out_off[i]:out_off[i + 1]]), float(out_p[i])) for i in range(n)]
+
+    def beam_stats(self) -> Dict[str, float]:
+        """The last beam search: steps, host-clock ms of its evals, of its row fetches + selections and of its re-parentings,
+        the K / V bytes the re-parenting launches moved, the tokens evaluated (prompts included), the steps that also evaluated
+        a prompt and the ms of their evals."""
+        v = (c_double * 8)()
+        self._lib.ctb_multi_beam_stats(self._m, v)
+        return dict(zip(("steps", "eval_ms", "select_ms", "reparent_ms", "reparent_bytes", "tokens", "prompt_steps", "prompt_eval_ms"), list(v)))
+
     def __del__(self):
         if self.__dict__.get("_m") is not None and self.__dict__.get("_lib") is not None:
             self._lib.ctb_multi_delete(self._m)

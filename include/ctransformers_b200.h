@@ -295,6 +295,34 @@ int ctb_multi_restore(ctb_multi* m, int slot, const void* buf, size_t size);
  * greedy pick), stream-ordered.  src must not be among dsts.  0, or -1 (+ stderr). */
 int ctb_multi_fork(ctb_multi* m, int src, int n, const int* dsts);
 
+/* Beam search: the reference's llama_beam_search (llama.cpp:4334-4579) driven as its examples/beam_search does (a beam is at its
+ * end when its last token is EOS), each result bit-identical.  Prompt i (tokens [prompt_off[i], prompt_off[i + 1])) is evaluated
+ * in one slot, chunked by batch_size as ctransformers_llm_batch_eval chunks it; its search holds n_beams slots, and prompts are
+ * admitted as slots free up.  Each step evaluates every live beam of every prompt in one batched eval; the beams are chosen on
+ * the host from their logits rows; then one launch moves K / V between slots where beams re-parent.  The response of prompt i
+ * (at most n_predict tokens, an EOS included when the winning beam ends in one) goes to out_tokens[out_off[i] .. out_off[i + 1])
+ * (room for n_prompts * n_predict ids, out_off for n_prompts + 1), the winner's renormalised p to out_p[i].  The slots used
+ * are reset afterwards.  0, or -1 (+ stderr) with every slot usable: n_beams outside 1 .. min(n_slots, n_vocab), an empty
+ * prompt, a prompt whose length plus n_predict exceeds the context, a token id out of range, or a continuation whose p
+ * underflows to 0 (undefined in the reference). */
+int ctb_multi_beam_search(ctb_multi* m, int n_prompts, const int* prompt_off, const int* prompt_tokens, int n_beams, int n_predict, int batch_size,
+                          int* out_off, int* out_tokens, float* out_p);
+/* the last beam search: steps, host-clock ms of the evals, of the row fetches + selections and of the re-parentings, the K / V
+ * bytes the re-parenting launches moved, the tokens evaluated (prompts included), the steps that also evaluated a prompt and
+ * the ms of their evals */
+int ctb_multi_beam_stats(ctb_multi* m, double* out8);
+/* Op level, for tests.  One selection step of the beam search on given rows: n_in beams (p, eob) with their logits rows
+ * ([n_in][n_vocab]; an eob beam's row is unused), n_next entries left from the step before (0 at the first step, then the
+ * previous step's beam count).  Writes the new beams in the reference's array order: the index of the beam each comes from,
+ * the token it adds (-1: an eob beam carried over), its renormalised p and eob flag.  Returns their count, or -1 (+ stderr),
+ * e.g. when a continuation's p underflows to 0. */
+int ctb_beam_step(int n_beams, int n_in, int n_next, const float* in_p, const unsigned char* in_eob, const float* rows, int n_vocab, int* out_parent,
+                  int* out_token, float* out_p, unsigned char* out_eob);
+/* Op level, for tests: the re-parenting launch of the beam search.  Slot dst[i] takes slot src[i]'s K / V at positions
+ * [lo[i], hi[i]) (whole 256-position blocks of V), its last results and greedy pick; no slot may be both a source and a
+ * destination.  Returns the K / V bytes moved, or -1 (+ stderr). */
+long ctb_multi_reparent(ctb_multi* m, int n, const int* src, const int* dst, const int* lo, const int* hi);
+
 /* Rows of every token: the logits row of every evaluated token, not only the last one's, each bit-identical to what the
  * reference's llama_eval returns for that token with the context flag logits_all set (llama.cpp:2949-2960), under the same
  * batch_size chunking and n_past clamp as ctransformers_llm_batch_eval.  Otherwise an eval with rows is an ordinary eval:
