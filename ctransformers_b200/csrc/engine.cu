@@ -76,7 +76,7 @@ struct PrefillState {
   size_t smem = 0;
   bool q3 = false;                  // the program holds Q3_K matrices (k_pstep<true>)
   bool ok = false, tried = false;
-  // multi-sequence mode (HParams::n_seq > 1): the same program on slot-addressed state (k_pstep<.., true>), plus the output head
+  // multi-sequence mode (HParams::multi): the same program on slot-addressed state (k_pstep<.., true>), plus the output head
   PPhase* d_mprog = nullptr;
   int n_mphases = 0;
   bool mq3 = false;
@@ -93,6 +93,13 @@ struct PrefillState {
   PPhase* d_rprog = nullptr;
   int n_rphases = 0;
   bool rq3 = false, rtried = false;
+  void* dalloc(size_t bytes) {      // zeroed device memory, freed with the state
+    void* p = nullptr;
+    CTB_CUDA(cudaMalloc(&p, bytes));
+    bufs.push_back(p);
+    CTB_CUDA(cudaMemset(p, 0, bytes));
+    return p;
+  }
   ~PrefillState() {
     for (void* b : bufs) cudaFree(b);
     if (h_state) cudaFreeHost(h_state);
@@ -819,10 +826,8 @@ void Engine::mark(int kind) {
 int Engine::profile_step(int token, int n_past, double ms_by_kind[4], int count_by_kind[4]) {
   DeviceGuard dev_guard(device_);
   if (tp_.world > 1) throw std::runtime_error("not available in tensor-parallel mode (every rank must run the same launches)");
-  spec_pending_ = false; spec_deferred_ = false; spec_pos_ = -1; spec_streak_ = 0;
-  if (h_state_cap_ < 1) { h_state_cap_ = 512; CTB_CUDA(cudaMallocHost(&h_state_, (size_t)h_state_cap_ * 16)); }
-  h_state_[0] = token; h_state_[1] = n_past; h_state_[2] = 0; h_state_[3] = n_past + 1;
-  CTB_CUDA(cudaMemcpyAsync(d_state_, h_state_, 16, cudaMemcpyHostToDevice, stream_));
+  drop_lookahead();
+  put_step(token, n_past, n_past + 1);
   const long keep = launches_per_step_;
   const bool keep_fused = fused_;
   profiling_ = true; fused_ = false;
@@ -848,7 +853,7 @@ int Engine::profile_step(int token, int n_past, double ms_by_kind[4], int count_
 double Engine::time_matvec_only(int reps, long* launches, unsigned mask) {
   if (!mask) mask = ~0u;
   if (tp_.world > 1) throw std::runtime_error("not available in tensor-parallel mode (every rank must run the same launches)");
-  spec_pending_ = false; spec_deferred_ = false; spec_pos_ = -1; spec_streak_ = 0;
+  drop_lookahead();
   DeviceGuard dev_guard(device_);
   std::vector<StepOp> sel;
   for (int i = 0; i <= n_body_; i++)
@@ -889,7 +894,7 @@ double Engine::time_matvec_only(int reps, long* launches, unsigned mask) {
 long Engine::trace_step(int token, int n_past, unsigned long long* out, long cap_words) {
   DeviceGuard dev_guard(device_);
   if (tp_.world > 1) throw std::runtime_error("not available in tensor-parallel mode (every rank must run the same launches)");
-  spec_pending_ = false; spec_deferred_ = false; spec_pos_ = -1; spec_streak_ = 0;
+  drop_lookahead();
   const int n = n_body_ + 1;
   for (int i = 0; i < n; i++)
     if (ops_[i].ph.kind == PH_MATVEC && !ops_[i].stream) return 0;
@@ -900,10 +905,8 @@ long Engine::trace_step(int token, int n_past, unsigned long long* out, long cap
   CTB_CUDA(cudaMemset(buf, 0, (size_t)n * step_grid_ * 64));
   StepLaunch L;
   L.grid = step_grid_; L.n_slots = step_slots_; L.smem = step_smem_; L.gen = !attn_fast_hd(hp_.head_dim()); L.q3 = step_q3_;
-  if (h_state_cap_ < 1) { h_state_cap_ = 512; CTB_CUDA(cudaMallocHost(&h_state_, (size_t)h_state_cap_ * 16)); }
   for (int rep = 0; rep < 3; rep++) {   // the last (warm) run is the one read back
-    h_state_[0] = token; h_state_[1] = n_past; h_state_[2] = 0; h_state_[3] = n_past + 1;
-    CTB_CUDA(cudaMemcpyAsync(d_state_, h_state_, 16, cudaMemcpyHostToDevice, stream_));
+    put_step(token, n_past, n_past + 1);
     CTB_CUDA(launch_step(L, stream_, d_prog_, d_bounds_, n, d_sync_, false, buf));
     CTB_CUDA(cudaStreamSynchronize(stream_));
   }
@@ -987,6 +990,8 @@ void Engine::after_eval(int next_pos) {
   }
 }
 
+void Engine::drop_lookahead() { spec_pending_ = false; spec_deferred_ = false; spec_pos_ = -1; spec_streak_ = 0; }
+
 void Engine::launch_deferred_spec() {
   if (!spec_deferred_) return;
   spec_deferred_ = false;
@@ -1013,12 +1018,17 @@ void Engine::eval(const int* tokens, int n, int n_past) {
   eval_list(tokens, pos.data(), nt.data(), n);
 }
 
-void Engine::decode_one(int token, int pos, int n_total, bool with_logits) {
+// Each copy reads its own ring entry, so a copy still pending in the stream reads what it was given (eval_list synchronises
+// before the ring wraps).
+void Engine::put_step(int token, int pos, int n_total) {
   if (h_state_cap_ < 1) { h_state_cap_ = 512; CTB_CUDA(cudaMallocHost(&h_state_, (size_t)h_state_cap_ * 16)); }
-  int* st = h_state_ + (size_t)(h_state_next_ % h_state_cap_) * 4;
-  h_state_next_++;
+  int* st = h_state_ + (size_t)(h_state_next_++ % h_state_cap_) * 4;
   st[0] = token; st[1] = pos; st[2] = 0; st[3] = n_total;
   CTB_CUDA(cudaMemcpyAsync(d_state_, st, 16, cudaMemcpyHostToDevice, stream_));
+}
+
+void Engine::decode_one(int token, int pos, int n_total, bool with_logits) {
+  put_step(token, pos, n_total);
   CTB_CUDA(cudaGraphLaunch(with_logits ? graph_full_ : graph_nolog_, stream_));
   single_steps_++;
 }
@@ -1207,17 +1217,10 @@ bool Engine::ensure_rows_prog() {
     if (p == d_logits_) { ld = hp_.n_vocab; return d_rows_; }
     throw std::runtime_error("rows: pointer outside the output head's buffers");
   };
-  auto dalloc = [&](size_t bytes) {
-    void* p = nullptr;
-    CTB_CUDA(cudaMalloc(&p, bytes));
-    P.bufs.push_back(p);
-    CTB_CUDA(cudaMemset(p, 0, bytes));
-    return p;
-  };
-  pb_matvec_phases(head.ph.mv, (uint8_t*)dalloc(pb_qbuf_bytes(head.ph.mv.K)), P.d_state, bat, rprog);
+  pb_matvec_phases(head.ph.mv, (uint8_t*)P.dalloc(pb_qbuf_bytes(head.ph.mv.K)), P.d_state, bat, rprog);
   P.n_rphases = (int)rprog.size();
   P.rq3 = pstep_q3(rprog);
-  PPhase* d = (PPhase*)dalloc((rprog.size() + 1) * sizeof(PPhase));
+  PPhase* d = (PPhase*)P.dalloc((rprog.size() + 1) * sizeof(PPhase));
   CTB_CUDA(cudaMemcpy(d, rprog.data(), rprog.size() * sizeof(PPhase), cudaMemcpyHostToDevice));
   P.d_rprog = d;
   return true;
@@ -1228,7 +1231,6 @@ void Engine::eval_list(const int* tokens, const int* pos, const int* n_total, in
   DeviceGuard dev_guard(device_);
   struct Release { Engine* e; ~Release() { e->sink_ = nullptr; } } release{this};   // a failed eval leaves no sink behind
   rows_begin(rows, n);
-  if (h_state_cap_ < 1) { h_state_cap_ = 512; CTB_CUDA(cudaMallocHost(&h_state_, (size_t)h_state_cap_ * 16)); }
   bool hit = false;
   if (spec_pos_ >= 0) {
     const bool was_pending = spec_pending_;   // (a deferred look-ahead nobody launched is simply dropped)
@@ -1274,26 +1276,19 @@ void Engine::eval_list(const int* tokens, const int* pos, const int* n_total, in
 }
 
 bool Engine::ensure_prefill() {
-  if ((!prefill_on_ && hp_.n_seq == 1) || tp_.world > 1) return false;   // (multi-sequence evals have no other path)
+  if ((!prefill_on_ && !hp_.multi) || tp_.world > 1) return false;   // (multi-sequence evals have no other path)
   if (pf_ && pf_->tried) return pf_->ok;
   if (!pf_) pf_ = new PrefillState();
   PrefillState& P = *pf_;
   P.tried = true;
   for (int i = 0; i < n_body_; i++)
     if (ops_[i].ph.kind == PH_MATVEC && !ops_[i].stream) return false;   // a non-K-quant layer matrix: single-token path only
-  auto dalloc = [&](size_t bytes) {
-    void* p = nullptr;
-    CTB_CUDA(cudaMalloc(&p, bytes));
-    P.bufs.push_back(p);
-    CTB_CUDA(cudaMemset(p, 0, bytes));
-    return p;
-  };
   const int n_embd = hp_.n_embd, gqa = hp_.n_embd_gqa();
   const int qkvw = n_embd + 2 * gqa;
   // decode buffer -> (batched buffer, floats between token rows)
   struct Map { const float* lo; size_t n; float* b; int ld; };
   std::vector<Map> maps;
-  auto add = [&](const float* dec, size_t n) { maps.push_back({dec, n, (float*)dalloc((size_t)PB_T * n * 4), (int)n}); };
+  auto add = [&](const float* dec, size_t n) { maps.push_back({dec, n, (float*)P.dalloc((size_t)PB_T * n * 4), (int)n}); };
   add(xa_, n_embd); add(xb_, n_embd); add(qkv_, qkvw); add(attn_, n_embd); add(attn_o_, n_embd); add(ffn_, hp_.n_ff); add(ffn2_, hp_.n_ff);
   auto bat = [&](const float* p, int& ld) -> float* {
     if (!p) { ld = 0; return nullptr; }
@@ -1301,7 +1296,7 @@ bool Engine::ensure_prefill() {
       if (p >= m.lo && p < m.lo + m.n) { ld = m.ld; return m.b + (p - m.lo); }
     throw std::runtime_error("prefill: pointer outside the step workspace");
   };
-  P.d_state = (int*)dalloc((PB_T * 4 + 4) * 4);
+  P.d_state = (int*)P.dalloc((PB_T * 4 + 4) * 4);
   CTB_CUDA(cudaMallocHost(&P.h_state, (size_t)PF_RING * (PB_T * 4 + 4) * 4));
   std::vector<PPhase> prog;
   int K_max = 0;
@@ -1326,17 +1321,17 @@ bool Engine::ensure_prefill() {
       ph.kind = PP_ATTN; prog.push_back(ph);
     } else {
       K_max = std::max(K_max, op.ph.mv.K);
-      pb_matvec_phases(op.ph.mv, (uint8_t*)dalloc(pb_qbuf_bytes(op.ph.mv.K)), P.d_state, bat, prog);
+      pb_matvec_phases(op.ph.mv, (uint8_t*)P.dalloc(pb_qbuf_bytes(op.ph.mv.K)), P.d_state, bat, prog);
     }
   }
   int ld;
   P.x_final = bat(ops_[n_body_].ph.mv.x, ld);
   P.n_phases = (int)prog.size();
   P.q3 = pstep_q3(prog);
-  P.d_prog = (PPhase*)dalloc((prog.size() + 1) * sizeof(PPhase));
+  P.d_prog = (PPhase*)P.dalloc((prog.size() + 1) * sizeof(PPhase));
   CTB_CUDA(cudaMemcpy(P.d_prog, prog.data(), prog.size() * sizeof(PPhase), cudaMemcpyHostToDevice));
-  if (hp_.n_seq > 1) {
-    P.d_mstate = (int*)dalloc(PB_STATE_MS * 4);
+  if (hp_.multi) {
+    P.d_mstate = (int*)P.dalloc(PB_STATE_MS * 4);
     CTB_CUDA(cudaMallocHost(&P.h_mstate, (size_t)PF_RING * PB_STATE_MS * 4));
     std::vector<PPhase> mprog = prog;
     for (PPhase& ph : mprog) { ph.state = P.d_mstate; ph.at.state = P.d_mstate; }
@@ -1344,18 +1339,18 @@ bool Engine::ensure_prefill() {
     P.mhead = head.stream;
     if (P.mhead) {   // the final norm (written as every token's embeddings) and the output matrix over every token of the launch
       add(d_logits_, hp_.n_vocab); add(d_embd_, n_embd);
-      pb_matvec_phases(head.ph.mv, (uint8_t*)dalloc(pb_qbuf_bytes(head.ph.mv.K)), P.d_mstate, bat, mprog);
+      pb_matvec_phases(head.ph.mv, (uint8_t*)P.dalloc(pb_qbuf_bytes(head.ph.mv.K)), P.d_mstate, bat, mprog);
       P.logits_b = bat(d_logits_, ld);
       P.embd_b = bat(d_embd_, ld);
       mprog[mprog.size() - 2].mv.norm_out = P.embd_b;
     }
     P.n_mphases = (int)mprog.size();
     P.mq3 = pstep_q3(mprog);
-    P.d_mprog = (PPhase*)dalloc((mprog.size() + 1) * sizeof(PPhase));
+    P.d_mprog = (PPhase*)P.dalloc((mprog.size() + 1) * sizeof(PPhase));
     CTB_CUDA(cudaMemcpy(P.d_mprog, mprog.data(), mprog.size() * sizeof(PPhase), cudaMemcpyHostToDevice));
-    P.d_mlogits = (float*)dalloc((size_t)hp_.n_seq * hp_.n_vocab * 4);
-    P.d_membd = (float*)dalloc((size_t)hp_.n_seq * n_embd * 4);
-    P.d_mpick = (int*)dalloc((size_t)hp_.n_seq * 8);
+    P.d_mlogits = (float*)P.dalloc((size_t)hp_.n_seq * hp_.n_vocab * 4);
+    P.d_membd = (float*)P.dalloc((size_t)hp_.n_seq * n_embd * 4);
+    P.d_mpick = (int*)P.dalloc((size_t)hp_.n_seq * 8);
   }
   if (!pstep_shape(pb_work_bytes(K_max, hp_.n_ctx, hp_.head_dim()), P.n_slots, P.smem)) return false;
   CTB_CUDA(pstep_set_smem_limit(P.smem));
@@ -1411,18 +1406,25 @@ std::string Engine::multi_refusal() {
   for (int i = 0; i < n_body_; i++)
     if (ops_[i].ph.kind == PH_MATVEC && !ops_[i].stream) return "layer matrices that are not K-quants (Q3_K / Q4_K / Q5_K / Q6_K)";
   DeviceGuard dev_guard(device_);
-  if (!ensure_prefill() || !pf_->d_mprog) return "a context of " + std::to_string(hp_.n_ctx) + " (the batched kernel's attention scratch does not fit in shared memory)";
+  if (!multi_ready()) return "a context of " + std::to_string(hp_.n_ctx) + " (the batched kernel's attention scratch does not fit in shared memory)";
   return "";
+}
+
+bool Engine::multi_ready() { return hp_.multi && ensure_prefill() && pf_->d_mprog; }
+
+void Engine::need_multi() {
+  if (!multi_ready()) throw std::runtime_error("this engine has no multi-sequence path");
 }
 
 void Engine::multi_eval(const std::vector<MultiTok>& toks, const std::vector<int>& starts, const RowSink* rows) {
   DeviceGuard dev_guard(device_);
-  if (hp_.n_seq < 2 || !ensure_prefill() || !pf_->d_mprog) throw std::runtime_error("this engine has no multi-sequence path");
+  need_multi();
   PrefillState& P = *pf_;
   struct Release { Engine* e; ~Release() { e->sink_ = nullptr; } } release{this};
   rows_begin(rows, (int)toks.size());
-  const int hd = hp_.head_dim(), n_embd = hp_.n_embd, n_vocab = hp_.n_vocab;
-  const size_t kslot = (size_t)hp_.n_layer * hp_.n_ctx * nkv_ * k_stride(hd), vslot = (size_t)hp_.n_layer * kv_ctx_pad(hp_.n_ctx) * nkv_ * hd;
+  const int n_embd = hp_.n_embd, n_vocab = hp_.n_vocab;
+  size_t kslot, vslot;
+  kv_slot_elems(kslot, vslot);
   if (kslot > 0xffffffffu || vslot > 0xffffffffu) throw std::runtime_error("multi-sequence: a slot's KV region is too large");
   CTB_CUDA(cudaEventRecord(ev0_, stream_));
   for (size_t l = 0; l + 1 < starts.size(); l++) {
@@ -1472,6 +1474,7 @@ void Engine::multi_eval(const std::vector<MultiTok>& toks, const std::vector<int
 
 void Engine::multi_fetch(int slot, float* logits, float* embd) {
   DeviceGuard dev_guard(device_);
+  need_multi();
   PrefillState& P = *pf_;
   CTB_CUDA(cudaMemcpyAsync(logits, P.d_mlogits + (size_t)slot * hp_.n_vocab, (size_t)hp_.n_vocab * 4, cudaMemcpyDeviceToHost, stream_));
   CTB_CUDA(cudaMemcpyAsync(embd, P.d_membd + (size_t)slot * hp_.n_embd, (size_t)hp_.n_embd * 4, cudaMemcpyDeviceToHost, stream_));
@@ -1480,7 +1483,7 @@ void Engine::multi_fetch(int slot, float* logits, float* embd) {
 
 const SampleGpuOut* Engine::multi_sample(const SampleRow* rows, int R, int* picks) {
   DeviceGuard dev_guard(device_);
-  if (!pf_ || !pf_->d_mlogits) throw std::runtime_error("this engine has no multi-sequence path");
+  need_multi();
   sample_enqueue(rows, R, pf_->d_mlogits, (size_t)hp_.n_vocab, true);
   CTB_CUDA(cudaStreamSynchronize(stream_));
   memcpy(picks, h_sample_, (size_t)hp_.n_seq * 8);
@@ -1489,10 +1492,7 @@ const SampleGpuOut* Engine::multi_sample(const SampleRow* rows, int R, int* pick
 
 void Engine::multi_reset(int slot) {
   DeviceGuard dev_guard(device_);
-  const int hd = hp_.head_dim();
-  const size_t kslot = (size_t)hp_.n_layer * hp_.n_ctx * nkv_ * k_stride(hd), vslot = (size_t)hp_.n_layer * kv_ctx_pad(hp_.n_ctx) * nkv_ * hd;
-  CTB_CUDA(cudaMemsetAsync(kc_ + (size_t)slot * kslot, 0, kslot * 2, stream_));
-  CTB_CUDA(cudaMemsetAsync(vc_ + (size_t)slot * vslot, 0, vslot * 2, stream_));
+  zero_slot(slot);
   CTB_CUDA(cudaStreamSynchronize(stream_));
 }
 
@@ -1505,14 +1505,30 @@ void Engine::kv_slot_elems(size_t& k, size_t& v) const {
   v = (size_t)hp_.n_layer * kv_ctx_pad(hp_.n_ctx) * nkv_ * hd;
 }
 
+void Engine::zero_slot(int slot) {
+  size_t k, v;
+  kv_slot_elems(k, v);
+  CTB_CUDA(cudaMemsetAsync(kc_ + (size_t)slot * k, 0, k * 2, stream_));
+  CTB_CUDA(cudaMemsetAsync(vc_ + (size_t)slot * v, 0, v * 2, stream_));
+}
+
 float* Engine::results_of(int slot, float** embd) {
-  if (hp_.n_seq == 1) {
+  if (!hp_.multi) {
     *embd = d_embd_keep_;
     return d_logits_keep_;
   }
-  if (!pf_ || !pf_->d_mlogits) throw std::runtime_error("this engine has no multi-sequence path");
+  need_multi();
   *embd = pf_->d_membd + (size_t)slot * hp_.n_embd;
   return pf_->d_mlogits + (size_t)slot * hp_.n_vocab;
+}
+
+void Engine::copy_results(int src, int dst) {
+  float *sem, *dem;
+  const float* slg = results_of(src, &sem);
+  float* dlg = results_of(dst, &dem);
+  CTB_CUDA(cudaMemcpyAsync(dlg, slg, (size_t)hp_.n_vocab * 4, cudaMemcpyDeviceToDevice, stream_));
+  CTB_CUDA(cudaMemcpyAsync(dem, sem, (size_t)hp_.n_embd * 4, cudaMemcpyDeviceToDevice, stream_));
+  CTB_CUDA(cudaMemcpyAsync(pf_->d_mpick + 2 * dst, pf_->d_mpick + 2 * src, 8, cudaMemcpyDeviceToDevice, stream_));
 }
 
 uint8_t* Engine::stage(size_t bytes) {
@@ -1583,11 +1599,8 @@ void Engine::state_load(int slot, int n_past, bool results, const void* in, int 
   uint8_t* h = stage(std::max<size_t>(state_bytes(n_past, results), 1));
   memcpy(h, in, state_bytes(n_past, results));
   zero_v_tail((uint16_t*)(h + kb), rows * hd, n_past);
-  if (hp_.n_seq == 1) {   // a look-ahead step may still be in the stream: it runs before the copies below
-    spec_pending_ = false; spec_deferred_ = false; spec_pos_ = -1; spec_streak_ = 0;
-  }
-  CTB_CUDA(cudaMemsetAsync(kc_ + slot * kslot, 0, kslot * 2, stream_));
-  CTB_CUDA(cudaMemsetAsync(vc_ + slot * vslot, 0, vslot * 2, stream_));
+  if (!hp_.multi) drop_lookahead();   // a look-ahead step may still be in the stream: it runs before the copies below
+  zero_slot(slot);
   if (n_past > 0) {
     CTB_CUDA(cudaMemcpy2DAsync(kc_ + slot * kslot, (size_t)hp_.n_ctx * ks * 2, h, (size_t)n_past * ks * 2, (size_t)n_past * ks * 2, rows,
                                cudaMemcpyHostToDevice, stream_));
@@ -1597,12 +1610,12 @@ void Engine::state_load(int slot, int n_past, bool results, const void* in, int 
   if (results) {
     CTB_CUDA(cudaMemcpyAsync(lg, h + kb + vb, (size_t)hp_.n_vocab * 4, cudaMemcpyHostToDevice, stream_));
     CTB_CUDA(cudaMemcpyAsync(em, h + kb + vb + (size_t)hp_.n_vocab * 4, (size_t)hp_.n_embd * 4, cudaMemcpyHostToDevice, stream_));
-    if (hp_.n_seq > 1) {
+    if (hp_.multi) {
       k_argmax<<<1, ARGMAX_THREADS, 0, stream_>>>(lg, hp_.n_vocab, pf_->d_mpick + 2 * slot);
       CTB_CUDA(cudaGetLastError());
     }
   }
-  if (hp_.n_seq == 1) {
+  if (!hp_.multi) {
     kv_high_ = n_past;
     host_fresh_ = false;
     if (results && n_past > 0) {
@@ -1610,11 +1623,7 @@ void Engine::state_load(int slot, int n_past, bool results, const void* in, int 
       // too, and the greedy pick of the look-ahead (after_eval), whose step then resumes once the caller decodes greedily
       CTB_CUDA(cudaMemcpyAsync(d_logits_, lg, (size_t)hp_.n_vocab * 4, cudaMemcpyDeviceToDevice, stream_));
       CTB_CUDA(cudaMemcpyAsync(d_embd_, em, (size_t)hp_.n_embd * 4, cudaMemcpyDeviceToDevice, stream_));
-      if (h_state_cap_ < 1) { h_state_cap_ = 512; CTB_CUDA(cudaMallocHost(&h_state_, (size_t)h_state_cap_ * 16)); }
-      int* st = h_state_ + (size_t)(h_state_next_ % h_state_cap_) * 4;
-      h_state_next_++;
-      st[0] = last_token; st[1] = n_past - 1; st[2] = 0; st[3] = n_past;
-      CTB_CUDA(cudaMemcpyAsync(d_state_, st, 16, cudaMemcpyHostToDevice, stream_));
+      put_step(last_token, n_past - 1, n_past);
       after_eval(n_past);
     }
   }
@@ -1623,19 +1632,14 @@ void Engine::state_load(int slot, int n_past, bool results, const void* in, int 
 
 void Engine::state_fork(int src, const int* dsts, int n) {
   DeviceGuard dev_guard(device_);
+  need_multi();
   size_t kslot, vslot;
   kv_slot_elems(kslot, vslot);
-  float* sem;
-  const float* slg = results_of(src, &sem);
   for (int i = 0; i < n; i++) {
     const int d = dsts[i];
-    float* dem;
-    float* dlg = results_of(d, &dem);
     CTB_CUDA(cudaMemcpyAsync(kc_ + d * kslot, kc_ + src * kslot, kslot * 2, cudaMemcpyDeviceToDevice, stream_));
     CTB_CUDA(cudaMemcpyAsync(vc_ + d * vslot, vc_ + src * vslot, vslot * 2, cudaMemcpyDeviceToDevice, stream_));
-    CTB_CUDA(cudaMemcpyAsync(dlg, slg, (size_t)hp_.n_vocab * 4, cudaMemcpyDeviceToDevice, stream_));
-    CTB_CUDA(cudaMemcpyAsync(dem, sem, (size_t)hp_.n_embd * 4, cudaMemcpyDeviceToDevice, stream_));
-    CTB_CUDA(cudaMemcpyAsync(pf_->d_mpick + 2 * d, pf_->d_mpick + 2 * src, 8, cudaMemcpyDeviceToDevice, stream_));
+    copy_results(src, d);
   }
   CTB_CUDA(cudaStreamSynchronize(stream_));
 }
@@ -1664,7 +1668,7 @@ __global__ void k_kv_reparent(const KvCopy* copies, uint16_t* kc, uint16_t* vc, 
 
 size_t Engine::kv_reparent(const std::vector<KvCopy>& copies) {
   DeviceGuard dev_guard(device_);
-  if (hp_.n_seq < 2 || !pf_ || !pf_->d_mlogits) throw std::runtime_error("this engine has no multi-sequence path");
+  need_multi();
   if (copies.empty()) return 0;
   if ((int)copies.size() > hp_.n_seq) throw std::runtime_error("kv_reparent: more copies than slots");
   std::vector<char> src(hp_.n_seq, 0), dst(hp_.n_seq, 0);
@@ -1689,21 +1693,14 @@ size_t Engine::kv_reparent(const std::vector<KvCopy>& copies) {
   CTB_CUDA(cudaMemcpyAsync(d_copies_, h_copies_, sizeof(KvCopy) * copies.size(), cudaMemcpyHostToDevice, stream_));
   k_kv_reparent<<<dim3((unsigned)lh, (unsigned)copies.size()), 256, 0, stream_>>>(d_copies_, kc_, vc_, kslot, vslot, hp_.n_ctx, ks, hd);
   CTB_CUDA(cudaGetLastError());
-  for (const KvCopy& c : copies) {
-    float *sem, *dem;
-    const float* slg = results_of(c.src, &sem);
-    float* dlg = results_of(c.dst, &dem);
-    CTB_CUDA(cudaMemcpyAsync(dlg, slg, (size_t)hp_.n_vocab * 4, cudaMemcpyDeviceToDevice, stream_));
-    CTB_CUDA(cudaMemcpyAsync(dem, sem, (size_t)hp_.n_embd * 4, cudaMemcpyDeviceToDevice, stream_));
-    CTB_CUDA(cudaMemcpyAsync(pf_->d_mpick + 2 * c.dst, pf_->d_mpick + 2 * c.src, 8, cudaMemcpyDeviceToDevice, stream_));
-  }
+  for (const KvCopy& c : copies) copy_results(c.src, c.dst);
   CTB_CUDA(cudaStreamSynchronize(stream_));
   return bytes;
 }
 
 const float* Engine::multi_rows(int slot0, int n) {
   DeviceGuard dev_guard(device_);
-  if (!pf_ || !pf_->d_mlogits) throw std::runtime_error("this engine has no multi-sequence path");
+  need_multi();
   if (slot0 < 0 || n < 0 || slot0 + n > hp_.n_seq) throw std::runtime_error("multi_rows: slots out of range");
   const size_t b = (size_t)n * hp_.n_vocab * 4;
   float* h = (float*)stage(std::max<size_t>(b, 1));
@@ -1714,14 +1711,12 @@ const float* Engine::multi_rows(int slot0, int n) {
 
 double Engine::decode_greedy(int first_token, int n_past, int n_steps, int* out_tokens) {
   if (n_steps <= 0) return 0.0;
-  spec_pending_ = false; spec_deferred_ = false; spec_pos_ = -1; spec_streak_ = 0;
+  drop_lookahead();
   if (n_steps > tokens_out_cap_) throw std::runtime_error("decode_greedy: too many steps");
   if (n_past + n_steps > hp_.n_ctx) throw std::runtime_error("decode_greedy: would run past the context length");
   kv_high_ = std::max(kv_high_, n_past + n_steps);
   DeviceGuard dev_guard(device_);
-  if (h_state_cap_ < 1) { h_state_cap_ = 512; CTB_CUDA(cudaMallocHost(&h_state_, (size_t)h_state_cap_ * 16)); }
-  h_state_[0] = first_token; h_state_[1] = n_past; h_state_[2] = 0; h_state_[3] = n_past + 1;
-  CTB_CUDA(cudaMemcpyAsync(d_state_, h_state_, 16, cudaMemcpyHostToDevice, stream_));
+  put_step(first_token, n_past, n_past + 1);
   CTB_CUDA(cudaEventRecord(ev0_, stream_));
   for (int s = 0; s < n_steps; s++) CTB_CUDA(cudaGraphLaunch(graph_greedy_, stream_));
   CTB_CUDA(cudaEventRecord(ev1_, stream_));

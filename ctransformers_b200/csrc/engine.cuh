@@ -35,7 +35,8 @@ struct HParams {
   int n_vocab = 0, n_ctx_train = 0, n_embd = 0, n_ff = 0, n_head = 0, n_head_kv = 0, n_layer = 0, n_rot = 0;
   float eps = 1e-5f, rope_base = 10000.f, rope_scale = 1.f;
   int n_ctx = 512;
-  int n_seq = 1;   // sequence slots of the KV cache (multi-sequence mode); slot 0 has the single-sequence layout
+  int n_seq = 1;   // sequence slots (KV regions) of the cache; slot 0 has the single-sequence layout
+  bool multi = false;   // a multi-sequence handle's engine (ctb_multi_create), whatever its n_seq: evals go through multi_eval
   int head_dim() const { return n_embd / n_head; }
   int n_embd_gqa() const { return head_dim() * n_head_kv; }
 };
@@ -99,7 +100,7 @@ class Engine {
   double time_matvec_only(int reps, long* launches, unsigned mask = 0);
   int profile_step(int token, int n_past, double ms_by_kind[4], int count_by_kind[4]);
   long trace_step(int token, int n_past, unsigned long long* out, long cap_words);
-  // Multi-sequence mode (hp.n_seq > 1): every slot has its own KV region.  multi_refusal: why the model cannot run it, "" when
+  // Multi-sequence mode (hp.multi): every slot has its own KV region.  multi_refusal: why the model cannot run it, "" when
   // it can.  multi_eval: tokens [starts[i], starts[i+1]) of toks share batched launch i (a slot's tokens within one launch at
   // consecutive positions); afterwards each slot whose eval ended holds its logits, embeddings and greedy pick on the device.
   std::string multi_refusal();
@@ -185,6 +186,7 @@ class Engine {
   int* h_state_ = nullptr;     // pinned ring of {token, n_past}
   int h_state_cap_ = 0;
   long h_state_next_ = 0;
+  void put_step(int token, int pos, int n_total);   // the next ring entry {token, pos, 0, n_total} to d_state_, on the stream
   int* h_tokens_out_ = nullptr;
   int* d_tokens_out_ = nullptr;
   int tokens_out_cap_ = 0;
@@ -198,6 +200,7 @@ class Engine {
   cudaEvent_t ev_sample_ = nullptr;
   void launch_deferred_spec();
   int spec_pos_ = -1, spec_streak_ = 0;
+  void drop_lookahead();         // forget the look-ahead and the streak that earned it (a step already enqueued still runs)
   int kv_high_ = 0;              // one past the highest position any eval has written
   int* h_spec_tok_ = nullptr;
   int* h_dbg_ = nullptr;         // host-mapped watchdog words of the persistent kernels
@@ -237,6 +240,8 @@ class Engine {
   void sample_enqueue(const SampleRow* rows, int R, const float* logits, size_t stride, bool picks);
   // batched prefill (prefill.cuh): built on first use
   struct PrefillState* pf_ = nullptr;
+  bool multi_ready();            // hp_.multi and the multi-sequence program is built
+  void need_multi();             // throws unless multi_ready()
   bool prefill_on_ = true;       // CTB_NO_PREFILL=1: prompts run through the single-token kernel
   int prefill_min_ = 4;          // shortest run of consecutive tokens worth a batched launch
   long prefill_launches_ = 0;    // k_pstep launches so far
@@ -274,7 +279,9 @@ class Engine {
   uint8_t* stage(size_t bytes);
   KvCopy *d_copies_ = nullptr, *h_copies_ = nullptr;   // kv_reparent's copy list (n_seq entries), device and pinned
   void kv_slot_elems(size_t& k, size_t& v) const;   // halves of one slot's K and V regions
+  void zero_slot(int slot);                         // zero the slot's K and V regions, on the stream
   float* results_of(int slot, float** embd);        // where the slot's last logits / embeddings live on the device
+  void copy_results(int src, int dst);              // multi-sequence: dst takes src's last logits, embeddings and greedy pick
 };
 
 size_t engine_arena_bytes(const GGUFFile& g, const HParams& hp);

@@ -243,27 +243,68 @@ static int state_error(const char* what, const std::exception& e) {
   return -1;
 }
 
+// What every handle loads: the model file, its architecture, hyper-parameters and vocabulary.  The model type is checked before
+// anything needs a device (a GGUF file: model_type "gguf" or the file's magic).  Returns the CUDA device count.
+static int load_model(LLM& L, const char* model_path, const char* model_type, int context_length) {
+  std::string type = model_type ? model_type : "";
+  type.erase(std::remove_if(type.begin(), type.end(), [](const char c) { return !std::isalnum((unsigned char)c); }), type.end());
+  if (!(type == "gguf" || file_is_gguf(model_path)))
+    throw std::runtime_error("model type '" + std::string(model_type ? model_type : "") + "' is not supported by this build (GGUF llama / falcon only)");
+  int ndev = 0;
+  if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev == 0) throw std::runtime_error("no CUDA device available; this library has no CPU fallback");
+  L.file.reset(new GGUFFile(model_path));
+  L.arch = L.file->need_str("general.architecture");
+  if (L.arch != "llama" && L.arch != "falcon") throw std::runtime_error("unknown model architecture: '" + L.arch + "'");
+  L.hp = read_hparams(*L.file, L.arch, context_length);
+  L.vocab.load(*L.file);
+  return ndev;
+}
+
+// Refuses a tensor-sharded LLM what that mode does not have: "the tensor-sharded mode " + why.
+static void not_sharded(LLM* llm, const char* why) {
+  if (llm->comm) throw std::invalid_argument(std::string("the tensor-sharded mode ") + why);
+}
+
+static void check_tokens(const int* tokens, int n, int n_vocab) {
+  if (n > 0 && !tokens) throw std::invalid_argument("no tokens");
+  for (int i = 0; i < n; i++)
+    if (tokens[i] < 0 || tokens[i] >= n_vocab) throw std::invalid_argument("token id out of range");
+}
+
+// targets: -1 (no target) or a token id
+static void check_targets(const int* targets, int n, int n_vocab) {
+  if (n > 0 && !targets) throw std::invalid_argument("no targets");
+  for (int i = 0; i < n; i++)
+    if (targets[i] < -1 || targets[i] >= n_vocab)
+      throw std::invalid_argument("target " + std::to_string(targets[i]) + " of token " + std::to_string(i) + " is out of range (-1 .. " + std::to_string(n_vocab - 1) + ")");
+}
+
+// The eval of an LLM, 0 or -1.  The engine gets the whole list at once so that prompt chunks can share batched launches.  With
+// a sink it also keeps every token's row.  Everything is checked before the first launch, so a refusal leaves the handle as it was.
+static int llm_eval(LLM* llm, const int* tokens, int n_tokens, int n_past, int batch_size, const RowSink* sink, const char* what) {
+  try {
+    if (sink) not_sharded(llm, "keeps no per-token rows");
+    check_tokens(tokens, n_tokens, llm->hp.n_vocab);
+    if (sink && sink->targets) check_targets(sink->targets, n_tokens, llm->hp.n_vocab);
+    else if (sink && n_tokens > 0 && !sink->host) throw std::invalid_argument("no memory for the rows");
+    if (n_tokens <= 0) return 0;
+    std::vector<int> pos(n_tokens), nt(n_tokens);
+    eval_positions(n_tokens, n_past, batch_size, llm->hp.n_ctx, pos.data(), nt.data());
+    llm->engine->eval_list(tokens, pos.data(), nt.data(), n_tokens, sink);
+    llm->has_logits = true;
+    return 0;
+  } catch (const std::exception& e) {
+    fprintf(stderr, "ctransformers-b200: %s failed: %s\n", what, e.what());
+    return -1;
+  } catch (...) { return -1; }
+}
+
 extern "C" {
 
 static LLM* create_llm(const char* model_path, const char* model_type, const ctransformers_config config, int rank, int world, const void* unique_id) {
   try {
-    std::string type = model_type ? model_type : "";
-    type.erase(std::remove_if(type.begin(), type.end(), [](const char c) { return !std::isalnum((unsigned char)c); }), type.end());
-    if (!(type == "gguf" || file_is_gguf(model_path))) {
-      fprintf(stderr, "Model type '%s' is not supported by this build (GGUF llama / falcon only).\n", model_type ? model_type : "");
-      return nullptr;
-    }
-    int ndev = 0;
-    if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev == 0) {
-      fprintf(stderr, "ctransformers-b200: no CUDA device available; this library has no CPU fallback.\n");
-      return nullptr;
-    }
     std::unique_ptr<LLM> llm(new LLM);
-    llm->file.reset(new GGUFFile(model_path));
-    llm->arch = llm->file->need_str("general.architecture");
-    if (llm->arch != "llama" && llm->arch != "falcon") throw std::runtime_error("unknown model architecture: '" + llm->arch + "'");
-    llm->hp = read_hparams(*llm->file, llm->arch, config.context_length);
-    llm->vocab.load(*llm->file);
+    const int ndev = load_model(*llm, model_path, model_type, config.context_length);
     int device = 0;
     if (const char* env = getenv("CT_DEVICE")) device = atoi(env);
     else if (const char* lr = getenv("LOCAL_RANK")) device = atoi(lr) % ndev;
@@ -353,19 +394,7 @@ const char* ctransformers_llm_architecture(LLM* llm) { return llm->arch.c_str();
 
 bool ctransformers_llm_batch_eval(LLM* llm, const int* tokens, const int n_tokens, const int n_past, const int batch_size, const int threads) {
   (void)threads;   // host thread count has no meaning on the GPU path
-  try {
-    // the engine gets the whole list at once so that prompt chunks can share batched launches
-    for (int i = 0; i < n_tokens; i++)
-      if (tokens[i] < 0 || tokens[i] >= llm->hp.n_vocab) throw std::runtime_error("token id out of range");
-    std::vector<int> pos(std::max(n_tokens, 0)), nt(std::max(n_tokens, 0));
-    eval_positions(n_tokens, n_past, batch_size, llm->hp.n_ctx, pos.data(), nt.data());
-    llm->engine->eval_list(tokens, pos.data(), nt.data(), n_tokens);
-    if (n_tokens > 0) llm->has_logits = true;
-    return true;
-  } catch (const std::exception& e) {
-    fprintf(stderr, "ctransformers-b200: eval failed: %s\n", e.what());
-    return false;
-  } catch (...) { return false; }
+  return llm_eval(llm, tokens, n_tokens, n_past, batch_size, nullptr, "eval") == 0;
 }
 
 float* ctransformers_llm_logits_data(LLM* llm) { return llm->engine->logits(); }
@@ -466,20 +495,16 @@ int ctb_state_info(const void* buf, size_t size, ctb_state_header* out) {
   return 0;
 }
 
-static void llm_states_ok(LLM* llm) {
-  if (llm->comm) throw std::runtime_error("the tensor-sharded mode has no sequence states");
-}
-
 size_t ctb_llm_state_size(LLM* llm, int n_tokens) {
   try {
-    llm_states_ok(llm);
+    not_sharded(llm, "has no sequence states");
     return state_size_for(*llm, n_tokens);
   } catch (...) { return 0; }
 }
 
 int ctb_llm_save_state(LLM* llm, const int* tokens, int n_tokens, void* buf, size_t cap) {
   try {
-    llm_states_ok(llm);
+    not_sharded(llm, "has no sequence states");
     save_state(*llm, 0, tokens, n_tokens, llm->has_logits, buf, cap);
     return 0;
   } catch (const std::exception& e) { return state_error("cannot save the state", e); }
@@ -487,54 +512,17 @@ int ctb_llm_save_state(LLM* llm, const int* tokens, int n_tokens, void* buf, siz
 
 int ctb_llm_load_state(LLM* llm, const void* buf, size_t size) {
   try {
-    llm_states_ok(llm);
+    not_sharded(llm, "has no sequence states");
     llm->has_logits = restore_state(*llm, 0, buf, size).has_results != 0;
     return 0;
   } catch (const std::exception& e) { return state_error("cannot load the state", e); }
 }
 
 // ---- rows of every token (the reference's logits_all) and their scores
-static void check_tokens(const int* tokens, int n, int n_vocab) {
-  if (n > 0 && !tokens) throw std::invalid_argument("no tokens");
-  for (int i = 0; i < n; i++)
-    if (tokens[i] < 0 || tokens[i] >= n_vocab) throw std::invalid_argument("token id out of range");
-}
-
-// targets: -1 (no target) or a token id
-static void check_targets(const int* targets, int n, int n_vocab) {
-  if (n > 0 && !targets) throw std::invalid_argument("no targets");
-  for (int i = 0; i < n; i++)
-    if (targets[i] < -1 || targets[i] >= n_vocab)
-      throw std::invalid_argument("target " + std::to_string(targets[i]) + " of token " + std::to_string(i) + " is out of range (-1 .. " + std::to_string(n_vocab - 1) + ")");
-}
-
-static void llm_rows_ok(LLM* llm) {
-  if (llm->comm) throw std::invalid_argument("the tensor-sharded mode keeps no per-token rows");
-}
-
-// ctransformers_llm_batch_eval with a RowSink: everything is checked before the first launch, so a refusal leaves the handle as it was
-static int llm_eval_rows(LLM* llm, const int* tokens, int n_tokens, int n_past, int batch_size, const RowSink& sink, const char* what) {
-  try {
-    llm_rows_ok(llm);
-    check_tokens(tokens, n_tokens, llm->hp.n_vocab);
-    if (sink.targets) check_targets(sink.targets, n_tokens, llm->hp.n_vocab);
-    else if (n_tokens > 0 && !sink.host) throw std::invalid_argument("no memory for the rows");
-    if (n_tokens <= 0) return 0;
-    std::vector<int> pos(n_tokens), nt(n_tokens);
-    eval_positions(n_tokens, n_past, batch_size, llm->hp.n_ctx, pos.data(), nt.data());
-    llm->engine->eval_list(tokens, pos.data(), nt.data(), n_tokens, &sink);
-    llm->has_logits = true;
-    return 0;
-  } catch (const std::exception& e) {
-    fprintf(stderr, "ctransformers-b200: %s failed: %s\n", what, e.what());
-    return -1;
-  } catch (...) { return -1; }
-}
-
 int ctb_llm_batch_eval_rows(LLM* llm, const int* tokens, int n_tokens, int n_past, int batch_size, float* rows) {
   RowSink s;
   s.host = rows;
-  return llm_eval_rows(llm, tokens, n_tokens, n_past, batch_size, s, "eval with rows");
+  return llm_eval(llm, tokens, n_tokens, n_past, batch_size, &s, "eval with rows");
 }
 
 int ctb_llm_batch_eval_scored(LLM* llm, const int* tokens, int n_tokens, int n_past, int batch_size, const int* targets, double* logprob, int* greedy) {
@@ -544,12 +532,12 @@ int ctb_llm_batch_eval_scored(LLM* llm, const int* tokens, int n_tokens, int n_p
     fprintf(stderr, "ctransformers-b200: scored eval failed: no memory for the scores\n");
     return -1;
   }
-  return llm_eval_rows(llm, tokens, n_tokens, n_past, batch_size, s, "scored eval");
+  return llm_eval(llm, tokens, n_tokens, n_past, batch_size, &s, "scored eval");
 }
 
 int ctb_llm_score_last(LLM* llm, int target, double* logprob, int* greedy) {
   try {
-    llm_rows_ok(llm);
+    not_sharded(llm, "keeps no per-token rows");
     if (!llm->has_logits) throw std::invalid_argument("nothing has been evaluated");
     check_targets(&target, 1, llm->hp.n_vocab);
     llm->engine->score_kept(target, logprob, greedy);
@@ -618,25 +606,14 @@ static bool multi_fetch(ctb_multi* m, int slot) {
 ctb_multi* ctb_multi_create(const char* model_path, const char* model_type, const ctransformers_config config, int n_slots) {
   try {
     if (n_slots < 1) throw std::runtime_error("n_slots must be at least 1");
-    std::string type = model_type ? model_type : "";
-    type.erase(std::remove_if(type.begin(), type.end(), [](const char c) { return !std::isalnum((unsigned char)c); }), type.end());
-    if (!(type == "gguf" || file_is_gguf(model_path))) throw std::runtime_error("model type '" + type + "' is not supported by this build (GGUF llama / falcon only)");
-    int ndev = 0;
-    if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev == 0) {
-      fprintf(stderr, "ctransformers-b200: no CUDA device available; this library has no CPU fallback.\n");
-      return nullptr;
-    }
-    if (g_tp_ranks > 0)
-      throw std::runtime_error("multi-sequence decoding in the tensor-sharded mode is not supported by the CUDA path");
     std::unique_ptr<ctb_multi> m(new ctb_multi);
     m->llm.reset(new LLM);
     LLM& L = *m->llm;
-    L.file.reset(new GGUFFile(model_path));
-    L.arch = L.file->need_str("general.architecture");
-    if (L.arch != "llama" && L.arch != "falcon") throw std::runtime_error("unknown model architecture: '" + L.arch + "'");
-    L.hp = read_hparams(*L.file, L.arch, config.context_length);
+    load_model(L, model_path, model_type, config.context_length);
+    if (g_tp_ranks > 0)
+      throw std::runtime_error("multi-sequence decoding in the tensor-sharded mode is not supported by the CUDA path");
     L.hp.n_seq = n_slots;
-    L.vocab.load(*L.file);
+    L.hp.multi = true;
     for (const auto& t : L.file->tensors)
       if (t.n_dims >= 2 && t.name.rfind("blk.", 0) == 0 && !type_is_kquant((int)t.type))
         throw std::runtime_error("multi-sequence decoding of layer matrices that are not K-quants (tensor '" + t.name + "', type " + std::to_string(t.type) +
@@ -675,47 +652,31 @@ int ctb_multi_info(ctb_multi* m, int* out6) {
   return 6;
 }
 
-bool ctb_multi_eval(ctb_multi* m, int n, const int* slots, const int* off, const int* tokens, const int* n_past, int batch_size) {
-  try {
-    std::vector<char> seen(m->n_slots, 0);
-    for (int i = 0; i < n; i++) {
-      if (!multi_slot_ok(m, slots[i])) return false;
-      if (seen[slots[i]]++) throw std::runtime_error("slot " + std::to_string(slots[i]) + " is listed twice");
-    }
-    for (int i = 0; n > 0 && i < off[n] - off[0]; i++)
-      if (tokens[off[0] + i] < 0 || tokens[off[0] + i] >= m->llm->hp.n_vocab) throw std::runtime_error("token id out of range");
-    std::vector<MultiTok> toks;
-    const std::vector<int> starts = multi_pack(n, slots, off, tokens, n_past, batch_size, m->llm->hp.n_ctx, toks);
-    if (toks.empty()) return true;
-    for (int i = 0; i < n; i++) m->fresh[slots[i]] = 0;
-    m->llm->engine->multi_eval(toks, starts);
-    for (int i = 0; i < n; i++)
-      if (off[i + 1] > off[i]) m->has[slots[i]] = 1;
-    return true;
-  } catch (const std::exception& e) {
-    fprintf(stderr, "ctransformers-b200: multi-sequence eval failed: %s\n", e.what());
-    return false;
-  } catch (...) { return false; }
+// slots[0 .. n) are in range (false, with a message, when one is not) and listed once (else it throws)
+static bool multi_slots_ok(ctb_multi* m, int n, const int* slots) {
+  std::vector<char> seen(m->n_slots, 0);
+  for (int i = 0; i < n; i++) {
+    if (!multi_slot_ok(m, slots[i])) return false;
+    if (seen[slots[i]]++) throw std::invalid_argument("slot " + std::to_string(slots[i]) + " is listed twice");
+  }
+  return true;
 }
 
-// ctb_multi_eval with a RowSink over the packed token list (call order); checked before the first launch
-static int multi_eval_rows(ctb_multi* m, int n, const int* slots, const int* off, const int* tokens, const int* n_past, int batch_size, const RowSink& sink,
-                           const char* what) {
+// The eval of a multi-sequence handle, 0 or -1; with a sink it also keeps the row of every token of the packed list (call order).
+// Everything is checked before the first launch.
+static int multi_eval(ctb_multi* m, int n, const int* slots, const int* off, const int* tokens, const int* n_past, int batch_size, const RowSink* sink,
+                      const char* what) {
   try {
-    std::vector<char> seen(m->n_slots, 0);
-    for (int i = 0; i < n; i++) {
-      if (!multi_slot_ok(m, slots[i])) return -1;
-      if (seen[slots[i]]++) throw std::invalid_argument("slot " + std::to_string(slots[i]) + " is listed twice");
-    }
+    if (!multi_slots_ok(m, n, slots)) return -1;
     const int total = n > 0 ? off[n] - off[0] : 0;
     check_tokens(tokens ? tokens + (n > 0 ? off[0] : 0) : nullptr, total, m->llm->hp.n_vocab);
-    if (sink.targets) check_targets(sink.targets, total, m->llm->hp.n_vocab);
-    else if (total > 0 && !sink.host) throw std::invalid_argument("no memory for the rows");
+    if (sink && sink->targets) check_targets(sink->targets, total, m->llm->hp.n_vocab);
+    else if (sink && total > 0 && !sink->host) throw std::invalid_argument("no memory for the rows");
     std::vector<MultiTok> toks;
     const std::vector<int> starts = multi_pack(n, slots, off, tokens, n_past, batch_size, m->llm->hp.n_ctx, toks);
     if (toks.empty()) return 0;
     for (int i = 0; i < n; i++) m->fresh[slots[i]] = 0;
-    m->llm->engine->multi_eval(toks, starts, &sink);
+    m->llm->engine->multi_eval(toks, starts, sink);
     for (int i = 0; i < n; i++)
       if (off[i + 1] > off[i]) m->has[slots[i]] = 1;
     return 0;
@@ -725,10 +686,14 @@ static int multi_eval_rows(ctb_multi* m, int n, const int* slots, const int* off
   } catch (...) { return -1; }
 }
 
+bool ctb_multi_eval(ctb_multi* m, int n, const int* slots, const int* off, const int* tokens, const int* n_past, int batch_size) {
+  return multi_eval(m, n, slots, off, tokens, n_past, batch_size, nullptr, "multi-sequence eval") == 0;
+}
+
 int ctb_multi_eval_rows(ctb_multi* m, int n, const int* slots, const int* off, const int* tokens, const int* n_past, int batch_size, float* rows) {
   RowSink s;
   s.host = rows;
-  return multi_eval_rows(m, n, slots, off, tokens, n_past, batch_size, s, "multi-sequence eval with rows");
+  return multi_eval(m, n, slots, off, tokens, n_past, batch_size, &s, "multi-sequence eval with rows");
 }
 
 int ctb_multi_eval_scored(ctb_multi* m, int n, const int* slots, const int* off, const int* tokens, const int* n_past, int batch_size, const int* targets,
@@ -739,7 +704,7 @@ int ctb_multi_eval_scored(ctb_multi* m, int n, const int* slots, const int* off,
     fprintf(stderr, "ctransformers-b200: multi-sequence scored eval failed: no memory for the scores\n");
     return -1;
   }
-  return multi_eval_rows(m, n, slots, off, tokens, n_past, batch_size, s, "multi-sequence scored eval");
+  return multi_eval(m, n, slots, off, tokens, n_past, batch_size, &s, "multi-sequence scored eval");
 }
 
 const float* ctb_multi_logits(ctb_multi* m, int slot) {
@@ -761,10 +726,8 @@ int ctb_multi_sample_many(ctb_multi* m, int n, const int* slots, const int* last
     if (n < 0) throw std::invalid_argument("a negative slot count");
     if (n > 0 && (!slots || !last_off || !top_k || !top_p || !temperature || !repetition_penalty || !seed || !out))
       throw std::invalid_argument("a missing argument array");
-    std::vector<char> seen(m->n_slots, 0);
+    if (!multi_slots_ok(m, n, slots)) return -1;
     for (int i = 0; i < n; i++) {
-      if (!multi_slot_ok(m, slots[i])) return -1;
-      if (seen[slots[i]]++) throw std::invalid_argument("slot " + std::to_string(slots[i]) + " is listed twice");
       if (!m->has[slots[i]]) throw std::invalid_argument("slot " + std::to_string(slots[i]) + " has no logits to sample from");
       if (last_off[i] < 0 || last_off[i + 1] < last_off[i]) throw std::invalid_argument("the window offsets of slot " + std::to_string(slots[i]) + " are not ascending");
     }

@@ -22,6 +22,15 @@ def per_slot(value, n: int, what: str) -> list:
     return values
 
 
+def _flatten(lists: Sequence[Sequence[int]]) -> Tuple[List[int], List[int]]:
+    """The lists concatenated, and the offsets where each starts (one more at the end): the library's (off, flat) form."""
+    off, flat = [0], []
+    for items in lists:
+        flat.extend(items)
+        off.append(len(flat))
+    return off, flat
+
+
 class MultiLLM:
     all_logits = None   # eval(..., logits_all=True): {slot: the rows of that slot's tokens}
 
@@ -60,41 +69,27 @@ class MultiLLM:
         LLM.eval chunks; all of them share batched launches.  logits_all=True also keeps the logits of every evaluated token:
         `all_logits` is then {slot: (n, vocab_size) float32 array}, each row what LLM.eval(..., logits_all=True) gives."""
         self.all_logits = None
-        if logits_all:
-            import numpy as np
-            slots = [self._slot(s) for s in tokens_by_slot]
-            total = sum(len(tokens_by_slot[s]) for s in slots)
-            rows = np.empty((total, self.vocab_size), np.float32)
-            self._eval_call(tokens_by_slot, batch_size, self._lib.ctb_multi_eval_rows, rows.ctypes.data_as(POINTER(c_float)))
-            self.all_logits, at = {}, 0
-            for s in slots:
-                self.all_logits[s], at = rows[at:at + len(tokens_by_slot[s])], at + len(tokens_by_slot[s])
+        if not logits_all:
+            self._eval_call(tokens_by_slot, batch_size, self._lib.ctb_multi_eval, ok=True)
             return
-        bs = _pick(batch_size, self._config.batch_size)
+        import numpy as np
         slots = [self._slot(s) for s in tokens_by_slot]
-        off, flat = [0], []
+        tokens_by_slot = {s: _check_ids(tokens_by_slot[s], self.vocab_size, f"slot {s}: token") for s in slots}
+        rows = np.empty((sum(map(len, tokens_by_slot.values())), self.vocab_size), np.float32)
+        self._eval_call(tokens_by_slot, batch_size, self._lib.ctb_multi_eval_rows, rows.ctypes.data_as(POINTER(c_float)))
+        self.all_logits, at = {}, 0
         for s in slots:
-            flat.extend(tokens_by_slot[s])
-            off.append(len(flat))
-        n = len(slots)
-        arr = (c_int * max(len(flat), 1))(*flat)
-        past = [len(self._context[s]) for s in slots]
-        if not self._lib.ctb_multi_eval(self._m, n, (c_int * max(n, 1))(*slots), (c_int * (n + 1))(*off), arr, (c_int * max(n, 1))(*past), bs):
-            raise RuntimeError("Failed to evaluate tokens.")
-        for s in slots:
-            self._context[s].extend(tokens_by_slot[s])
+            self.all_logits[s], at = rows[at:at + len(tokens_by_slot[s])], at + len(tokens_by_slot[s])
 
-    def _eval_call(self, tokens_by_slot, batch_size, fn, *out) -> None:
-        """One ctb_multi_eval_rows / ctb_multi_eval_scored call: the slots' lists concatenated in dict order."""
+    def _eval_call(self, tokens_by_slot, batch_size, fn, *out, ok=0) -> None:
+        """One ctb_multi_eval / ctb_multi_eval_rows / ctb_multi_eval_scored call, which returns `ok` on success: the slots'
+        lists concatenated in dict order, each after its slot's context."""
         bs = _pick(batch_size, self._config.batch_size)
         slots = [self._slot(s) for s in tokens_by_slot]
-        off, flat = [0], []
-        for s in slots:
-            flat.extend(_check_ids(tokens_by_slot[s], self.vocab_size, f"slot {s}: token"))
-            off.append(len(flat))
+        off, flat = _flatten([tokens_by_slot[s] for s in slots])
         n = len(slots)
         past = [len(self._context[s]) for s in slots]
-        if fn(self._m, n, _ints(slots), (c_int * (n + 1))(*off), _ints(flat), _ints(past), bs, *out) != 0:
+        if fn(self._m, n, _ints(slots), _ints(off), _ints(flat), _ints(past), bs, *out) != ok:
             raise RuntimeError("Failed to evaluate tokens.")
         for s in slots:
             self._context[s].extend(tokens_by_slot[s])
@@ -165,10 +160,9 @@ class MultiLLM:
         for name, value in (("top_k", top_k), ("top_p", top_p), ("temperature", temperature), ("repetition_penalty", repetition_penalty),
                             ("last_n_tokens", last_n_tokens), ("seed", seed)):
             args[name] = [_pick(v, getattr(cfg, name)) for v in per_slot(value, n, name)]
-        off, flat = [0], []
-        for s, last_n in zip(slots, args["last_n_tokens"]):
-            flat.extend(self._context[s][-(last_n if last_n >= 0 else self.context_length):])   # (last_n 0: the whole context, as LLM.sample)
-            off.append(len(flat))
+        windows = [self._context[s][-(last_n if last_n >= 0 else self.context_length):]   # (last_n 0: the whole context, as LLM.sample)
+                   for s, last_n in zip(slots, args["last_n_tokens"])]
+        off, flat = _flatten(windows)
         out = (c_int * max(n, 1))()
         floats = lambda v: (c_float * max(n, 1))(*v)
         if self._lib.ctb_multi_sample_many(self._m, n, _ints(slots), _ints(off), _ints(flat), _ints(args["top_k"]), floats(args["top_p"]),
@@ -289,10 +283,7 @@ class MultiLLM:
                 raise ValueError(f"prompt {i} is empty")
             if len(p) + max_new_tokens > self.context_length:
                 raise ValueError(f"prompt {i}: {len(p)} tokens and {max_new_tokens} more exceed the context length {self.context_length}")
-        off, flat = [0], []
-        for p in prompts:
-            flat.extend(p)
-            off.append(len(flat))
+        off, flat = _flatten(prompts)
         n = len(prompts)
         out_off = (c_int * (n + 1))()
         out_tok = (c_int * max(n * max_new_tokens, 1))()

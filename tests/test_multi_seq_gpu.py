@@ -232,6 +232,39 @@ def test_sample_equals_single_sequence_draw(model_dir):
             llm.eval([draws[s]])
 
 
+
+def test_one_slot_handle_equals_llm(model_dir):
+    """A one-slot handle runs the multi-sequence path like any other: it evaluates, samples, saves and restores, and scores
+    bit for bit as an LLM fed the same calls."""
+    from ctransformers_b200.llm import _ints
+    name = "llama_tiny_q4km"
+    path, ctx = build(name, model_dir)
+    m, llm = multi(path, ctx, 1), load(path, ctx)
+    prompt = modelcases.seeded_prompt(name, 37, seed=37)
+    m.eval({0: prompt}, batch_size=8)
+    llm.eval(prompt, batch_size=8)
+    for step in range(5):
+        if step == 3:                                       # the slot starts over from its saved state
+            saved = m.save(0)
+            m.reset(0)
+            m.restore(0, saved)
+        lg, em = multi_state(m, 0)
+        want_lg, want_em = llm_state(llm)
+        same(lg, want_lg, f"logits at step {step}")
+        same(em, want_em, f"embeddings at step {step}")
+        kw = dict(top_k=40, top_p=0.9, temperature=0.8, seed=100 + step)
+        t = m.sample(0, **kw)
+        assert t == llm.sample(**kw), f"step {step}"
+        m.eval({0: [t]})
+        llm.eval([t])
+    toks = modelcases.seeded_prompt(name, 11, seed=50)     # token i scored under the logits after token i - 1, as LLM.score scores
+    lp, gr = np.zeros(len(toks)), np.zeros(len(toks), np.int32)
+    assert m._lib.ctb_multi_eval_scored(m._m, 1, _ints([0]), _ints([0, len(toks)]), _ints(toks), _ints([len(m.context(0))]), 8,
+                                        _ints(toks[1:] + [-1]), lp.ctypes.data_as(C.POINTER(C.c_double)), gr.ctypes.data_as(C.POINTER(C.c_int))) == 0
+    want_lp, want_gr = llm.score(toks, batch_size=8)
+    assert lp[:-1].tobytes() == want_lp[1:].tobytes()
+    assert (gr[:-1] != 0).tolist() == want_gr[1:].tolist()
+
 def test_generate_many_equals_generate(model_dir):
     """Four prompts through two slots: each result is what LLM.generate gives that prompt, greedy."""
     name = "llama_tiny_q4km"
