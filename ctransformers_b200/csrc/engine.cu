@@ -63,26 +63,28 @@ struct StepOp {
 // advance the on-device decode state after k_argmax's greedy pick (state[4])
 __global__ void k_advance(int* state, int* out_tokens) { advance_state(state, out_tokens, state[4]); }
 
+// one program of the batched kernel (k_pstep): its phases on the host, their device copy, and whether it holds Q3_K matrices
+// (the k_pstep<true> build)
+struct PProg {
+  std::vector<PPhase> phases;
+  DevMem d;
+  bool q3 = false;
+};
+
 // ---- batched prefill (prefill.cuh): the per-token schedule rewritten over PB_T-row buffers
 struct PrefillState {
-  std::vector<void*> bufs;          // cudaMalloc'ed
-  PPhase* d_prog = nullptr;
-  int n_phases = 0;
+  std::vector<DevMem> bufs;         // the batched buffers and the QUANT phases' scratch (dalloc)
+  PProg prog;
   int* d_state = nullptr;           // [PB_T][4] + n_tok
-  int* h_state = nullptr;           // pinned, PF_RING launches deep
-  int h_next = 0;
+  StateRing ring;                   // d_state of each launch, PF_RING launches deep
   float* x_final = nullptr;         // batched buffer that holds the last layer's output rows
   int n_slots = 0;
   size_t smem = 0;
-  bool q3 = false;                  // the program holds Q3_K matrices (k_pstep<true>)
   bool ok = false, tried = false;
   // multi-sequence mode (HParams::multi): the same program on slot-addressed state (k_pstep<.., true>), plus the output head
-  PPhase* d_mprog = nullptr;
-  int n_mphases = 0;
-  bool mq3 = false;
+  PProg mprog;
   int* d_mstate = nullptr;          // PB_STATE_MS ints
-  int* h_mstate = nullptr;          // pinned, PF_RING launches deep
-  int mh_next = 0;
+  StateRing mring;                  // d_mstate of each launch, PF_RING launches deep
   bool mhead = false;               // K-quant head: its QUANT + GEMM phases end the launch, every token's row in logits_b / embd_b
   float *logits_b = nullptr, *embd_b = nullptr;
   float *d_mlogits = nullptr, *d_membd = nullptr;   // [n_seq][n_vocab], [n_seq][n_embd]: each slot's last results
@@ -90,20 +92,21 @@ struct PrefillState {
   long m_launches = 0;
   // rows of every token (RowSink), single sequence: the single-sequence program followed by a K-quant head's QUANT + GEMM phases,
   // every token's logits row of a launch in Engine::d_rows_ (built on first use)
-  PPhase* d_rprog = nullptr;
-  int n_rphases = 0;
-  bool rq3 = false, rtried = false;
+  PProg rprog;
+  bool rtried = false;
   void* dalloc(size_t bytes) {      // zeroed device memory, freed with the state
-    void* p = nullptr;
-    CTB_CUDA(cudaMalloc(&p, bytes));
-    bufs.push_back(p);
-    CTB_CUDA(cudaMemset(p, 0, bytes));
-    return p;
+    bufs.emplace_back(bytes);
+    CTB_CUDA(cudaMemset(bufs.back().get(), 0, bytes));
+    return bufs.back().get();
   }
-  ~PrefillState() {
-    for (void* b : bufs) cudaFree(b);
-    if (h_state) cudaFreeHost(h_state);
-    if (h_mstate) cudaFreeHost(h_mstate);
+  void upload(PProg& p) {           // p.phases to the device (zeroed one phase past the end)
+    p.q3 = pstep_q3(p.phases);
+    p.d = DevMem((p.phases.size() + 1) * sizeof(PPhase));
+    CTB_CUDA(cudaMemset(p.d.get(), 0, (p.phases.size() + 1) * sizeof(PPhase)));
+    CTB_CUDA(cudaMemcpy(p.d.get(), p.phases.data(), p.phases.size() * sizeof(PPhase), cudaMemcpyHostToDevice));
+  }
+  cudaError_t launch(const PProg& p, int grid, cudaStream_t st, unsigned* d_sync, bool multi = false) const {
+    return launch_pstep(grid, n_slots, smem, st, p.d.as<PPhase>(), (int)p.phases.size(), d_sync, p.q3, multi);
   }
 };
 constexpr int PF_RING = 64;
@@ -139,7 +142,7 @@ void* Engine::alloc(size_t bytes, size_t align) {
   const size_t off = align_up(arena_used_, align);
   if (off + bytes > arena_size_) throw std::runtime_error("device arena exhausted");
   arena_used_ = off + bytes;
-  return arena_ + off;
+  return arena_.as<uint8_t>() + off;
 }
 
 // ---- load pipeline (reference: llama_model_loader::load_all_data, llama.cpp:1417-1487 + ggml_cuda_transform_tensor,
@@ -148,18 +151,18 @@ void* Engine::alloc(size_t bytes, size_t align) {
 // into pinned memory while chunk i is on the wire (cudaMemcpyAsync from pinned memory is truly asynchronous) and chunk i-1 is
 // being repacked on the GPU; buffers are recycled behind events, nothing synchronises per tensor.
 struct Uploader {
-  uint8_t* host[UP_BUFS] = {nullptr, nullptr, nullptr};
+  HostMem host[UP_BUFS];
   uint8_t* dev[UP_BUFS] = {nullptr, nullptr, nullptr};
-  cudaEvent_t done[UP_BUFS] = {nullptr, nullptr, nullptr};
-  cudaStream_t st[UP_BUFS] = {nullptr, nullptr, nullptr};
+  Event done[UP_BUFS];
+  Stream st[UP_BUFS];   // (declared after the buffers: a stream's work is done before they are freed)
   int next = 0;
   size_t bytes = 0;
   void init(uint8_t* dev_base) {
     for (int i = 0; i < UP_BUFS; i++) {
-      CTB_CUDA(cudaMallocHost(&host[i], UP_CHUNK));
+      host[i] = HostMem(UP_CHUNK);
       dev[i] = dev_base + (size_t)i * UP_CHUNK;
-      CTB_CUDA(cudaEventCreateWithFlags(&done[i], cudaEventDisableTiming));
-      CTB_CUDA(cudaStreamCreateWithFlags(&st[i], cudaStreamNonBlocking));
+      done[i] = Event(cudaEventDisableTiming);
+      st[i] = Stream(cudaStreamNonBlocking);
     }
   }
   // copies [src, src+n) to the device staging buffer of the next slot; returns the slot (its stream carries the copy)
@@ -167,21 +170,13 @@ struct Uploader {
     const int i = next;
     next = (next + 1) % UP_BUFS;
     CTB_CUDA(cudaEventSynchronize(done[i]));        // the slot's previous chunk has been repacked
-    memcpy(host[i], src, n);
-    CTB_CUDA(cudaMemcpyAsync(dev[i], host[i], n, cudaMemcpyHostToDevice, st[i]));
+    memcpy(host[i].get(), src, n);
+    CTB_CUDA(cudaMemcpyAsync(dev[i], host[i].get(), n, cudaMemcpyHostToDevice, st[i]));
     bytes += n;
     return i;
   }
   void finish(int i) { CTB_CUDA(cudaEventRecord(done[i], st[i])); }
-  void drain() { for (int i = 0; i < UP_BUFS; i++) if (st[i]) CTB_CUDA(cudaStreamSynchronize(st[i])); }
-  void release() {
-    for (int i = 0; i < UP_BUFS; i++) {
-      if (st[i]) { cudaStreamSynchronize(st[i]); cudaStreamDestroy(st[i]); }
-      if (done[i]) cudaEventDestroy(done[i]);
-      if (host[i]) cudaFreeHost(host[i]);
-      st[i] = nullptr; done[i] = nullptr; host[i] = nullptr;
-    }
-  }
+  void drain() { for (int i = 0; i < UP_BUFS; i++) CTB_CUDA(cudaStreamSynchronize(st[i])); }
 };
 
 // rows [row0, row1) and elements [k0, k1) of every row (whole quantization blocks) are kept: a tensor-parallel shard
@@ -285,15 +280,10 @@ TPShard tp_shard(int n_embd, int n_head, int n_head_kv, int n_ff, int rank, int 
   return s;
 }
 
-Engine::Engine(const GGUFFile& g, const HParams& hp, int device, const TPShard& tp) : hp_(hp), tp_(tp), device_(device) {
-  // everything acquired below is released by release() if the constructor throws (the destructor does not run then)
-  try {
-    init(g);
-  } catch (...) {
-    release();
-    throw;
-  }
-}
+Engine::Engine(const HParams& hp, int device, const TPShard& tp) : hp_(hp), tp_(tp), device_(device) {}
+
+// Delegating first makes the engine constructed before init runs, so ~Engine also runs when init throws.
+Engine::Engine(const GGUFFile& g, const HParams& hp, int device, const TPShard& tp) : Engine(hp, device, tp) { init(g); }
 
 void Engine::init(const GGUFFile& g) {
   CTB_CUDA(cudaSetDevice(device_));
@@ -304,15 +294,14 @@ void Engine::init(const GGUFFile& g) {
   for (const auto& t : g.tensors)
     if (t.n_dims >= 2 && !supported_matrix_type(t.type))
       throw std::runtime_error("tensor '" + t.name + "': quantization type " + std::to_string(t.type) + " is not supported by the CUDA path");
-  CTB_CUDA(cudaStreamCreateWithFlags(&stream_, cudaStreamNonBlocking));
-  CTB_CUDA(cudaEventCreate(&ev0_));
-  CTB_CUDA(cudaEventCreate(&ev1_));
+  stream_ = Stream(cudaStreamNonBlocking);
+  ev0_ = Event(cudaEventDefault);
+  ev1_ = Event(cudaEventDefault);
 
   arena_size_ = engine_arena_bytes(g, hp_);
-  CTB_CUDA(cudaMalloc(&arena_, arena_size_));
+  arena_ = DevMem(arena_size_);
   const auto t_load0 = std::chrono::steady_clock::now();
   Uploader up;
-  struct UpGuard { Uploader& u; ~UpGuard() { u.release(); } } up_guard{up};
   up.init((uint8_t*)alloc(UP_CHUNK * UP_BUFS));
 
   // ---- weights (shapes follow from the hyper-parameters: llama.cpp:1878-1934 llama, 1948-2012 falcon)
@@ -413,26 +402,28 @@ void Engine::init(const GGUFFile& g) {
   d_sync_ = (unsigned*)alloc(64);
   CTB_CUDA(cudaMemset(d_state_, 0, 64));
   CTB_CUDA(cudaMemset(d_sync_, 0, 64));
-  CTB_CUDA(cudaMallocHost(&h_logits_, (size_t)hp_.n_vocab * 4));
-  CTB_CUDA(cudaMallocHost(&h_embd_, (size_t)hp_.n_embd * 4));
-  memset(h_logits_, 0, (size_t)hp_.n_vocab * 4);
-  memset(h_embd_, 0, (size_t)hp_.n_embd * 4);
+  h_logits_ = HostMem((size_t)hp_.n_vocab * 4);
+  h_embd_ = HostMem((size_t)hp_.n_embd * 4);
+  memset(h_logits_.get(), 0, (size_t)hp_.n_vocab * 4);
+  memset(h_embd_.get(), 0, (size_t)hp_.n_embd * 4);
+  step_ring_ = StateRing(d_state_, 4, 512);
 
   if (const char* e = getenv("CTB_NO_PDL")) pdl_ = !(e[0] == '1');
   if (const char* e = getenv("CTB_NO_SPEC")) spec_on_ = !(e[0] == '1');
   if (const char* e = getenv("CTB_STEP_FUSE")) fused_ = !(e[0] == '0');
   if (const char* e = getenv("CTB_NO_PREFILL")) prefill_on_ = !(e[0] == '1');
   if (const char* e = getenv("CTB_PREFILL_MIN")) prefill_min_ = std::max(1, atoi(e));
-  CTB_CUDA(cudaMallocHost(&h_spec_tok_, 16));
+  h_spec_tok_ = HostMem(16);
   {   // the kernels' watchdog words: host memory the device can write and the host can read after a trapped launch
-    CTB_CUDA(cudaHostAlloc(&h_dbg_, 64, cudaHostAllocMapped));
-    memset(h_dbg_, 0, 64);
+    h_dbg_ = HostMem(64, true);
+    memset(h_dbg_.get(), 0, 64);
     int* d = nullptr;
-    CTB_CUDA(cudaHostGetDevicePointer(&d, h_dbg_, 0));
+    CTB_CUDA(cudaHostGetDevicePointer(&d, h_dbg_.get(), 0));
     CTB_CUDA(st_set_debug_words(d));
-    g_watchdog_words = h_dbg_;
+    g_watchdog_words = h_dbg_.as<int>();
   }
-  CTB_CUDA(cudaEventCreateWithFlags(&ev_pick_, cudaEventDisableTiming));
+  ev_pick_ = Event(cudaEventDisableTiming);
+  ev_sample_ = Event(cudaEventDisableTiming);
   CTB_CUDA(matvec_set_smem_limit(MV_SMEM_LIMIT));
   CTB_CUDA(cudaFuncSetAttribute(attn_kernel(hp_.head_dim()), cudaFuncAttributeMaxDynamicSharedMemorySize, (int)attn_smem_bytes(hp_.n_ctx, hp_.head_dim())));
   if (tp_.world > 1) tp_setup_peer();
@@ -444,56 +435,15 @@ void Engine::init(const GGUFFile& g) {
   build_graphs();
 }
 
-void Engine::release() {
-  cudaSetDevice(device_);
+Engine::~Engine() {
+  cudaSetDevice(device_);   // the members free on the engine's device, behind its work
   cudaDeviceSynchronize();
-  destroy_graphs();
-  delete pf_;
-  pf_ = nullptr;
-  if (h_logits_) cudaFreeHost(h_logits_);
-  if (h_embd_) cudaFreeHost(h_embd_);
-  if (h_state_) cudaFreeHost(h_state_);
-  if (h_tokens_out_) cudaFreeHost(h_tokens_out_);
-  if (d_tokens_out_) cudaFree(d_tokens_out_);
   for (int r = 0; r < 8; r++)
     if (xc_ll_[r] && r != tp_.rank) cudaIpcCloseMemHandle(xc_ll_[r]);
   if (xc_region_) cudaFree(xc_region_);
-  xc_region_ = nullptr;
-  for (int r = 0; r < 8; r++) xc_ll_[r] = nullptr;
-  if (arena_) cudaFree(arena_);
-  if (h_spec_tok_) cudaFreeHost(h_spec_tok_);
-  if (h_dbg_) cudaFreeHost(h_dbg_);
-  h_dbg_ = nullptr;
-  if (h_sample_) cudaFreeHost(h_sample_);
-  if (d_sample_) cudaFree(d_sample_);
-  h_sample_ = d_sample_ = nullptr;
-  if (h_stage_) cudaFreeHost(h_stage_);
-  h_stage_ = nullptr;
-  stage_cap_ = 0;
-  if (d_copies_) cudaFree(d_copies_);
-  if (h_copies_) cudaFreeHost(h_copies_);
-  d_copies_ = h_copies_ = nullptr;
-  if (d_rows_) cudaFree(d_rows_);
-  if (d_score_) cudaFree(d_score_);
-  if (h_score_) cudaFreeHost(h_score_);
-  d_rows_ = nullptr; d_score_ = h_score_ = nullptr; score_cap_ = 0;
-  if (ev_pick_) cudaEventDestroy(ev_pick_);
-  if (ev_sample_) cudaEventDestroy(ev_sample_);
-  ev_sample_ = nullptr;
-  if (ev0_) cudaEventDestroy(ev0_);
-  if (ev1_) cudaEventDestroy(ev1_);
-  if (stream_ && own_stream_) cudaStreamDestroy(stream_);
-  h_logits_ = h_embd_ = nullptr; h_state_ = nullptr; h_tokens_out_ = nullptr; d_tokens_out_ = nullptr; arena_ = nullptr; h_spec_tok_ = nullptr;
-  ev_pick_ = ev0_ = ev1_ = nullptr; stream_ = nullptr;
 }
 
-Engine::~Engine() { release(); }
-
-void Engine::set_stream(cudaStream_t s) {
-  if (own_stream_ && stream_) { cudaStreamSynchronize(stream_); cudaStreamDestroy(stream_); }
-  stream_ = s;
-  own_stream_ = false;
-}
+void Engine::set_stream(cudaStream_t s) { stream_.set_stream(s); }
 
 static MVSeg seg(const DevMat& w, float* out, int epi = EPI_STORE, const float* res = nullptr, const float* res2 = nullptr) {
   MVSeg s;
@@ -517,9 +467,9 @@ void Engine::push_matvec(MVParams& p, int kind) {
   ops_.push_back(op);
 }
 
-void Engine::tp_all_reduce(float* buf, int n) {
+void Engine::tp_all_reduce(float* buf, int n, cudaStream_t st) {
   const NcclApi& nccl = NcclApi::get();
-  nccl.check(nccl.AllReduce(buf, buf, (size_t)n, ncclFloat, ncclSum, (ncclComm_t)tp_.comm, stream_), "all-reduce");
+  nccl.check(nccl.AllReduce(buf, buf, (size_t)n, ncclFloat, ncclSum, (ncclComm_t)tp_.comm, st), "all-reduce");
 }
 
 // Fused exchange set-up: allocate this rank's region, hand its CUDA IPC handle to the peers (the NCCL communicator carries the 64
@@ -754,11 +704,23 @@ void Engine::upload_prog(Phase* dst, int* dst_bounds, const std::vector<StepOp>&
   CTB_CUDA(cudaMemcpy(dst_bounds, b.data(), b.size() * 4, cudaMemcpyHostToDevice));
 }
 
-// Enqueue ops[0, n) on stream_.  Fused mode: maximal runs of ops the step kernel can take become ONE k_step launch (a
-// K-quant model: the whole token); anything else (Q4_0 / Q8_0 / F16 / F32 mat-vecs) runs as its own kernel.  Un-fused mode
-// (CTB_STEP_FUSE=0): one kernel per op, K-quant mat-vecs as one-phase k_step launches.
-void Engine::enqueue_ops(const std::vector<StepOp>& ops, const Phase* d_prog, const int* d_bounds, int n) {
-  launches_per_step_ = 0;
+struct ProfMark {
+  Event ev;
+  int kind;   // the class (profile_step) of the kernel that ends here, or -1 where one starts
+};
+
+// Enqueue ops[0, n) on st; returns the kernels launched.  Fused mode: maximal runs of ops the step kernel can take become ONE
+// k_step launch (a K-quant model: the whole token); anything else (Q4_0 / Q8_0 / F16 / F32 mat-vecs) runs as its own kernel.
+// Un-fused mode (CTB_STEP_FUSE=0): one kernel per op, K-quant mat-vecs as one-phase k_step launches.  marks: an event before and
+// after every kernel.
+long Engine::enqueue_ops(const std::vector<StepOp>& ops, const Phase* d_prog, const int* d_bounds, int n, cudaStream_t st, bool fused,
+                         std::vector<ProfMark>* marks) {
+  long launches = 0;
+  auto mark = [&](int kind) {
+    if (!marks) return;
+    marks->push_back({Event(cudaEventDefault), kind});
+    CTB_CUDA(cudaEventRecord(marks->back().ev, st));
+  };
   StepLaunch step_shape_;
   step_shape_.grid = step_grid_; step_shape_.n_slots = step_slots_; step_shape_.smem = step_smem_; step_shape_.gen = !attn_fast_hd(hp_.head_dim());
   step_shape_.q3 = step_q3_;
@@ -766,12 +728,12 @@ void Engine::enqueue_ops(const std::vector<StepOp>& ops, const Phase* d_prog, co
   int i = 0;
   while (i < n) {
     const StepOp& op = ops[i];
-    if (fused_ && capable(op)) {
+    if (fused && capable(op)) {
       int j = i;
       while (j < n && capable(ops[j])) j++;
       mark(-1);
-      CTB_CUDA(launch_step(step_shape_, stream_, d_prog + i, d_bounds + (size_t)i * (sm_count_ + 1), j - i, d_sync_, false, nullptr, tp_peer_));
-      launches_per_step_++;
+      CTB_CUDA(launch_step(step_shape_, st, d_prog + i, d_bounds + (size_t)i * (sm_count_ + 1), j - i, d_sync_, false, nullptr, tp_peer_));
+      launches++;
       mark(0);
       i = j;
       continue;
@@ -779,47 +741,39 @@ void Engine::enqueue_ops(const std::vector<StepOp>& ops, const Phase* d_prog, co
     mark(-1);
     switch (op.ph.kind) {
       case PH_EMBED:
-        k_embed<<<1, 256, 0, stream_>>>(op.ph.em);
-        launches_per_step_++;
+        k_embed<<<1, 256, 0, st>>>(op.ph.em);
+        launches++;
         mark(3);
         break;
       case PH_ATTN:
-        CTB_CUDA(launch_kernel(attn_kernel(hp_.head_dim()), dim3(nh_, 1, attn_groups(hp_.head_dim())), dim3(ATTN_THREADS), attn_smem_bytes(hp_.n_ctx, hp_.head_dim()), stream_, pdl_, op.ph.at));
-        launches_per_step_++;
+        CTB_CUDA(launch_kernel(attn_kernel(hp_.head_dim()), dim3(nh_, 1, attn_groups(hp_.head_dim())), dim3(ATTN_THREADS), attn_smem_bytes(hp_.n_ctx, hp_.head_dim()), st, pdl_, op.ph.at));
+        launches++;
         mark(1);
         break;
       case PH_XCHG:
-        tp_all_reduce(op.ph.em.out, op.ph.em.K);
+        tp_all_reduce(op.ph.em.out, op.ph.em.K, st);
         mark(3);
         break;
       case PH_PICK:
-        k_argmax<<<1, ARGMAX_THREADS, 0, stream_>>>(d_logits_, hp_.n_vocab, d_state_ + 4);
-        k_advance<<<1, 1, 0, stream_>>>(d_state_, d_tokens_out_);
-        launches_per_step_ += 2;
+        k_argmax<<<1, ARGMAX_THREADS, 0, st>>>(d_logits_, hp_.n_vocab, d_state_ + 4);
+        k_advance<<<1, 1, 0, st>>>(d_state_, d_tokens_out_.as<int>());
+        launches += 2;
         mark(3);
         break;
       default:
         if (op.stream) {
-          CTB_CUDA(launch_step(step_shape_, stream_, d_prog + i, d_bounds + (size_t)i * (sm_count_ + 1), 1, d_sync_));
+          CTB_CUDA(launch_step(step_shape_, st, d_prog + i, d_bounds + (size_t)i * (sm_count_ + 1), 1, d_sync_));
         } else {
           const MVLaunch L = matvec_launch_shape(op.ph.mv, sm_count_);
-          CTB_CUDA(launch_matvec_kernel(L, stream_, op.ph.mv, pdl_));
+          CTB_CUDA(launch_matvec_kernel(L, st, op.ph.mv, pdl_));
         }
-        launches_per_step_++;
+        launches++;
         mark(0);
     }
     i++;
   }
   CTB_CUDA(cudaGetLastError());
-}
-
-void Engine::mark(int kind) {
-  if (!profiling_) return;
-  cudaEvent_t e;
-  CTB_CUDA(cudaEventCreate(&e));
-  CTB_CUDA(cudaEventRecord(e, stream_));
-  prof_ev_.push_back(e);
-  prof_kind_.push_back(kind);
+  return launches;
 }
 
 // One eager decode step, one kernel per op (un-fused), a CUDA event around every kernel: the kernel classes' share of a step.
@@ -828,22 +782,16 @@ int Engine::profile_step(int token, int n_past, double ms_by_kind[4], int count_
   if (tp_.world > 1) throw std::runtime_error("not available in tensor-parallel mode (every rank must run the same launches)");
   drop_lookahead();
   put_step(token, n_past, n_past + 1);
-  const long keep = launches_per_step_;
-  const bool keep_fused = fused_;
-  profiling_ = true; fused_ = false;
-  try { enqueue_ops(ops_, d_prog_, d_bounds_, n_body_ + 1); } catch (...) { profiling_ = false; fused_ = keep_fused; throw; }
-  profiling_ = false; fused_ = keep_fused;
-  launches_per_step_ = keep;
+  std::vector<ProfMark> marks;
+  enqueue_ops(ops_, d_prog_, d_bounds_, n_body_ + 1, stream_, false, &marks);
   CTB_CUDA(cudaStreamSynchronize(stream_));
   int n = 0;
-  for (size_t i = 1; i < prof_ev_.size(); i++) {
+  for (size_t i = 1; i < marks.size(); i++) {
     float ms = 0;
-    cudaEventElapsedTime(&ms, prof_ev_[i - 1], prof_ev_[i]);
-    const int k = prof_kind_[i];
+    cudaEventElapsedTime(&ms, marks[i - 1].ev, marks[i].ev);
+    const int k = marks[i].kind;
     if (k >= 0 && k < 4) { ms_by_kind[k] += ms; count_by_kind[k]++; n++; }
   }
-  for (cudaEvent_t e : prof_ev_) cudaEventDestroy(e);
-  prof_ev_.clear(); prof_kind_.clear();
   return n;
 }
 
@@ -860,24 +808,18 @@ double Engine::time_matvec_only(int reps, long* launches, unsigned mask) {
     if (ops_[i].ph.kind == PH_MATVEC && ((mask >> ops_[i].mvk) & 1)) sel.push_back(ops_[i]);
   if (sel.empty()) { if (launches) *launches = 0; return 0.0; }
   upload_prog(d_prog_mv_, d_bounds_mv_, sel);
-  cudaStream_t user = stream_, cap;
-  CTB_CUDA(cudaStreamCreateWithFlags(&cap, cudaStreamNonBlocking));
-  const long keep = launches_per_step_;
-  cudaGraphExec_t ex = nullptr;
-  stream_ = cap;
-  try {
+  GraphExec ex;
+  {
+    const Stream cap(cudaStreamNonBlocking);
     cudaGraph_t g;
     CTB_CUDA(cudaStreamBeginCapture(cap, cudaStreamCaptureModeThreadLocal));
-    enqueue_ops(sel, d_prog_mv_, d_bounds_mv_, (int)sel.size());
+    enqueue_ops(sel, d_prog_mv_, d_bounds_mv_, (int)sel.size(), cap, fused_);
     CTB_CUDA(cudaStreamEndCapture(cap, &g));
-    CTB_CUDA(cudaGraphInstantiate(&ex, g, 0));
+    ex = GraphExec(g);
     cudaGraphDestroy(g);
-  } catch (...) { stream_ = user; launches_per_step_ = keep; cudaStreamDestroy(cap); throw; }
+  }
   if (launches) *launches = (long)sel.size();
-  stream_ = user; launches_per_step_ = keep;
-  cudaStreamDestroy(cap);
-  cudaEvent_t e0, e1;
-  CTB_CUDA(cudaEventCreate(&e0)); CTB_CUDA(cudaEventCreate(&e1));
+  const Event e0(cudaEventDefault), e1(cudaEventDefault);
   for (int i = 0; i < 3; i++) CTB_CUDA(cudaGraphLaunch(ex, stream_));
   CTB_CUDA(cudaEventRecord(e0, stream_));
   for (int i = 0; i < reps; i++) CTB_CUDA(cudaGraphLaunch(ex, stream_));
@@ -885,7 +827,6 @@ double Engine::time_matvec_only(int reps, long* launches, unsigned mask) {
   CTB_CUDA(cudaStreamSynchronize(stream_));
   float ms = 0;
   cudaEventElapsedTime(&ms, e0, e1);
-  cudaEventDestroy(e0); cudaEventDestroy(e1); cudaGraphExecDestroy(ex);
   return (double)ms / reps;
 }
 
@@ -900,66 +841,42 @@ long Engine::trace_step(int token, int n_past, unsigned long long* out, long cap
     if (ops_[i].ph.kind == PH_MATVEC && !ops_[i].stream) return 0;
   const long need = 2L * n + 8L * n * step_grid_;
   if (need > cap_words) return -need;
-  unsigned long long* buf = nullptr;
-  CTB_CUDA(cudaMalloc(&buf, (size_t)n * step_grid_ * 64));
-  CTB_CUDA(cudaMemset(buf, 0, (size_t)n * step_grid_ * 64));
+  const DevMem buf((size_t)n * step_grid_ * 64);
+  CTB_CUDA(cudaMemset(buf.get(), 0, (size_t)n * step_grid_ * 64));
   StepLaunch L;
   L.grid = step_grid_; L.n_slots = step_slots_; L.smem = step_smem_; L.gen = !attn_fast_hd(hp_.head_dim()); L.q3 = step_q3_;
   for (int rep = 0; rep < 3; rep++) {   // the last (warm) run is the one read back
     put_step(token, n_past, n_past + 1);
-    CTB_CUDA(launch_step(L, stream_, d_prog_, d_bounds_, n, d_sync_, false, buf));
+    CTB_CUDA(launch_step(L, stream_, d_prog_, d_bounds_, n, d_sync_, false, buf.as<unsigned long long>()));
     CTB_CUDA(cudaStreamSynchronize(stream_));
   }
   for (int i = 0; i < n; i++) { out[2 * i] = (unsigned long long)ops_[i].ph.kind; out[2 * i + 1] = (unsigned long long)ops_[i].mvk; }
-  const cudaError_t e = cudaMemcpy(out + 2 * n, buf, (size_t)n * step_grid_ * 64, cudaMemcpyDeviceToHost);
-  cudaFree(buf);
-  CTB_CUDA(e);
+  CTB_CUDA(cudaMemcpy(out + 2 * n, buf.get(), (size_t)n * step_grid_ * 64, cudaMemcpyDeviceToHost));
   return n;
 }
 
-void Engine::destroy_graphs() {
-  if (graph_full_) cudaGraphExecDestroy(graph_full_);
-  if (graph_nolog_) cudaGraphExecDestroy(graph_nolog_);
-  if (graph_greedy_) cudaGraphExecDestroy(graph_greedy_);
-  graph_full_ = graph_nolog_ = graph_greedy_ = nullptr;
-}
-
 void Engine::build_graphs() {
-  destroy_graphs();
-  if (!d_tokens_out_) {
-    tokens_out_cap_ = std::max(hp_.n_ctx, 4096);
-    CTB_CUDA(cudaMalloc(&d_tokens_out_, (size_t)tokens_out_cap_ * 4));
-    CTB_CUDA(cudaMallocHost(&h_tokens_out_, (size_t)tokens_out_cap_ * 4));
-  }
-  cudaStream_t user = stream_;
-  cudaStream_t cap;
-  CTB_CUDA(cudaStreamCreateWithFlags(&cap, cudaStreamNonBlocking));
-  stream_ = cap;
-  ops_.back().ph.pk.out_tokens = d_tokens_out_;
+  tokens_out_cap_ = std::max(hp_.n_ctx, 4096);
+  d_tokens_out_ = DevMem((size_t)tokens_out_cap_ * 4);
+  h_tokens_out_ = HostMem((size_t)tokens_out_cap_ * 4);
+  const Stream cap(cudaStreamNonBlocking);
+  ops_.back().ph.pk.out_tokens = d_tokens_out_.as<int>();
   upload_prog(d_prog_, d_bounds_, ops_);
+  long launches = 0;
   auto capture = [&](bool logits, bool greedy) {
     cudaGraph_t g;
     CTB_CUDA(cudaStreamBeginCapture(cap, cudaStreamCaptureModeThreadLocal));
     // (fused tensor-parallel exchange: the head phase consumes the last layer's exchange, so every program contains it)
-    enqueue_ops(ops_, d_prog_, d_bounds_, n_body_ + (logits || tp_peer_ ? 1 : 0) + (greedy ? 1 : 0));
+    launches = enqueue_ops(ops_, d_prog_, d_bounds_, n_body_ + (logits || tp_peer_ ? 1 : 0) + (greedy ? 1 : 0), cap, fused_);
     CTB_CUDA(cudaStreamEndCapture(cap, &g));
-    cudaGraphExec_t ex;
-    CTB_CUDA(cudaGraphInstantiate(&ex, g, 0));
+    GraphExec ex(g);
     cudaGraphDestroy(g);
     return ex;
   };
-  try {
-    graph_nolog_ = capture(false, false);
-    graph_greedy_ = capture(true, true);
-    graph_full_ = capture(true, false);
-  } catch (...) {
-    stream_ = user;
-    cudaStreamDestroy(cap);
-    throw;
-  }
-  stats.launches = launches_per_step_;
-  stream_ = user;
-  cudaStreamDestroy(cap);
+  graph_nolog_ = capture(false, false);
+  graph_greedy_ = capture(true, true);
+  graph_full_ = capture(true, false);
+  stats.launches = launches;
 }
 
 // After an eval: pick the greedy next token on the device and — once the caller has proven to decode greedily (its last
@@ -974,8 +891,8 @@ void Engine::after_eval(int next_pos) {
   // that re-evaluates an earlier position and later continues past it keeps its cache contents.
   if (!spec_on_ || next_pos >= hp_.n_ctx || next_pos < kv_high_) return;
   k_argmax<<<1, ARGMAX_THREADS, 0, stream_>>>(d_logits_, hp_.n_vocab, d_state_ + 4);
-  k_advance<<<1, 1, 0, stream_>>>(d_state_, d_tokens_out_);
-  CTB_CUDA(cudaMemcpyAsync(h_spec_tok_, d_state_ + 4, 8, cudaMemcpyDeviceToHost, stream_));   // {greedy pick, how many logits equal the maximum}
+  k_advance<<<1, 1, 0, stream_>>>(d_state_, d_tokens_out_.as<int>());
+  CTB_CUDA(cudaMemcpyAsync(h_spec_tok_.get(), d_state_ + 4, 8, cudaMemcpyDeviceToHost, stream_));   // {greedy pick, how many logits equal the maximum}
   CTB_CUDA(cudaEventRecord(ev_pick_, stream_));
   spec_pos_ = next_pos;
   if (spec_streak_ >= 2) {
@@ -1008,7 +925,8 @@ int Engine::greedy_pick() {
   CTB_CUDA(cudaEventSynchronize(ev_pick_));
   sampler_mode_ = false;
   launch_deferred_spec();
-  return h_spec_tok_[1] == 1 ? h_spec_tok_[0] : -1;
+  const int* pick = h_spec_tok_.as<int>();
+  return pick[1] == 1 ? pick[0] : -1;
 }
 
 void Engine::eval(const int* tokens, int n, int n_past) {
@@ -1018,13 +936,8 @@ void Engine::eval(const int* tokens, int n, int n_past) {
   eval_list(tokens, pos.data(), nt.data(), n);
 }
 
-// Each copy reads its own ring entry, so a copy still pending in the stream reads what it was given (eval_list synchronises
-// before the ring wraps).
 void Engine::put_step(int token, int pos, int n_total) {
-  if (h_state_cap_ < 1) { h_state_cap_ = 512; CTB_CUDA(cudaMallocHost(&h_state_, (size_t)h_state_cap_ * 16)); }
-  int* st = h_state_ + (size_t)(h_state_next_++ % h_state_cap_) * 4;
-  st[0] = token; st[1] = pos; st[2] = 0; st[3] = n_total;
-  CTB_CUDA(cudaMemcpyAsync(d_state_, st, 16, cudaMemcpyHostToDevice, stream_));
+  CTB_CUDA(step_ring_.put(stream_, [&](int* st) { st[0] = token; st[1] = pos; st[2] = 0; st[3] = n_total; }));
 }
 
 void Engine::decode_one(int token, int pos, int n_total, bool with_logits) {
@@ -1045,15 +958,15 @@ void Engine::host_views() {
   eager_ = true;
   if (host_fresh_) return;
   DeviceGuard dev_guard(device_);
-  CTB_CUDA(cudaMemcpyAsync(h_logits_, d_logits_keep_, (size_t)hp_.n_vocab * 4, cudaMemcpyDeviceToHost, stream_));
-  CTB_CUDA(cudaMemcpyAsync(h_embd_, d_embd_keep_, (size_t)hp_.n_embd * 4, cudaMemcpyDeviceToHost, stream_));
+  CTB_CUDA(cudaMemcpyAsync(h_logits_.get(), d_logits_keep_, (size_t)hp_.n_vocab * 4, cudaMemcpyDeviceToHost, stream_));
+  CTB_CUDA(cudaMemcpyAsync(h_embd_.get(), d_embd_keep_, (size_t)hp_.n_embd * 4, cudaMemcpyDeviceToHost, stream_));
   CTB_CUDA(cudaStreamSynchronize(stream_));
   host_fresh_ = true;
 }
 
 std::vector<float> Engine::logits_copy() {
   std::vector<float> v((size_t)hp_.n_vocab);
-  if (host_fresh_) { memcpy(v.data(), h_logits_, v.size() * 4); return v; }
+  if (host_fresh_) { memcpy(v.data(), h_logits_.get(), v.size() * 4); return v; }
   DeviceGuard dev_guard(device_);
   CTB_CUDA(cudaMemcpyAsync(v.data(), d_logits_keep_, v.size() * 4, cudaMemcpyDeviceToHost, stream_));
   CTB_CUDA(cudaStreamSynchronize(stream_));
@@ -1066,14 +979,12 @@ void Engine::sample_enqueue(const SampleRow* rows, int R, const float* logits, s
   const int S = hp_.n_seq;
   if (R < 0 || R > S) throw std::runtime_error("device sampler: " + std::to_string(R) + " rows for " + std::to_string(S) + " slots");
   const size_t picks_b = (size_t)S * 8, outs_b = (size_t)S * sizeof(SampleGpuOut);
-  if (!d_sample_) {
-    const size_t bytes = picks_b + outs_b + sg_block_ints(S, S * SG_MAX_LAST) * 4;
-    CTB_CUDA(cudaMalloc(&d_sample_, bytes));
-    CTB_CUDA(cudaMallocHost(&h_sample_, bytes));
-  }
-  SampleGpuOut* d_out = (SampleGpuOut*)(d_sample_ + picks_b);
-  int* h_blk = (int*)(h_sample_ + picks_b + outs_b);
-  int* d_blk = (int*)(d_sample_ + picks_b + outs_b);
+  const size_t bytes = picks_b + outs_b + sg_block_ints(S, S * SG_MAX_LAST) * 4;
+  uint8_t* d_buf = (uint8_t*)d_sample_.grow(bytes);
+  uint8_t* h_buf = (uint8_t*)h_sample_.grow(bytes);
+  SampleGpuOut* d_out = (SampleGpuOut*)(d_buf + picks_b);
+  int* h_blk = (int*)(h_buf + picks_b + outs_b);
+  int* d_blk = (int*)(d_buf + picks_b + outs_b);
   int n_tok = 0;
   for (int r = 0; r < R; r++) {
     if (!sg_accepts(rows[r].n_last, rows[r].k) || rows[r].slot < 0 || rows[r].slot >= S) throw std::runtime_error("device sampler: a row it does not take");
@@ -1086,22 +997,21 @@ void Engine::sample_enqueue(const SampleRow* rows, int R, const float* logits, s
     CTB_CUDA(cudaGetLastError());
   }
   // one copy back: the picks (first in the buffer) and then the R results
-  if (picks) CTB_CUDA(cudaMemcpyAsync(d_sample_, pf_->d_mpick, picks_b, cudaMemcpyDeviceToDevice, stream_));
+  if (picks) CTB_CUDA(cudaMemcpyAsync(d_buf, pf_->d_mpick, picks_b, cudaMemcpyDeviceToDevice, stream_));
   const size_t from = picks ? 0 : picks_b, to = picks_b + (size_t)R * sizeof(SampleGpuOut);
-  if (to > from) CTB_CUDA(cudaMemcpyAsync(h_sample_ + from, d_sample_ + from, to - from, cudaMemcpyDeviceToHost, stream_));
+  if (to > from) CTB_CUDA(cudaMemcpyAsync(h_buf + from, d_buf + from, to - from, cudaMemcpyDeviceToHost, stream_));
 }
 
 int Engine::topk_candidates(const int* last, int n_last, float penalty, int k, int* ids, float* logits) {
   if (!sg_accepts(n_last, k)) return -1;
   DeviceGuard dev_guard(device_);
-  if (!ev_sample_) CTB_CUDA(cudaEventCreateWithFlags(&ev_sample_, cudaEventDisableTiming));
   sampler_mode_ = true;
   const SampleRow row{0, last, n_last, penalty, k};
   sample_enqueue(&row, 1, d_logits_keep_, 0, false);
   CTB_CUDA(cudaEventRecord(ev_sample_, stream_));
   launch_deferred_spec();                          // the look-ahead step runs while the host finishes the draw
   CTB_CUDA(cudaEventSynchronize(ev_sample_));
-  return sg_take(*(const SampleGpuOut*)(h_sample_ + (size_t)hp_.n_seq * 8), ids, logits);
+  return sg_take(*(const SampleGpuOut*)(h_sample_.as<uint8_t>() + (size_t)hp_.n_seq * 8), ids, logits);
 }
 
 void Engine::finish_eval(int next_pos, bool hit) {
@@ -1109,8 +1019,8 @@ void Engine::finish_eval(int next_pos, bool hit) {
   CTB_CUDA(cudaMemcpyAsync(d_logits_keep_, d_logits_, (size_t)hp_.n_vocab * 4, cudaMemcpyDeviceToDevice, stream_));
   CTB_CUDA(cudaMemcpyAsync(d_embd_keep_, d_embd_, (size_t)hp_.n_embd * 4, cudaMemcpyDeviceToDevice, stream_));
   if (eager_) {
-    CTB_CUDA(cudaMemcpyAsync(h_logits_, d_logits_, (size_t)hp_.n_vocab * 4, cudaMemcpyDeviceToHost, stream_));
-    CTB_CUDA(cudaMemcpyAsync(h_embd_, d_embd_, (size_t)hp_.n_embd * 4, cudaMemcpyDeviceToHost, stream_));
+    CTB_CUDA(cudaMemcpyAsync(h_logits_.get(), d_logits_, (size_t)hp_.n_vocab * 4, cudaMemcpyDeviceToHost, stream_));
+    CTB_CUDA(cudaMemcpyAsync(h_embd_.get(), d_embd_, (size_t)hp_.n_embd * 4, cudaMemcpyDeviceToHost, stream_));
   }
   host_fresh_ = eager_;
   CTB_CUDA(cudaEventRecord(ev1_, stream_));
@@ -1123,26 +1033,24 @@ void Engine::finish_eval(int next_pos, bool hit) {
 }
 
 // ---- rows of every token (RowSink)
-void Engine::rows_begin(const RowSink* rows, int n) {
+Engine::SinkGuard Engine::rows_begin(const RowSink* rows, int n) {
   sink_ = nullptr; rows_pending_ = 0; rows_done_ = 0; rows_n_ = n;
-  if (!rows) return;
+  if (!rows) return SinkGuard{this};
   if (tp_.world > 1) throw std::runtime_error("the tensor-sharded mode keeps no per-token rows");
-  if (!d_rows_) CTB_CUDA(cudaMalloc(&d_rows_, (size_t)PB_T * hp_.n_vocab * 4));
+  d_rows_.grow((size_t)PB_T * hp_.n_vocab * 4);
   if (rows->targets) {
     if (n > score_cap_) {
-      if (d_score_) CTB_CUDA(cudaFree(d_score_));
-      if (h_score_) CTB_CUDA(cudaFreeHost(h_score_));
-      d_score_ = h_score_ = nullptr; score_cap_ = 0;
       const int cap = std::max(n, 1024);
-      CTB_CUDA(cudaMalloc(&d_score_, (size_t)cap * 16));
-      CTB_CUDA(cudaMallocHost(&h_score_, (size_t)cap * 16));
+      d_score_.grow((size_t)cap * 16);
+      h_score_.grow((size_t)cap * 16);
       score_cap_ = cap;
     }
-    d_lp_ = (double*)d_score_; d_tgt_ = (int*)(d_score_ + (size_t)score_cap_ * 8); d_gr_ = d_tgt_ + score_cap_;
-    memcpy(h_score_ + (size_t)score_cap_ * 8, rows->targets, (size_t)n * 4);
-    CTB_CUDA(cudaMemcpyAsync(d_tgt_, h_score_ + (size_t)score_cap_ * 8, (size_t)n * 4, cudaMemcpyHostToDevice, stream_));
+    d_lp_ = d_score_.as<double>(); d_tgt_ = (int*)(d_score_.as<uint8_t>() + (size_t)score_cap_ * 8); d_gr_ = d_tgt_ + score_cap_;
+    memcpy(h_score_.as<uint8_t>() + (size_t)score_cap_ * 8, rows->targets, (size_t)n * 4);
+    CTB_CUDA(cudaMemcpyAsync(d_tgt_, h_score_.as<uint8_t>() + (size_t)score_cap_ * 8, (size_t)n * 4, cudaMemcpyHostToDevice, stream_));
   }
   sink_ = rows;
+  return SinkGuard{this};
 }
 
 void Engine::rows_take(const float* src, int m) {
@@ -1158,7 +1066,7 @@ void Engine::rows_take(const float* src, int m) {
 }
 
 void Engine::rows_push(const float* row) {
-  CTB_CUDA(cudaMemcpyAsync(d_rows_ + (size_t)rows_pending_ * hp_.n_vocab, row, (size_t)hp_.n_vocab * 4, cudaMemcpyDeviceToDevice, stream_));
+  CTB_CUDA(cudaMemcpyAsync(d_rows_.as<float>() + (size_t)rows_pending_ * hp_.n_vocab, row, (size_t)hp_.n_vocab * 4, cudaMemcpyDeviceToDevice, stream_));
   if (++rows_pending_ == PB_T) rows_drain();
 }
 
@@ -1166,7 +1074,7 @@ void Engine::rows_drain() {
   if (!sink_ || !rows_pending_) return;
   const int m = rows_pending_;
   rows_pending_ = 0;
-  rows_take(d_rows_, m);
+  rows_take(d_rows_.as<float>(), m);
 }
 
 void Engine::rows_finish() {
@@ -1174,25 +1082,23 @@ void Engine::rows_finish() {
   rows_drain();
   if (rows_done_ != rows_n_) throw std::runtime_error("rows: " + std::to_string(rows_done_) + " rows for " + std::to_string(rows_n_) + " tokens");
   if (sink_->targets) {
-    CTB_CUDA(cudaMemcpyAsync(h_score_, d_lp_, (size_t)rows_n_ * 8, cudaMemcpyDeviceToHost, stream_));
-    CTB_CUDA(cudaMemcpyAsync(h_score_ + (size_t)score_cap_ * 12, d_gr_, (size_t)rows_n_ * 4, cudaMemcpyDeviceToHost, stream_));
+    CTB_CUDA(cudaMemcpyAsync(h_score_.get(), d_lp_, (size_t)rows_n_ * 8, cudaMemcpyDeviceToHost, stream_));
+    CTB_CUDA(cudaMemcpyAsync(h_score_.as<uint8_t>() + (size_t)score_cap_ * 12, d_gr_, (size_t)rows_n_ * 4, cudaMemcpyDeviceToHost, stream_));
   }
 }
 
 void Engine::rows_end() {
   if (sink_ && sink_->targets) {
-    if (sink_->logprob) memcpy(sink_->logprob, h_score_, (size_t)rows_n_ * 8);
-    if (sink_->greedy) memcpy(sink_->greedy, h_score_ + (size_t)score_cap_ * 12, (size_t)rows_n_ * 4);
+    if (sink_->logprob) memcpy(sink_->logprob, h_score_.get(), (size_t)rows_n_ * 8);
+    if (sink_->greedy) memcpy(sink_->greedy, h_score_.as<uint8_t>() + (size_t)score_cap_ * 12, (size_t)rows_n_ * 4);
   }
-  sink_ = nullptr;
 }
 
 void Engine::score_kept(int target, double* logprob, int* greedy) {
   DeviceGuard dev_guard(device_);
   RowSink s;
   s.targets = &target; s.logprob = logprob; s.greedy = greedy;
-  struct Release { Engine* e; ~Release() { e->sink_ = nullptr; } } release{this};
-  rows_begin(&s, 1);
+  const SinkGuard sink = rows_begin(&s, 1);
   rows_take(d_logits_keep_, 1);
   rows_finish();
   CTB_CUDA(cudaStreamSynchronize(stream_));
@@ -1204,33 +1110,27 @@ void Engine::score_kept(int target, double* logprob, int* greedy) {
 // last token's (head_from).  False for a head that is not a K-quant: its rows then come from head_from, one row at a time.
 bool Engine::ensure_rows_prog() {
   PrefillState& P = *pf_;
-  if (P.rtried) return P.d_rprog != nullptr;
+  if (P.rtried) return (bool)P.rprog.d;
   P.rtried = true;
   const StepOp& head = ops_[n_body_];
   if (!head.stream) return false;
-  std::vector<PPhase> rprog(P.n_phases);
-  CTB_CUDA(cudaMemcpy(rprog.data(), P.d_prog, rprog.size() * sizeof(PPhase), cudaMemcpyDeviceToHost));
+  P.rprog.phases = P.prog.phases;
   const float* hx = head.ph.mv.x;
   auto bat = [&](const float* p, int& ld) -> float* {
     if (!p) { ld = 0; return nullptr; }
     if (p == hx) { ld = hp_.n_embd; return P.x_final; }
-    if (p == d_logits_) { ld = hp_.n_vocab; return d_rows_; }
+    if (p == d_logits_) { ld = hp_.n_vocab; return d_rows_.as<float>(); }
     throw std::runtime_error("rows: pointer outside the output head's buffers");
   };
-  pb_matvec_phases(head.ph.mv, (uint8_t*)P.dalloc(pb_qbuf_bytes(head.ph.mv.K)), P.d_state, bat, rprog);
-  P.n_rphases = (int)rprog.size();
-  P.rq3 = pstep_q3(rprog);
-  PPhase* d = (PPhase*)P.dalloc((rprog.size() + 1) * sizeof(PPhase));
-  CTB_CUDA(cudaMemcpy(d, rprog.data(), rprog.size() * sizeof(PPhase), cudaMemcpyHostToDevice));
-  P.d_rprog = d;
+  pb_matvec_phases(head.ph.mv, (uint8_t*)P.dalloc(pb_qbuf_bytes(head.ph.mv.K)), P.d_state, bat, P.rprog.phases);
+  P.upload(P.rprog);
   return true;
 }
 
 void Engine::eval_list(const int* tokens, const int* pos, const int* n_total, int n, const RowSink* rows) {
   if (n <= 0) return;
   DeviceGuard dev_guard(device_);
-  struct Release { Engine* e; ~Release() { e->sink_ = nullptr; } } release{this};   // a failed eval leaves no sink behind
-  rows_begin(rows, n);
+  const SinkGuard sink = rows_begin(rows, n);
   bool hit = false;
   if (spec_pos_ >= 0) {
     const bool was_pending = spec_pending_;   // (a deferred look-ahead nobody launched is simply dropped)
@@ -1238,7 +1138,7 @@ void Engine::eval_list(const int* tokens, const int* pos, const int* n_total, in
     bool guessed = false;
     if (n == 1 && pos[0] == spec_pos_ && n_total[0] == pos[0] + 1) {
       CTB_CUDA(cudaEventSynchronize(ev_pick_));
-      guessed = h_spec_tok_[0] == tokens[0];
+      guessed = h_spec_tok_.as<int>()[0] == tokens[0];
     }
     spec_streak_ = guessed ? spec_streak_ + 1 : 0;
     hit = guessed && was_pending;
@@ -1262,7 +1162,6 @@ void Engine::eval_list(const int* tokens, const int* pos, const int* n_total, in
         for (int k = i; k < j; k++) {
           decode_one(tokens[k], pos[k], n_total[k], k == n - 1 || sink_);   // (the full step's body is the same as the short one's)
           if (sink_) rows_push(d_logits_);
-          if ((k - i) % 128 == 127) CTB_CUDA(cudaStreamSynchronize(stream_));   // keeps the pinned state ring from wrapping under the GPU
         }
       }
       i = j;
@@ -1278,7 +1177,7 @@ void Engine::eval_list(const int* tokens, const int* pos, const int* n_total, in
 bool Engine::ensure_prefill() {
   if ((!prefill_on_ && !hp_.multi) || tp_.world > 1) return false;   // (multi-sequence evals have no other path)
   if (pf_ && pf_->tried) return pf_->ok;
-  if (!pf_) pf_ = new PrefillState();
+  if (!pf_) pf_.reset(new PrefillState());
   PrefillState& P = *pf_;
   P.tried = true;
   for (int i = 0; i < n_body_; i++)
@@ -1297,8 +1196,8 @@ bool Engine::ensure_prefill() {
     throw std::runtime_error("prefill: pointer outside the step workspace");
   };
   P.d_state = (int*)P.dalloc((PB_T * 4 + 4) * 4);
-  CTB_CUDA(cudaMallocHost(&P.h_state, (size_t)PF_RING * (PB_T * 4 + 4) * 4));
-  std::vector<PPhase> prog;
+  P.ring = StateRing(P.d_state, PB_T * 4 + 4, PF_RING);
+  std::vector<PPhase>& prog = P.prog.phases;
   int K_max = 0;
   for (int i = 0; i < n_body_; i++) {
     const StepOp& op = ops_[i];
@@ -1326,14 +1225,12 @@ bool Engine::ensure_prefill() {
   }
   int ld;
   P.x_final = bat(ops_[n_body_].ph.mv.x, ld);
-  P.n_phases = (int)prog.size();
-  P.q3 = pstep_q3(prog);
-  P.d_prog = (PPhase*)P.dalloc((prog.size() + 1) * sizeof(PPhase));
-  CTB_CUDA(cudaMemcpy(P.d_prog, prog.data(), prog.size() * sizeof(PPhase), cudaMemcpyHostToDevice));
+  P.upload(P.prog);
   if (hp_.multi) {
     P.d_mstate = (int*)P.dalloc(PB_STATE_MS * 4);
-    CTB_CUDA(cudaMallocHost(&P.h_mstate, (size_t)PF_RING * PB_STATE_MS * 4));
-    std::vector<PPhase> mprog = prog;
+    P.mring = StateRing(P.d_mstate, PB_STATE_MS, PF_RING);
+    std::vector<PPhase>& mprog = P.mprog.phases;
+    mprog = prog;
     for (PPhase& ph : mprog) { ph.state = P.d_mstate; ph.at.state = P.d_mstate; }
     const StepOp& head = ops_[n_body_];
     P.mhead = head.stream;
@@ -1344,10 +1241,7 @@ bool Engine::ensure_prefill() {
       P.embd_b = bat(d_embd_, ld);
       mprog[mprog.size() - 2].mv.norm_out = P.embd_b;
     }
-    P.n_mphases = (int)mprog.size();
-    P.mq3 = pstep_q3(mprog);
-    P.d_mprog = (PPhase*)P.dalloc((mprog.size() + 1) * sizeof(PPhase));
-    CTB_CUDA(cudaMemcpy(P.d_mprog, mprog.data(), mprog.size() * sizeof(PPhase), cudaMemcpyHostToDevice));
+    P.upload(P.mprog);
     P.d_mlogits = (float*)P.dalloc((size_t)hp_.n_seq * hp_.n_vocab * 4);
     P.d_membd = (float*)P.dalloc((size_t)hp_.n_seq * n_embd * 4);
     P.d_mpick = (int*)P.dalloc((size_t)hp_.n_seq * 8);
@@ -1365,16 +1259,14 @@ void Engine::prefill_batch(const int* tokens, const int* pos, const int* n_total
   PrefillState& P = *pf_;
   const bool rp = rows && ensure_rows_prog();
   if (rp) rows_drain();   // the launch writes d_rows_
-  if (P.h_next % PF_RING == PF_RING - 1) CTB_CUDA(cudaStreamSynchronize(stream_));   // pinned state ring
-  int* st = P.h_state + (size_t)(P.h_next++ % PF_RING) * (PB_T * 4 + 4);
-  for (int i = 0; i < PB_T; i++) {
-    const int k = std::min(i, n - 1);
-    st[i * 4] = tokens[k]; st[i * 4 + 1] = pos[k]; st[i * 4 + 2] = 0; st[i * 4 + 3] = n_total[k];
-  }
-  st[PB_T * 4] = n;
-  CTB_CUDA(cudaMemcpyAsync(P.d_state, st, (PB_T * 4 + 4) * 4, cudaMemcpyHostToDevice, stream_));
-  if (rp) CTB_CUDA(launch_pstep(step_grid_, P.n_slots, P.smem, stream_, P.d_rprog, P.n_rphases, d_sync_, P.rq3));
-  else CTB_CUDA(launch_pstep(step_grid_, P.n_slots, P.smem, stream_, P.d_prog, P.n_phases, d_sync_, P.q3));
+  CTB_CUDA(P.ring.put(stream_, [&](int* st) {
+    for (int i = 0; i < PB_T; i++) {
+      const int k = std::min(i, n - 1);
+      st[i * 4] = tokens[k]; st[i * 4 + 1] = pos[k]; st[i * 4 + 2] = 0; st[i * 4 + 3] = n_total[k];
+    }
+    st[PB_T * 4] = n;
+  }));
+  CTB_CUDA(P.launch(rp ? P.rprog : P.prog, step_grid_, stream_, d_sync_));
   prefill_launches_++;
   if (rp) {
     rows_pending_ = n;
@@ -1391,13 +1283,8 @@ void Engine::prefill_batch(const int* tokens, const int* pos, const int* n_total
 void Engine::head_from(const float* row) {
   const StepOp& head = ops_[n_body_];
   CTB_CUDA(cudaMemcpyAsync(const_cast<float*>(head.ph.mv.x), row, (size_t)hp_.n_embd * 4, cudaMemcpyDeviceToDevice, stream_));
-  const bool keep = fused_;
-  fused_ = false;                                    // just this one op, the way the un-fused schedule launches it
-  std::vector<StepOp> one(1, head);
-  const long keepl = launches_per_step_;
-  try { enqueue_ops(one, d_prog_ + n_body_, d_bounds_ + (size_t)n_body_ * (sm_count_ + 1), 1); } catch (...) { fused_ = keep; throw; }
-  fused_ = keep;
-  launches_per_step_ = keepl;
+  // just this one op, the way the un-fused schedule launches it
+  enqueue_ops(std::vector<StepOp>(1, head), d_prog_ + n_body_, d_bounds_ + (size_t)n_body_ * (sm_count_ + 1), 1, stream_, false);
 }
 
 // ---- multi-sequence mode
@@ -1410,7 +1297,7 @@ std::string Engine::multi_refusal() {
   return "";
 }
 
-bool Engine::multi_ready() { return hp_.multi && ensure_prefill() && pf_->d_mprog; }
+bool Engine::multi_ready() { return hp_.multi && ensure_prefill() && pf_->mprog.d; }
 
 void Engine::need_multi() {
   if (!multi_ready()) throw std::runtime_error("this engine has no multi-sequence path");
@@ -1420,8 +1307,7 @@ void Engine::multi_eval(const std::vector<MultiTok>& toks, const std::vector<int
   DeviceGuard dev_guard(device_);
   need_multi();
   PrefillState& P = *pf_;
-  struct Release { Engine* e; ~Release() { e->sink_ = nullptr; } } release{this};
-  rows_begin(rows, (int)toks.size());
+  const SinkGuard sink = rows_begin(rows, (int)toks.size());
   const int n_embd = hp_.n_embd, n_vocab = hp_.n_vocab;
   size_t kslot, vslot;
   kv_slot_elems(kslot, vslot);
@@ -1430,16 +1316,15 @@ void Engine::multi_eval(const std::vector<MultiTok>& toks, const std::vector<int
   for (size_t l = 0; l + 1 < starts.size(); l++) {
     const int a = starts[l], n = starts[l + 1] - a;
     if (n < 1 || n > PB_T) throw std::runtime_error("multi-sequence: bad launch size");
-    if (P.mh_next % PF_RING == PF_RING - 1) CTB_CUDA(cudaStreamSynchronize(stream_));   // pinned state ring
-    int* st = P.h_mstate + (size_t)(P.mh_next++ % PF_RING) * PB_STATE_MS;
-    for (int i = 0; i < PB_T; i++) {
-      const MultiTok& t = toks[a + std::min(i, n - 1)];
-      st[i * 4] = t.token; st[i * 4 + 1] = t.pos; st[i * 4 + 2] = 0; st[i * 4 + 3] = t.n_total;
-      st[PB_S + i] = t.slot;
-    }
-    st[PB_T * 4] = n; st[PB_T * 4 + 1] = (int)(unsigned)kslot; st[PB_T * 4 + 2] = (int)(unsigned)vslot; st[PB_T * 4 + 3] = 0;
-    CTB_CUDA(cudaMemcpyAsync(P.d_mstate, st, PB_STATE_MS * 4, cudaMemcpyHostToDevice, stream_));
-    CTB_CUDA(launch_pstep(step_grid_, P.n_slots, P.smem, stream_, P.d_mprog, P.n_mphases, d_sync_, P.mq3, true));
+    CTB_CUDA(P.mring.put(stream_, [&](int* st) {
+      for (int i = 0; i < PB_T; i++) {
+        const MultiTok& t = toks[a + std::min(i, n - 1)];
+        st[i * 4] = t.token; st[i * 4 + 1] = t.pos; st[i * 4 + 2] = 0; st[i * 4 + 3] = t.n_total;
+        st[PB_S + i] = t.slot;
+      }
+      st[PB_T * 4] = n; st[PB_T * 4 + 1] = (int)(unsigned)kslot; st[PB_T * 4 + 2] = (int)(unsigned)vslot; st[PB_T * 4 + 3] = 0;
+    }));
+    CTB_CUDA(P.launch(P.mprog, step_grid_, stream_, d_sync_, true));
     P.m_launches++;
     if (sink_ && P.mhead) rows_take(P.logits_b, n);   // every token's row of the launch
     for (int r = 0; r < n; r++) {
@@ -1486,8 +1371,8 @@ const SampleGpuOut* Engine::multi_sample(const SampleRow* rows, int R, int* pick
   need_multi();
   sample_enqueue(rows, R, pf_->d_mlogits, (size_t)hp_.n_vocab, true);
   CTB_CUDA(cudaStreamSynchronize(stream_));
-  memcpy(picks, h_sample_, (size_t)hp_.n_seq * 8);
-  return (const SampleGpuOut*)(h_sample_ + (size_t)hp_.n_seq * 8);
+  memcpy(picks, h_sample_.get(), (size_t)hp_.n_seq * 8);
+  return (const SampleGpuOut*)(h_sample_.as<uint8_t>() + (size_t)hp_.n_seq * 8);
 }
 
 void Engine::multi_reset(int slot) {
@@ -1531,17 +1416,6 @@ void Engine::copy_results(int src, int dst) {
   CTB_CUDA(cudaMemcpyAsync(pf_->d_mpick + 2 * dst, pf_->d_mpick + 2 * src, 8, cudaMemcpyDeviceToDevice, stream_));
 }
 
-uint8_t* Engine::stage(size_t bytes) {
-  if (bytes > stage_cap_) {
-    if (h_stage_) CTB_CUDA(cudaFreeHost(h_stage_));
-    h_stage_ = nullptr;
-    stage_cap_ = 0;
-    CTB_CUDA(cudaMallocHost(&h_stage_, bytes));
-    stage_cap_ = bytes;
-  }
-  return h_stage_;
-}
-
 int Engine::state_k_stride() const { return k_stride(hp_.head_dim()); }
 
 // V rows hold position t at v_perm(t), a permutation within each block of 256 positions: a state keeps whole blocks,
@@ -1570,7 +1444,7 @@ void Engine::state_save(int slot, int n_past, bool results, void* out) {
   size_t kslot, vslot;
   kv_slot_elems(kslot, vslot);
   const size_t rows = (size_t)hp_.n_layer * nkv_, kb = rows * n_past * ks * 2, vb = rows * hd * v_pad(n_past) * 2;
-  uint8_t* h = stage(std::max<size_t>(state_bytes(n_past, results), 1));
+  uint8_t* h = (uint8_t*)h_stage_.grow(std::max<size_t>(state_bytes(n_past, results), 1));
   if (n_past > 0) {
     CTB_CUDA(cudaMemcpy2DAsync(h, (size_t)n_past * ks * 2, kc_ + slot * kslot, (size_t)hp_.n_ctx * ks * 2, (size_t)n_past * ks * 2, rows,
                                cudaMemcpyDeviceToHost, stream_));
@@ -1596,7 +1470,7 @@ void Engine::state_load(int slot, int n_past, bool results, const void* in, int 
   const size_t rows = (size_t)hp_.n_layer * nkv_, kb = rows * n_past * ks * 2, vb = rows * hd * v_pad(n_past) * 2;
   float* em = nullptr;
   float* lg = results ? results_of(slot, &em) : nullptr;
-  uint8_t* h = stage(std::max<size_t>(state_bytes(n_past, results), 1));
+  uint8_t* h = (uint8_t*)h_stage_.grow(std::max<size_t>(state_bytes(n_past, results), 1));
   memcpy(h, in, state_bytes(n_past, results));
   zero_v_tail((uint16_t*)(h + kb), rows * hd, n_past);
   if (!hp_.multi) drop_lookahead();   // a look-ahead step may still be in the stream: it runs before the copies below
@@ -1680,18 +1554,16 @@ size_t Engine::kv_reparent(const std::vector<KvCopy>& copies) {
   }
   for (int s = 0; s < hp_.n_seq; s++)
     if (src[s] && dst[s]) throw std::runtime_error("kv_reparent: slot " + std::to_string(s) + " is both a source and a destination");
-  if (!d_copies_) {
-    CTB_CUDA(cudaMalloc(&d_copies_, sizeof(KvCopy) * hp_.n_seq));
-    CTB_CUDA(cudaMallocHost(&h_copies_, sizeof(KvCopy) * hp_.n_seq));
-  }
+  KvCopy* d_copies = (KvCopy*)d_copies_.grow(sizeof(KvCopy) * hp_.n_seq);
+  KvCopy* h_copies = (KvCopy*)h_copies_.grow(sizeof(KvCopy) * hp_.n_seq);
   const int hd = hp_.head_dim(), ks = k_stride(hd);
   size_t kslot, vslot, bytes = 0;
   kv_slot_elems(kslot, vslot);
   const size_t lh = (size_t)hp_.n_layer * nkv_;
   for (const KvCopy& c : copies) bytes += lh * ((size_t)(c.hi - c.lo) * ks + (size_t)hd * (((c.hi + 255) & ~255) - (c.lo & ~255))) * 2;
-  std::copy(copies.begin(), copies.end(), h_copies_);
-  CTB_CUDA(cudaMemcpyAsync(d_copies_, h_copies_, sizeof(KvCopy) * copies.size(), cudaMemcpyHostToDevice, stream_));
-  k_kv_reparent<<<dim3((unsigned)lh, (unsigned)copies.size()), 256, 0, stream_>>>(d_copies_, kc_, vc_, kslot, vslot, hp_.n_ctx, ks, hd);
+  std::copy(copies.begin(), copies.end(), h_copies);
+  CTB_CUDA(cudaMemcpyAsync(d_copies, h_copies, sizeof(KvCopy) * copies.size(), cudaMemcpyHostToDevice, stream_));
+  k_kv_reparent<<<dim3((unsigned)lh, (unsigned)copies.size()), 256, 0, stream_>>>(d_copies, kc_, vc_, kslot, vslot, hp_.n_ctx, ks, hd);
   CTB_CUDA(cudaGetLastError());
   for (const KvCopy& c : copies) copy_results(c.src, c.dst);
   CTB_CUDA(cudaStreamSynchronize(stream_));
@@ -1703,7 +1575,7 @@ const float* Engine::multi_rows(int slot0, int n) {
   need_multi();
   if (slot0 < 0 || n < 0 || slot0 + n > hp_.n_seq) throw std::runtime_error("multi_rows: slots out of range");
   const size_t b = (size_t)n * hp_.n_vocab * 4;
-  float* h = (float*)stage(std::max<size_t>(b, 1));
+  float* h = (float*)h_stage_.grow(std::max<size_t>(b, 1));
   CTB_CUDA(cudaMemcpyAsync(h, pf_->d_mlogits + (size_t)slot0 * hp_.n_vocab, b, cudaMemcpyDeviceToHost, stream_));
   CTB_CUDA(cudaStreamSynchronize(stream_));
   return h;
@@ -1720,14 +1592,14 @@ double Engine::decode_greedy(int first_token, int n_past, int n_steps, int* out_
   CTB_CUDA(cudaEventRecord(ev0_, stream_));
   for (int s = 0; s < n_steps; s++) CTB_CUDA(cudaGraphLaunch(graph_greedy_, stream_));
   CTB_CUDA(cudaEventRecord(ev1_, stream_));
-  CTB_CUDA(cudaMemcpyAsync(h_tokens_out_, d_tokens_out_, (size_t)n_steps * 4, cudaMemcpyDeviceToHost, stream_));
-  CTB_CUDA(cudaMemcpyAsync(h_logits_, d_logits_, (size_t)hp_.n_vocab * 4, cudaMemcpyDeviceToHost, stream_));
-  CTB_CUDA(cudaMemcpyAsync(h_embd_, d_embd_, (size_t)hp_.n_embd * 4, cudaMemcpyDeviceToHost, stream_));
+  CTB_CUDA(cudaMemcpyAsync(h_tokens_out_.get(), d_tokens_out_.get(), (size_t)n_steps * 4, cudaMemcpyDeviceToHost, stream_));
+  CTB_CUDA(cudaMemcpyAsync(h_logits_.get(), d_logits_, (size_t)hp_.n_vocab * 4, cudaMemcpyDeviceToHost, stream_));
+  CTB_CUDA(cudaMemcpyAsync(h_embd_.get(), d_embd_, (size_t)hp_.n_embd * 4, cudaMemcpyDeviceToHost, stream_));
   CTB_CUDA(cudaMemcpyAsync(d_logits_keep_, d_logits_, (size_t)hp_.n_vocab * 4, cudaMemcpyDeviceToDevice, stream_));
   CTB_CUDA(cudaMemcpyAsync(d_embd_keep_, d_embd_, (size_t)hp_.n_embd * 4, cudaMemcpyDeviceToDevice, stream_));
   CTB_CUDA(cudaStreamSynchronize(stream_));
   host_fresh_ = true;
-  memcpy(out_tokens, h_tokens_out_, (size_t)n_steps * 4);
+  memcpy(out_tokens, h_tokens_out_.get(), (size_t)n_steps * 4);
   float ms = 0;
   cudaEventElapsedTime(&ms, ev0_, ev1_);
   stats.last_eval_ms = ms;

@@ -13,6 +13,7 @@
 #include <string>
 #include <vector>
 
+#include "cuda_owned.cuh"
 #include "device_types.cuh"
 #include "gguf.hpp"
 
@@ -50,6 +51,7 @@ struct LayerW {
 
 struct Phase;    // stream.cuh: one phase of the persistent step kernel
 struct StepOp;   // engine.cu: one op of the per-token schedule
+struct ProfMark; // engine.cu: an event recorded behind a kernel of profile_step, and the kernel's class
 struct MVParams;
 struct Uploader;
 struct PrefillState;
@@ -137,8 +139,8 @@ class Engine {
   // Host views of the last token's logits / hidden state (the reference hands out ctx->logits.data(), mutable by the caller,
   // llama.cc:47-51).  Until a caller asks for one, nothing is copied per eval (lazy); from the first request on every eval
   // refreshes them, because the caller may keep the pointer.
-  float* logits() { host_views(); return h_logits_; }
-  float* embeddings() { host_views(); return h_embd_; }
+  float* logits() { host_views(); return h_logits_.as<float>(); }
+  float* embeddings() { host_views(); return h_embd_.as<float>(); }
   bool lazy_logits() const { return !eager_; }
   std::vector<float> logits_copy();   // this eval's logits without switching the engine to eager host views
   // Device half of the sampler (sample_gpu.cuh): candidates >= the k-th largest penalised logit.  Returns their count, or -1
@@ -152,20 +154,20 @@ class Engine {
   cudaStream_t stream() const { return stream_; }
 
  private:
+  Engine(const HParams& hp, int device, const TPShard& tp);   // (the public constructor delegates here first: see engine.cu)
   HParams hp_;
   TPShard tp_;
   int nh_ = 0, nkv_ = 0, nff_ = 0;   // this rank's query heads, KV heads and n_ff slice (the whole model when world == 1)
-  void tp_all_reduce(float* buf, int n);
+  void tp_all_reduce(float* buf, int n, cudaStream_t st);
   // fused exchange (stream.cuh: XchgParams): this rank's region  uint2 ll[2][world][n_embd]  and every peer's, IPC-mapped
   bool tp_peer_ = false;
   uint8_t* xc_region_ = nullptr;
   uint2* xc_ll_[8] = {nullptr};
   void tp_setup_peer();
   int device_ = 0;
-  cudaStream_t stream_ = nullptr;
-  bool own_stream_ = true;
+  Stream stream_;
   // arena
-  uint8_t* arena_ = nullptr;
+  DevMem arena_;
   size_t arena_size_ = 0, arena_used_ = 0;
   void* alloc(size_t bytes, size_t align = 256);
 
@@ -182,34 +184,29 @@ class Engine {
   int* d_state_ = nullptr;     // {token, n_past}
   float *xa_ = nullptr, *xb_ = nullptr, *qkv_ = nullptr, *attn_ = nullptr, *attn_o_ = nullptr, *ffn_ = nullptr, *ffn2_ = nullptr, *d_logits_ = nullptr, *d_embd_ = nullptr, *d_logits_keep_ = nullptr, *d_embd_keep_ = nullptr;
   // host (pinned) results
-  float *h_logits_ = nullptr, *h_embd_ = nullptr;
-  int* h_state_ = nullptr;     // pinned ring of {token, n_past}
-  int h_state_cap_ = 0;
-  long h_state_next_ = 0;
+  HostMem h_logits_, h_embd_;
+  StateRing step_ring_;        // {token, n_past} of the single-token steps
   void put_step(int token, int pos, int n_total);   // the next ring entry {token, pos, 0, n_total} to d_state_, on the stream
-  int* h_tokens_out_ = nullptr;
-  int* d_tokens_out_ = nullptr;
+  HostMem h_tokens_out_;
+  DevMem d_tokens_out_;
   int tokens_out_cap_ = 0;
 
-  cudaGraphExec_t graph_full_ = nullptr, graph_nolog_ = nullptr, graph_greedy_ = nullptr;
-  cudaEvent_t ev0_ = nullptr, ev1_ = nullptr, ev_pick_ = nullptr;
+  Event ev0_, ev1_, ev_pick_;
   // speculative next step (see after_eval)
   bool spec_on_ = true, spec_pending_ = false;
   bool spec_deferred_ = false;   // a look-ahead step is due but waits for the device sampler to be enqueued first
   bool sampler_mode_ = false;    // the caller's last sample() ran the device sampler kernel (not the greedy pick)
-  cudaEvent_t ev_sample_ = nullptr;
+  Event ev_sample_;
   void launch_deferred_spec();
   int spec_pos_ = -1, spec_streak_ = 0;
   void drop_lookahead();         // forget the look-ahead and the streak that earned it (a step already enqueued still runs)
   int kv_high_ = 0;              // one past the highest position any eval has written
-  int* h_spec_tok_ = nullptr;
-  int* h_dbg_ = nullptr;         // host-mapped watchdog words of the persistent kernels
+  HostMem h_spec_tok_;
+  HostMem h_dbg_;                // host-mapped watchdog words of the persistent kernels
   void after_eval(int next_pos);
   int sm_count_ = 132;
-  long launches_per_step_ = 0;
 
   void init(const GGUFFile& g);
-  void release();
   // rows [row0, row1) and K range [k0, k1) of the tensor (defaults: all of it); the shape check is against the FULL tensor
   DevMat upload_matrix(const GGUFTensor& t, struct Uploader& up, int want_K, int want_M, int row0 = 0, int row1 = -1, int k0 = 0, int k1 = -1);
   const float* upload_vector(const GGUFFile& g, const std::string& name, bool required, int want_n);
@@ -228,18 +225,19 @@ class Engine {
   void build_ops();
   void push_matvec(struct MVParams& p, int kind);
   void upload_prog(Phase* dst, int* dst_bounds, const std::vector<StepOp>& ops);
-  void enqueue_ops(const std::vector<StepOp>& ops, const Phase* d_prog, const int* d_bounds, int n);
+  long enqueue_ops(const std::vector<StepOp>& ops, const Phase* d_prog, const int* d_bounds, int n, cudaStream_t st, bool fused,
+                   std::vector<ProfMark>* marks = nullptr);
   void build_graphs();
-  void destroy_graphs();
   bool eager_ = false;           // host logits / embeddings are refreshed by every eval
   bool host_fresh_ = true;
   void host_views();
   // the device sampler's buffers, allocated on first use outside the arena for n_seq rows, the same layout on the device and
   // in pinned memory: every slot's greedy pick (int[n_seq][2]), the results (SampleGpuOut[n_seq]), the argument block
-  uint8_t *d_sample_ = nullptr, *h_sample_ = nullptr;
+  DevMem d_sample_;
+  HostMem h_sample_;
   void sample_enqueue(const SampleRow* rows, int R, const float* logits, size_t stride, bool picks);
   // batched prefill (prefill.cuh): built on first use
-  struct PrefillState* pf_ = nullptr;
+  std::unique_ptr<PrefillState> pf_;
   bool multi_ready();            // hp_.multi and the multi-sequence program is built
   void need_multi();             // throws unless multi_ready()
   bool prefill_on_ = true;       // CTB_NO_PREFILL=1: prompts run through the single-token kernel
@@ -250,38 +248,37 @@ class Engine {
   void prefill_batch(const int* tokens, const int* pos, const int* n_total, int n, bool last, bool rows = false);
   // rows of an eval (RowSink), allocated on first use outside the arena: d_rows_ holds up to PB_T rows on their way out
   const RowSink* sink_ = nullptr;
-  float* d_rows_ = nullptr;
+  DevMem d_rows_;
   int rows_pending_ = 0, rows_done_ = 0;
   int rows_n_ = 0;
-  uint8_t *d_score_ = nullptr, *h_score_ = nullptr;   // [cap] doubles logprob, [cap] ints target, [cap] ints greedy; device and pinned
+  DevMem d_score_;               // [cap] doubles logprob, [cap] ints target, [cap] ints greedy; device and pinned
+  HostMem h_score_;
   int score_cap_ = 0;
   double* d_lp_ = nullptr;
   int *d_tgt_ = nullptr, *d_gr_ = nullptr;
-  void rows_begin(const RowSink* rows, int n);
+  struct SinkGuard { Engine* e; ~SinkGuard() { e->sink_ = nullptr; } };
+  SinkGuard rows_begin(const RowSink* rows, int n);   // the eval's sink, released when the guard goes (also when the eval throws)
   void rows_finish();                        // enqueue the scores' copy to the host (before finish_eval's event)
   void rows_take(const float* src, int m);   // m rows at src (n_vocab apart) leave for the sink
   void rows_push(const float* row);          // one row through d_rows_
   void rows_drain();
-  void rows_end();                           // after the stream is synchronised: the scores to the caller; the sink is released
+  void rows_end();                           // after the stream is synchronised: the scores to the caller
   bool ensure_rows_prog();
   void decode_one(int token, int pos, int n_total, bool with_logits);
   void head_from(const float* row);   // the output head (un-fused, as the single-token schedule launches it) on one hidden row
   void finish_eval(int next_pos, bool hit);
   enum : int { MVK_QKV = 0, MVK_WO = 1, MVK_UP = 2, MVK_DOWN = 3, MVK_OUT = 4 };   // which projection a mat-vec launch is
-  bool profiling_ = false;
   bool pdl_ = true;              // programmatic dependent launch between the kernels of a step (CTB_NO_PDL=1 turns it off)
-  std::vector<cudaEvent_t> prof_ev_;
-  std::vector<int> prof_kind_;
-  void mark(int kind);
   // sequence states
-  uint8_t* h_stage_ = nullptr;   // pinned staging of state_save / state_load, grown on demand
-  size_t stage_cap_ = 0;
-  uint8_t* stage(size_t bytes);
-  KvCopy *d_copies_ = nullptr, *h_copies_ = nullptr;   // kv_reparent's copy list (n_seq entries), device and pinned
+  HostMem h_stage_;              // pinned staging of state_save / state_load, grown on demand
+  DevMem d_copies_;              // kv_reparent's copy list (n_seq entries), device and pinned
+  HostMem h_copies_;
   void kv_slot_elems(size_t& k, size_t& v) const;   // halves of one slot's K and V regions
   void zero_slot(int slot);                         // zero the slot's K and V regions, on the stream
   float* results_of(int slot, float** embd);        // where the slot's last logits / embeddings live on the device
   void copy_results(int src, int dst);              // multi-sequence: dst takes src's last logits, embeddings and greedy pick
+  // the step's graphs, declared last so that they go before the buffers they launch on
+  GraphExec graph_full_, graph_nolog_, graph_greedy_;
 };
 
 size_t engine_arena_bytes(const GGUFFile& g, const HParams& hp);

@@ -6,13 +6,13 @@
 #include <cstring>
 #include <ctime>
 #include <functional>
-#include <memory>
 #include <stdexcept>
 #include <string>
 #include <vector>
 
 #include "../../include/ctransformers_b200.h"
 #include "attention.cuh"
+#include "cuda_owned.cuh"
 #include "matvec.cuh"
 #include "prefill.cuh"
 #include "repack.cuh"
@@ -31,14 +31,6 @@ namespace {
     cudaError_t e__ = (expr);                                                                              \
     if (e__ != cudaSuccess) throw std::runtime_error(std::string("CUDA error: ") + cudaGetErrorString(e__) + " (" #expr ")"); \
   } while (0)
-
-struct DevBuf {
-  void* p = nullptr;
-  explicit DevBuf(size_t n) { OPS_CUDA(cudaMalloc(&p, n ? n : 1)); }
-  ~DevBuf() { if (p) cudaFree(p); }
-  DevBuf(const DevBuf&) = delete;
-  template <typename T> T* as() const { return (T*)p; }
-};
 
 struct OpsTables {
   uint16_t *silu = nullptr, *gelu = nullptr, *ex = nullptr;
@@ -72,36 +64,32 @@ int block_elems(int type) {
   return (type == GT_Q4_0 || type == GT_Q5_0 || type == GT_Q8_0 || type == GT_Q4_1 || type == GT_Q5_1) ? 32 : 1;
 }
 
-struct OwnedMat {
-  DevMat m;
-  std::vector<void*> bufs;
-  ~OwnedMat() { for (void* b : bufs) cudaFree(b); }
-};
-
-void upload(OwnedMat& o, int type, const void* blocks, int K, int M) {
+// the matrix in the engine's device layout, its planes in buffers that `keep` owns
+DevMat upload(std::vector<DevMem>& keep, int type, const void* blocks, int K, int M) {
   if (K % block_elems(type)) throw std::runtime_error("K is not a multiple of the block size");
   const size_t bytes = raw_row_bytes(type, K) * M;
-  DevBuf raw(bytes);
-  OPS_CUDA(cudaMemcpy(raw.p, blocks, bytes, cudaMemcpyHostToDevice));
-  o.m.type = type; o.m.K = K; o.m.M = M; o.m.nb = K / block_elems(type); o.m.bytes = bytes;
+  DevMem raw(bytes);
+  OPS_CUDA(cudaMemcpy(raw.get(), blocks, bytes, cudaMemcpyHostToDevice));
+  DevMat m;
+  m.type = type; m.K = K; m.M = M; m.nb = K / block_elems(type); m.bytes = bytes;
   if (type_is_kquant(type)) {   // the stream layout of the step kernel
-    const size_t sb = st_matrix_bytes(type, M, o.m.nb);
-    uint16_t* st = nullptr;
-    OPS_CUDA(cudaMalloc((void**)&st, sb));
-    o.bufs.push_back(st);
-    k_repack_stream<<<(int)std::min<size_t>((sb / 2 + 255) / 256, 4096), 256>>>(type, raw.as<uint8_t>(), M, o.m.nb, st);
+    const size_t sb = st_matrix_bytes(type, M, m.nb);
+    keep.emplace_back(sb);
+    uint16_t* st = keep.back().as<uint16_t>();
+    k_repack_stream<<<(int)std::min<size_t>((sb / 2 + 255) / 256, 4096), 256>>>(type, raw.as<uint8_t>(), M, m.nb, st);
     OPS_CUDA(cudaDeviceSynchronize());
-    o.m.st = (const uint8_t*)st;
-    return;
+    m.st = (const uint8_t*)st;
+    return m;
   }
-  const PlaneSizes ps = plane_sizes(type, M, o.m.nb, bytes);
+  const PlaneSizes ps = plane_sizes(type, M, m.nb, bytes);
   uint16_t* pl[4] = {nullptr, nullptr, nullptr, nullptr};
   const size_t sz[4] = {ps.qs, ps.qh, ps.d, ps.mn};
   for (int i = 0; i < 4; i++)
-    if (sz[i]) { OPS_CUDA(cudaMalloc((void**)&pl[i], sz[i])); o.bufs.push_back(pl[i]); }
+    if (sz[i]) { keep.emplace_back(sz[i]); pl[i] = keep.back().as<uint16_t>(); }
   k_repack<<<(int)std::min<size_t>((bytes / 2 + 255) / 256, 4096), 256>>>(type, raw.as<uint16_t>(), bytes / 2, pl[0], pl[1], pl[2], pl[3]);
   OPS_CUDA(cudaDeviceSynchronize());
-  o.m.qs = (const uint8_t*)pl[0]; o.m.qh = (const uint8_t*)pl[1]; o.m.d = pl[2]; o.m.mn = pl[3];
+  m.qs = (const uint8_t*)pl[0]; m.qh = (const uint8_t*)pl[1]; m.d = pl[2]; m.mn = pl[3];
+  return m;
 }
 
 int sm_count() {
@@ -122,12 +110,12 @@ void run_phases(std::vector<Phase> phs) {
   unsigned* d_sync = sync_words();
   const StepLaunch L = step_launch_shape(phs.data(), (int)phs.size(), sm_count(), max_dyn_smem(k_step<true, false, false>));
   const std::vector<int> hb = step_bounds(phs.data(), (int)phs.size(), L.grid);
-  DevBuf dbounds(hb.size() * 4);
-  OPS_CUDA(cudaMemcpy(dbounds.p, hb.data(), hb.size() * 4, cudaMemcpyHostToDevice));
+  DevMem dbounds(hb.size() * 4);
+  OPS_CUDA(cudaMemcpy(dbounds.get(), hb.data(), hb.size() * 4, cudaMemcpyHostToDevice));
   if (L.n_slots < ST_W) throw std::runtime_error("rows too long for the step kernel's shared memory");
   OPS_CUDA(step_set_smem_limit(L.smem));
-  DevBuf dprog((phs.size() + 1) * sizeof(Phase));
-  OPS_CUDA(cudaMemcpy(dprog.p, phs.data(), phs.size() * sizeof(Phase), cudaMemcpyHostToDevice));
+  DevMem dprog((phs.size() + 1) * sizeof(Phase));
+  OPS_CUDA(cudaMemcpy(dprog.get(), phs.data(), phs.size() * sizeof(Phase), cudaMemcpyHostToDevice));
   OPS_CUDA(launch_step(L, 0, dprog.as<Phase>(), dbounds.as<int>(), (int)phs.size(), d_sync));
   OPS_CUDA(cudaGetLastError());
   OPS_CUDA(cudaDeviceSynchronize());
@@ -195,12 +183,12 @@ int guarded(const char* what, const std::function<void()>& fn) {
 }
 
 void stage_to_host(const float* x, const float* w, const float* b, float* y_norm, int mode, float eps, int K, int act, std::vector<uint8_t>& dump) {
-  DevBuf dx((size_t)K * 4), dw((size_t)K * 4), db((size_t)K * 4), dy((size_t)K * 4);
-  OPS_CUDA(cudaMemcpy(dx.p, x, (size_t)K * 4, cudaMemcpyHostToDevice));
-  if (w) OPS_CUDA(cudaMemcpy(dw.p, w, (size_t)K * 4, cudaMemcpyHostToDevice));
-  if (b) OPS_CUDA(cudaMemcpy(db.p, b, (size_t)K * 4, cudaMemcpyHostToDevice));
+  DevMem dx((size_t)K * 4), dw((size_t)K * 4), db((size_t)K * 4), dy((size_t)K * 4);
+  OPS_CUDA(cudaMemcpy(dx.get(), x, (size_t)K * 4, cudaMemcpyHostToDevice));
+  if (w) OPS_CUDA(cudaMemcpy(dw.get(), w, (size_t)K * 4, cudaMemcpyHostToDevice));
+  if (b) OPS_CUDA(cudaMemcpy(db.get(), b, (size_t)K * 4, cudaMemcpyHostToDevice));
   const size_t n = act_smem_bytes(act, K);
-  DevBuf dd(n);
+  DevMem dd(n);
   if (n > 48 * 1024) OPS_CUDA(cudaFuncSetAttribute(k_stage_dump, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)n));
   MVParams q{};
   q.x = dx.as<float>(); q.norm_w = w ? dw.as<float>() : nullptr; q.norm_b = b ? db.as<float>() : nullptr; q.norm_out = dy.as<float>();
@@ -208,8 +196,8 @@ void stage_to_host(const float* x, const float* w, const float* b, float* y_norm
   k_stage_dump<<<1, MV_THREADS, n>>>(q, act, dd.as<uint8_t>());
   OPS_CUDA(cudaGetLastError());
   dump.resize(n);
-  OPS_CUDA(cudaMemcpy(dump.data(), dd.p, n, cudaMemcpyDeviceToHost));
-  if (y_norm) OPS_CUDA(cudaMemcpy(y_norm, dy.p, (size_t)K * 4, cudaMemcpyDeviceToHost));
+  OPS_CUDA(cudaMemcpy(dump.data(), dd.get(), n, cudaMemcpyDeviceToHost));
+  if (y_norm) OPS_CUDA(cudaMemcpy(y_norm, dy.get(), (size_t)K * 4, cudaMemcpyDeviceToHost));
 }
 
 // KV caches in the reference's layouts (K [pos][n_kv*hd], V transposed [n_kv*hd][v_ld]), positions [0, n_pos)  <->  the
@@ -236,10 +224,10 @@ void kv_from_device(const std::vector<uint16_t>& kp, const std::vector<uint16_t>
 
 // k_argmax over n device logits, as Engine::after_eval launches it: {pick, logits equal to the picked one}
 void argmax_on_device(const float* d_logits, int n, int* pick2) {
-  DevBuf dout(8);
+  DevMem dout(8);
   k_argmax<<<1, ARGMAX_THREADS>>>(d_logits, n, dout.as<int>());
   OPS_CUDA(cudaGetLastError());
-  OPS_CUDA(cudaMemcpy(pick2, dout.p, 8, cudaMemcpyDeviceToHost));
+  OPS_CUDA(cudaMemcpy(pick2, dout.get(), 8, cudaMemcpyDeviceToHost));
 }
 
 // k_sample_topk over rows rows[0 ..) of a [rows][n] device buffer in one launch, as Engine::multi_sample launches it: result i is
@@ -256,11 +244,11 @@ std::vector<SampleGpuOut> topk_rows_on_device(const float* d_logits, int n, cons
     const int q = rows[r];
     sg_put(blk.data(), R, r, q, last_tokens + last_off[q], last_off[q + 1] - last_off[q], penalty[q], k[q], n);
   }
-  DevBuf dblk(blk.size() * 4), dout((size_t)R * sizeof(SampleGpuOut));
-  OPS_CUDA(cudaMemcpy(dblk.p, blk.data(), blk.size() * 4, cudaMemcpyHostToDevice));
+  DevMem dblk(blk.size() * 4), dout((size_t)R * sizeof(SampleGpuOut));
+  OPS_CUDA(cudaMemcpy(dblk.get(), blk.data(), blk.size() * 4, cudaMemcpyHostToDevice));
   sg_launch(sg_rows(dblk.as<int>(), R, d_logits, (size_t)n, dout.as<SampleGpuOut>()), R, n, 0);
   OPS_CUDA(cudaGetLastError());
-  OPS_CUDA(cudaMemcpy(o.data(), dout.p, (size_t)R * sizeof(SampleGpuOut), cudaMemcpyDeviceToHost));
+  OPS_CUDA(cudaMemcpy(o.data(), dout.get(), (size_t)R * sizeof(SampleGpuOut), cudaMemcpyDeviceToHost));
   return o;
 }
 
@@ -284,17 +272,17 @@ extern "C" {
 
 int ctb_mul_mat(int type, const void* w_blocks, const float* x, float* dst, int K, int M, int N) {
   return guarded("ctb_mul_mat", [&] {
-    OwnedMat w;
-    upload(w, type, w_blocks, K, M);
-    DevBuf dx((size_t)K * N * 4), dy((size_t)M * N * 4);
-    OPS_CUDA(cudaMemcpy(dx.p, x, (size_t)K * N * 4, cudaMemcpyHostToDevice));
+    std::vector<DevMem> keep;
+    const DevMat w = upload(keep, type, w_blocks, K, M);
+    DevMem dx((size_t)K * N * 4), dy((size_t)M * N * 4);
+    OPS_CUDA(cudaMemcpy(dx.get(), x, (size_t)K * N * 4, cudaMemcpyHostToDevice));
     for (int n = 0; n < N; n++) {
       MVParams p{};
       p.x = dx.as<float>() + (size_t)n * K; p.norm_mode = NORM_NONE; p.K = K; p.act = act_format_for(type); p.nseg = 1;
-      p.seg[0].w = w.m; p.seg[0].out = dy.as<float>() + (size_t)n * M; p.seg[0].epi = EPI_STORE;
+      p.seg[0].w = w; p.seg[0].out = dy.as<float>() + (size_t)n * M; p.seg[0].epi = EPI_STORE;
       run_matvec(p);
     }
-    OPS_CUDA(cudaMemcpy(dst, dy.p, (size_t)M * N * 4, cudaMemcpyDeviceToHost));
+    OPS_CUDA(cudaMemcpy(dst, dy.get(), (size_t)M * N * 4, cudaMemcpyDeviceToHost));
   });
 }
 
@@ -369,19 +357,19 @@ int ctb_norm_path(int path, int mode, const float* x, const float* w, const floa
     if (n < 256 || n % 256) throw std::runtime_error("the step kernel takes n a positive multiple of 256");
     // one mat-vec phase of the step kernel over 16 all-zero Q4_K rows: what is checked is the normalised vector CTA 0 writes
     const std::vector<uint8_t> zeros(raw_row_bytes(GT_Q4_K, n) * 16, 0);
-    OwnedMat wm;
-    upload(wm, GT_Q4_K, zeros.data(), n, 16);
-    DevBuf dx((size_t)n * 4), dw((size_t)n * 4), db((size_t)n * 4), dy((size_t)n * 4), dout(16 * 4);
-    OPS_CUDA(cudaMemcpy(dx.p, x, (size_t)n * 4, cudaMemcpyHostToDevice));
-    if (w) OPS_CUDA(cudaMemcpy(dw.p, w, (size_t)n * 4, cudaMemcpyHostToDevice));
-    if (b) OPS_CUDA(cudaMemcpy(db.p, b, (size_t)n * 4, cudaMemcpyHostToDevice));
+    std::vector<DevMem> keep;
+    const DevMat wm = upload(keep, GT_Q4_K, zeros.data(), n, 16);
+    DevMem dx((size_t)n * 4), dw((size_t)n * 4), db((size_t)n * 4), dy((size_t)n * 4), dout(16 * 4);
+    OPS_CUDA(cudaMemcpy(dx.get(), x, (size_t)n * 4, cudaMemcpyHostToDevice));
+    if (w) OPS_CUDA(cudaMemcpy(dw.get(), w, (size_t)n * 4, cudaMemcpyHostToDevice));
+    if (b) OPS_CUDA(cudaMemcpy(db.get(), b, (size_t)n * 4, cudaMemcpyHostToDevice));
     MVParams p{};
     p.x = dx.as<float>(); p.norm_w = w ? dw.as<float>() : nullptr; p.norm_b = b && mode == NORM_LAYER ? db.as<float>() : nullptr;
     p.norm_out = dy.as<float>(); p.norm_mode = mode; p.eps = eps; p.K = n; p.act = ACT_Q8_K; p.nseg = 1;
-    p.seg[0].w = wm.m; p.seg[0].out = dout.as<float>(); p.seg[0].epi = EPI_STORE;
+    p.seg[0].w = wm; p.seg[0].out = dout.as<float>(); p.seg[0].epi = EPI_STORE;
     p.silu_tab = tables().silu; p.gelu_tab = tables().gelu;
     run_phases({matvec_phase(p)});
-    OPS_CUDA(cudaMemcpy(y, dy.p, (size_t)n * 4, cudaMemcpyDeviceToHost));
+    OPS_CUDA(cudaMemcpy(y, dy.get(), (size_t)n * 4, cudaMemcpyDeviceToHost));
   });
 }
 
@@ -390,12 +378,12 @@ int ctb_rope(float* x, int n_heads, int head_dim, int pos, int mode, float freq_
     const int half = head_dim / 2;
     const std::vector<float2> tab = rope_table(pos + 1, head_dim, head_dim, freq_base, freq_scale);
     const size_t nq = (size_t)n_heads * head_dim;
-    DevBuf dq(nq * 4), dtab(tab.size() * 8);
-    OPS_CUDA(cudaMemcpy(dq.p, x, nq * 4, cudaMemcpyHostToDevice));
-    OPS_CUDA(cudaMemcpy(dtab.p, tab.data(), tab.size() * 8, cudaMemcpyHostToDevice));
+    DevMem dq(nq * 4), dtab(tab.size() * 8);
+    OPS_CUDA(cudaMemcpy(dq.get(), x, nq * 4, cudaMemcpyHostToDevice));
+    OPS_CUDA(cudaMemcpy(dtab.get(), tab.data(), tab.size() * 8, cudaMemcpyHostToDevice));
     k_rope_dump<<<n_heads, half>>>(dq.as<float>(), dtab.as<float2>(), pos, head_dim, (mode & 2) ? 1 : 0);
     OPS_CUDA(cudaGetLastError());
-    OPS_CUDA(cudaMemcpy(x, dq.p, nq * 4, cudaMemcpyDeviceToHost));
+    OPS_CUDA(cudaMemcpy(x, dq.get(), nq * 4, cudaMemcpyDeviceToHost));
   });
 }
 
@@ -417,15 +405,15 @@ int ctb_attention(const float* q, const uint16_t* kcache, const uint16_t* vcache
         vcur[(size_t)kh * head_dim + e] = __half2float(__ushort_as_half(vcache[((size_t)kh * head_dim + e) * T + pos]));
       }
     std::vector<float2> ident((size_t)n_total * (head_dim / 2), make_float2(1.f, 0.f));
-    DevBuf dq(nq * 4), dk(kp.size() * 2), dv(vp.size() * 2), dout(nq * 4), dst(16), dkc(kcur.size() * 4), dvc(vcur.size() * 4), dtab(ident.size() * 8);
-    OPS_CUDA(cudaMemcpy(dq.p, q, nq * 4, cudaMemcpyHostToDevice));
-    OPS_CUDA(cudaMemcpy(dk.p, kp.data(), kp.size() * 2, cudaMemcpyHostToDevice));
-    OPS_CUDA(cudaMemcpy(dv.p, vp.data(), vp.size() * 2, cudaMemcpyHostToDevice));
-    OPS_CUDA(cudaMemcpy(dkc.p, kcur.data(), kcur.size() * 4, cudaMemcpyHostToDevice));
-    OPS_CUDA(cudaMemcpy(dvc.p, vcur.data(), vcur.size() * 4, cudaMemcpyHostToDevice));
-    OPS_CUDA(cudaMemcpy(dtab.p, ident.data(), ident.size() * 8, cudaMemcpyHostToDevice));
+    DevMem dq(nq * 4), dk(kp.size() * 2), dv(vp.size() * 2), dout(nq * 4), dst(16), dkc(kcur.size() * 4), dvc(vcur.size() * 4), dtab(ident.size() * 8);
+    OPS_CUDA(cudaMemcpy(dq.get(), q, nq * 4, cudaMemcpyHostToDevice));
+    OPS_CUDA(cudaMemcpy(dk.get(), kp.data(), kp.size() * 2, cudaMemcpyHostToDevice));
+    OPS_CUDA(cudaMemcpy(dv.get(), vp.data(), vp.size() * 2, cudaMemcpyHostToDevice));
+    OPS_CUDA(cudaMemcpy(dkc.get(), kcur.data(), kcur.size() * 4, cudaMemcpyHostToDevice));
+    OPS_CUDA(cudaMemcpy(dvc.get(), vcur.data(), vcur.size() * 4, cudaMemcpyHostToDevice));
+    OPS_CUDA(cudaMemcpy(dtab.get(), ident.data(), ident.size() * 8, cudaMemcpyHostToDevice));
     const int st[4] = {0, pos, 0, n_total};
-    OPS_CUDA(cudaMemcpy(dst.p, st, 16, cudaMemcpyHostToDevice));
+    OPS_CUDA(cudaMemcpy(dst.get(), st, 16, cudaMemcpyHostToDevice));
     AttnParams ap{};
     ap.q = dq.as<float>(); ap.k = dkc.as<float>(); ap.v = dvc.as<float>(); ap.kc = dk.as<uint16_t>(); ap.vc = dv.as<uint16_t>();
     ap.out = dout.as<float>(); ap.exp_tab = tables().ex; ap.rope = dtab.as<float2>(); ap.state = dst.as<int>(); ap.kq_scale = kq_scale;
@@ -434,7 +422,7 @@ int ctb_attention(const float* q, const uint16_t* kcache, const uint16_t* vcache
     OPS_CUDA(cudaFuncSetAttribute(attn_kernel(head_dim), cudaFuncAttributeMaxDynamicSharedMemorySize, (int)std::max<size_t>(smem, 48 * 1024)));
     attn_kernel(head_dim)<<<dim3(n_head, 1, attn_groups(head_dim)), ATTN_THREADS, smem>>>(ap);
     OPS_CUDA(cudaGetLastError());
-    OPS_CUDA(cudaMemcpy(out, dout.p, nq * 4, cudaMemcpyDeviceToHost));
+    OPS_CUDA(cudaMemcpy(out, dout.get(), nq * 4, cudaMemcpyDeviceToHost));
   });
 }
 
@@ -460,16 +448,16 @@ int ctb_attention_path(int path, const float* q, const float* k_new, const float
       st[(size_t)i * 4 + 1] = pos0 + k; st[(size_t)i * 4 + 3] = n_total[k];
     }
     if (path == 3) st[(size_t)PB_T * 4] = n_tok;
-    DevBuf dq(nq * n_tok * 4), dk(nkv * n_tok * 4), dv(nkv * n_tok * 4), dkc(kp.size() * 2), dvc(vp.size() * 2), dout(nq * n_tok * 4),
+    DevMem dq(nq * n_tok * 4), dk(nkv * n_tok * 4), dv(nkv * n_tok * 4), dkc(kp.size() * 2), dvc(vp.size() * 2), dout(nq * n_tok * 4),
         dtab(tab.size() * 8), dst(st.size() * 4);
-    OPS_CUDA(cudaMemcpy(dq.p, q, nq * n_tok * 4, cudaMemcpyHostToDevice));
-    OPS_CUDA(cudaMemcpy(dk.p, k_new, nkv * n_tok * 4, cudaMemcpyHostToDevice));
-    OPS_CUDA(cudaMemcpy(dv.p, v_new, nkv * n_tok * 4, cudaMemcpyHostToDevice));
-    OPS_CUDA(cudaMemcpy(dkc.p, kp.data(), kp.size() * 2, cudaMemcpyHostToDevice));
-    OPS_CUDA(cudaMemcpy(dvc.p, vp.data(), vp.size() * 2, cudaMemcpyHostToDevice));
-    OPS_CUDA(cudaMemcpy(dtab.p, tab.data(), tab.size() * 8, cudaMemcpyHostToDevice));
-    OPS_CUDA(cudaMemcpy(dst.p, st.data(), st.size() * 4, cudaMemcpyHostToDevice));
-    OPS_CUDA(cudaMemset(dout.p, 0, nq * n_tok * 4));
+    OPS_CUDA(cudaMemcpy(dq.get(), q, nq * n_tok * 4, cudaMemcpyHostToDevice));
+    OPS_CUDA(cudaMemcpy(dk.get(), k_new, nkv * n_tok * 4, cudaMemcpyHostToDevice));
+    OPS_CUDA(cudaMemcpy(dv.get(), v_new, nkv * n_tok * 4, cudaMemcpyHostToDevice));
+    OPS_CUDA(cudaMemcpy(dkc.get(), kp.data(), kp.size() * 2, cudaMemcpyHostToDevice));
+    OPS_CUDA(cudaMemcpy(dvc.get(), vp.data(), vp.size() * 2, cudaMemcpyHostToDevice));
+    OPS_CUDA(cudaMemcpy(dtab.get(), tab.data(), tab.size() * 8, cudaMemcpyHostToDevice));
+    OPS_CUDA(cudaMemcpy(dst.get(), st.data(), st.size() * 4, cudaMemcpyHostToDevice));
+    OPS_CUDA(cudaMemset(dout.get(), 0, nq * n_tok * 4));
     AttnParams ap{};
     ap.q = dq.as<float>(); ap.k = dk.as<float>(); ap.v = dv.as<float>(); ap.kc = dkc.as<uint16_t>(); ap.vc = dvc.as<uint16_t>();
     ap.out = dout.as<float>(); ap.exp_tab = tables().ex; ap.rope = dtab.as<float2>(); ap.state = dst.as<int>(); ap.kq_scale = kq_scale;
@@ -484,8 +472,8 @@ int ctb_attention_path(int path, const float* q, const float* k_new, const float
       ph.at = ap; ph.state = dst.as<int>();
       PPhase prog[2] = {ph, ph};
       prog[0].kind = PP_KV; prog[1].kind = PP_ATTN;
-      DevBuf dprog(sizeof(prog));
-      OPS_CUDA(cudaMemcpy(dprog.p, prog, sizeof(prog), cudaMemcpyHostToDevice));
+      DevMem dprog(sizeof(prog));
+      OPS_CUDA(cudaMemcpy(dprog.get(), prog, sizeof(prog), cudaMemcpyHostToDevice));
       OPS_CUDA(pstep_set_smem_limit(smem));
       OPS_CUDA(launch_pstep(sm_count(), n_slots, smem, 0, dprog.as<PPhase>(), 2, sync_words()));
     } else {   // one launch per token, in order, like decode_one
@@ -511,9 +499,9 @@ int ctb_attention_path(int path, const float* q, const float* k_new, const float
       }
     }
     OPS_CUDA(cudaDeviceSynchronize());
-    OPS_CUDA(cudaMemcpy(out, dout.p, nq * n_tok * 4, cudaMemcpyDeviceToHost));
-    OPS_CUDA(cudaMemcpy(kp.data(), dkc.p, kp.size() * 2, cudaMemcpyDeviceToHost));
-    OPS_CUDA(cudaMemcpy(vp.data(), dvc.p, vp.size() * 2, cudaMemcpyDeviceToHost));
+    OPS_CUDA(cudaMemcpy(out, dout.get(), nq * n_tok * 4, cudaMemcpyDeviceToHost));
+    OPS_CUDA(cudaMemcpy(kp.data(), dkc.get(), kp.size() * 2, cudaMemcpyDeviceToHost));
+    OPS_CUDA(cudaMemcpy(vp.data(), dvc.get(), vp.size() * 2, cudaMemcpyDeviceToHost));
     kv_from_device(kp, vp, n_kv, hd, n_ctx, kcache, vcache);
   });
 }
@@ -544,25 +532,23 @@ int ctb_prefill_mul_mat(int nseg, const int* types, const void* const* w_blocks,
     int slots = 0;
     size_t smem = 0;
     if (!pstep_shape(pb_work_bytes(K, n_ctx, head_dim), slots, smem)) throw std::runtime_error("no batched prefill at this n_ctx: its attention scratch does not fit");
-    std::unique_ptr<OwnedMat> mats[MV_MAX_SEG];
-    for (int s = 0; s < nseg; s++) {
-      mats[s].reset(new OwnedMat());
-      upload(*mats[s], types[s], w_blocks[s], K, rows[s]);
-    }
+    std::vector<DevMem> keep;
+    DevMat mats[MV_MAX_SEG];
+    for (int s = 0; s < nseg; s++) mats[s] = upload(keep, types[s], w_blocks[s], K, rows[s]);
     // PB_T-row token buffers, reused by every launch like the engine's batched buffers (rows past a short batch keep the previous
     // launch's values), and the QUANT phase's qbuf zeroed like the engine's
-    DevBuf dx((size_t)PB_T * K * 4), dx2((size_t)PB_T * K * 4), dout((size_t)PB_T * W * 4), dres((size_t)PB_T * W * 4), dres2((size_t)PB_T * W * 4),
+    DevMem dx((size_t)PB_T * K * 4), dx2((size_t)PB_T * K * 4), dout((size_t)PB_T * W * 4), dres((size_t)PB_T * W * 4), dres2((size_t)PB_T * W * 4),
         dnw((size_t)K * 4), dnb((size_t)K * 4), dq(pb_qbuf_bytes(K)), dst((PB_T * 4 + 4) * 4);
-    OPS_CUDA(cudaMemset(dq.p, 0, pb_qbuf_bytes(K)));
-    OPS_CUDA(cudaMemset(dout.p, 0, (size_t)PB_T * W * 4));
-    if (norm_w) OPS_CUDA(cudaMemcpy(dnw.p, norm_w, (size_t)K * 4, cudaMemcpyHostToDevice));
-    if (norm_b) OPS_CUDA(cudaMemcpy(dnb.p, norm_b, (size_t)K * 4, cudaMemcpyHostToDevice));
+    OPS_CUDA(cudaMemset(dq.get(), 0, pb_qbuf_bytes(K)));
+    OPS_CUDA(cudaMemset(dout.get(), 0, (size_t)PB_T * W * 4));
+    if (norm_w) OPS_CUDA(cudaMemcpy(dnw.get(), norm_w, (size_t)K * 4, cudaMemcpyHostToDevice));
+    if (norm_b) OPS_CUDA(cudaMemcpy(dnb.get(), norm_b, (size_t)K * 4, cudaMemcpyHostToDevice));
     MVParams m{};
     m.x = dx.as<float>(); m.x2 = x2 ? dx2.as<float>() : nullptr; m.x_mode = x2 ? 1 : 0;
     m.norm_w = norm_w ? dnw.as<float>() : nullptr; m.norm_b = norm_b ? dnb.as<float>() : nullptr; m.norm_mode = norm_mode; m.eps = eps;
     m.K = K; m.act = ACT_Q8_K; m.nseg = nseg; m.silu_tab = tables().silu; m.gelu_tab = tables().gelu;
     for (int s = 0; s < nseg; s++) {
-      m.seg[s].w = mats[s]->m; m.seg[s].out = dout.as<float>() + off[s]; m.seg[s].epi = epi[s];
+      m.seg[s].w = mats[s]; m.seg[s].out = dout.as<float>() + off[s]; m.seg[s].epi = epi[s];
       if (epi[s] == EPI_ADD || epi[s] == EPI_ADD2) m.seg[s].res = dres.as<float>() + off[s];
       if (epi[s] == EPI_ADD2) m.seg[s].res2 = dres2.as<float>() + off[s];
     }
@@ -577,8 +563,8 @@ int ctb_prefill_mul_mat(int nseg, const int* types, const void* const* w_blocks,
     };
     std::vector<PPhase> prog;
     pb_matvec_phases(m, dq.as<uint8_t>(), dst.as<int>(), bat, prog);
-    DevBuf dprog((prog.size() + 1) * sizeof(PPhase));
-    OPS_CUDA(cudaMemcpy(dprog.p, prog.data(), prog.size() * sizeof(PPhase), cudaMemcpyHostToDevice));
+    DevMem dprog((prog.size() + 1) * sizeof(PPhase));
+    OPS_CUDA(cudaMemcpy(dprog.get(), prog.data(), prog.size() * sizeof(PPhase), cudaMemcpyHostToDevice));
     OPS_CUDA(pstep_set_smem_limit(smem));
     // launches of at most PB_T tokens over the same program and buffers, as eval_list cuts a run of prompt tokens
     for (int b = 0; b < n_tok; b += PB_T) {
@@ -589,14 +575,14 @@ int ctb_prefill_mul_mat(int nseg, const int* types, const void* const* w_blocks,
         st[i * 4 + 1] = b + k; st[i * 4 + 3] = b + k + 1;
       }
       st[PB_T * 4] = n;
-      OPS_CUDA(cudaMemcpy(dst.p, st.data(), st.size() * 4, cudaMemcpyHostToDevice));
-      OPS_CUDA(cudaMemcpy(dx.p, x + (size_t)b * K, (size_t)n * K * 4, cudaMemcpyHostToDevice));
-      if (x2) OPS_CUDA(cudaMemcpy(dx2.p, x2 + (size_t)b * K, (size_t)n * K * 4, cudaMemcpyHostToDevice));
-      if (res) OPS_CUDA(cudaMemcpy(dres.p, res + (size_t)b * W, (size_t)n * W * 4, cudaMemcpyHostToDevice));
-      if (res2) OPS_CUDA(cudaMemcpy(dres2.p, res2 + (size_t)b * W, (size_t)n * W * 4, cudaMemcpyHostToDevice));
+      OPS_CUDA(cudaMemcpy(dst.get(), st.data(), st.size() * 4, cudaMemcpyHostToDevice));
+      OPS_CUDA(cudaMemcpy(dx.get(), x + (size_t)b * K, (size_t)n * K * 4, cudaMemcpyHostToDevice));
+      if (x2) OPS_CUDA(cudaMemcpy(dx2.get(), x2 + (size_t)b * K, (size_t)n * K * 4, cudaMemcpyHostToDevice));
+      if (res) OPS_CUDA(cudaMemcpy(dres.get(), res + (size_t)b * W, (size_t)n * W * 4, cudaMemcpyHostToDevice));
+      if (res2) OPS_CUDA(cudaMemcpy(dres2.get(), res2 + (size_t)b * W, (size_t)n * W * 4, cudaMemcpyHostToDevice));
       OPS_CUDA(launch_pstep(sm_count(), slots, smem, 0, dprog.as<PPhase>(), (int)prog.size(), sync_words(), pstep_q3(prog)));
       OPS_CUDA(cudaDeviceSynchronize());
-      OPS_CUDA(cudaMemcpy(out + (size_t)b * W, dout.p, (size_t)n * W * 4, cudaMemcpyDeviceToHost));
+      OPS_CUDA(cudaMemcpy(out + (size_t)b * W, dout.get(), (size_t)n * W * 4, cudaMemcpyDeviceToHost));
     }
     if (n_slots) *n_slots = slots;
   });
@@ -604,15 +590,14 @@ int ctb_prefill_mul_mat(int nseg, const int* types, const void* const* w_blocks,
 
 int ctb_ffn_gate(int type, const void* w1_blocks, const void* w3_blocks, const float* x, float* out, int K, int M) {
   return guarded("ctb_ffn_gate", [&] {
-    OwnedMat w1, w3;
-    upload(w1, type, w1_blocks, K, M);
-    upload(w3, type, w3_blocks, K, M);
-    DevBuf dx((size_t)K * 4), dg((size_t)M * 4), du((size_t)M * 4), dy((size_t)M * 4);
-    OPS_CUDA(cudaMemcpy(dx.p, x, (size_t)K * 4, cudaMemcpyHostToDevice));
+    std::vector<DevMem> keep;
+    const DevMat w1 = upload(keep, type, w1_blocks, K, M), w3 = upload(keep, type, w3_blocks, K, M);
+    DevMem dx((size_t)K * 4), dg((size_t)M * 4), du((size_t)M * 4), dy((size_t)M * 4);
+    OPS_CUDA(cudaMemcpy(dx.get(), x, (size_t)K * 4, cudaMemcpyHostToDevice));
     // as the engine does it: gate and up rows in one launch, SiLU(gate)*up where the down projection stages its input
     MVParams p{};
     p.x = dx.as<float>(); p.norm_mode = NORM_NONE; p.K = K; p.act = act_format_for(type); p.nseg = 2;
-    p.seg[0].w = w1.m; p.seg[0].out = dg.as<float>(); p.seg[0].epi = EPI_SILU; p.seg[1].w = w3.m; p.seg[1].out = du.as<float>();
+    p.seg[0].w = w1; p.seg[0].out = dg.as<float>(); p.seg[0].epi = EPI_SILU; p.seg[1].w = w3; p.seg[1].out = du.as<float>();
     run_matvec(p);
     const size_t smem = (size_t)M * 4 + 64;
     OPS_CUDA(cudaFuncSetAttribute(k_gate_dump, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)std::max<size_t>(smem, 48 * 1024)));
@@ -620,7 +605,7 @@ int ctb_ffn_gate(int type, const void* w1_blocks, const void* w3_blocks, const f
     q.x = dg.as<float>(); q.x2 = du.as<float>(); q.x_mode = 1; q.norm_mode = NORM_NONE; q.K = M;
     k_gate_dump<<<1, MV_THREADS, smem>>>(q, dy.as<float>());
     OPS_CUDA(cudaGetLastError());
-    OPS_CUDA(cudaMemcpy(out, dy.p, (size_t)M * 4, cudaMemcpyDeviceToHost));
+    OPS_CUDA(cudaMemcpy(out, dy.get(), (size_t)M * 4, cudaMemcpyDeviceToHost));
   });
 }
 
@@ -654,14 +639,14 @@ int ctb_matvec_partition(const int* types, const int* rows, int nseg, int K, int
 int ctb_get_row(int type, const void* table_blocks, int K, int n_rows, int row, float* out) {
   return guarded("ctb_get_row", [&] {
     const size_t rb = raw_row_bytes(type, K);
-    DevBuf dt(rb * n_rows), dtok(4), dout((size_t)K * 4);
-    OPS_CUDA(cudaMemcpy(dt.p, table_blocks, rb * n_rows, cudaMemcpyHostToDevice));
-    OPS_CUDA(cudaMemcpy(dtok.p, &row, 4, cudaMemcpyHostToDevice));
+    DevMem dt(rb * n_rows), dtok(4), dout((size_t)K * 4);
+    OPS_CUDA(cudaMemcpy(dt.get(), table_blocks, rb * n_rows, cudaMemcpyHostToDevice));
+    OPS_CUDA(cudaMemcpy(dtok.get(), &row, 4, cudaMemcpyHostToDevice));
     EmbedParams em{};
     em.table = dt.as<uint8_t>(); em.row_bytes = rb; em.tokens = dtok.as<int>(); em.out = dout.as<float>(); em.type = type; em.K = K; em.n_vocab = n_rows;
     k_embed<<<1, 256>>>(em);
     OPS_CUDA(cudaGetLastError());
-    OPS_CUDA(cudaMemcpy(out, dout.p, (size_t)K * 4, cudaMemcpyDeviceToHost));
+    OPS_CUDA(cudaMemcpy(out, dout.get(), (size_t)K * 4, cudaMemcpyDeviceToHost));
   });
 }
 
@@ -669,8 +654,8 @@ int ctb_argmax_path(int path, const float* logits, int n, int* out) {
   return guarded("ctb_argmax_path", [&] {
     if (path < 0 || path > 1) throw std::runtime_error("unknown argmax path " + std::to_string(path));
     if (n < 1) throw std::runtime_error("no logits");
-    DevBuf dlog((size_t)n * 4);
-    OPS_CUDA(cudaMemcpy(dlog.p, logits, (size_t)n * 4, cudaMemcpyHostToDevice));
+    DevMem dlog((size_t)n * 4);
+    OPS_CUDA(cudaMemcpy(dlog.get(), logits, (size_t)n * 4, cudaMemcpyHostToDevice));
     if (path == 0) {
       argmax_on_device(dlog.as<float>(), n, out);
       return;
@@ -678,14 +663,14 @@ int ctb_argmax_path(int path, const float* logits, int n, int* out) {
     // one PH_PICK phase of the step kernel on the decode state out[0..4], as the last phase of the engine's step program
     const int step = out[2];
     if (step < 0 || step >= (1 << 20)) throw std::runtime_error("step out of range");
-    DevBuf dstate(5 * 4), dtok((size_t)(step + 1) * 4);
-    OPS_CUDA(cudaMemcpy(dstate.p, out, 5 * 4, cudaMemcpyHostToDevice));
-    OPS_CUDA(cudaMemset(dtok.p, 0xff, (size_t)(step + 1) * 4));
+    DevMem dstate(5 * 4), dtok((size_t)(step + 1) * 4);
+    OPS_CUDA(cudaMemcpy(dstate.get(), out, 5 * 4, cudaMemcpyHostToDevice));
+    OPS_CUDA(cudaMemset(dtok.get(), 0xff, (size_t)(step + 1) * 4));
     Phase ph{};
     ph.kind = PH_PICK;
     ph.pk.logits = dlog.as<float>(); ph.pk.state = dstate.as<int>(); ph.pk.out_tokens = dtok.as<int>(); ph.pk.n = n;
     run_phases({ph});
-    OPS_CUDA(cudaMemcpy(out, dstate.p, 5 * 4, cudaMemcpyDeviceToHost));
+    OPS_CUDA(cudaMemcpy(out, dstate.get(), 5 * 4, cudaMemcpyDeviceToHost));
     OPS_CUDA(cudaMemcpy(out + 5, dtok.as<int>() + step, 4, cudaMemcpyDeviceToHost));
   });
 }
@@ -694,8 +679,8 @@ int ctb_sample_topk(const float* logits, int n, const int* last_tokens, int n_la
   int count = -1;
   const int rc = guarded("ctb_sample_topk", [&] {
     if (n < 1 || !sg_accepts(n_last, k)) throw std::runtime_error("n < 1, or a window or k the device sampler does not take");
-    DevBuf dlog((size_t)n * 4);
-    OPS_CUDA(cudaMemcpy(dlog.p, logits, (size_t)n * 4, cudaMemcpyHostToDevice));
+    DevMem dlog((size_t)n * 4);
+    OPS_CUDA(cudaMemcpy(dlog.get(), logits, (size_t)n * 4, cudaMemcpyHostToDevice));
     const SampleGpuOut o = topk_on_device(dlog.as<float>(), n, last_tokens, n_last, repetition_penalty, k);
     if (o.nan) { count = -2; return; }
     count = o.count;
@@ -711,8 +696,8 @@ int ctb_sample_device(const float* logits, int n, const int* last_tokens, int n_
     if (n < 1) throw std::runtime_error("no logits");
     if (seed < 0) seed = (int)time(nullptr);
     std::mt19937 rng((unsigned)seed);
-    DevBuf dlog((size_t)n * 4);
-    OPS_CUDA(cudaMemcpy(dlog.p, logits, (size_t)n * 4, cudaMemcpyHostToDevice));
+    DevMem dlog((size_t)n * 4);
+    OPS_CUDA(cudaMemcpy(dlog.get(), logits, (size_t)n * 4, cudaMemcpyHostToDevice));
     bool dev = false;
     tok = sample_lazy(
         n, last_tokens, n_last, top_k, top_p, temperature, repetition_penalty, rng, dev,
@@ -740,8 +725,8 @@ int ctb_sample_topk_rows(const float* logits, int n_rows, int n, const int* last
       count[r] = -1;
       if (sg_accepts(last_off[r + 1] - last_off[r], k[r])) rows.push_back(r);
     }
-    DevBuf dlog((size_t)n_rows * n * 4);
-    OPS_CUDA(cudaMemcpy(dlog.p, logits, (size_t)n_rows * n * 4, cudaMemcpyHostToDevice));
+    DevMem dlog((size_t)n_rows * n * 4);
+    OPS_CUDA(cudaMemcpy(dlog.get(), logits, (size_t)n_rows * n * 4, cudaMemcpyHostToDevice));
     const std::vector<SampleGpuOut> o = topk_rows_on_device(dlog.as<float>(), n, rows, last_off, last_tokens, repetition_penalty, k);
     for (size_t i = 0; i < rows.size(); i++) {
       const int r = rows[i];
@@ -758,8 +743,8 @@ int ctb_sample_device_rows(const float* logits, int n_rows, int n, const int* la
                            const float* temperature, const float* repetition_penalty, const int* seed, int* tokens, int* used_device) {
   return guarded("ctb_sample_device_rows", [&] {
     check_rows(n_rows, n, last_off, last_tokens);
-    DevBuf dlog((size_t)n_rows * n * 4);
-    OPS_CUDA(cudaMemcpy(dlog.p, logits, (size_t)n_rows * n * 4, cudaMemcpyHostToDevice));
+    DevMem dlog((size_t)n_rows * n * 4);
+    OPS_CUDA(cudaMemcpy(dlog.get(), logits, (size_t)n_rows * n * 4, cudaMemcpyHostToDevice));
     // the device half as ctb_multi_sample_many runs it: every row's pick, one top-k launch over the rows that need a cut
     std::vector<int> picks((size_t)2 * n_rows), rows, row_of(n_rows, -1);
     for (int r = 0; r < n_rows; r++) {
@@ -789,13 +774,13 @@ int ctb_row_logprob(const float* rows, int n_rows, int n_vocab, const int* targe
     if (n_rows < 1 || n_vocab < 1) throw std::runtime_error("no rows");
     for (int r = 0; r < n_rows; r++)
       if (targets[r] < -1 || targets[r] >= n_vocab) throw std::runtime_error("target " + std::to_string(targets[r]) + " of row " + std::to_string(r) + " is out of range");
-    DevBuf drows((size_t)n_rows * n_vocab * 4), dt((size_t)n_rows * 4), dlp((size_t)n_rows * 8), dg((size_t)n_rows * 4);
-    OPS_CUDA(cudaMemcpy(drows.p, rows, (size_t)n_rows * n_vocab * 4, cudaMemcpyHostToDevice));
-    OPS_CUDA(cudaMemcpy(dt.p, targets, (size_t)n_rows * 4, cudaMemcpyHostToDevice));
+    DevMem drows((size_t)n_rows * n_vocab * 4), dt((size_t)n_rows * 4), dlp((size_t)n_rows * 8), dg((size_t)n_rows * 4);
+    OPS_CUDA(cudaMemcpy(drows.get(), rows, (size_t)n_rows * n_vocab * 4, cudaMemcpyHostToDevice));
+    OPS_CUDA(cudaMemcpy(dt.get(), targets, (size_t)n_rows * 4, cudaMemcpyHostToDevice));
     rl_launch(drows.as<float>(), n_rows, n_vocab, dt.as<int>(), dlp.as<double>(), dg.as<int>(), 0);
     OPS_CUDA(cudaGetLastError());
-    OPS_CUDA(cudaMemcpy(logprob, dlp.p, (size_t)n_rows * 8, cudaMemcpyDeviceToHost));
-    OPS_CUDA(cudaMemcpy(greedy, dg.p, (size_t)n_rows * 4, cudaMemcpyDeviceToHost));
+    OPS_CUDA(cudaMemcpy(logprob, dlp.get(), (size_t)n_rows * 8, cudaMemcpyDeviceToHost));
+    OPS_CUDA(cudaMemcpy(greedy, dg.get(), (size_t)n_rows * 4, cudaMemcpyDeviceToHost));
   });
 }
 
