@@ -104,19 +104,19 @@ using DevMem = Mem<false>;
 using HostMem = Mem<true>;
 
 // The pinned entries (cap of them, `ints` ints each) through which launch state reaches one device target: put() fills the next
-// entry and copies it to the target on the stream.  The copy runs later, so an entry is reused only after the copy that read
-// it has run: when the ring wraps, it first synchronises the stream.
+// entry and copies its first n ints to the target on the stream.  The copy runs later, so an entry is reused only after the
+// copy that read it has run: when the ring wraps, it first synchronises the stream.
 class StateRing {
  public:
   StateRing() = default;
   StateRing(int* target, int ints, int cap) : h_((size_t)ints * cap * 4), d_(target), ints_(ints), cap_(cap) {}
   template <typename Fill>
-  cudaError_t put(cudaStream_t s, Fill&& fill) {
+  cudaError_t put(cudaStream_t s, int n, Fill&& fill) {
     if (next_ > 0 && next_ % cap_ == 0)
       if (const cudaError_t e = cudaStreamSynchronize(s)) return e;
     int* e = h_.as<int>() + (size_t)(next_++ % cap_) * ints_;
     fill(e);
-    return cudaMemcpyAsync(d_, e, (size_t)ints_ * 4, cudaMemcpyHostToDevice, s);
+    return cudaMemcpyAsync(d_, e, (size_t)n * 4, cudaMemcpyHostToDevice, s);
   }
 
  private:

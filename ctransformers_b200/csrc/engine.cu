@@ -63,50 +63,31 @@ struct StepOp {
 // advance the on-device decode state after k_argmax's greedy pick (state[4])
 __global__ void k_advance(int* state, int* out_tokens) { advance_state(state, out_tokens, state[4]); }
 
-// one program of the batched kernel (k_pstep): its phases on the host, their device copy, and whether it holds Q3_K matrices
-// (the k_pstep<true> build)
-struct PProg {
-  std::vector<PPhase> phases;
-  DevMem d;
-  bool q3 = false;
-};
-
-// ---- batched prefill (prefill.cuh): the per-token schedule rewritten over PB_T-row buffers
+// ---- batched prefill (prefill.cuh): the per-token schedule rewritten over PB_T-row buffers, as one program of k_pstep: the
+// body, then, when the output head is a K-quant, its QUANT + GEMM phases over every token of the launch (logits rows in
+// Engine::d_rows_, embeddings rows in embd_rows).  A launch runs the body alone or the whole program.
 struct PrefillState {
   std::vector<DevMem> bufs;         // the batched buffers and the QUANT phases' scratch (dalloc)
-  PProg prog;
-  int* d_state = nullptr;           // [PB_T][4] + n_tok
+  std::vector<PPhase> phases;
+  DevMem d_phases;                  // their device copy (zeroed one phase past the end)
+  int n_body = 0;                   // phases of the body: all of them when the head has no phases here
+  bool q3_body = false, q3_all = false;   // the body / the whole program holds Q3_K matrices: the k_pstep<true> build
+  int* d_state = nullptr;           // PB_STATE_MS ints: [PB_T][4] + n_tok, the slot strides, each token's slot (PB_S)
   StateRing ring;                   // d_state of each launch, PF_RING launches deep
   float* x_final = nullptr;         // batched buffer that holds the last layer's output rows
+  float* embd_rows = nullptr;       // [PB_T][n_embd]: the head's QUANT phase writes every token's embeddings (the MS builds)
   int n_slots = 0;
   size_t smem = 0;
   bool ok = false, tried = false;
-  // multi-sequence mode (HParams::multi): the same program on slot-addressed state (k_pstep<.., true>), plus the output head
-  PProg mprog;
-  int* d_mstate = nullptr;          // PB_STATE_MS ints
-  StateRing mring;                  // d_mstate of each launch, PF_RING launches deep
-  bool mhead = false;               // K-quant head: its QUANT + GEMM phases end the launch, every token's row in logits_b / embd_b
-  float *logits_b = nullptr, *embd_b = nullptr;
-  float *d_mlogits = nullptr, *d_membd = nullptr;   // [n_seq][n_vocab], [n_seq][n_embd]: each slot's last results
-  int* d_mpick = nullptr;                           // [n_seq][2]: k_argmax of each slot's logits
-  long m_launches = 0;
-  // rows of every token (RowSink), single sequence: the single-sequence program followed by a K-quant head's QUANT + GEMM phases,
-  // every token's logits row of a launch in Engine::d_rows_ (built on first use)
-  PProg rprog;
-  bool rtried = false;
+  long m_launches = 0;              // multi-sequence launches
   void* dalloc(size_t bytes) {      // zeroed device memory, freed with the state
     bufs.emplace_back(bytes);
     CTB_CUDA(cudaMemset(bufs.back().get(), 0, bytes));
     return bufs.back().get();
   }
-  void upload(PProg& p) {           // p.phases to the device (zeroed one phase past the end)
-    p.q3 = pstep_q3(p.phases);
-    p.d = DevMem((p.phases.size() + 1) * sizeof(PPhase));
-    CTB_CUDA(cudaMemset(p.d.get(), 0, (p.phases.size() + 1) * sizeof(PPhase)));
-    CTB_CUDA(cudaMemcpy(p.d.get(), p.phases.data(), p.phases.size() * sizeof(PPhase), cudaMemcpyHostToDevice));
-  }
-  cudaError_t launch(const PProg& p, int grid, cudaStream_t st, unsigned* d_sync, bool multi = false) const {
-    return launch_pstep(grid, n_slots, smem, st, p.d.as<PPhase>(), (int)p.phases.size(), d_sync, p.q3, multi);
+  bool head() const { return n_body < (int)phases.size(); }
+  cudaError_t launch(bool whole, int grid, cudaStream_t st, unsigned* d_sync, bool multi) const {
+    return launch_pstep(grid, n_slots, smem, st, d_phases.as<PPhase>(), whole ? (int)phases.size() : n_body, d_sync, whole ? q3_all : q3_body, multi);
   }
 };
 constexpr int PF_RING = 64;
@@ -132,7 +113,8 @@ size_t engine_arena_bytes(const GGUFFile& g, const HParams& hp) {
   total += 3 * align_up(65536 * 2, 256);
   total += align_up((size_t)hp.n_ctx * (hp.head_dim() / 2) * 8, 256);
   const size_t qkv = (size_t)hp.n_embd + 2 * (size_t)hp.n_embd_gqa();
-  total += 4 * (2 * (size_t)hp.n_embd + qkv + 4 * (size_t)hp.n_embd + 2 * (size_t)hp.n_ff + 2 * (size_t)hp.n_vocab) + 64 * 256 + 8192;
+  total += 4 * (2 * (size_t)hp.n_embd + qkv + 3 * (size_t)hp.n_embd + 2 * (size_t)hp.n_ff + (size_t)hp.n_vocab) + 64 * 256 + 8192;
+  total += (size_t)hp.n_seq * (4 * ((size_t)hp.n_vocab + hp.n_embd) + 8) + 256;   // every slot's kept results
   total += ((size_t)hp.n_layer * 10 + 8) * (sizeof(Phase) * 2 + 2 * 1024) + 8192;   // the step programs and their per-CTA tile ranges
   total += 1 << 20;
   return total;
@@ -397,8 +379,13 @@ void Engine::init(const GGUFFile& g) {
   ffn2_ = (float*)alloc((size_t)nff_ * 4);
   d_logits_ = (float*)alloc((size_t)hp_.n_vocab * 4);
   d_embd_ = (float*)alloc(hp_.n_embd * 4);
-  d_logits_keep_ = (float*)alloc((size_t)hp_.n_vocab * 4);
-  d_embd_keep_ = (float*)alloc(hp_.n_embd * 4);
+  {
+    const size_t nl = (size_t)hp_.n_seq * hp_.n_vocab, ne = (size_t)hp_.n_seq * hp_.n_embd, bytes = (nl + ne) * 4 + (size_t)hp_.n_seq * 8;
+    kept_logits_ = (float*)alloc(bytes);
+    kept_embd_ = kept_logits_ + nl;
+    kept_pick_ = (int*)(kept_embd_ + ne);
+    CTB_CUDA(cudaMemset(kept_logits_, 0, bytes));
+  }
   d_sync_ = (unsigned*)alloc(64);
   CTB_CUDA(cudaMemset(d_state_, 0, 64));
   CTB_CUDA(cudaMemset(d_sync_, 0, 64));
@@ -929,15 +916,8 @@ int Engine::greedy_pick() {
   return pick[1] == 1 ? pick[0] : -1;
 }
 
-void Engine::eval(const int* tokens, int n, int n_past) {
-  if (n <= 0) return;
-  std::vector<int> pos(n), nt(n, n_past + n);   // n_total: row length of this eval's attention mat-muls
-  for (int i = 0; i < n; i++) pos[i] = n_past + i;
-  eval_list(tokens, pos.data(), nt.data(), n);
-}
-
 void Engine::put_step(int token, int pos, int n_total) {
-  CTB_CUDA(step_ring_.put(stream_, [&](int* st) { st[0] = token; st[1] = pos; st[2] = 0; st[3] = n_total; }));
+  CTB_CUDA(step_ring_.put(stream_, 4, [&](int* st) { st[0] = token; st[1] = pos; st[2] = 0; st[3] = n_total; }));
 }
 
 void Engine::decode_one(int token, int pos, int n_total, bool with_logits) {
@@ -958,8 +938,8 @@ void Engine::host_views() {
   eager_ = true;
   if (host_fresh_) return;
   DeviceGuard dev_guard(device_);
-  CTB_CUDA(cudaMemcpyAsync(h_logits_.get(), d_logits_keep_, (size_t)hp_.n_vocab * 4, cudaMemcpyDeviceToHost, stream_));
-  CTB_CUDA(cudaMemcpyAsync(h_embd_.get(), d_embd_keep_, (size_t)hp_.n_embd * 4, cudaMemcpyDeviceToHost, stream_));
+  CTB_CUDA(cudaMemcpyAsync(h_logits_.get(), kept_logits_, (size_t)hp_.n_vocab * 4, cudaMemcpyDeviceToHost, stream_));
+  CTB_CUDA(cudaMemcpyAsync(h_embd_.get(), kept_embd_, (size_t)hp_.n_embd * 4, cudaMemcpyDeviceToHost, stream_));
   CTB_CUDA(cudaStreamSynchronize(stream_));
   host_fresh_ = true;
 }
@@ -968,14 +948,14 @@ std::vector<float> Engine::logits_copy() {
   std::vector<float> v((size_t)hp_.n_vocab);
   if (host_fresh_) { memcpy(v.data(), h_logits_.get(), v.size() * 4); return v; }
   DeviceGuard dev_guard(device_);
-  CTB_CUDA(cudaMemcpyAsync(v.data(), d_logits_keep_, v.size() * 4, cudaMemcpyDeviceToHost, stream_));
+  CTB_CUDA(cudaMemcpyAsync(v.data(), kept_logits_, v.size() * 4, cudaMemcpyDeviceToHost, stream_));
   CTB_CUDA(cudaStreamSynchronize(stream_));
   return v;
 }
 
-// Upload the rows' argument block, launch k_sample_topk over them and copy their results back (with every slot's greedy pick when
-// `picks`), all on the engine stream; the caller synchronises.
-void Engine::sample_enqueue(const SampleRow* rows, int R, const float* logits, size_t stride, bool picks) {
+// Upload the rows' argument block, launch k_sample_topk over them (each on its slot's kept logits) and copy their results back
+// (with every slot's greedy pick when `picks`), all on the engine stream; the caller synchronises.
+void Engine::sample_enqueue(const SampleRow* rows, int R, bool picks) {
   const int S = hp_.n_seq;
   if (R < 0 || R > S) throw std::runtime_error("device sampler: " + std::to_string(R) + " rows for " + std::to_string(S) + " slots");
   const size_t picks_b = (size_t)S * 8, outs_b = (size_t)S * sizeof(SampleGpuOut);
@@ -993,11 +973,11 @@ void Engine::sample_enqueue(const SampleRow* rows, int R, const float* logits, s
   for (int r = 0; r < R; r++) sg_put(h_blk, R, r, rows[r].slot, rows[r].last, rows[r].n_last, rows[r].penalty, rows[r].k, hp_.n_vocab);
   if (R > 0) {
     CTB_CUDA(cudaMemcpyAsync(d_blk, h_blk, sg_block_ints(R, n_tok) * 4, cudaMemcpyHostToDevice, stream_));
-    sg_launch(sg_rows(d_blk, R, logits, stride, d_out), R, hp_.n_vocab, stream_);
+    sg_launch(sg_rows(d_blk, R, kept_logits_, (size_t)hp_.n_vocab, d_out), R, hp_.n_vocab, stream_);
     CTB_CUDA(cudaGetLastError());
   }
   // one copy back: the picks (first in the buffer) and then the R results
-  if (picks) CTB_CUDA(cudaMemcpyAsync(d_buf, pf_->d_mpick, picks_b, cudaMemcpyDeviceToDevice, stream_));
+  if (picks) CTB_CUDA(cudaMemcpyAsync(d_buf, kept_pick_, picks_b, cudaMemcpyDeviceToDevice, stream_));
   const size_t from = picks ? 0 : picks_b, to = picks_b + (size_t)R * sizeof(SampleGpuOut);
   if (to > from) CTB_CUDA(cudaMemcpyAsync(h_buf + from, d_buf + from, to - from, cudaMemcpyDeviceToHost, stream_));
 }
@@ -1007,7 +987,7 @@ int Engine::topk_candidates(const int* last, int n_last, float penalty, int k, i
   DeviceGuard dev_guard(device_);
   sampler_mode_ = true;
   const SampleRow row{0, last, n_last, penalty, k};
-  sample_enqueue(&row, 1, d_logits_keep_, 0, false);
+  sample_enqueue(&row, 1, false);
   CTB_CUDA(cudaEventRecord(ev_sample_, stream_));
   launch_deferred_spec();                          // the look-ahead step runs while the host finishes the draw
   CTB_CUDA(cudaEventSynchronize(ev_sample_));
@@ -1016,8 +996,8 @@ int Engine::topk_candidates(const int* last, int n_last, float penalty, int k, i
 
 void Engine::finish_eval(int next_pos, bool hit) {
   // the look-ahead step (after_eval) overwrites d_logits_ / d_embd_: keep this eval's results where a late request finds them
-  CTB_CUDA(cudaMemcpyAsync(d_logits_keep_, d_logits_, (size_t)hp_.n_vocab * 4, cudaMemcpyDeviceToDevice, stream_));
-  CTB_CUDA(cudaMemcpyAsync(d_embd_keep_, d_embd_, (size_t)hp_.n_embd * 4, cudaMemcpyDeviceToDevice, stream_));
+  CTB_CUDA(cudaMemcpyAsync(kept_logits_, d_logits_, (size_t)hp_.n_vocab * 4, cudaMemcpyDeviceToDevice, stream_));
+  CTB_CUDA(cudaMemcpyAsync(kept_embd_, d_embd_, (size_t)hp_.n_embd * 4, cudaMemcpyDeviceToDevice, stream_));
   if (eager_) {
     CTB_CUDA(cudaMemcpyAsync(h_logits_.get(), d_logits_, (size_t)hp_.n_vocab * 4, cudaMemcpyDeviceToHost, stream_));
     CTB_CUDA(cudaMemcpyAsync(h_embd_.get(), d_embd_, (size_t)hp_.n_embd * 4, cudaMemcpyDeviceToHost, stream_));
@@ -1099,32 +1079,10 @@ void Engine::score_kept(int target, double* logprob, int* greedy) {
   RowSink s;
   s.targets = &target; s.logprob = logprob; s.greedy = greedy;
   const SinkGuard sink = rows_begin(&s, 1);
-  rows_take(d_logits_keep_, 1);
+  rows_take(kept_logits_, 1);
   rows_finish();
   CTB_CUDA(cudaStreamSynchronize(stream_));
   rows_end();
-}
-
-// The single-sequence program followed by the output head's QUANT + GEMM phases, built the way ensure_prefill ends the
-// multi-sequence program: the head runs over every token of the launch and leaves its rows in d_rows_.  The embeddings stay the
-// last token's (head_from).  False for a head that is not a K-quant: its rows then come from head_from, one row at a time.
-bool Engine::ensure_rows_prog() {
-  PrefillState& P = *pf_;
-  if (P.rtried) return (bool)P.rprog.d;
-  P.rtried = true;
-  const StepOp& head = ops_[n_body_];
-  if (!head.stream) return false;
-  P.rprog.phases = P.prog.phases;
-  const float* hx = head.ph.mv.x;
-  auto bat = [&](const float* p, int& ld) -> float* {
-    if (!p) { ld = 0; return nullptr; }
-    if (p == hx) { ld = hp_.n_embd; return P.x_final; }
-    if (p == d_logits_) { ld = hp_.n_vocab; return d_rows_.as<float>(); }
-    throw std::runtime_error("rows: pointer outside the output head's buffers");
-  };
-  pb_matvec_phases(head.ph.mv, (uint8_t*)P.dalloc(pb_qbuf_bytes(head.ph.mv.K)), P.d_state, bat, P.rprog.phases);
-  P.upload(P.rprog);
-  return true;
 }
 
 void Engine::eval_list(const int* tokens, const int* pos, const int* n_total, int n, const RowSink* rows) {
@@ -1195,9 +1153,9 @@ bool Engine::ensure_prefill() {
       if (p >= m.lo && p < m.lo + m.n) { ld = m.ld; return m.b + (p - m.lo); }
     throw std::runtime_error("prefill: pointer outside the step workspace");
   };
-  P.d_state = (int*)P.dalloc((PB_T * 4 + 4) * 4);
-  P.ring = StateRing(P.d_state, PB_T * 4 + 4, PF_RING);
-  std::vector<PPhase>& prog = P.prog.phases;
+  P.d_state = (int*)P.dalloc(PB_STATE_MS * 4);
+  P.ring = StateRing(P.d_state, PB_STATE_MS, PF_RING);
+  std::vector<PPhase>& prog = P.phases;
   int K_max = 0;
   for (int i = 0; i < n_body_; i++) {
     const StepOp& op = ops_[i];
@@ -1223,29 +1181,21 @@ bool Engine::ensure_prefill() {
       pb_matvec_phases(op.ph.mv, (uint8_t*)P.dalloc(pb_qbuf_bytes(op.ph.mv.K)), P.d_state, bat, prog);
     }
   }
+  const StepOp& head = ops_[n_body_];
   int ld;
-  P.x_final = bat(ops_[n_body_].ph.mv.x, ld);
-  P.upload(P.prog);
-  if (hp_.multi) {
-    P.d_mstate = (int*)P.dalloc(PB_STATE_MS * 4);
-    P.mring = StateRing(P.d_mstate, PB_STATE_MS, PF_RING);
-    std::vector<PPhase>& mprog = P.mprog.phases;
-    mprog = prog;
-    for (PPhase& ph : mprog) { ph.state = P.d_mstate; ph.at.state = P.d_mstate; }
-    const StepOp& head = ops_[n_body_];
-    P.mhead = head.stream;
-    if (P.mhead) {   // the final norm (written as every token's embeddings) and the output matrix over every token of the launch
-      add(d_logits_, hp_.n_vocab); add(d_embd_, n_embd);
-      pb_matvec_phases(head.ph.mv, (uint8_t*)P.dalloc(pb_qbuf_bytes(head.ph.mv.K)), P.d_mstate, bat, mprog);
-      P.logits_b = bat(d_logits_, ld);
-      P.embd_b = bat(d_embd_, ld);
-      mprog[mprog.size() - 2].mv.norm_out = P.embd_b;
-    }
-    P.upload(P.mprog);
-    P.d_mlogits = (float*)P.dalloc((size_t)hp_.n_seq * hp_.n_vocab * 4);
-    P.d_membd = (float*)P.dalloc((size_t)hp_.n_seq * n_embd * 4);
-    P.d_mpick = (int*)P.dalloc((size_t)hp_.n_seq * 8);
+  P.x_final = bat(head.ph.mv.x, ld);
+  P.n_body = (int)prog.size();
+  P.q3_body = pstep_q3(prog);
+  if (head.stream) {   // a K-quant head: the final norm (written as every token's embeddings) and the output matrix over every token
+    maps.push_back({d_logits_, (size_t)hp_.n_vocab, (float*)d_rows_.grow((size_t)PB_T * hp_.n_vocab * 4), hp_.n_vocab});
+    pb_matvec_phases(head.ph.mv, (uint8_t*)P.dalloc(pb_qbuf_bytes(head.ph.mv.K)), P.d_state, bat, prog);
+    P.embd_rows = (float*)P.dalloc((size_t)PB_T * n_embd * 4);
+    prog[prog.size() - 2].mv.norm_out = P.embd_rows;
   }
+  P.q3_all = pstep_q3(prog);
+  P.d_phases = DevMem((prog.size() + 1) * sizeof(PPhase));
+  CTB_CUDA(cudaMemset(P.d_phases.get(), 0, (prog.size() + 1) * sizeof(PPhase)));
+  CTB_CUDA(cudaMemcpy(P.d_phases.get(), prog.data(), prog.size() * sizeof(PPhase), cudaMemcpyHostToDevice));
   if (!pstep_shape(pb_work_bytes(K_max, hp_.n_ctx, hp_.head_dim()), P.n_slots, P.smem)) return false;
   CTB_CUDA(pstep_set_smem_limit(P.smem));
   P.ok = true;
@@ -1254,23 +1204,17 @@ bool Engine::ensure_prefill() {
 
 // n <= PB_T tokens at consecutive positions through all layers in one launch; `last`: the list ends here, so the head
 // mat-vec (logits + final-norm hidden state of the last token) follows on the single-token kernel.
-// rows: every token's logits row goes to the sink (RowSink), from the launch itself (ensure_rows_prog) or from head_from per row.
+// rows: every token's logits row goes to the sink (RowSink), from the launch's head phases or, for a head that is not a K-quant,
+// from head_from per row.
 void Engine::prefill_batch(const int* tokens, const int* pos, const int* n_total, int n, bool last, bool rows) {
   PrefillState& P = *pf_;
-  const bool rp = rows && ensure_rows_prog();
-  if (rp) rows_drain();   // the launch writes d_rows_
-  CTB_CUDA(P.ring.put(stream_, [&](int* st) {
-    for (int i = 0; i < PB_T; i++) {
-      const int k = std::min(i, n - 1);
-      st[i * 4] = tokens[k]; st[i * 4 + 1] = pos[k]; st[i * 4 + 2] = 0; st[i * 4 + 3] = n_total[k];
-    }
-    st[PB_T * 4] = n;
-  }));
-  CTB_CUDA(P.launch(rp ? P.rprog : P.prog, step_grid_, stream_, d_sync_));
+  MultiTok toks[PB_T];
+  for (int i = 0; i < n; i++) toks[i] = MultiTok{0, tokens[i], pos[i], n_total[i], false};
+  const bool whole = rows && P.head();
+  launch_batch(toks, n, whole);
   prefill_launches_++;
-  if (rp) {
-    rows_pending_ = n;
-    rows_drain();
+  if (whole) {
+    rows_take(d_rows_.as<float>(), n);
   } else if (rows) {
     for (int r = 0; r < n; r++) {
       head_from(P.x_final + (size_t)r * hp_.n_embd);
@@ -1278,6 +1222,26 @@ void Engine::prefill_batch(const int* tokens, const int* pos, const int* n_total
     }
   }
   if (last) head_from(P.x_final + (size_t)(n - 1) * hp_.n_embd);
+}
+
+// One k_pstep launch of toks[0, n), n <= PB_T: the body, or with `whole` the whole program, whose head phases write every
+// token's logits row to d_rows_ (so the single-token rows still waiting there go to the sink first).  The launch state holds
+// the token entries (the last one repeated up to PB_T) and n; the multi-sequence build also reads the slot strides and each
+// token's slot, the single-sequence build only the first PB_S ints, which are all a single-sequence launch uploads.
+void Engine::launch_batch(const MultiTok* toks, int n, bool whole) {
+  PrefillState& P = *pf_;
+  if (whole) rows_drain();
+  size_t kslot, vslot;
+  kv_slot_elems(kslot, vslot);
+  CTB_CUDA(P.ring.put(stream_, hp_.multi ? PB_STATE_MS : PB_S, [&](int* st) {
+    for (int i = 0; i < PB_T; i++) {
+      const MultiTok& t = toks[std::min(i, n - 1)];
+      st[i * 4] = t.token; st[i * 4 + 1] = t.pos; st[i * 4 + 2] = 0; st[i * 4 + 3] = t.n_total;
+      st[PB_S + i] = t.slot;
+    }
+    st[PB_T * 4] = n; st[PB_T * 4 + 1] = (int)(unsigned)kslot; st[PB_T * 4 + 2] = (int)(unsigned)vslot; st[PB_T * 4 + 3] = 0;
+  }));
+  CTB_CUDA(P.launch(whole, step_grid_, stream_, d_sync_, hp_.multi));
 }
 
 void Engine::head_from(const float* row) {
@@ -1297,7 +1261,7 @@ std::string Engine::multi_refusal() {
   return "";
 }
 
-bool Engine::multi_ready() { return hp_.multi && ensure_prefill() && pf_->mprog.d; }
+bool Engine::multi_ready() { return hp_.multi && ensure_prefill(); }
 
 void Engine::need_multi() {
   if (!multi_ready()) throw std::runtime_error("this engine has no multi-sequence path");
@@ -1316,27 +1280,19 @@ void Engine::multi_eval(const std::vector<MultiTok>& toks, const std::vector<int
   for (size_t l = 0; l + 1 < starts.size(); l++) {
     const int a = starts[l], n = starts[l + 1] - a;
     if (n < 1 || n > PB_T) throw std::runtime_error("multi-sequence: bad launch size");
-    CTB_CUDA(P.mring.put(stream_, [&](int* st) {
-      for (int i = 0; i < PB_T; i++) {
-        const MultiTok& t = toks[a + std::min(i, n - 1)];
-        st[i * 4] = t.token; st[i * 4 + 1] = t.pos; st[i * 4 + 2] = 0; st[i * 4 + 3] = t.n_total;
-        st[PB_S + i] = t.slot;
-      }
-      st[PB_T * 4] = n; st[PB_T * 4 + 1] = (int)(unsigned)kslot; st[PB_T * 4 + 2] = (int)(unsigned)vslot; st[PB_T * 4 + 3] = 0;
-    }));
-    CTB_CUDA(P.launch(P.mprog, step_grid_, stream_, d_sync_, true));
+    launch_batch(&toks[a], n, P.head());
     P.m_launches++;
-    if (sink_ && P.mhead) rows_take(P.logits_b, n);   // every token's row of the launch
+    if (sink_ && P.head()) rows_take(d_rows_.as<float>(), n);   // every token's row of the launch
     for (int r = 0; r < n; r++) {
       const MultiTok& t = toks[a + r];
-      if (!t.last && !(sink_ && !P.mhead)) continue;   // (its logits, if the launch computed them, are dropped)
-      float* lg = P.d_mlogits + (size_t)t.slot * n_vocab;
-      float* em = P.d_membd + (size_t)t.slot * n_embd;
+      if (!t.last && !(sink_ && !P.head())) continue;   // (its logits, if the launch computed them, are dropped)
+      float* lg = kept_logits(t.slot);
+      float* em = kept_embd(t.slot);
       const float* lsrc = d_logits_;
       const float* esrc = d_embd_;
-      if (P.mhead) {
-        lsrc = P.logits_b + (size_t)r * n_vocab;
-        esrc = P.embd_b + (size_t)r * n_embd;
+      if (P.head()) {
+        lsrc = d_rows_.as<float>() + (size_t)r * n_vocab;
+        esrc = P.embd_rows + (size_t)r * n_embd;
       } else {
         head_from(P.x_final + (size_t)r * n_embd);   // a head that is not a K-quant: k_matvec, one row at a time
         if (sink_) rows_push(d_logits_);
@@ -1344,7 +1300,7 @@ void Engine::multi_eval(const std::vector<MultiTok>& toks, const std::vector<int
       if (!t.last) continue;
       CTB_CUDA(cudaMemcpyAsync(lg, lsrc, (size_t)n_vocab * 4, cudaMemcpyDeviceToDevice, stream_));
       CTB_CUDA(cudaMemcpyAsync(em, esrc, (size_t)n_embd * 4, cudaMemcpyDeviceToDevice, stream_));
-      k_argmax<<<1, ARGMAX_THREADS, 0, stream_>>>(lg, n_vocab, P.d_mpick + 2 * t.slot);
+      k_argmax<<<1, ARGMAX_THREADS, 0, stream_>>>(lg, n_vocab, kept_pick_ + 2 * t.slot);
       CTB_CUDA(cudaGetLastError());
     }
   }
@@ -1360,16 +1316,15 @@ void Engine::multi_eval(const std::vector<MultiTok>& toks, const std::vector<int
 void Engine::multi_fetch(int slot, float* logits, float* embd) {
   DeviceGuard dev_guard(device_);
   need_multi();
-  PrefillState& P = *pf_;
-  CTB_CUDA(cudaMemcpyAsync(logits, P.d_mlogits + (size_t)slot * hp_.n_vocab, (size_t)hp_.n_vocab * 4, cudaMemcpyDeviceToHost, stream_));
-  CTB_CUDA(cudaMemcpyAsync(embd, P.d_membd + (size_t)slot * hp_.n_embd, (size_t)hp_.n_embd * 4, cudaMemcpyDeviceToHost, stream_));
+  CTB_CUDA(cudaMemcpyAsync(logits, kept_logits(slot), (size_t)hp_.n_vocab * 4, cudaMemcpyDeviceToHost, stream_));
+  CTB_CUDA(cudaMemcpyAsync(embd, kept_embd(slot), (size_t)hp_.n_embd * 4, cudaMemcpyDeviceToHost, stream_));
   CTB_CUDA(cudaStreamSynchronize(stream_));
 }
 
 const SampleGpuOut* Engine::multi_sample(const SampleRow* rows, int R, int* picks) {
   DeviceGuard dev_guard(device_);
   need_multi();
-  sample_enqueue(rows, R, pf_->d_mlogits, (size_t)hp_.n_vocab, true);
+  sample_enqueue(rows, R, true);
   CTB_CUDA(cudaStreamSynchronize(stream_));
   memcpy(picks, h_sample_.get(), (size_t)hp_.n_seq * 8);
   return (const SampleGpuOut*)(h_sample_.as<uint8_t>() + (size_t)hp_.n_seq * 8);
@@ -1397,23 +1352,10 @@ void Engine::zero_slot(int slot) {
   CTB_CUDA(cudaMemsetAsync(vc_ + (size_t)slot * v, 0, v * 2, stream_));
 }
 
-float* Engine::results_of(int slot, float** embd) {
-  if (!hp_.multi) {
-    *embd = d_embd_keep_;
-    return d_logits_keep_;
-  }
-  need_multi();
-  *embd = pf_->d_membd + (size_t)slot * hp_.n_embd;
-  return pf_->d_mlogits + (size_t)slot * hp_.n_vocab;
-}
-
 void Engine::copy_results(int src, int dst) {
-  float *sem, *dem;
-  const float* slg = results_of(src, &sem);
-  float* dlg = results_of(dst, &dem);
-  CTB_CUDA(cudaMemcpyAsync(dlg, slg, (size_t)hp_.n_vocab * 4, cudaMemcpyDeviceToDevice, stream_));
-  CTB_CUDA(cudaMemcpyAsync(dem, sem, (size_t)hp_.n_embd * 4, cudaMemcpyDeviceToDevice, stream_));
-  CTB_CUDA(cudaMemcpyAsync(pf_->d_mpick + 2 * dst, pf_->d_mpick + 2 * src, 8, cudaMemcpyDeviceToDevice, stream_));
+  CTB_CUDA(cudaMemcpyAsync(kept_logits(dst), kept_logits(src), (size_t)hp_.n_vocab * 4, cudaMemcpyDeviceToDevice, stream_));
+  CTB_CUDA(cudaMemcpyAsync(kept_embd(dst), kept_embd(src), (size_t)hp_.n_embd * 4, cudaMemcpyDeviceToDevice, stream_));
+  CTB_CUDA(cudaMemcpyAsync(kept_pick_ + 2 * dst, kept_pick_ + 2 * src, 8, cudaMemcpyDeviceToDevice, stream_));
 }
 
 int Engine::state_k_stride() const { return k_stride(hp_.head_dim()); }
@@ -1452,10 +1394,8 @@ void Engine::state_save(int slot, int n_past, bool results, void* out) {
                                rows * hd, cudaMemcpyDeviceToHost, stream_));
   }
   if (results) {
-    float* em;
-    const float* lg = results_of(slot, &em);
-    CTB_CUDA(cudaMemcpyAsync(h + kb + vb, lg, (size_t)hp_.n_vocab * 4, cudaMemcpyDeviceToHost, stream_));
-    CTB_CUDA(cudaMemcpyAsync(h + kb + vb + (size_t)hp_.n_vocab * 4, em, (size_t)hp_.n_embd * 4, cudaMemcpyDeviceToHost, stream_));
+    CTB_CUDA(cudaMemcpyAsync(h + kb + vb, kept_logits(slot), (size_t)hp_.n_vocab * 4, cudaMemcpyDeviceToHost, stream_));
+    CTB_CUDA(cudaMemcpyAsync(h + kb + vb + (size_t)hp_.n_vocab * 4, kept_embd(slot), (size_t)hp_.n_embd * 4, cudaMemcpyDeviceToHost, stream_));
   }
   CTB_CUDA(cudaStreamSynchronize(stream_));
   zero_v_tail((uint16_t*)(h + kb), rows * hd, n_past);
@@ -1468,8 +1408,8 @@ void Engine::state_load(int slot, int n_past, bool results, const void* in, int 
   size_t kslot, vslot;
   kv_slot_elems(kslot, vslot);
   const size_t rows = (size_t)hp_.n_layer * nkv_, kb = rows * n_past * ks * 2, vb = rows * hd * v_pad(n_past) * 2;
-  float* em = nullptr;
-  float* lg = results ? results_of(slot, &em) : nullptr;
+  float* lg = kept_logits(slot);
+  float* em = kept_embd(slot);
   uint8_t* h = (uint8_t*)h_stage_.grow(std::max<size_t>(state_bytes(n_past, results), 1));
   memcpy(h, in, state_bytes(n_past, results));
   zero_v_tail((uint16_t*)(h + kb), rows * hd, n_past);
@@ -1485,7 +1425,7 @@ void Engine::state_load(int slot, int n_past, bool results, const void* in, int 
     CTB_CUDA(cudaMemcpyAsync(lg, h + kb + vb, (size_t)hp_.n_vocab * 4, cudaMemcpyHostToDevice, stream_));
     CTB_CUDA(cudaMemcpyAsync(em, h + kb + vb + (size_t)hp_.n_vocab * 4, (size_t)hp_.n_embd * 4, cudaMemcpyHostToDevice, stream_));
     if (hp_.multi) {
-      k_argmax<<<1, ARGMAX_THREADS, 0, stream_>>>(lg, hp_.n_vocab, pf_->d_mpick + 2 * slot);
+      k_argmax<<<1, ARGMAX_THREADS, 0, stream_>>>(lg, hp_.n_vocab, kept_pick_ + 2 * slot);
       CTB_CUDA(cudaGetLastError());
     }
   }
@@ -1576,7 +1516,7 @@ const float* Engine::multi_rows(int slot0, int n) {
   if (slot0 < 0 || n < 0 || slot0 + n > hp_.n_seq) throw std::runtime_error("multi_rows: slots out of range");
   const size_t b = (size_t)n * hp_.n_vocab * 4;
   float* h = (float*)h_stage_.grow(std::max<size_t>(b, 1));
-  CTB_CUDA(cudaMemcpyAsync(h, pf_->d_mlogits + (size_t)slot0 * hp_.n_vocab, b, cudaMemcpyDeviceToHost, stream_));
+  CTB_CUDA(cudaMemcpyAsync(h, kept_logits(slot0), b, cudaMemcpyDeviceToHost, stream_));
   CTB_CUDA(cudaStreamSynchronize(stream_));
   return h;
 }
@@ -1595,8 +1535,8 @@ double Engine::decode_greedy(int first_token, int n_past, int n_steps, int* out_
   CTB_CUDA(cudaMemcpyAsync(h_tokens_out_.get(), d_tokens_out_.get(), (size_t)n_steps * 4, cudaMemcpyDeviceToHost, stream_));
   CTB_CUDA(cudaMemcpyAsync(h_logits_.get(), d_logits_, (size_t)hp_.n_vocab * 4, cudaMemcpyDeviceToHost, stream_));
   CTB_CUDA(cudaMemcpyAsync(h_embd_.get(), d_embd_, (size_t)hp_.n_embd * 4, cudaMemcpyDeviceToHost, stream_));
-  CTB_CUDA(cudaMemcpyAsync(d_logits_keep_, d_logits_, (size_t)hp_.n_vocab * 4, cudaMemcpyDeviceToDevice, stream_));
-  CTB_CUDA(cudaMemcpyAsync(d_embd_keep_, d_embd_, (size_t)hp_.n_embd * 4, cudaMemcpyDeviceToDevice, stream_));
+  CTB_CUDA(cudaMemcpyAsync(kept_logits_, d_logits_, (size_t)hp_.n_vocab * 4, cudaMemcpyDeviceToDevice, stream_));
+  CTB_CUDA(cudaMemcpyAsync(kept_embd_, d_embd_, (size_t)hp_.n_embd * 4, cudaMemcpyDeviceToDevice, stream_));
   CTB_CUDA(cudaStreamSynchronize(stream_));
   host_fresh_ = true;
   memcpy(out_tokens, h_tokens_out_.get(), (size_t)n_steps * 4);

@@ -86,8 +86,6 @@ class Engine {
   Engine(const Engine&) = delete;
   Engine& operator=(const Engine&) = delete;
 
-  // Evaluate n tokens starting at position n_past; afterwards logits()/embeddings() hold the last token's.
-  void eval(const int* tokens, int n, int n_past);
   // Evaluate a token list with explicit per-token position and n_total (= n_past + N of the reference eval call the token
   // belongs to, llm.h:40-54): consecutive positions go through the batched prefill kernel, PB_T tokens per launch.
   // rows: also keep every token's logits row (RowSink); logits() / embeddings() / the greedy look-ahead come out the same.
@@ -117,9 +115,9 @@ class Engine {
   void multi_reset(int slot);                               // zero the slot's KV region: a reused slot is a fresh one
   long multi_launches() const;
   // Sequence states (include/ctransformers_b200.h ctb_state_header): the slot's K / V at positions [0, n_past) as
-  // K [layer][kv_head][pos][k_stride] then V [layer][kv_channel][pos], fp16, then with `results` its last logits and embeddings
-  // (a multi-sequence slot's rows, or the single-sequence eval's kept results).  Every copy is stream-ordered on the engine
-  // stream, behind whatever is already in it (a look-ahead step writes position n_past, which a state does not hold).
+  // K [layer][kv_head][pos][k_stride] then V [layer][kv_channel][pos], fp16, then with `results` its kept logits and embeddings.
+  // Every copy is stream-ordered on the engine stream, behind whatever is already in it (a look-ahead step writes position
+  // n_past, which a state does not hold).
   size_t state_bytes(int n_past, bool results) const;
   int state_k_stride() const;   // halves of a K row
   void state_save(int slot, int n_past, bool results, void* out);
@@ -182,7 +180,14 @@ class Engine {
   uint16_t *kc_ = nullptr, *vc_ = nullptr;
   // workspace
   int* d_state_ = nullptr;     // {token, n_past}
-  float *xa_ = nullptr, *xb_ = nullptr, *qkv_ = nullptr, *attn_ = nullptr, *attn_o_ = nullptr, *ffn_ = nullptr, *ffn2_ = nullptr, *d_logits_ = nullptr, *d_embd_ = nullptr, *d_logits_keep_ = nullptr, *d_embd_keep_ = nullptr;
+  float *xa_ = nullptr, *xb_ = nullptr, *qkv_ = nullptr, *attn_ = nullptr, *attn_o_ = nullptr, *ffn_ = nullptr, *ffn2_ = nullptr, *d_logits_ = nullptr, *d_embd_ = nullptr;
+  // every slot's last results (a single-sequence engine's are slot 0's), where a look-ahead step (after_eval) leaves them alone:
+  // logits [n_seq][n_vocab], embeddings [n_seq][n_embd], and the multi-sequence slots' greedy picks [n_seq][2] (the single
+  // sequence's is the look-ahead's, d_state_ + 4)
+  float *kept_logits_ = nullptr, *kept_embd_ = nullptr;
+  int* kept_pick_ = nullptr;
+  float* kept_logits(int slot) const { return kept_logits_ + (size_t)slot * hp_.n_vocab; }
+  float* kept_embd(int slot) const { return kept_embd_ + (size_t)slot * hp_.n_embd; }
   // host (pinned) results
   HostMem h_logits_, h_embd_;
   StateRing step_ring_;        // {token, n_past} of the single-token steps
@@ -235,10 +240,10 @@ class Engine {
   // in pinned memory: every slot's greedy pick (int[n_seq][2]), the results (SampleGpuOut[n_seq]), the argument block
   DevMem d_sample_;
   HostMem h_sample_;
-  void sample_enqueue(const SampleRow* rows, int R, const float* logits, size_t stride, bool picks);
-  // batched prefill (prefill.cuh): built on first use
+  void sample_enqueue(const SampleRow* rows, int R, bool picks);
+  // batched prefill (prefill.cuh): one program, built on first use
   std::unique_ptr<PrefillState> pf_;
-  bool multi_ready();            // hp_.multi and the multi-sequence program is built
+  bool multi_ready();            // hp_.multi and the batched program is built
   void need_multi();             // throws unless multi_ready()
   bool prefill_on_ = true;       // CTB_NO_PREFILL=1: prompts run through the single-token kernel
   int prefill_min_ = 4;          // shortest run of consecutive tokens worth a batched launch
@@ -246,7 +251,9 @@ class Engine {
   long single_steps_ = 0;        // tokens of batch_eval that went through the single-token step
   bool ensure_prefill();
   void prefill_batch(const int* tokens, const int* pos, const int* n_total, int n, bool last, bool rows = false);
-  // rows of an eval (RowSink), allocated on first use outside the arena: d_rows_ holds up to PB_T rows on their way out
+  void launch_batch(const MultiTok* toks, int n, bool whole);   // one k_pstep launch: the body, or `whole` with the head phases
+  // rows of an eval (RowSink), allocated outside the arena when the batched program or a rows eval first needs them: d_rows_
+  // holds up to PB_T rows on their way out, written by a launch's head phases or one at a time (rows_push)
   const RowSink* sink_ = nullptr;
   DevMem d_rows_;
   int rows_pending_ = 0, rows_done_ = 0;
@@ -263,7 +270,6 @@ class Engine {
   void rows_push(const float* row);          // one row through d_rows_
   void rows_drain();
   void rows_end();                           // after the stream is synchronised: the scores to the caller
-  bool ensure_rows_prog();
   void decode_one(int token, int pos, int n_total, bool with_logits);
   void head_from(const float* row);   // the output head (un-fused, as the single-token schedule launches it) on one hidden row
   void finish_eval(int next_pos, bool hit);
@@ -275,7 +281,6 @@ class Engine {
   HostMem h_copies_;
   void kv_slot_elems(size_t& k, size_t& v) const;   // halves of one slot's K and V regions
   void zero_slot(int slot);                         // zero the slot's K and V regions, on the stream
-  float* results_of(int slot, float** embd);        // where the slot's last logits / embeddings live on the device
   void copy_results(int src, int dst);              // multi-sequence: dst takes src's last logits, embeddings and greedy pick
   // the step's graphs, declared last so that they go before the buffers they launch on
   GraphExec graph_full_, graph_nolog_, graph_greedy_;
