@@ -8,6 +8,8 @@
 #include <stdexcept>
 
 #include "attention.cuh"
+#include "grammar.hpp"
+#include "grammar_gpu.cuh"
 #include "matvec.cuh"
 #include "prefill.cuh"
 #include "repack.cuh"
@@ -1544,6 +1546,130 @@ double Engine::decode_greedy(int first_token, int n_past, int n_steps, int* out_
   cudaEventElapsedTime(&ms, ev0_, ev1_);
   stats.last_eval_ms = ms;
   return ms;
+}
+
+// ----------------------------------------------------------------------------- grammar-constrained sampling (grammar_gpu.cuh)
+void Engine::grammar_pieces(const std::vector<int>& off, const std::vector<uint8_t>& bytes) {
+  if ((int)off.size() != hp_.n_vocab + 1) throw std::runtime_error("grammar pieces: one offset per token and one more are needed");
+  DeviceGuard dev_guard(device_);
+  const size_t ob = off.size() * 4;
+  uint8_t* d = (uint8_t*)d_pieces_.grow(ob + bytes.size() + 1);
+  CTB_CUDA(cudaMemcpy(d, off.data(), ob, cudaMemcpyHostToDevice));
+  if (!bytes.empty()) CTB_CUDA(cudaMemcpy(d + ob, bytes.data(), bytes.size(), cudaMemcpyHostToDevice));
+  pieces_ready_ = true;
+}
+
+// The launch buffer, the same layout on the device and in pinned memory: the top-k results SampleGpuOut[R], the allowed bits
+// [R][gm_words], stats int[R][2] (uploaded as zeros), the k_sample_topk block of the rows with a cut (sample_gpu.cuh sg_put), then the k_grammar_mask block:
+// rows [R][GM_ROW_INTS], every grammar's elements and rule offsets (once per grammar), the stacks' nodes, their tops, the windows.
+const SampleGpuOut* Engine::grammar_rows(const GrammarRow* rows, int R, int eos, int* stats, unsigned* bits) {
+  if (!pieces_ready_) throw std::runtime_error("grammar mask: the vocabulary's pieces are not on the device");
+  if (R <= 0 || R > hp_.n_seq) throw std::runtime_error("grammar mask: " + std::to_string(R) + " rows for " + std::to_string(hp_.n_seq) + " slots");
+  // the engine's device before the first grow: the buffers below are allocated on the current device, and the engine may run
+  // on another one than the caller's (CT_DEVICE, one replica per GPU)
+  DeviceGuard dev_guard(device_);
+  const int V = hp_.n_vocab;
+  std::vector<int> rec((size_t)R * GM_ROW_INTS), elems, roff, nodes, heads, last;
+  std::vector<std::pair<const Grammar*, std::pair<int, int>>> seen;   // grammar -> (its first element, its rule offsets' start)
+  std::vector<int> cut;                                // rows with a top-k cut
+  for (int r = 0; r < R; r++) {
+    const GrammarRow& w = rows[r];
+    if (w.slot < 0 || w.slot >= hp_.n_seq) throw std::runtime_error("grammar mask: slot out of range");
+    // a grammar's elements and rule offsets go into the block once, however many rows use it
+    int base = -1, rbase = -1;
+    for (const auto& g : seen)
+      if (g.first == w.g) { base = g.second.first; rbase = g.second.second; }
+    if (base < 0) {
+      base = (int)elems.size() / 2;
+      rbase = (int)roff.size();
+      for (const GElem& x : w.g->elems) { elems.push_back((int)x.type); elems.push_back((int)x.value); }
+      for (int o : w.g->off) roff.push_back(base + o);
+      seen.push_back({w.g, {base, rbase}});
+    }
+    int* q = rec.data() + (size_t)r * GM_ROW_INTS;
+    q[0] = w.slot;
+    q[1] = rbase;
+    q[2] = (int)heads.size();
+    q[3] = (int)w.s->stacks.size();
+    for (const GStack& st : w.s->stacks) {
+      int parent = -1;
+      for (int e : st) {
+        nodes.push_back(base + e);
+        nodes.push_back(parent);
+        parent = (int)nodes.size() / 2 - 1;
+      }
+      heads.push_back(parent);
+    }
+    q[4] = (int)w.s->partial.value;
+    q[5] = w.s->partial.n_remain;
+    q[6] = w.s->eos_ok() ? 1 : 0;
+    const int nl = sg_window(w.n_last);
+    q[7] = (int)last.size();
+    q[8] = nl;
+    last.insert(last.end(), w.last, w.last + nl);
+    memcpy(q + 9, &w.penalty, 4);
+    if (w.k > 0) {
+      if (!sg_accepts(0, w.k)) throw std::runtime_error("grammar mask: a top-k cut the device sampler does not take");
+      cut.push_back(r);
+    }
+  }
+  const int C = (int)cut.size();
+  const size_t bits_b = (size_t)R * gm_words(V) * 4;
+  const size_t outs_b = (size_t)R * sizeof(SampleGpuOut) + bits_b, stats_b = (size_t)R * 8, sg_b = sg_block_ints(C, 0) * 4;
+  const size_t gm_ints = rec.size() + elems.size() + roff.size() + nodes.size() + heads.size() + last.size();
+  const size_t bytes = outs_b + stats_b + sg_b + gm_ints * 4;
+  const size_t res_b = (size_t)R * sizeof(SampleGpuOut);
+  uint8_t* d_buf = (uint8_t*)d_gm_.grow(bytes);
+  uint8_t* h_buf = (uint8_t*)h_gm_.grow(bytes);
+  memset(h_buf + outs_b, 0, stats_b);
+  int* h_sg = (int*)(h_buf + outs_b + stats_b);
+  for (int c = 0; c < C; c++) sg_put(h_sg, C, c, cut[c], nullptr, 0, 1.0f, rows[cut[c]].k, V);
+  int* h = (int*)(h_buf + outs_b + stats_b + sg_b);
+  size_t at = 0;
+  auto put = [&](const std::vector<int>& v) { const size_t a = at; std::copy(v.begin(), v.end(), h + at); at += v.size(); return a; };
+  const size_t o_rec = put(rec), o_el = put(elems), o_roff = put(roff), o_nodes = put(nodes), o_heads = put(heads), o_last = put(last);
+  float* scratch = (float*)d_gm_rows_.grow((size_t)R * V * 4);
+  sampler_mode_ = true;
+  CTB_CUDA(cudaMemcpyAsync(d_buf + outs_b, h_buf + outs_b, bytes - outs_b, cudaMemcpyHostToDevice, stream_));
+  const int* d = (const int*)(d_buf + outs_b + stats_b + sg_b);
+  const int* pieces = d_pieces_.as<int>();
+  GmArgs a{kept_logits_, d + o_rec, (const uint32_t*)(d + o_el), d + o_roff, d + o_nodes, d + o_heads, d + o_last, pieces,
+           (const uint8_t*)(pieces + V + 1), scratch, (int*)(d_buf + outs_b), (unsigned*)(d_buf + res_b), V, eos};
+  k_grammar_mask<<<dim3((V + GM_THREADS - 1) / GM_THREADS, R), GM_THREADS, 0, stream_>>>(a);
+  CTB_CUDA(cudaGetLastError());
+  if (C > 0) {
+    sg_launch(sg_rows((const int*)(d_buf + outs_b + stats_b), C, scratch, (size_t)V, (SampleGpuOut*)d_buf), C, V, stream_);
+    CTB_CUDA(cudaGetLastError());
+  }
+  CTB_CUDA(cudaMemcpyAsync(h_buf, d_buf, outs_b + stats_b, cudaMemcpyDeviceToHost, stream_));
+  CTB_CUDA(cudaEventRecord(ev_sample_, stream_));
+  launch_deferred_spec();                          // the look-ahead step runs while the host finishes the draw
+  CTB_CUDA(cudaEventSynchronize(ev_sample_));
+  memcpy(stats, h_buf + outs_b, stats_b);
+  if (bits) memcpy(bits, h_buf + res_b, bits_b);
+  // results in row order: row cut[c]'s cut is at [c]; hand them out at [row]
+  std::vector<SampleGpuOut> tmp(cut.size());
+  for (int c = 0; c < C; c++) tmp[c] = ((const SampleGpuOut*)h_buf)[c];
+  SampleGpuOut* outs = (SampleGpuOut*)h_buf;
+  for (int c = 0; c < C; c++) outs[cut[c]] = tmp[c];
+  return outs;
+}
+
+std::vector<std::vector<float>> Engine::grammar_scratch(const std::vector<int>& rows) {
+  std::vector<std::vector<float>> out(rows.size(), std::vector<float>((size_t)hp_.n_vocab));
+  DeviceGuard dev_guard(device_);
+  for (size_t i = 0; i < rows.size(); i++)
+    CTB_CUDA(cudaMemcpyAsync(out[i].data(), d_gm_rows_.as<float>() + (size_t)rows[i] * hp_.n_vocab, out[i].size() * 4, cudaMemcpyDeviceToHost, stream_));
+  CTB_CUDA(cudaStreamSynchronize(stream_));
+  return out;
+}
+
+std::vector<float> Engine::slot_logits(int slot) {
+  std::vector<float> v((size_t)hp_.n_vocab);
+  DeviceGuard dev_guard(device_);
+  CTB_CUDA(cudaMemcpyAsync(v.data(), kept_logits(slot), v.size() * 4, cudaMemcpyDeviceToHost, stream_));
+  CTB_CUDA(cudaStreamSynchronize(stream_));
+  return v;
 }
 
 }  // namespace ctb

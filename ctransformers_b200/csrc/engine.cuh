@@ -65,6 +65,12 @@ constexpr int MULTI_LAUNCH_TOKENS = 32;   // tokens of one batched launch (prefi
 // engine), the repetition window, penalty and k.
 struct SampleRow { int slot; const int* last; int n_last; float penalty; int k; };
 
+// One row of the grammar mask (grammar_gpu.cuh: k_grammar_mask): whose logits, the grammar and its state (grammar.hpp), the
+// repetition window and penalty, and the top-k cut to run on the masked row afterwards (0: none).
+struct Grammar;
+struct GrammarState;
+struct GrammarRow { int slot; const Grammar* g; const GrammarState* s; const int* last; int n_last; float penalty; int k; };
+
 // Where an eval's per-token logits rows go (the reference's logits_all, llama.cpp:2949-2960): every evaluated token's row, in
 // call order, either copied to host[i * n_vocab] or reduced on the device by k_row_logprob (score_gpu.cuh) against
 // targets[i] into logprob[i] / greedy[i].  Exactly one of host / targets is set.
@@ -146,6 +152,18 @@ class Engine {
   int topk_candidates(const int* last, int n_last, float penalty, int k, int* ids, float* logits);
   // The last eval's greedy pick when the engine has it and it is unambiguous (a unique maximum), else -1.
   int greedy_pick();
+  // Grammar-constrained sampling (engine.cu, grammar_gpu.cuh).  grammar_pieces: the vocabulary's pieces, uploaded once (off[n_vocab + 1] into
+  // bytes, each piece cut at its first NUL).  grammar_rows: one upload of the rows' argument block (pinned), one k_grammar_mask
+  // launch writing each row's penalised, masked logits to scratch row r, one k_sample_topk launch over the scratch rows whose k is
+  // not 0 (penalty 1, no window), one copy back, one synchronise.  stats[2 r] = the allowed tokens of row r, stats[2 r + 1] = 1
+  // when the device reached a bound on it (its scratch row is then not the mask); bits (optional): the allowed tokens of row r
+  // as bits, [R][(n_vocab + 31) / 32].  Returns the top-k results (row r's at [r]), valid until the next call.
+  bool has_grammar_pieces() const { return pieces_ready_; }
+  void grammar_pieces(const std::vector<int>& off, const std::vector<uint8_t>& bytes);
+  const struct SampleGpuOut* grammar_rows(const GrammarRow* rows, int R, int eos, int* stats, unsigned* bits = nullptr);
+  // scratch rows of the last grammar_rows call, one copy each and one synchronise for all of them
+  std::vector<std::vector<float>> grammar_scratch(const std::vector<int>& rows);
+  std::vector<float> slot_logits(int slot);    // a copy of the slot's kept logits
   const HParams& hparams() const { return hp_; }
   EvalStats stats;
   void set_stream(cudaStream_t s);   // run on a caller-owned stream (bench: torch's current stream)
@@ -241,6 +259,10 @@ class Engine {
   DevMem d_sample_;
   HostMem h_sample_;
   void sample_enqueue(const SampleRow* rows, int R, bool picks);
+  // grammar mask: the piece table, the launch buffer (results, stats, argument blocks; device and pinned) and the scratch rows
+  bool pieces_ready_ = false;
+  DevMem d_pieces_, d_gm_, d_gm_rows_;
+  HostMem h_gm_;
   // batched prefill (prefill.cuh): one program, built on first use
   std::unique_ptr<PrefillState> pf_;
   bool multi_ready();            // hp_.multi and the batched program is built

@@ -11,6 +11,7 @@
 #include <algorithm>
 #include <atomic>
 #include <cctype>
+#include <cmath>
 #include <chrono>
 #include <cstdio>
 #include <cstring>
@@ -24,6 +25,7 @@
 #include "beam.hpp"
 #include "engine.cuh"
 #include "gguf.hpp"
+#include "grammar.hpp"
 #include "sample_gpu.cuh"
 #include "sampler.hpp"
 #include "tp_nccl.hpp"
@@ -51,6 +53,7 @@ struct LLM {
   std::mt19937 rng;
   bool has_logits = false;
   long gpu_samples = 0;   // sample() calls answered by the device-side penalty + top-k
+  long grammar_paths[3] = {0, 0, 0};   // constrained draws: device, host mask after a device bound, host cut (ctb_llm_grammar_paths)
   uint64_t fingerprint = 0;   // of the model file, computed on first use (model_fingerprint)
 };
 
@@ -1130,3 +1133,297 @@ int ctb_sample(const float* logits, int n_vocab, const int* last_tokens, int n_l
 }
 
 }  // extern "C"
+
+// ----------------------------------------------------------------------------- grammar-constrained sampling
+struct ctb_grammar { std::shared_ptr<const Grammar> g; };
+struct ctb_grammar_state { std::shared_ptr<const Grammar> g; GrammarState s; };
+
+ctb_grammar* ctb_grammar_parse(const char* text, char* err, int cap, long* err_pos) {
+  auto report = [&](const std::string& m, long pos) {
+    if (err && cap > 0) { const size_t n = std::min(m.size(), (size_t)cap - 1); memcpy(err, m.data(), n); err[n] = 0; }
+    if (err_pos) *err_pos = pos;
+  };
+  try {
+    if (!text) throw GrammarError("no grammar text", 0);
+    std::unique_ptr<ctb_grammar> g(new ctb_grammar);
+    g->g = std::make_shared<const Grammar>(grammar_parse(text));
+    report("", -1);
+    return g.release();
+  } catch (const GrammarError& e) {
+    report(e.what(), e.pos);
+  } catch (const std::exception& e) {
+    report(e.what(), 0);
+  }
+  return nullptr;
+}
+void ctb_grammar_free(ctb_grammar* g) { delete g; }
+int ctb_grammar_info(const ctb_grammar* g, int* out3) {
+  out3[0] = g->g->n_rules(); out3[1] = (int)g->g->elems.size(); out3[2] = (int)g->g->symbols.size();
+  return 3;
+}
+int ctb_grammar_rules(const ctb_grammar* g, int* off, unsigned* elems) {
+  std::copy(g->g->off.begin(), g->g->off.end(), off);
+  for (size_t i = 0; i < g->g->elems.size(); i++) { elems[2 * i] = g->g->elems[i].type; elems[2 * i + 1] = g->g->elems[i].value; }
+  return g->g->n_rules();
+}
+int ctb_grammar_symbol(const ctb_grammar* g, int i, char* name, int cap, unsigned* id) {
+  if (i < 0 || i >= (int)g->g->symbols.size()) return 0;
+  const auto& s = g->g->symbols[i];
+  *id = s.second;
+  if ((int)s.first.size() > cap) return -(int)s.first.size();
+  memcpy(name, s.first.data(), s.first.size());
+  return (int)s.first.size();
+}
+ctb_grammar_state* ctb_grammar_start(const ctb_grammar* g) {
+  try { return new ctb_grammar_state{g->g, grammar_start(*g->g)}; } catch (...) { return nullptr; }
+}
+ctb_grammar_state* ctb_grammar_state_copy(const ctb_grammar_state* s) {
+  try { return new ctb_grammar_state(*s); } catch (...) { return nullptr; }
+}
+void ctb_grammar_state_free(ctb_grammar_state* s) { delete s; }
+int ctb_grammar_state_eos_ok(const ctb_grammar_state* s) { return s->s.eos_ok() ? 1 : 0; }
+int ctb_grammar_state_stacks(const ctb_grammar_state* s, int* out, int cap, int* partial2) {
+  std::vector<int> v;   // per stack: its length, then its elements bottom first
+  for (const auto& st : s->s.stacks) { v.push_back((int)st.size()); v.insert(v.end(), st.begin(), st.end()); }
+  partial2[0] = (int)s->s.partial.value;
+  partial2[1] = s->s.partial.n_remain;
+  if ((int)v.size() > cap) return -(int)v.size();
+  std::copy(v.begin(), v.end(), out);
+  return (int)v.size();
+}
+
+static int grammar_accept_or_refuse(ctb_grammar_state* s, bool is_eos, const std::string& piece) {
+  try {
+    grammar_accept(*s->g, s->s, is_eos, piece);
+    return 0;
+  } catch (const std::exception& e) {
+    fprintf(stderr, "ctransformers-b200: grammar accept failed: %s\n", e.what());
+    return -1;
+  }
+}
+int ctb_grammar_accept_piece(ctb_grammar_state* s, const char* piece, int len, int is_eos) {
+  return grammar_accept_or_refuse(s, is_eos != 0, std::string(piece ? piece : "", piece ? std::max(len, 0) : 0));
+}
+static int llm_grammar_accept(LLM* llm, ctb_grammar_state* s, int token) {
+  if (token < 0 || token >= llm->hp.n_vocab) {
+    fprintf(stderr, "ctransformers-b200: grammar accept failed: token %d is out of range\n", token);
+    return -1;
+  }
+  return grammar_accept_or_refuse(s, token == llm->vocab.eos, token == llm->vocab.eos ? std::string() : llm->vocab.piece(token));
+}
+int ctb_llm_grammar_accept(LLM* llm, ctb_grammar_state* s, int token) { return llm_grammar_accept(llm, s, token); }
+int ctb_multi_grammar_accept(ctb_multi* m, ctb_grammar_state* s, int token) { return llm_grammar_accept(m->llm.get(), s, token); }
+
+int ctb_grammar_mask_pieces(const ctb_grammar_state* s, int n_vocab, const int* off, const char* bytes, int eos, unsigned char* allowed) {
+  try {
+    grammar_mask(*s->g, s->s, n_vocab, eos, [&](int t) { return std::string(bytes + off[t], bytes + off[t + 1]); }, allowed);
+    return 0;
+  } catch (const std::exception& e) {
+    fprintf(stderr, "ctransformers-b200: grammar mask failed: %s\n", e.what());
+    return -1;
+  }
+}
+
+// the host mask over the model's vocabulary
+static void host_mask(LLM* llm, const ctb_grammar_state* s, uint8_t* allowed) {
+  grammar_mask(*s->g, s->s, llm->hp.n_vocab, llm->vocab.eos, [&](int t) { return llm->vocab.piece(t); }, allowed);
+}
+
+// The rows below hold logits after the repetition penalty and the grammar mask (llama.cc:53-84 with llama_sample_grammar
+// between the penalty and top-k, as examples/main/main.cpp:650-695 places it): the host version of what k_grammar_mask writes.
+static std::vector<float> host_masked(LLM* llm, std::vector<float> v, const int* last, int n_last, float penalty, const ctb_grammar_state* s) {
+  if (n_last > 0 && penalty != 1.0f)
+    for (size_t i = 0; i < v.size(); i++) {
+      if (std::find(last, last + n_last, (int)i) == last + n_last) continue;
+      if (v[i] <= 0) v[i] *= penalty; else v[i] /= penalty;
+    }
+  std::vector<uint8_t> ok(v.size());
+  host_mask(llm, s, ok.data());
+  size_t n_ok = 0;
+  for (size_t i = 0; i < v.size(); i++) {
+    if (!ok[i]) v[i] = -INFINITY;
+    n_ok += ok[i];
+  }
+  if (!n_ok) throw std::invalid_argument("the grammar allows no token here");
+  return v;
+}
+
+static void grammar_pieces_once(LLM* llm) {
+  Engine& e = *llm->engine;
+  if (e.has_grammar_pieces()) return;
+  std::vector<int> off(1, 0);
+  std::vector<uint8_t> bytes;
+  for (int t = 0; t < llm->hp.n_vocab; t++) {
+    const std::string p = llm->vocab.piece(t);
+    const size_t n = std::find(p.begin(), p.end(), '\0') - p.begin();   // the reference decodes the piece as a C string
+    bytes.insert(bytes.end(), p.begin(), p.begin() + n);
+    off.push_back((int)bytes.size());
+  }
+  e.grammar_pieces(off, bytes);
+}
+
+// The device's top-k cut of a constrained row: its candidates' count (ids / logits filled), or -1 when the row has fewer allowed
+// tokens than the cut (equal -inf keys make the cut ambiguous) or the device took no cut.
+static int grammar_cut(const SampleGpuOut& res, int allowed, int top_k, int V, int* ids, float* lg) {
+  return sg_accepts(0, top_k) && allowed >= std::min(std::max(top_k, 1), V) ? sg_take(res, ids, lg) : -1;
+}
+// whether the draw of a row the device finished takes the host sampler on its masked row (sample_lazy's test)
+static bool grammar_needs_host_cut(const SampleGpuOut& res, int allowed, int top_k, int V) {
+  int ids[SG_MAX_OUT];
+  float lg[SG_MAX_OUT];
+  std::vector<Candidate> c;
+  const int count = grammar_cut(res, allowed, top_k, V, ids, lg);
+  return !(count > 0 && device_candidates_usable(ids, lg, count, top_k, V, c));
+}
+
+// One constrained draw from the device's results for its row: the device's top-k cut when it is usable (as many allowed tokens as
+// the cut and an unambiguous cut), else the host sampler on the masked row (scratch: that row when the caller fetched it already);
+// a row the device could not finish is masked on the host from the slot's logits.
+static int grammar_draw(LLM* llm, long* paths, int r, int slot, const int* stats, const SampleGpuOut& res, const int* last, int n_last, int top_k,
+                        float top_p, float temperature, float penalty, const ctb_grammar_state* s, const std::vector<float>* scratch = nullptr) {
+  Engine& e = *llm->engine;
+  const int V = llm->hp.n_vocab;
+  if (stats[2 * r + 1]) {
+    paths[1]++;
+    const std::vector<float> v = host_masked(llm, e.slot_logits(slot), last, n_last, penalty, s);
+    return sample_token(v.data(), V, nullptr, 0, top_k, top_p, temperature, 1.0f, llm->rng);
+  }
+  const int allowed = stats[2 * r];
+  if (allowed == 0) throw std::invalid_argument("the grammar allows no token here");
+  bool used_device = false;
+  const int t = sample_lazy(
+      V, nullptr, 0, top_k, top_p, temperature, 1.0f, llm->rng, used_device, [] { return -1; },
+      [&](const int*, int, float, int, int* ids, float* lg) { return grammar_cut(res, allowed, top_k, V, ids, lg); },
+      [&] { return scratch ? *scratch : std::move(e.grammar_scratch({r})[0]); });
+  paths[used_device ? 0 : 2]++;
+  return t;
+}
+
+int ctb_llm_sample_grammar(LLM* llm, const int* last_tokens, int n_last, int top_k, float top_p, float temperature, float repetition_penalty,
+                           int seed, const ctb_grammar_state* s) {
+  try {
+    not_sharded(llm, "does not sample with a grammar");
+    if (!s) throw std::invalid_argument("no grammar state");
+    if (!llm->has_logits) throw std::invalid_argument("nothing has been evaluated");
+    if (n_last > 0 && !last_tokens) throw std::invalid_argument("no window tokens");
+    if (seed < 0) seed = (int)time(nullptr);
+    llm->rng.seed((unsigned)seed);
+    Engine& e = *llm->engine;
+    if (!e.lazy_logits()) {
+      // a host view of the logits is held (and may have been changed by the caller): mask on the host over that view
+      const float* view = e.logits();
+      const std::vector<float> v = host_masked(llm, std::vector<float>(view, view + llm->hp.n_vocab), last_tokens, n_last, repetition_penalty, s);
+      llm->grammar_paths[2]++;
+      return sample_token(v.data(), llm->hp.n_vocab, nullptr, 0, top_k, top_p, temperature, 1.0f, llm->rng);
+    }
+    grammar_pieces_once(llm);
+    const GrammarRow row{0, s->g.get(), &s->s, last_tokens, n_last, repetition_penalty, sg_accepts(0, top_k) ? top_k : 0};
+    int stats[2];
+    const SampleGpuOut* res = e.grammar_rows(&row, 1, llm->vocab.eos, stats);
+    return grammar_draw(llm, llm->grammar_paths, 0, 0, stats, res[0], last_tokens, n_last, top_k, top_p, temperature, repetition_penalty, s);
+  } catch (const std::exception& e) {
+    fprintf(stderr, "ctransformers-b200: grammar sampling failed: %s\n", e.what());
+    return -1;
+  } catch (...) { return -1; }
+}
+
+// the device mask of a state on one slot's engine; a row the device could not finish is masked on the host
+static int engine_mask(LLM* llm, long* paths, int slot, const ctb_grammar_state* s, unsigned char* allowed) {
+  try {
+    not_sharded(llm, "does not sample with a grammar");
+    if (!s || !allowed) throw std::invalid_argument("a missing argument");
+    grammar_pieces_once(llm);
+    const int V = llm->hp.n_vocab;
+    const GrammarRow row{slot, s->g.get(), &s->s, nullptr, 0, 1.0f, 0};
+    int stats[2];
+    std::vector<unsigned> bits((size_t)(V + 31) / 32);
+    llm->engine->grammar_rows(&row, 1, llm->vocab.eos, stats, bits.data());
+    if (stats[1]) {
+      paths[1]++;
+      host_mask(llm, s, allowed);
+      return 0;
+    }
+    for (int t = 0; t < V; t++) allowed[t] = (bits[t / 32] >> (t % 32)) & 1u;
+    return 0;
+  } catch (const std::exception& e) {
+    fprintf(stderr, "ctransformers-b200: grammar mask failed: %s\n", e.what());
+    return -1;
+  } catch (...) { return -1; }
+}
+int ctb_llm_grammar_mask(LLM* llm, const ctb_grammar_state* s, unsigned char* allowed) {
+  return engine_mask(llm, llm->grammar_paths, 0, s, allowed);
+}
+int ctb_multi_grammar_mask(ctb_multi* m, int slot, const ctb_grammar_state* s, unsigned char* allowed) {
+  if (!multi_slot_ok(m, slot)) return -1;
+  return engine_mask(m->llm.get(), m->llm->grammar_paths, slot, s, allowed);
+}
+
+int ctb_multi_sample_grammar_many(ctb_multi* m, int n, const int* slots, const int* last_off, const int* last_tokens, const int* top_k,
+                                  const float* top_p, const float* temperature, const float* repetition_penalty, const int* seed,
+                                  const ctb_grammar_state* const* states, int* out) {
+  try {
+    if (n < 0) throw std::invalid_argument("a negative slot count");
+    if (n > 0 && (!slots || !last_off || !top_k || !top_p || !temperature || !repetition_penalty || !seed || !out || !states))
+      throw std::invalid_argument("a missing argument array");
+    if (!multi_slots_ok(m, n, slots)) return -1;
+    for (int i = 0; i < n; i++) {
+      if (!m->has[slots[i]]) throw std::invalid_argument("slot " + std::to_string(slots[i]) + " has no logits to sample from");
+      if (last_off[i] < 0 || last_off[i + 1] < last_off[i]) throw std::invalid_argument("the window offsets of slot " + std::to_string(slots[i]) + " are not ascending");
+    }
+    if (n > 0 && last_off[n] > last_off[0] && !last_tokens) throw std::invalid_argument("no window tokens");
+    // the unconstrained draws: exactly ctb_multi_sample_many on them
+    std::vector<int> free_i, u_slots, u_off(1, 0), u_last, u_k, u_seed, u_out;
+    std::vector<float> u_p, u_t, u_pen;
+    std::vector<GrammarRow> rows;
+    std::vector<int> row_i;
+    for (int i = 0; i < n; i++) {
+      const int* w = last_tokens ? last_tokens + last_off[i] : nullptr;
+      const int nl = last_off[i + 1] - last_off[i];
+      if (states[i]) {
+        rows.push_back(GrammarRow{slots[i], states[i]->g.get(), &states[i]->s, w, nl, repetition_penalty[i], sg_accepts(0, top_k[i]) ? top_k[i] : 0});
+        row_i.push_back(i);
+        continue;
+      }
+      free_i.push_back(i);
+      u_slots.push_back(slots[i]);
+      if (nl > 0) u_last.insert(u_last.end(), w, w + nl);
+      u_off.push_back((int)u_last.size());
+      u_k.push_back(top_k[i]); u_p.push_back(top_p[i]); u_t.push_back(temperature[i]); u_pen.push_back(repetition_penalty[i]);
+      u_seed.push_back(seed[i]);
+    }
+    if (!free_i.empty()) {
+      u_out.resize(free_i.size());
+      if (ctb_multi_sample_many(m, (int)free_i.size(), u_slots.data(), u_off.data(), u_last.data(), u_k.data(), u_p.data(), u_t.data(), u_pen.data(),
+                                u_seed.data(), u_out.data()) != 0)
+        return -1;
+      for (size_t j = 0; j < free_i.size(); j++) out[free_i[j]] = u_out[j];
+    }
+    if (rows.empty()) return 0;
+    LLM& L = *m->llm;
+    grammar_pieces_once(&L);
+    std::vector<int> stats(2 * rows.size());
+    const SampleGpuOut* res = L.engine->grammar_rows(rows.data(), (int)rows.size(), L.vocab.eos, stats.data());
+    std::vector<SampleGpuOut> results(res, res + rows.size());
+    // the masked rows the host cuts come back together: one copy each, one synchronise
+    std::vector<int> host_rows, at(rows.size(), -1);
+    for (size_t r = 0; r < rows.size(); r++)
+      if (!stats[2 * r + 1] && stats[2 * r] > 0 && grammar_needs_host_cut(results[r], stats[2 * r], top_k[row_i[r]], L.hp.n_vocab)) {
+        at[r] = (int)host_rows.size();
+        host_rows.push_back((int)r);
+      }
+    const std::vector<std::vector<float>> scratch = host_rows.empty() ? std::vector<std::vector<float>>() : L.engine->grammar_scratch(host_rows);
+    for (size_t r = 0; r < rows.size(); r++) {
+      const int i = row_i[r];
+      L.rng.seed((unsigned)(seed[i] < 0 ? (int)time(nullptr) : seed[i]));
+      out[i] = grammar_draw(&L, L.grammar_paths, (int)r, slots[i], stats.data(), results[r], rows[r].last, rows[r].n_last, top_k[i], top_p[i],
+                            temperature[i], repetition_penalty[i], states[i], at[r] >= 0 ? &scratch[at[r]] : nullptr);
+    }
+    return 0;
+  } catch (const std::exception& e) {
+    fprintf(stderr, "ctransformers-b200: multi-sequence grammar sampling failed: %s\n", e.what());
+    return -1;
+  } catch (...) { return -1; }
+}
+
+int ctb_llm_grammar_paths(LLM* llm, long* out3) { std::copy(llm->grammar_paths, llm->grammar_paths + 3, out3); return 3; }
+int ctb_multi_grammar_paths(ctb_multi* m, long* out3) { return ctb_llm_grammar_paths(m->llm.get(), out3); }

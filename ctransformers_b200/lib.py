@@ -133,6 +133,26 @@ EXTRA_PROTOTYPES = {
     "ctb_multi_reparent": (C.c_long, [_P, C.c_int, _IP, _IP, _IP, _IP]),
     "ctb_multi_beam_search": (C.c_int, [_P, C.c_int, _IP, _IP, C.c_int, C.c_int, C.c_int, _IP, _IP, _FP]),
     "ctb_multi_beam_stats": (C.c_int, [_P, _DP]),
+    "ctb_grammar_parse": (_P, [C.c_char_p, C.c_char_p, C.c_int, C.POINTER(C.c_long)]),
+    "ctb_grammar_free": (None, [_P]),
+    "ctb_grammar_info": (C.c_int, [_P, _IP]),
+    "ctb_grammar_rules": (C.c_int, [_P, _IP, C.POINTER(C.c_uint)]),
+    "ctb_grammar_symbol": (C.c_int, [_P, C.c_int, C.c_char_p, C.c_int, C.POINTER(C.c_uint)]),
+    "ctb_grammar_start": (_P, [_P]),
+    "ctb_grammar_state_copy": (_P, [_P]),
+    "ctb_grammar_state_free": (None, [_P]),
+    "ctb_grammar_state_eos_ok": (C.c_int, [_P]),
+    "ctb_grammar_state_stacks": (C.c_int, [_P, _IP, C.c_int, _IP]),
+    "ctb_grammar_accept_piece": (C.c_int, [_P, C.c_char_p, C.c_int, C.c_int]),
+    "ctb_llm_grammar_accept": (C.c_int, [_P, _P, C.c_int]),
+    "ctb_multi_grammar_accept": (C.c_int, [_P, _P, C.c_int]),
+    "ctb_grammar_mask_pieces": (C.c_int, [_P, C.c_int, _IP, C.c_char_p, C.c_int, _P]),
+    "ctb_llm_grammar_mask": (C.c_int, [_P, _P, _P]),
+    "ctb_multi_grammar_mask": (C.c_int, [_P, C.c_int, _P, _P]),
+    "ctb_llm_sample_grammar": (C.c_int, [_P, _IP, C.c_int, C.c_int, C.c_float, C.c_float, C.c_float, C.c_int, _P]),
+    "ctb_multi_sample_grammar_many": (C.c_int, [_P, C.c_int, _IP, _IP, _IP, _IP, _FP, _FP, _FP, _IP, C.POINTER(_P), _IP]),
+    "ctb_llm_grammar_paths": (C.c_int, [_P, C.POINTER(C.c_long)]),
+    "ctb_multi_grammar_paths": (C.c_int, [_P, C.POINTER(C.c_long)]),
 }
 
 

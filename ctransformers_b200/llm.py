@@ -7,13 +7,14 @@ Same class names, method names, keyword arguments, defaults and error behaviour,
 import re
 import warnings
 from collections.abc import MutableSequence
-from ctypes import POINTER, byref, c_double, c_float, c_int
+from ctypes import POINTER, byref, c_double, c_float, c_int, c_long
 from dataclasses import dataclass, fields
 from functools import partial
 from pathlib import Path
 from typing import Generator, List, Optional, Sequence, Union
 
 from . import state
+from .grammar import as_state
 from .lib import ConfigStruct, load_library
 from .state import SequenceState
 
@@ -251,16 +252,39 @@ class LLM:
             raise ValueError("perplexity needs a scored token: give a context or at least two tokens")
         return float(np.exp(-np.mean(scored)))
 
-    def sample(self, *, top_k=None, top_p=None, temperature=None, repetition_penalty=None, last_n_tokens=None, seed=None) -> int:
+    def sample(self, *, top_k=None, top_p=None, temperature=None, repetition_penalty=None, last_n_tokens=None, seed=None, grammar=None) -> int:
+        """grammar: a GrammarState (ctransformers_b200.grammar).  The draw is then the reference's chain with llama_sample_grammar
+        between the repetition penalty and top-k; the state is not advanced (accept does that).  Raises ValueError when the
+        grammar allows no token."""
         cfg = self._config
         last_n = _pick(last_n_tokens, cfg.last_n_tokens)
         if last_n < 0:
             last_n = self.context_length
         recent = self._context[-last_n:]   # (last_n == 0 selects the whole context, exactly like the reference's slice, llm.py:443)
         arr = (c_int * len(recent))(*recent)
-        return self.ctransformers_llm_sample(arr, len(recent), _pick(top_k, cfg.top_k), _pick(top_p, cfg.top_p),
-                                             _pick(temperature, cfg.temperature), _pick(repetition_penalty, cfg.repetition_penalty),
-                                             _pick(seed, cfg.seed))
+        args = (arr, len(recent), _pick(top_k, cfg.top_k), _pick(top_p, cfg.top_p), _pick(temperature, cfg.temperature),
+                _pick(repetition_penalty, cfg.repetition_penalty), _pick(seed, cfg.seed))
+        if grammar is None:
+            return self.ctransformers_llm_sample(*args)
+        token = self._lib.ctb_llm_sample_grammar(self._llm, *args, grammar._s)
+        if token < 0:
+            raise ValueError("grammar sampling failed: the grammar allows no token here, or the handle is tensor-sharded")
+        return token
+
+    def grammar_mask(self, grammar) -> "np.ndarray":
+        """The tokens the GrammarState allows next, as a bool array over the vocabulary (computed on the GPU)."""
+        import numpy as np
+        out = np.zeros(self.vocab_size, np.uint8)
+        if self._lib.ctb_llm_grammar_mask(self._llm, grammar._s, out.ctypes.data) != 0:
+            raise RuntimeError("Failed to compute the grammar mask.")
+        return out.astype(bool)
+
+    def grammar_paths(self) -> dict:
+        """Constrained draws so far: answered on the device, masked on the host because the device reached a bound, and cut on
+        the host (fewer allowed tokens than top_k, or an ambiguous cut)."""
+        out = (c_long * 3)()
+        self._lib.ctb_llm_grammar_paths(self._llm, out)
+        return {"device": out[0], "host_mask": out[1], "host_cut": out[2]}
 
     def save_state(self) -> SequenceState:
         """What this LLM has evaluated (its tokens, K / V cache and last results), for load_state here or in any LLM or MultiLLM
@@ -294,12 +318,16 @@ class LLM:
         return tokens[keep:]
 
     def generate(self, tokens: Sequence[int], *, top_k=None, top_p=None, temperature=None, repetition_penalty=None, last_n_tokens=None,
-                 seed=None, batch_size=None, threads=None, reset=None) -> Generator[int, None, None]:
+                 seed=None, batch_size=None, threads=None, reset=None, grammar=None) -> Generator[int, None, None]:
+        """grammar: a Grammar, GBNF text or GrammarState (advanced in place); every token is then one the grammar allows."""
+        state = None if grammar is None else as_state(grammar)
         tokens = self.prepare_inputs_for_generation(tokens, reset=reset)
         self.eval(tokens, batch_size=batch_size, threads=threads)
         while True:
             token = self.sample(top_k=top_k, top_p=top_p, temperature=temperature, repetition_penalty=repetition_penalty,
-                                last_n_tokens=last_n_tokens, seed=seed)
+                                last_n_tokens=last_n_tokens, seed=seed, grammar=state)
+            if state is not None:
+                state.accept(self, token)
             self.eval([token], batch_size=batch_size, threads=threads)
             if self.is_eos_token(token):
                 break
@@ -340,10 +368,11 @@ class LLM:
             yield text
 
     def __call__(self, prompt: str, *, max_new_tokens=None, top_k=None, top_p=None, temperature=None, repetition_penalty=None,
-                 last_n_tokens=None, seed=None, batch_size=None, threads=None, stop=None, stream=None, reset=None):
+                 last_n_tokens=None, seed=None, batch_size=None, threads=None, stop=None, stream=None, reset=None, grammar=None):
+        extra = {} if grammar is None else {"grammar": grammar}
         pieces = self._stream(prompt, max_new_tokens=max_new_tokens, stop=stop, top_k=top_k, top_p=top_p, temperature=temperature,
                               repetition_penalty=repetition_penalty, last_n_tokens=last_n_tokens, seed=seed, batch_size=batch_size,
-                              threads=threads, reset=reset)
+                              threads=threads, reset=reset, **extra)
         return pieces if _pick(stream, self._config.stream) else "".join(pieces)
 
     def embed(self, input: Union[str, Sequence[int]], *, batch_size=None, threads=None) -> List[float]:

@@ -1,13 +1,14 @@
 """Many independent sequences on one GPU (include/ctransformers_b200.h ctb_multi_*): every slot behaves like its own LLM with the
 same config, bit for bit, while the slots listed in one eval share batched launches — one pass over the weights per launch of
 up to 32 tokens instead of one per token of every sequence."""
-from ctypes import POINTER, c_double, c_float, c_int
+from ctypes import POINTER, c_double, c_float, c_int, c_long, c_void_p
 from pathlib import Path
 from functools import partial
 from typing import Dict, List, Optional, Sequence, Tuple
 
 from .lib import load_library
 from . import state
+from .grammar import as_state
 from .llm import Config, Vector, _check_ids, _ints, _pick, is_gguf
 from .state import SequenceState
 
@@ -144,16 +145,20 @@ class MultiLLM:
             raise RuntimeError("No logits to pick from: every slot must have been evaluated.")
         return list(out[: len(slots)])
 
-    def sample(self, slot: int, *, top_k=None, top_p=None, temperature=None, repetition_penalty=None, last_n_tokens=None, seed=None) -> int:
-        """LLM.sample on this slot: the same defaults, its own last_n_tokens window."""
+    def sample(self, slot: int, *, top_k=None, top_p=None, temperature=None, repetition_penalty=None, last_n_tokens=None, seed=None,
+               grammar=None) -> int:
+        """LLM.sample on this slot: the same defaults, its own last_n_tokens window (grammar: a GrammarState, as LLM.sample)."""
+        extra = {} if grammar is None else {"grammars": [grammar]}
         return self.sample_many([slot], top_k=top_k, top_p=top_p, temperature=temperature, repetition_penalty=repetition_penalty,
-                                last_n_tokens=last_n_tokens, seed=seed)[0]
+                                last_n_tokens=last_n_tokens, seed=seed, **extra)[0]
 
     def sample_many(self, slots: Sequence[int], *, top_k=None, top_p=None, temperature=None, repetition_penalty=None, last_n_tokens=None,
-                    seed=None) -> List[int]:
+                    seed=None, grammars=None) -> List[int]:
         """sample() of every listed slot, in one call: draw i is what LLM.sample returns with the i-th settings on an LLM fed
         slot slots[i]'s history.  Each setting is one value for every slot or a sequence with one value per slot (None: the
-        config's).  The penalty and top-k cut of all slots run in one device launch; the host finishes each draw."""
+        config's).  The penalty and top-k cut of all slots run in one device launch; the host finishes each draw.
+        grammars: one GrammarState or None (unconstrained) per slot; draw i is then LLM.sample(..., grammar=grammars[i]), and the
+        masks of all constrained slots are computed in one device launch."""
         slots = [self._slot(s) for s in slots]
         n, cfg = len(slots), self._config
         args = {}
@@ -165,10 +170,33 @@ class MultiLLM:
         off, flat = _flatten(windows)
         out = (c_int * max(n, 1))()
         floats = lambda v: (c_float * max(n, 1))(*v)
+        if grammars is not None:
+            if isinstance(grammars, (str, bytes)) or not hasattr(grammars, "__len__") or len(grammars) != n:
+                raise ValueError(f"grammars: one state (or None) for each of the {n} slots")
+            states = (c_void_p * max(n, 1))(*[None if g is None else g._s for g in grammars])
+            if self._lib.ctb_multi_sample_grammar_many(self._m, n, _ints(slots), _ints(off), _ints(flat), _ints(args["top_k"]), floats(args["top_p"]),
+                                                       floats(args["temperature"]), floats(args["repetition_penalty"]), _ints(args["seed"]),
+                                                       states, out) != 0:
+                raise ValueError(f"Failed to sample slots {slots} with grammars: the grammar allows no token, or a slot has no logits.")
+            return list(out[:n])
         if self._lib.ctb_multi_sample_many(self._m, n, _ints(slots), _ints(off), _ints(flat), _ints(args["top_k"]), floats(args["top_p"]),
                                            floats(args["temperature"]), floats(args["repetition_penalty"]), _ints(args["seed"]), out) != 0:
             raise RuntimeError(f"Failed to sample slots {slots}: each must have logits and be listed once.")
         return list(out[:n])
+
+    def grammar_mask(self, slot: int, grammar) -> "np.ndarray":
+        """LLM.grammar_mask for this handle's vocabulary (computed on the GPU)."""
+        import numpy as np
+        out = np.zeros(self.vocab_size, np.uint8)
+        if self._lib.ctb_multi_grammar_mask(self._m, self._slot(slot), grammar._s, out.ctypes.data) != 0:
+            raise RuntimeError("Failed to compute the grammar mask.")
+        return out.astype(bool)
+
+    def grammar_paths(self) -> dict:
+        """LLM.grammar_paths over every slot of this handle."""
+        out = (c_long * 3)()
+        self._lib.ctb_multi_grammar_paths(self._m, out)
+        return {"device": out[0], "host_mask": out[1], "host_cut": out[2]}
 
     def device_samples(self) -> int:
         """Draws so far that the device answered (the rest ran the host sampler on a slot's logits)."""
@@ -207,14 +235,19 @@ class MultiLLM:
         self._context[slot] = state.restore(self._lib, saved, partial(self._lib.ctb_multi_restore, self._m, slot))
 
     def generate_many(self, prompts: Sequence[Sequence[int]], max_new_tokens: int, *, n: int = 1, seeds: Optional[Sequence[int]] = None,
-                      batch_size: Optional[int] = None, **sampling) -> list:
+                      batch_size: Optional[int] = None, grammar=None, **sampling) -> list:
         """Generates for every prompt, up to n_slots at once: a sequence ends at EOS (not included) or after max_new_tokens, and
         its slot takes the next waiting prompt, whose prompt tokens then share launches with the other slots' decode tokens.
         Each result equals LLM.generate of that prompt on a fresh LLM with the same sampling arguments.
 
         n > 1 draws n samples of every prompt: the prompt is evaluated once, in one slot, which is then forked into n - 1 more;
         sample j draws with seed seeds[j] (required: equal seeds draw equal samples).  The result of a prompt is then the list
-        of its n samples, sample j equal to LLM.generate(prompt, seed=seeds[j], ...) on a fresh LLM."""
+        of its n samples, sample j equal to LLM.generate(prompt, seed=seeds[j], ...) on a fresh LLM.
+
+        grammar (a Grammar or GBNF text): every sequence draws under its own state of it, as LLM.generate(..., grammar=grammar);
+        a forked sample starts from a copy of its prompt's state."""
+        gram = None if grammar is None else as_state(grammar)
+        states: Dict[int, object] = {}
         if not 1 <= n <= self.n_slots:
             raise ValueError(f"n = {n}: each prompt's samples need a slot each, and there are {self.n_slots}")
         if (n > 1 or seeds is not None) and (seeds is None or len(seeds) != n):
@@ -234,6 +267,8 @@ class MultiLLM:
                 pending[group[0]], forks[group[0]] = list(prompts[i]), group[1:]
                 for j, s in enumerate(group):
                     owner[s], results[i][j] = (i, j), []
+                    if gram is not None:
+                        states[s] = gram.copy()
 
         admit()
         while owner:
@@ -245,11 +280,15 @@ class MultiLLM:
             forks = {}
             order = sorted(owner)
             kw = sampling if seeds is None else {**sampling, "seed": [seeds[owner[s][1]] for s in order]}
+            if gram is not None:
+                kw = {**kw, "grammars": [states[s] for s in order]}
             for slot, tok in zip(order, self.sample_many(order, **kw)):
                 i, j = owner[slot]
                 if tok == self.eos_token_id or max_new_tokens <= 0:
                     done = True
                 else:
+                    if gram is not None:
+                        states[slot].accept(self, tok)
                     results[i][j].append(tok)
                     done = len(results[i][j]) >= max_new_tokens
                     pending[slot] = [tok]

@@ -145,8 +145,16 @@ def random_blocks(t, ne0, rows, sigma, rng):
 
 
 # ----------------------------------------------------------------------------------------- vocabulary
-def make_spm_vocab(n_vocab):
-    """<unk>,<s>,</s>, 256 byte tokens, then pieces: printable ASCII singles, '▁'-prefixed words, merges."""
+# Pieces beyond ASCII for the grammar tests (extra_pieces=True): whole multi-byte characters, pieces that end inside a sequence,
+# pieces that start with a continuation byte, a piece with a NUL inside, an invalid sequence, and overlong-encoded NULs.
+EXTRA_PIECES = ["é".encode(), "ü".encode(), "日本".encode(), "😀".encode(), "▁café".encode(), "日".encode()[:2], "😀".encode()[:3],
+                "é".encode()[1:] + b"x", "日".encode()[2:], b"a\x00b", b"\xff\xfe", "ñ".encode()[:1], "{\"".encode(), "\":".encode(),
+                b"\xc0\x80", b"a\xe0\x80\x80b", b"\xe0\x80"]
+
+
+def make_spm_vocab(n_vocab, extra_pieces=False):
+    """<unk>,<s>,</s>, 256 byte tokens, then pieces: printable ASCII singles, '▁'-prefixed words, merges.  extra_pieces: the
+    EXTRA_PIECES (as bytes) before the fillers; without it the vocabulary is what it always was."""
     assert n_vocab >= 259 + 64
     toks, scores, types = ["<unk>", "<s>", "</s>"], [0.0, 0.0, 0.0], [2, 3, 3]
     for b in range(256):
@@ -171,6 +179,8 @@ def make_spm_vocab(n_vocab):
             add(w[:k], -3.0 - 0.01 * k)
         for k in range(1, len(w) + 1):
             add("▁" + w[:k], -2.0 - 0.01 * k)
+    for piece in EXTRA_PIECES if extra_pieces else ():
+        add(piece, -8.0)
     i = 0
     while len(toks) < n_vocab:
         add(f"▁tok{i}", -10.0 - i * 1e-4)
@@ -178,10 +188,11 @@ def make_spm_vocab(n_vocab):
     return toks, scores, types
 
 
-def make_bpe_vocab(n_vocab):
+def make_bpe_vocab(n_vocab, extra_pieces=False):
     """GPT-2 style vocabulary for Falcon GGUFs: the 256 raw single-byte strings (the reference BPE looks pieces up
     verbatim and dereferences a missing byte, llama.cpp:3316-3326, and it tokenizes "\\n" at load, llama.cpp:1748-1752),
-    then merged pieces with their merge list, then fillers.  Tokens are returned as bytes."""
+    then merged pieces with their merge list, then fillers.  Tokens are returned as bytes.  extra_pieces: the EXTRA_PIECES
+    before the fillers (no merges lead to them)."""
     toks = [bytes([b]) for b in range(256)]
     merges = []
     seen = set(toks)
@@ -195,6 +206,9 @@ def make_bpe_vocab(n_vocab):
                 ga = lambda x: x.replace(b" ", "Ġ".encode())   # merges live in GPT-2's byte-level alphabet (llama.cpp:962-974)
                 merges.append(ga(wb[:k - 1]) + b" " + ga(wb[k - 1:k]))
                 toks.append(piece); seen.add(piece)
+    for piece in EXTRA_PIECES if extra_pieces else ():
+        if piece not in seen:
+            toks.append(piece); seen.add(piece)
     i = 0
     while len(toks) < n_vocab:
         toks.append(f"<filler{i}>".encode()); i += 1
@@ -301,10 +315,11 @@ def _output_type(out_t, n_embd):
 
 
 def write_llama(path, shape: LlamaShape = LLAMA2_7B, ftype="Q4_K_M", seed=0, quantizer=None, sigma=0.02, emb_sigma=1.0, token_rows=None,
-                tensor_types=None):
+                tensor_types=None, extra_pieces=False):
     """Llama-architecture GGUF.  Returns dict(path, weight_bytes_per_token, tensor_types).  token_rows {token id: row}: token_embd
     is written as F32 with these rows (the rest drawn), so a test can choose exactly what the first layer's norm sees.
-    tensor_types {tensor kind, e.g. "attn_k": type}: that matrix of every layer in the given type instead of the ftype's."""
+    tensor_types {tensor kind, e.g. "attn_k": type}: that matrix of every layer in the given type instead of the ftype's.
+    extra_pieces: the vocabulary also holds EXTRA_PIECES (make_spm_vocab)."""
     _, _, out_t, emb_t = _type_plan(ftype)
     out_t = _output_type(out_t, shape.n_embd)
     tensor_types = tensor_types or {}
@@ -322,7 +337,7 @@ def write_llama(path, shape: LlamaShape = LLAMA2_7B, ftype="Q4_K_M", seed=0, qua
     w.add_f32(f"{a}.attention.layer_norm_rms_epsilon", shape.rms_eps)
     if shape.rope_base != 10000.0:
         w.add_f32(f"{a}.rope.freq_base", shape.rope_base)
-    toks, scores, types = make_spm_vocab(shape.n_vocab)
+    toks, scores, types = make_spm_vocab(shape.n_vocab, extra_pieces)
     w.add_str("tokenizer.ggml.model", "llama")
     w.add_arr_str("tokenizer.ggml.tokens", toks)
     w.add_arr_f32("tokenizer.ggml.scores", scores)
@@ -374,9 +389,9 @@ def write_llama(path, shape: LlamaShape = LLAMA2_7B, ftype="Q4_K_M", seed=0, qua
 
 
 def write_falcon(path, shape: FalconShape = FALCON_7B_SHAPED, ftype="Q5_K_M", seed=0, quantizer=None, sigma=0.02, emb_sigma=1.0, token_rows=None,
-                 tensor_types=None):
-    """Falcon-architecture GGUF (fused attn_qkv, LayerNorm with bias, gpt2/BPE vocabulary); token_rows and tensor_types as for
-    write_llama."""
+                 tensor_types=None, extra_pieces=False):
+    """Falcon-architecture GGUF (fused attn_qkv, LayerNorm with bias, gpt2/BPE vocabulary); token_rows, tensor_types and
+    extra_pieces as for write_llama."""
     main, _, _, emb_t = _type_plan(ftype)
     tensor_types = tensor_types or {}
     out_t = Q8_0 if ftype not in ("F16", "F32") else main
@@ -391,7 +406,7 @@ def write_falcon(path, shape: FalconShape = FALCON_7B_SHAPED, ftype="Q5_K_M", se
     w.add_u32(f"{a}.attention.head_count", shape.n_head)
     w.add_u32(f"{a}.attention.head_count_kv", shape.n_head_kv)
     w.add_f32(f"{a}.attention.layer_norm_epsilon", shape.eps)
-    toks, scores, types, merges = make_bpe_vocab(shape.n_vocab)
+    toks, scores, types, merges = make_bpe_vocab(shape.n_vocab, extra_pieces)
     w.add_str("tokenizer.ggml.model", "gpt2")
     w.add_arr_str("tokenizer.ggml.tokens", toks)
     w.add_arr_f32("tokenizer.ggml.scores", scores)

@@ -350,6 +350,54 @@ int ctb_multi_eval_rows(ctb_multi* m, int n, const int* slots, const int* off, c
 int ctb_multi_eval_scored(ctb_multi* m, int n, const int* slots, const int* off, const int* tokens, const int* n_past, int batch_size,
                           const int* targets, double* logprob, int* greedy);
 
+/* ---- grammar-constrained sampling (csrc/grammar.hpp, csrc/grammar_gpu.cuh): the reference's llama_sample_grammar and
+ * llama_grammar_accept_token over grammars in the GBNF text format of its grammar_parser::parse.
+ *
+ * ctb_grammar_parse: NULL on refusal (a syntax error, no `root`, a rule referenced but never defined, left recursion), with the
+ *   message in err (cap bytes, NUL-terminated) and the byte offset where parsing stopped in *err_pos.
+ * ctb_grammar_info: {n_rules, n_elements, n_symbols}.  ctb_grammar_rules: rule r is elements[off[r] .. off[r + 1]) of
+ *   elems (type, value pairs: llama_grammar_element).  ctb_grammar_symbol: symbol i (in id order): its name (bytes written, or
+ *   -needed) and *id.
+ * A state (stacks + partial UTF-8 sequence) keeps its grammar alive.  ctb_grammar_start: the state llama_grammar_init gives.
+ * ctb_grammar_accept_piece / ctb_llm_grammar_accept / ctb_multi_grammar_accept: llama_grammar_accept_token with the piece given,
+ *   or the model's piece of token; 0, or -1 (+ stderr) when the state does not allow the token (the state is left as it was).
+ * ctb_grammar_mask_pieces: the host mask over n_vocab pieces (piece t = bytes[off[t] .. off[t + 1])): allowed[t] = 1 where
+ *   llama_sample_grammar leaves token t's logit finite.
+ * ctb_llm_grammar_mask / ctb_multi_grammar_mask: that mask over the model's vocabulary, computed by k_grammar_mask on the
+ *   device (a row the device cannot finish is answered by the host code).
+ * ctb_llm_sample_grammar: ctransformers_llm_sample with llama_sample_grammar between the repetition penalty and top-k; the token,
+ *   or -1 (+ stderr) when no token is allowed or the handle is tensor-sharded.
+ * ctb_multi_sample_grammar_many: ctb_multi_sample_many with state states[i] for draw i (NULL: unconstrained, drawn as
+ *   ctb_multi_sample_many draws); every constrained row goes into one k_grammar_mask launch.
+ * ctb_llm_grammar_paths / ctb_multi_grammar_paths: out3 = {constrained draws the device answered, rows the host masked because
+ *   the device reached a bound, draws whose top-k cut the host made on the masked row (fewer allowed tokens than top_k, or an
+ *   ambiguous cut)}. */
+typedef struct ctb_grammar ctb_grammar;
+typedef struct ctb_grammar_state ctb_grammar_state;
+ctb_grammar* ctb_grammar_parse(const char* text, char* err, int cap, long* err_pos);
+void ctb_grammar_free(ctb_grammar* g);
+int ctb_grammar_info(const ctb_grammar* g, int* out3);
+int ctb_grammar_rules(const ctb_grammar* g, int* off, unsigned* elems);
+int ctb_grammar_symbol(const ctb_grammar* g, int i, char* name, int cap, unsigned* id);
+ctb_grammar_state* ctb_grammar_start(const ctb_grammar* g);
+ctb_grammar_state* ctb_grammar_state_copy(const ctb_grammar_state* s);
+void ctb_grammar_state_free(ctb_grammar_state* s);
+int ctb_grammar_state_eos_ok(const ctb_grammar_state* s);
+int ctb_grammar_state_stacks(const ctb_grammar_state* s, int* out, int cap, int* partial2);   /* ints written, or -needed */
+int ctb_grammar_accept_piece(ctb_grammar_state* s, const char* piece, int len, int is_eos);
+int ctb_llm_grammar_accept(LLM* llm, ctb_grammar_state* s, int token);
+int ctb_multi_grammar_accept(ctb_multi* m, ctb_grammar_state* s, int token);
+int ctb_grammar_mask_pieces(const ctb_grammar_state* s, int n_vocab, const int* off, const char* bytes, int eos, unsigned char* allowed);
+int ctb_llm_grammar_mask(LLM* llm, const ctb_grammar_state* s, unsigned char* allowed);
+int ctb_multi_grammar_mask(ctb_multi* m, int slot, const ctb_grammar_state* s, unsigned char* allowed);
+int ctb_llm_sample_grammar(LLM* llm, const int* last_tokens, int n_last, int top_k, float top_p, float temperature, float repetition_penalty,
+                           int seed, const ctb_grammar_state* s);
+int ctb_multi_sample_grammar_many(ctb_multi* m, int n, const int* slots, const int* last_off, const int* last_tokens, const int* top_k,
+                                  const float* top_p, const float* temperature, const float* repetition_penalty, const int* seed,
+                                  const ctb_grammar_state* const* states, int* out);
+int ctb_llm_grammar_paths(LLM* llm, long* out3);
+int ctb_multi_grammar_paths(ctb_multi* m, long* out3);
+
 #ifdef __cplusplus
 }
 #endif
