@@ -64,16 +64,29 @@ __device__ __forceinline__ uint16_t f2h(float f) { return __half_as_ushort(__flo
 __device__ __forceinline__ void pdl_trigger() { asm volatile("griddepcontrol.launch_dependents;"); }
 __device__ __forceinline__ void pdl_wait() { asm volatile("griddepcontrol.wait;" ::: "memory"); }
 
-// launch with the programmatic-serialization attribute when pdl is set (the kernel may then start while its predecessor drains)
+// launch with the programmatic-serialization attribute when pdl is set (the kernel may then start while its predecessor drains),
+// and in clusters of `cluster` CTAs along x when that is more than 1
 template <typename... KArgs, typename... Args>
-static inline cudaError_t launch_kernel(void (*kernel)(KArgs...), dim3 grid, dim3 block, size_t smem, cudaStream_t st, bool pdl, Args&&... args) {
+static inline cudaError_t launch_kernel_cluster(void (*kernel)(KArgs...), dim3 grid, dim3 block, size_t smem, cudaStream_t st, bool pdl, unsigned cluster,
+                                                Args&&... args) {
   cudaLaunchConfig_t cfg{};
   cfg.gridDim = grid; cfg.blockDim = block; cfg.dynamicSmemBytes = smem; cfg.stream = st;
-  cudaLaunchAttribute at[1];
-  at[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-  at[0].val.programmaticStreamSerializationAllowed = 1;
-  cfg.attrs = at; cfg.numAttrs = pdl ? 1 : 0;
+  cudaLaunchAttribute at[2];
+  unsigned n = 0;
+  if (pdl) {
+    at[n].id = cudaLaunchAttributeProgrammaticStreamSerialization;
+    at[n++].val.programmaticStreamSerializationAllowed = 1;
+  }
+  if (cluster > 1) {
+    at[n].id = cudaLaunchAttributeClusterDimension;
+    at[n].val.clusterDim.x = cluster; at[n].val.clusterDim.y = 1; at[n++].val.clusterDim.z = 1;
+  }
+  cfg.attrs = at; cfg.numAttrs = n;
   return cudaLaunchKernelEx(&cfg, kernel, std::forward<Args>(args)...);
+}
+template <typename... KArgs, typename... Args>
+static inline cudaError_t launch_kernel(void (*kernel)(KArgs...), dim3 grid, dim3 block, size_t smem, cudaStream_t st, bool pdl, Args&&... args) {
+  return launch_kernel_cluster(kernel, grid, block, smem, st, pdl, 1u, std::forward<Args>(args)...);
 }
 
 // dynamic shared memory a kernel can opt in to on the current device: the per-block limit less its static shared memory

@@ -666,7 +666,7 @@ void Engine::build_ops() {
   for (const StepOp& op : ops_) any_stream |= op.ph.kind == PH_MATVEC && op.stream;
   std::vector<Phase> phs;
   for (const StepOp& op : ops_) if (op.ph.kind != PH_XCHG && (op.ph.kind != PH_MATVEC || op.stream)) phs.push_back(op.ph);
-  const StepLaunch sl = step_launch_shape(phs.data(), (int)phs.size(), sm_count_, max_dyn_smem(k_step<true, false, false>));
+  const StepLaunch sl = step_launch_plan(phs.data(), (int)phs.size(), sm_count_);
   step_grid_ = sl.grid; step_slots_ = sl.n_slots; step_smem_ = sl.smem; step_q3_ = sl.q3;
   if (const char* e = getenv("CTB_ST_SLOTS")) {   // A/B knob: fewer ring slots = less prefetch in flight
     const int want = atoi(e);
@@ -675,8 +675,14 @@ void Engine::build_ops() {
   ring_attn_ = st_attn_ring_ok(hp_.n_ctx, step_slots_) && !getenv("CTB_NO_RING_ATTN");
   for (StepOp& op : ops_) if (op.ph.kind == PH_ATTN) op.ph.q6 = ring_attn_ ? 1 : 0;
   if (any_stream && step_slots_ < ST_W) throw std::runtime_error("model rows are too long for the step kernel's shared memory");
-  if (any_stream) CTB_CUDA(step_set_smem_limit(step_smem_));
-  else fused_ = false;
+  if (any_stream) {
+    CTB_CUDA(step_set_smem_limit(step_smem_));
+    StepLaunch pl = sl;
+    pl.n_slots = step_slots_; pl.smem = step_smem_;
+    step_pair_ = step_pair_choose(pl, phs.data(), (int)phs.size());
+  } else {
+    fused_ = false;
+  }
   d_prog_ = (Phase*)alloc((ops_.size() + 1) * sizeof(Phase), 256);
   d_prog_mv_ = (Phase*)alloc((ops_.size() + 1) * sizeof(Phase), 256);
   d_bounds_ = (int*)alloc((ops_.size() + 1) * (size_t)(sm_count_ + 1) * 4, 256);      // per-CTA tile ranges, one row per phase
@@ -713,6 +719,7 @@ long Engine::enqueue_ops(const std::vector<StepOp>& ops, const Phase* d_prog, co
   StepLaunch step_shape_;
   step_shape_.grid = step_grid_; step_shape_.n_slots = step_slots_; step_shape_.smem = step_smem_; step_shape_.gen = !attn_fast_hd(hp_.head_dim());
   step_shape_.q3 = step_q3_;
+  step_shape_.pair = step_pair_;
   auto capable = [&](const StepOp& op) { return op.ph.kind != PH_XCHG && (op.ph.kind != PH_MATVEC || op.stream); };
   int i = 0;
   while (i < n) {
@@ -833,7 +840,7 @@ long Engine::trace_step(int token, int n_past, unsigned long long* out, long cap
   const DevMem buf((size_t)n * step_grid_ * 64);
   CTB_CUDA(cudaMemset(buf.get(), 0, (size_t)n * step_grid_ * 64));
   StepLaunch L;
-  L.grid = step_grid_; L.n_slots = step_slots_; L.smem = step_smem_; L.gen = !attn_fast_hd(hp_.head_dim()); L.q3 = step_q3_;
+  L.grid = step_grid_; L.n_slots = step_slots_; L.smem = step_smem_; L.gen = !attn_fast_hd(hp_.head_dim()); L.q3 = step_q3_; L.pair = step_pair_;
   for (int rep = 0; rep < 3; rep++) {   // the last (warm) run is the one read back
     put_step(token, n_past, n_past + 1);
     CTB_CUDA(launch_step(L, stream_, d_prog_, d_bounds_, n, d_sync_, false, buf.as<unsigned long long>()));

@@ -139,6 +139,7 @@ class Engine {
   const float* multi_rows(int slot0, int n);
   // Which implementations the evals run (include/ctransformers_b200.h ctb_llm_paths): entries written, or -needed.
   int paths(int* out, int cap);
+  int step_cluster() const { return step_pair_ ? 2 : 1; }   // CTAs per cluster of the step kernel's launch
 
   // Host views of the last token's logits / hidden state (the reference hands out ctx->logits.data(), mutable by the caller,
   // llama.cc:47-51).  Until a caller asks for one, nothing is copied per eval (lazy); from the first request on every eval
@@ -244,6 +245,7 @@ class Engine {
   size_t step_smem_ = 0;                 // dynamic shared memory
   bool fused_ = true;            // CTB_STEP_FUSE=0: one kernel per op
   bool step_q3_ = false;         // some mat-vec phase holds a Q3_K matrix: the k_step<.., .., true> build
+  bool step_pair_ = false;       // k_step runs as clusters of two CTAs (step_pair_choose)
   bool ring_attn_ = false;       // the step kernel's attention phases take cached K / V through the ring (st_attn_ring_ok)
   void build_ops();
   void push_matvec(struct MVParams& p, int kind);

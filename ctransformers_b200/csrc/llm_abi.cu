@@ -476,6 +476,8 @@ long ctb_llm_paths(LLM* llm, int* out, int cap) {
   }
 }
 
+int ctb_llm_step_cluster(LLM* llm) { return llm->engine->step_cluster(); }
+
 double ctb_llm_time_matvec_only(LLM* llm, int reps, long* launches) { return ctb_llm_time_matvec_kinds(llm, reps, launches, 0); }
 
 double ctb_llm_time_matvec_kinds(LLM* llm, int reps, long* launches, unsigned kind_mask) {

@@ -43,12 +43,13 @@ enum : int { EPI_STORE = 0, EPI_ADD = 1, EPI_GELU = 2, EPI_ADD2 = 3, EPI_SILU = 
 // what a timed-out wait was waiting for (the code st_fail records), and the text the host reports for it
 enum WaitCode : int {
   W_GRID_BARRIER = 1, W_FOLD_FLAG, W_FREE_WEIGHT_SLOT, W_WEIGHT_ITEM, W_FREE_K_SLOT, W_FREE_V_SLOT, W_K_ITEM, W_V_ITEM, W_XCHG,
-  W_PF_GRID_BARRIER, W_PF_FREE_SLOT, W_PF_WEIGHT_ITEM, W_CODES
+  W_PF_GRID_BARRIER, W_PF_FREE_SLOT, W_PF_WEIGHT_ITEM, W_PAIR, W_CODES
 };
 constexpr const char* WAIT_TEXT[] = {"?", "grid barrier (aux = phase)", "fold hand-off flag (aux = chunk)", "producer: free weight slot (aux = item)",
                                      "consumer: weight item (aux = item)", "producer: free K slot (attention)", "producer: free V slot (attention)",
                                      "consumer: K item (attention)", "consumer: V item (attention)", "tensor-parallel exchange: a peer's element (aux = exchange number)",
-                                     "prefill grid barrier (aux = phase)", "prefill producer: free slot (aux = item)", "prefill consumer: weight item (aux = item)"};
+                                     "prefill grid barrier (aux = phase)", "prefill producer: free slot (aux = item)", "prefill consumer: weight item (aux = item)",
+                                     "cluster peer: its half of the staged input (aux = exchange round)"};
 static_assert(sizeof(WAIT_TEXT) / sizeof(WAIT_TEXT[0]) == W_CODES, "one text per wait code");
 
 static __device__ int* g_st_dbg = nullptr;   // set by the host (st_set_debug_words): 4 ints of mapped pinned host memory, or null
@@ -238,11 +239,91 @@ __device__ __forceinline__ void load16x(const MVParams& xs, int base, int valid,
 
 // Norm weight / bias of this thread's first 16 elements: constants of the model, so they are fetched before the kernel waits
 // for its predecessor (pdl_wait) and are in registers when the input vector arrives.
+// lo: the first element this CTA stages (stage_q8k_pair; 0 otherwise).
 struct NormPre { float w0[16], bias0[16]; };
-__device__ __forceinline__ void preload_norm(NormPre& np, const MVParams& p) {
-  const int t = threadIdx.x;
-  if (p.norm_mode != NORM_NONE && p.norm_w) load16(p.norm_w + t * 16, p.K - t * 16, np.w0);
-  if (p.norm_mode != NORM_NONE && p.norm_b) load16(p.norm_b + t * 16, p.K - t * 16, np.bias0);
+__device__ __forceinline__ void preload_norm(NormPre& np, const MVParams& p, int lo = 0) {
+  const int t = lo + (int)threadIdx.x * 16;
+  if (p.norm_mode != NORM_NONE && p.norm_w) load16(p.norm_w + t, p.K - t, np.w0);
+  if (p.norm_mode != NORM_NONE && p.norm_b) load16(p.norm_b + t, p.K - t, np.bias0);
+}
+
+// ---------------------------------------------------------------------------------------------
+// Distributed shared memory of a cluster of two CTAs (stage_q8k_pair): a thread stores into the other CTA's shared memory
+// through the address mapa gives for the same offset there.
+__device__ __forceinline__ uint32_t cluster_ctarank() {
+  uint32_t r;
+  asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
+  return r;
+}
+__device__ __forceinline__ uint32_t dsmem_map(const void* p, uint32_t rank) {
+  uint32_t a;
+  asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(a) : "r"((uint32_t)__cvta_generic_to_shared(p)), "r"(rank));
+  return a;
+}
+__device__ __forceinline__ void dsmem_st_u32(uint32_t a, uint32_t v) { asm volatile("st.shared::cluster.u32 [%0], %1;" ::"r"(a), "r"(v) : "memory"); }
+__device__ __forceinline__ void dsmem_st_u16(uint32_t a, uint16_t v) { asm volatile("st.shared::cluster.u16 [%0], %1;" ::"r"(a), "h"(v) : "memory"); }
+__device__ __forceinline__ void dsmem_st_f64(uint32_t a, double v) { asm volatile("st.shared::cluster.f64 [%0], %1;" ::"r"(a), "d"(v) : "memory"); }
+
+// The two CTAs of a pair hand each other data in numbered rounds.  Round r: every thread stores its data into both CTAs, the
+// CTA meets at its named barrier, thread 0 arrives (release, cluster scope) on the peer's mbarrier bar[r & 1], and every thread
+// waits (acquire, cluster scope) on its own bar[r & 1] for the peer's arrival.  The named barrier orders all of this CTA's
+// stores before thread 0's release; each waiting thread's acquire then orders the peer's stores before its own loads.  A CTA
+// arrives for round r + 2 only after it has waited for round r + 1, which the peer sends after it has finished waiting for
+// round r, so two mbarriers (and two reduction buffers) never hold two rounds at once.  Every round's data lands in a CTA
+// that is still waiting for it, so no CTA stores into one that has exited.
+struct PairX {
+  uint64_t* bar;    // [2] mbarriers of this CTA, arrival count 1 (initialised before the launch's first cluster barrier)
+  double* red;      // [2 rounds][2 ranks][3][NT / 32] per-warp partials of the norm statistic
+  uint32_t rank;    // %cluster_ctarank
+  uint32_t round;   // rounds done so far: the same in both CTAs
+};
+// blocks [pair_block0(nb, r), pair_block0(nb, r + 1)) of a vector of nb Q8_K blocks are rank r's; an odd block goes to rank 0
+__host__ __device__ inline int pair_block0(int nb, int rank) { return rank <= 0 ? 0 : (rank == 1 ? (nb + 1) / 2 : nb); }
+
+template <int NT, int BAR>
+__device__ __forceinline__ void pair_round(PairX& px) {
+  bar_sync<BAR, NT>();
+  uint64_t* bar = px.bar + (px.round & 1u);
+  if (threadIdx.x == 0) asm volatile("mbarrier.arrive.release.cluster.shared::cluster.b64 _, [%0];" ::"r"(dsmem_map(bar, px.rank ^ 1u)) : "memory");
+  const uint32_t addr = (uint32_t)__cvta_generic_to_shared(bar), parity = (px.round >> 1) & 1u;
+  bounded_wait([&] {
+    uint32_t ok;
+    asm volatile("{\n .reg .pred p;\n mbarrier.try_wait.parity.acquire.cluster.shared::cta.b64 p, [%1], %2;\n selp.u32 %0, 1, 0, p;\n}"
+                 : "=r"(ok) : "r"(addr), "r"(parity) : "memory");
+    return ok != 0;
+  }, W_PAIR, (int)px.round);
+  px.round++;
+}
+
+// block_sum2_max_f64 over both CTAs of the pair: the per-warp partials of both go to both, and every thread adds them in one
+// fixed order, rank 0's warps first, so both CTAs hold the same s, a and g.
+template <int NT, int BAR>
+__device__ __forceinline__ void pair_sum2_max_f64(double& s, double& a, double& g, bool a_is_s, PairX& px) {
+  constexpr int NW = NT / 32;
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) {
+    s += __shfl_xor_sync(0xffffffffu, s, o);
+    if (!a_is_s) {
+      a += __shfl_xor_sync(0xffffffffu, a, o);
+      g = fmax(g, __shfl_xor_sync(0xffffffffu, g, o));
+    }
+  }
+  double* buf = px.red + (px.round & 1u) * (2 * 3 * NW);
+  if ((threadIdx.x & 31) == 0) {
+    const int w = threadIdx.x >> 5;
+    double* mine = buf + px.rank * (3 * NW);
+    mine[w] = s; mine[NW + w] = a; mine[2 * NW + w] = g;
+    const uint32_t peer = dsmem_map(mine, px.rank ^ 1u);
+    dsmem_st_f64(peer + 8 * w, s); dsmem_st_f64(peer + 8 * (NW + w), a); dsmem_st_f64(peer + 8 * (2 * NW + w), g);
+  }
+  pair_round<NT, BAR>(px);
+  s = 0.0;
+  a = 0.0;
+#pragma unroll
+  for (int r = 0; r < 2; r++)
+#pragma unroll
+    for (int w = 0; w < NW; w++) { s += buf[r * 3 * NW + w]; a += buf[r * 3 * NW + NW + w]; g = fmax(g, buf[r * 3 * NW + 2 * NW + w]); }
+  if (a_is_s) a = s;
 }
 
 // One norm statistic, (float)(Σ term(x_i) / K), as the reference computes it: its double sum runs over the elements one after
@@ -289,11 +370,13 @@ static __device__ __noinline__ double seq_sum_warp0(const float* x, const float*
   return seq;
 }
 
-template <int NT, int BAR, bool XC>
+// PAIR: the terms are spread over the two CTAs of a pair (stage_q8k_pair), which add all partial sums in the same order.
+template <int NT, int BAR, bool XC, bool PAIR = false>
 __device__ __forceinline__ float norm_stat(double s, double a, double g, bool a_is_s, int kind, float mean, const MVParams& xs, double* red,
-                                           unsigned epoch) {
+                                           unsigned epoch, PairX* px = nullptr) {
   const int K = xs.K;
-  if (a_is_s) a = s = block_sum_f64<NT, BAR>(s, red);
+  if constexpr (PAIR) pair_sum2_max_f64<NT, BAR>(s, a, g, a_is_s, *px);
+  else if (a_is_s) a = s = block_sum_f64<NT, BAR>(s, red);
   else block_sum2_max_f64<NT, BAR>(s, a, g, red);
   // inf / NaN terms give the same sum in every order (a double sum of float terms cannot overflow); so does an exact sum
   if (!isfinite(s) || (!a_is_s && __dmul_ru(a, g) < 0x1p52)) return (float)(s / (double)K);
@@ -305,6 +388,74 @@ __device__ __forceinline__ float norm_stat(double s, double a, double g, bool a_
   if (threadIdx.x == 0) red[0] = seq;
   bar_sync<BAR, NT>();
   return (float)(red[0] / (double)K);
+}
+
+// ggml_rms_norm / ggml_norm of 16 elements given the statistic (mean, scale), then the separate weight and bias (ggml_mul, ggml_add)
+__device__ __forceinline__ void norm_apply16(float (&v)[16], const float (&w)[16], const float (&bb)[16], int norm_mode, float mean, float scale, bool has_w,
+                                             bool has_b) {
+#pragma unroll
+  for (int e = 0; e < 16; e++) {
+    float y = v[e];
+    if (norm_mode == NORM_LAYER) y = __fsub_rn(y, mean);
+    y = __fmul_rn(y, scale);
+    if (has_w) y = __fmul_rn(y, w[e]);
+    if (has_b) y = __fadd_rn(y, bb[e]);
+    v[e] = y;
+  }
+}
+
+// One thread's 16 elements of a Q8_K block (16 lanes, a half-warp, share a block; every lane of the warp calls): reference
+// quantize_row_q8_K_reference (k_quants.c:1191-1226): the first element with the largest |x| fixes the sign; iscale = -128/max;
+// q = min(127, nearest_int(iscale*x)); the reference BINARY fuses iscale*x + 12582912.f (vfmadd), so the exact product is
+// rounded once — __fmaf_rn.  d = 1/iscale; bsums per 16.  PAIR: the same words also go to the other CTA of the pair, whose
+// image has the same layout at pqs (qs), pdd (d) and pbs (bsums).
+template <bool PAIR = false>
+__device__ __forceinline__ void quant_q8k16(const float (&v)[16], int base, int valid, int lane, int8_t* qs, float* dd, int16_t* bs, uint32_t pqs = 0,
+                                            uint32_t pdd = 0, uint32_t pbs = 0) {
+  float amax = 0.f, mx = 0.f;
+#pragma unroll
+  for (int e = 0; e < 16; e++) { const float ax = fabsf(v[e]); if (ax > amax) { amax = ax; mx = v[e]; } }
+  float gmax = amax;
+#pragma unroll
+  for (int o = 8; o > 0; o >>= 1) gmax = fmaxf(gmax, __shfl_xor_sync(0xffffffffu, gmax, o));
+  const unsigned who = __ballot_sync(0xffffffffu, amax == gmax);
+  const int hbase = lane & 16, hl = lane & 15;
+  const unsigned mine = (who >> hbase) & 0xffffu;
+  const float maxv = __shfl_sync(0xffffffffu, mx, hbase + __ffs(mine) - 1);
+  if (valid > 0) {
+    const int b = base >> 8;
+    int q[16];
+    int sum = 0;
+    if (gmax == 0.f) {
+#pragma unroll
+      for (int e = 0; e < 16; e++) q[e] = 0;
+      if (hl == 0) {
+        dd[b] = 0.f;
+        if (PAIR) dsmem_st_u32(pdd + 4 * b, 0u);
+      }
+    } else {
+      const float iscale = __fdiv_rn(-128.f, maxv);
+#pragma unroll
+      for (int e = 0; e < 16; e++) {
+        const float val = __fmaf_rn(iscale, v[e], 12582912.f);
+        q[e] = min(127, (__float_as_int(val) & 0x007fffff) - 0x00400000);
+        sum += q[e];
+      }
+      if (hl == 0) {
+        const float d = __fdiv_rn(1.f, iscale);
+        dd[b] = d;
+        if (PAIR) dsmem_st_u32(pdd + 4 * b, __float_as_uint(d));
+      }
+    }
+    bs[b * 16 + hl] = (int16_t)sum;
+    if (PAIR) dsmem_st_u16(pbs + 2 * (b * 16 + hl), (uint16_t)(int16_t)sum);
+#pragma unroll
+    for (int j = 0; j < 4; j++) {
+      const int wi = hl * 4 + j, o = q8k_word_offset(b, wi >> 3, wi & 7);
+      *(uint32_t*)(qs + o) = pack4(q + 4 * j);
+      if (PAIR) dsmem_st_u32(pqs + o, pack4(q + 4 * j));
+    }
+  }
 }
 
 // The first NT threads of the CTA must call (named barrier BAR); each owns 16 consecutive elements per pass.
@@ -392,59 +543,14 @@ __device__ __forceinline__ void stage_activation(const MVParams& xs, const NormP
         if (nw) load16(nw + base, valid, w);
         if (nb_) load16(nb_ + base, valid, bb);
       }
-#pragma unroll
-      for (int e = 0; e < 16; e++) {
-        float y = v[e];
-        if (norm_mode == NORM_LAYER) y = __fsub_rn(y, mean);
-        y = __fmul_rn(y, scale);
-        if (nw) y = __fmul_rn(y, w[e]);
-        if (nb_) y = __fadd_rn(y, bb[e]);
-        v[e] = y;
-      }
+      norm_apply16(v, w, bb, norm_mode, mean, scale, nw != nullptr, nb_ != nullptr);
     }
     if (write_norm && norm_out && valid > 0) {
 #pragma unroll
       for (int e = 0; e < 16; e++) if (e < valid) norm_out[base + e] = v[e];
     }
     if (act == ACT_Q8_K) {
-      // reference quantize_row_q8_K_reference (k_quants.c:1191-1226): the first element with the largest |x| fixes the sign;
-      // iscale = -128/max; q = min(127, nearest_int(iscale*x)); the reference BINARY fuses iscale*x + 12582912.f (vfmadd), so
-      // the exact product is rounded once — __fmaf_rn.  d = 1/iscale; bsums per 16.  16 lanes (a half-warp) share a block.
-      float amax = 0.f, mx = 0.f;
-#pragma unroll
-      for (int e = 0; e < 16; e++) { const float ax = fabsf(v[e]); if (ax > amax) { amax = ax; mx = v[e]; } }
-      float gmax = amax;
-#pragma unroll
-      for (int o = 8; o > 0; o >>= 1) gmax = fmaxf(gmax, __shfl_xor_sync(0xffffffffu, gmax, o));
-      const unsigned who = __ballot_sync(0xffffffffu, amax == gmax);
-      const int hbase = lane & 16, hl = lane & 15;
-      const unsigned mine = (who >> hbase) & 0xffffu;
-      const float maxv = __shfl_sync(0xffffffffu, mx, hbase + __ffs(mine) - 1);
-      if (valid > 0) {
-        const int b = base >> 8;
-        int q[16];
-        int sum = 0;
-        if (gmax == 0.f) {
-#pragma unroll
-          for (int e = 0; e < 16; e++) q[e] = 0;
-          if (hl == 0) dd[b] = 0.f;
-        } else {
-          const float iscale = __fdiv_rn(-128.f, maxv);
-#pragma unroll
-          for (int e = 0; e < 16; e++) {
-            const float val = __fmaf_rn(iscale, v[e], 12582912.f);
-            q[e] = min(127, (__float_as_int(val) & 0x007fffff) - 0x00400000);
-            sum += q[e];
-          }
-          if (hl == 0) dd[b] = __fdiv_rn(1.f, iscale);
-        }
-        bs[b * 16 + hl] = (int16_t)sum;
-#pragma unroll
-        for (int j = 0; j < 4; j++) {
-          const int wi = hl * 4 + j;
-          *(uint32_t*)(qs + q8k_word_offset(b, wi >> 3, wi & 7)) = pack4(q + 4 * j);
-        }
-      }
+      quant_q8k16(v, base, valid, lane, qs, dd, bs);
     } else if (act == ACT_Q8_0) {
       // quantize_row_q8_0, AVX2 variant (ggml.c:1232-1268): d = amax/127 kept as fp16, id = 127/amax, round-half-even
       float amax = 0.f;
@@ -489,6 +595,82 @@ __device__ __forceinline__ void stage_activation(const MVParams& xs, const NormP
     }
   }
   bar_sync<BAR, NT>();
+}
+
+// stage_activation's Q8_K staging split over the two CTAs of a cluster (the paired k_step launch, stream.cuh): rank r loads,
+// normalises and quantizes the whole blocks [pair_block0(nb, r), pair_block0(nb, r + 1)) and stores them into both CTAs'
+// images; the norm statistic's per-warp partials cross over too (pair_sum2_max_f64).  Each block is quantized from the same
+// floats by the same code as in stage_activation, and norm_stat gives the reference's float whatever the order of
+// the partial sums (its bound holds for every order, and its fallback adds the whole vector in element order), so both images
+// are stage_activation's bits.  A thread holds at most two groups of 16 (the host pairs only programs where that suffices:
+// step_pair_fits), and both are loaded before either is used.  write_norm: this pair writes norm_out, each rank its blocks.
+template <int NT, int BAR>
+__device__ __forceinline__ void stage_q8k_pair(const MVParams& xs, const NormPre& np, uint8_t* smem, double* red, PairX& px, bool write_norm) {
+  const int K = xs.K, nb = K >> 8, norm_mode = xs.norm_mode, t = threadIdx.x, lane = t & 31;
+  const int lo = pair_block0(nb, (int)px.rank) * 256, hi = pair_block0(nb, (int)px.rank + 1) * 256;
+  const int base[2] = {lo + t * 16, lo + (t + NT) * 16};
+  float v[2][16];   // zeros past hi
+  load16x(xs, base[0], hi - base[0], v[0]);
+  load16x(xs, base[1], hi - base[1], v[1]);
+  // ---- statistics
+  float mean = 0.f, scale = 1.f;
+  if (norm_mode == NORM_RMS) {
+    double ss = 0.0;
+#pragma unroll
+    for (int h = 0; h < 2; h++)
+#pragma unroll
+      for (int e = 0; e < 16; e++) ss += (double)__fmul_rn(v[h][e], v[h][e]);
+    const float m = norm_stat<NT, BAR, false, true>(ss, ss, 0.0, true, NORM_TERM_SQ, 0.f, xs, red, 0, &px);
+    scale = __fdiv_rn(1.0f, __fsqrt_rn(__fadd_rn(m, xs.eps)));
+  } else if (norm_mode == NORM_LAYER) {
+    double s1 = 0.0, a1 = 0.0;
+    unsigned emin = 255;
+#pragma unroll
+    for (int h = 0; h < 2; h++)
+#pragma unroll
+      for (int e = 0; e < 16; e++) {
+        s1 += (double)v[h][e];
+        a1 += (double)fabsf(v[h][e]);
+        emin = min_exp(emin, v[h][e]);
+      }
+    mean = norm_stat<NT, BAR, false, true>(s1, a1, lsb_inv(emin), false, NORM_TERM_X, 0.f, xs, red, 0, &px);
+    double s2 = 0.0;
+#pragma unroll
+    for (int h = 0; h < 2; h++)
+      if (base[h] < hi) {
+#pragma unroll
+        for (int e = 0; e < 16; e++) { const float d = __fsub_rn(v[h][e], mean); s2 += (double)__fmul_rn(d, d); }
+      }
+    const float var = norm_stat<NT, BAR, false, true>(s2, s2, 0.0, true, NORM_TERM_DEV, mean, xs, red, 0, &px);
+    scale = __fdiv_rn(1.0f, __fsqrt_rn(__fadd_rn(var, xs.eps)));
+  }
+  // ---- normalise + quantize into both images
+  int8_t* qs = (int8_t*)smem;
+  float* dd = (float*)(smem + (((size_t)K + 15) & ~(size_t)15));
+  int16_t* bs = (int16_t*)((uint8_t*)dd + q8k_d_bytes(K));
+  const uint32_t peer = px.rank ^ 1u, pqs = dsmem_map(qs, peer), pdd = dsmem_map(dd, peer), pbs = dsmem_map(bs, peer);
+#pragma unroll
+  for (int h = 0; h < 2; h++) {
+    if (lo + (((h * NT + t) * 16) & ~511) >= hi) continue;   // warp-uniform: this warp has no elements in this group
+    const int valid = hi - base[h];
+    if (norm_mode != NORM_NONE) {
+      float w[16], bb[16];
+      if (h == 0) {
+#pragma unroll
+        for (int e = 0; e < 16; e++) { w[e] = np.w0[e]; bb[e] = np.bias0[e]; }
+      } else {
+        if (xs.norm_w) load16(xs.norm_w + base[h], valid, w);
+        if (xs.norm_b) load16(xs.norm_b + base[h], valid, bb);
+      }
+      norm_apply16(v[h], w, bb, norm_mode, mean, scale, xs.norm_w != nullptr, xs.norm_b != nullptr);
+    }
+    if (write_norm && xs.norm_out && valid > 0) {
+#pragma unroll
+      for (int e = 0; e < 16; e++) xs.norm_out[base[h] + e] = v[h][e];
+    }
+    quant_q8k16<true>(v[h], base[h], valid, lane, qs, dd, bs, pqs, pdd, pbs);
+  }
+  pair_round<NT, BAR>(px);
 }
 
 // ---------------------------------------------------------------------------------------------

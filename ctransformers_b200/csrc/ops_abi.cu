@@ -105,15 +105,22 @@ unsigned* sync_words() {
   return d_sync;
 }
 
+// the step kernel's launch shape for a program, exactly as the engine chooses it (shared-memory limits set)
+StepLaunch plan_phases(const std::vector<Phase>& phs) {
+  StepLaunch L = step_launch_plan(phs.data(), (int)phs.size(), sm_count());
+  if (L.n_slots < ST_W) throw std::runtime_error("rows too long for the step kernel's shared memory");
+  OPS_CUDA(step_set_smem_limit(L.smem));
+  step_pair_choose(L, phs.data(), (int)phs.size());
+  return L;
+}
+
 // a program of phases through the persistent step kernel, exactly as the engine launches it
 void run_phases(std::vector<Phase> phs) {
   unsigned* d_sync = sync_words();
-  const StepLaunch L = step_launch_shape(phs.data(), (int)phs.size(), sm_count(), max_dyn_smem(k_step<true, false, false>));
+  const StepLaunch L = plan_phases(phs);
   const std::vector<int> hb = step_bounds(phs.data(), (int)phs.size(), L.grid);
   DevMem dbounds(hb.size() * 4);
   OPS_CUDA(cudaMemcpy(dbounds.get(), hb.data(), hb.size() * 4, cudaMemcpyHostToDevice));
-  if (L.n_slots < ST_W) throw std::runtime_error("rows too long for the step kernel's shared memory");
-  OPS_CUDA(step_set_smem_limit(L.smem));
   DevMem dprog((phs.size() + 1) * sizeof(Phase));
   OPS_CUDA(cudaMemcpy(dprog.get(), phs.data(), phs.size() * sizeof(Phase), cudaMemcpyHostToDevice));
   OPS_CUDA(launch_step(L, 0, dprog.as<Phase>(), dbounds.as<int>(), (int)phs.size(), d_sync));
@@ -373,6 +380,18 @@ int ctb_norm_path(int path, int mode, const float* x, const float* w, const floa
   });
 }
 
+int ctb_norm_path_cluster(int n) {
+  int cluster = -1;
+  const int rc = guarded("ctb_norm_path_cluster", [&] {
+    if (n < 256 || n % 256) throw std::runtime_error("the step kernel takes n a positive multiple of 256");
+    MVParams p{};
+    p.K = n; p.act = ACT_Q8_K; p.nseg = 1; p.norm_mode = NORM_RMS;
+    p.seg[0].w.type = GT_Q4_K; p.seg[0].w.K = n; p.seg[0].w.M = 16; p.seg[0].w.nb = n / 256;
+    cluster = step_paired(plan_phases({matvec_phase(p)}), false) ? 2 : 1;
+  });
+  return rc == 0 ? cluster : rc;
+}
+
 int ctb_rope(float* x, int n_heads, int head_dim, int pos, int mode, float freq_base, float freq_scale) {
   return guarded("ctb_rope", [&] {
     const int half = head_dim / 2;
@@ -480,7 +499,7 @@ int ctb_attention_path(int path, const float* q, const float* k_new, const float
       if (path == 1) {
         Phase ph{};
         ph.kind = PH_ATTN; ph.q6 = 1; ph.at = ap;
-        const StepLaunch L = step_launch_shape(&ph, 1, sm_count(), max_dyn_smem(k_step<true, false, false>));
+        const StepLaunch L = step_launch_plan(&ph, 1, sm_count());
         if (!st_attn_ring_ok(n_ctx, L.n_slots)) throw std::runtime_error("the step kernel's ring cannot carry K / V at this n_ctx");
       }
       const size_t smem = attn_smem_bytes(n_ctx, hd);
@@ -634,6 +653,17 @@ int ctb_matvec_partition(const int* types, const int* rows, int nseg, int K, int
   meta[0] = n_sm; meta[1] = ST_SLOT; meta[2] = ST_MAXT; meta[3] = ts.ntiles; meta[4] = ST_W; meta[5] = ST_ROWS; meta[6] = (int)max_items;
   meta[7] = st_chunk_blocks(GT_Q4_K) | (st_chunk_blocks(GT_Q5_K) << 8) | (st_chunk_blocks(GT_Q6_K) << 16) | (st_chunk_blocks(GT_Q3_K) << 24);
   return 0;
+}
+
+// Host-side view of how the paired step kernel splits the staging of a K-wide input (no GPU needed): block0[r] = first Q8_K
+// block of cluster rank r (block0[2] = the end); returns 1 when a program of such phases can run paired (step_pair_fits), else 0.
+int ctb_stage_pair_split(int K, int* block0) {
+  if (K <= 0 || K % 256 != 0) return -1;
+  for (int r = 0; r < 3; r++) block0[r] = pair_block0(K / 256, r);
+  Phase ph{};
+  ph.kind = PH_MATVEC;
+  ph.mv.K = K;
+  return step_pair_fits(&ph, 1) ? 1 : 0;
 }
 
 int ctb_get_row(int type, const void* table_blocks, int K, int n_rows, int row, float* out) {

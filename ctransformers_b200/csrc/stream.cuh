@@ -30,6 +30,8 @@
 //
 // Algorithmic HBM bytes: the GGUF bytes of the weights, once per token (same byte count in the stream layout).
 #pragma once
+#include <stdexcept>
+#include <string>
 #include "matvec.cuh"
 
 namespace ctb {
@@ -823,8 +825,8 @@ __device__ __forceinline__ void st_attn_phase(const Phase& ph, uint8_t* act_smem
     }
   }
 }
-// (one copy per kernel build, Q3: ptxas fits an out-of-line function's registers to all its callers at once)
-template <bool Q3>
+// (one copy per kernel build, Q3 and PAIR: ptxas fits an out-of-line function's registers to all its callers at once)
+template <bool Q3, bool PAIR>
 static __device__ __noinline__ uint32_t st_attn_phase_gen(const Phase& ph, uint8_t* act_smem, uint8_t* ring, uint64_t* full_bar, uint64_t* empty_bar, int n_slots,
                                                    uint32_t seq, float* pick_v, double* red) {
   st_attn_phase<true>(ph, act_smem, ring, full_bar, empty_bar, n_slots, seq, pick_v, red);
@@ -889,14 +891,16 @@ __device__ __forceinline__ void st_producer(const StepArgs& args, uint8_t* ring,
 // Consumer side of one mat-vec phase.  `seq` is the running item number (identical in every warp and in the producer).
 // XC: the build of the kernel that can exchange partial vectors between ranks (tensor-parallel mode); the single-GPU build
 // carries none of that code.  Q3: the build for programs that hold Q3_K matrices (the others carry none of its code).
-template <bool XC, bool Q3>
+// PAIR: the build launched as clusters of two CTAs, which stage the input together (stage_q8k_pair).
+template <bool XC, bool Q3, bool PAIR>
 __device__ __forceinline__ void st_matvec_phase(const Phase& ph, const NormPre& np, uint8_t* ring, uint8_t* act_smem, double* red, uint64_t* full_bar, uint64_t* empty_bar,
                                                 float (*mailbox)[ST_STATE * 32], int* flags, uint32_t S, uint32_t& seq, const int* tb, unsigned long long* tr,
-                                                unsigned xc_base) {
+                                                unsigned xc_base, PairX& px) {
   const MVParams& p = ph.mv;
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const unsigned epoch = XC ? xc_base + (unsigned)ph.xc.index + 1u : 0u;   // number of the exchange this phase consumes / produces (if any)
-  stage_activation<ST_NT, ST_BAR, XC>(p, np, ACT_Q8_K, act_smem, red, blockIdx.x == 0, epoch);
+  if constexpr (PAIR) stage_q8k_pair<ST_NT, ST_BAR>(p, np, act_smem, red, px, blockIdx.x < 2);
+  else stage_activation<ST_NT, ST_BAR, XC>(p, np, ACT_Q8_K, act_smem, red, blockIdx.x == 0, epoch);
   StAct a = st_act_extras<ST_NT, ST_BAR>(act_smem, p.K, ph.q6 != 0);
   a.xc = XC && ph.xc.role == 2 ? &ph.xc : nullptr;
   a.epoch = epoch;
@@ -977,8 +981,10 @@ __device__ __forceinline__ void grid_rearm(unsigned* sync, bool set_xc = false, 
 // and the kernels of the other models (GEN = false) have no trace of them.  The tensor-sharded mode takes heads of 64 / 128
 // only, so there is no exchange kernel with GEN.  Q3: some phase of the program holds a Q3_K matrix or embedding table.  The
 // builds without it compile to the same instructions as before Q3_K was added; with the Q3_K code inlined into every build,
-// ptxas spilled more in the builds of the other models (DESIGN.md §6).
-template <bool XC, bool GEN, bool Q3>
+// ptxas spilled more in the builds of the other models (DESIGN.md §6).  PAIR: launched as clusters of two CTAs, which
+// stage every mat-vec input together (stage_q8k_pair); the builds without it carry none of that code.  The exchange build
+// (XC) is never paired: its staging sums the peers' partial vectors and CTA 0 alone writes sum_out.
+template <bool XC, bool GEN, bool Q3, bool PAIR = false>
 static __global__ void __launch_bounds__(ST_THREADS, 1) k_step(const __grid_constant__ StepArgs args) {
   extern __shared__ __align__(16) uint8_t smem[];
   __shared__ __align__(8) uint64_t full_bar[ST_MAX_SLOTS];
@@ -990,10 +996,23 @@ static __global__ void __launch_bounds__(ST_THREADS, 1) k_step(const __grid_cons
   __shared__ int pick_i[ST_W];
   __shared__ __align__(16) Phase ph_s[2];   // this phase's descriptor and the next one's (fetched with cp.async a phase ahead)
   __shared__ int tb_s[2][2];                // first / end tile of this CTA, same double buffering
+  __shared__ __align__(8) uint64_t pair_bar[PAIR ? 2 : 1];    // PAIR: the exchange rounds of stage_q8k_pair (PairX)
+  __shared__ double pair_red[PAIR ? 2 * 2 * 3 * ST_W : 1];
   const int warp = threadIdx.x >> 5;
   uint8_t* ring = smem;
   uint8_t* act_smem = smem + (size_t)args.n_slots * ST_SLOT;
   ring_init(full_bar, empty_bar, args.n_slots, 1);
+  PairX px{pair_bar, pair_red, 0u, 0u};
+  if constexpr (PAIR) {
+    if (threadIdx.x == 0) {
+      mbar_init(&pair_bar[0], 1);
+      mbar_init(&pair_bar[1], 1);
+      asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+    }
+    px.rank = cluster_ctarank();
+    // both CTAs' mbarriers are initialised before either CTA arrives on the other's
+    asm volatile("barrier.cluster.arrive.release.aligned;\n barrier.cluster.wait.acquire.aligned;" ::: "memory");
+  }
   pdl_trigger();
   pdl_wait();           // (the producer reads device state too: the position decides how many K / V items an attention phase has)
   if (warp == ST_W) {
@@ -1037,14 +1056,15 @@ static __global__ void __launch_bounds__(ST_THREADS, 1) k_step(const __grid_cons
     const Phase& ph = ph_s[ip & 1];
     fetch_phase(ip + 1);
     NormPre np;
-    if (ph.kind == PH_MATVEC) preload_norm(np, ph.mv);
+    if (ph.kind == PH_MATVEC) preload_norm(np, ph.mv, PAIR ? pair_block0(ph.mv.K >> 8, (int)px.rank) * 256 : 0);
     if (tr && threadIdx.x == 0) tr[0] = globaltimer_ns();
     if (XC && ph.kind == PH_MATVEC && ph.xc.role == 1) xc_done++;
     if (ph.kind == PH_MATVEC) {
       // (the tile bounds were written by threads 0/1 above; the barriers inside the activation staging order them)
-      st_matvec_phase<XC, Q3>(ph, np, ring, act_smem, red, full_bar, empty_bar, mailbox, flags, (uint32_t)(args.n_slots / ST_W), seq, &tb_s[ip & 1][0], tr, xc_base);
+      st_matvec_phase<XC, Q3, PAIR>(ph, np, ring, act_smem, red, full_bar, empty_bar, mailbox, flags, (uint32_t)(args.n_slots / ST_W), seq, &tb_s[ip & 1][0], tr,
+                                    xc_base, px);
     } else if (ph.kind == PH_ATTN) {
-      if (GEN) seq = st_attn_phase_gen<Q3>(ph, act_smem, ring, full_bar, empty_bar, args.n_slots, seq, pick_v, red);
+      if (GEN) seq = st_attn_phase_gen<Q3, PAIR>(ph, act_smem, ring, full_bar, empty_bar, args.n_slots, seq, pick_v, red);
       else st_attn_phase<false>(ph, act_smem, ring, full_bar, empty_bar, args.n_slots, seq, pick_v, red);
     } else if (ph.kind == PH_EMBED) {
       if (blockIdx.x == 0) embed_row<Q3>(ph.em, ph.em.tokens[0], ph.em.out, threadIdx.x, ST_NT);
@@ -1062,7 +1082,7 @@ static __global__ void __launch_bounds__(ST_THREADS, 1) k_step(const __grid_cons
 
 // ---------------------------------------------------------------------------------------------
 // Host side
-struct StepLaunch { int grid; int n_slots; size_t smem; bool gen = false, q3 = false; /* k_step<.., GEN, Q3>: see k_step */ };
+struct StepLaunch { int grid; int n_slots; size_t smem; bool gen = false, q3 = false, pair = false; /* k_step<.., GEN, Q3, PAIR>: see k_step */ };
 
 // shared-memory budget: ring slots fill what the largest activation image of the program leaves
 inline StepLaunch step_launch_shape(const Phase* phases, int n, int n_sm, size_t max_dyn_smem, size_t extra_act = 0) {
@@ -1133,13 +1153,70 @@ static inline cudaError_t step_set_smem_limit(size_t bytes) {
   return cudaSuccess;
 }
 
+// Programs with Q3_K matrices are never paired: with the paired staging inlined, their builds spilled more than the unpaired
+// ones (DESIGN.md §6), so there are no paired Q3 builds.
+inline bool step_paired(const StepLaunch& L, bool xchg) { return L.pair && !L.q3 && !xchg; }
+using StepKernel = void (*)(StepArgs);
+inline StepKernel step_kernel(const StepLaunch& L, bool xchg) {
+  if (xchg) return L.q3 ? k_step<true, false, true> : k_step<true, false, false>;
+  if (step_paired(L, xchg)) return L.gen ? k_step<false, true, false, true> : k_step<false, false, false, true>;
+  return L.q3 ? (L.gen ? k_step<false, true, true> : k_step<false, false, true>) : (L.gen ? k_step<false, true, false> : k_step<false, false, false>);
+}
+
+// Can every mat-vec phase of the program be staged by a pair of CTAs?  Rank 0 holds the larger half of the blocks, 16
+// elements per thread and group, at most two groups (stage_q8k_pair): K <= 80 blocks = 20480 with 320 consumer threads.
+inline bool step_pair_fits(const Phase* phases, int n) {
+  for (int i = 0; i < n; i++)
+    if (phases[i].kind == PH_MATVEC && pair_block0(phases[i].mv.K >> 8, 1) * 16 > 2 * ST_NT) return false;
+  return true;
+}
+
+// the environment knob CTB_ST_CLUSTER=0 keeps the step kernel one CTA per cluster
+inline bool step_pair_wanted() {
+  const char* e = getenv("CTB_ST_CLUSTER");
+  return !(e && e[0] == '0');
+}
+
+// step_launch_shape with the dynamic shared memory of the builds that may run the program: the paired builds hold the
+// exchange state of stage_q8k_pair in static shared memory, so a program that may run paired sizes its ring for them.
+inline StepLaunch step_launch_plan(const Phase* phases, int n, int n_sm, size_t extra_act = 0) {
+  StepLaunch L = step_launch_shape(phases, n, n_sm, max_dyn_smem(k_step<true, false, false>), extra_act);
+  if (!L.q3 && step_pair_wanted())
+    L = step_launch_shape(phases, n, n_sm, std::min(max_dyn_smem(k_step<false, false, false, true>), max_dyn_smem(k_step<false, true, false, true>)), extra_act);
+  return L;
+}
+
+// Launch the step kernel as clusters of two CTAs, which split every activation staging between them (stage_q8k_pair), when
+// pairs are wanted, the program has no Q3_K matrix (step_paired), the grid pairs up, the program fits the split, and all
+// grid / 2 clusters are resident at once at this shared-memory size: the grid barrier needs every CTA running.  L must come
+// from step_launch_plan (possibly with fewer ring slots).  Sets the shared-memory limit of the paired build it chooses.
+inline bool step_pair_choose(StepLaunch& L, const Phase* phases, int n) {
+  L.pair = false;
+  if (!step_pair_wanted() || L.q3 || L.grid % 2 || !step_pair_fits(phases, n)) return false;
+  StepLaunch P = L;
+  P.pair = true;
+  const StepKernel k = step_kernel(P, false);
+  auto check = [](cudaError_t e) {   // (the ring was sized for the paired build: a failure here is an error, not a reason to fall back)
+    if (e != cudaSuccess) throw std::runtime_error(std::string("pairing the step kernel: ") + cudaGetErrorString(e));
+  };
+  check(cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)L.smem));
+  cudaLaunchConfig_t cfg{};
+  cfg.gridDim = dim3(L.grid); cfg.blockDim = dim3(ST_THREADS); cfg.dynamicSmemBytes = L.smem;
+  cudaLaunchAttribute at[1];
+  at[0].id = cudaLaunchAttributeClusterDimension;
+  at[0].val.clusterDim.x = 2; at[0].val.clusterDim.y = 1; at[0].val.clusterDim.z = 1;
+  cfg.attrs = at; cfg.numAttrs = 1;
+  int clusters = 0;
+  check(cudaOccupancyMaxActiveClusters(&clusters, k, &cfg));
+  L.pair = clusters >= L.grid / 2;
+  return L.pair;
+}
+
 static inline cudaError_t launch_step(const StepLaunch& L, cudaStream_t st, const Phase* d_prog, const int* d_bounds, int n_phases, unsigned* d_sync, bool pdl = false,
                                       unsigned long long* trace = nullptr, bool xchg = false) {
   StepArgs a;
   a.prog = d_prog; a.bounds = d_bounds; a.n_phases = n_phases; a.n_slots = L.n_slots; a.sync = d_sync; a.trace = trace;
-  auto kernel = L.q3 ? (xchg ? k_step<true, false, true> : (L.gen ? k_step<false, true, true> : k_step<false, false, true>))
-                     : (xchg ? k_step<true, false, false> : (L.gen ? k_step<false, true, false> : k_step<false, false, false>));
-  return launch_kernel(kernel, dim3(L.grid), dim3(ST_THREADS), L.smem, st, pdl, a);
+  return launch_kernel_cluster(step_kernel(L, xchg), dim3(L.grid), dim3(ST_THREADS), L.smem, st, pdl, step_paired(L, xchg) ? 2u : 1u, a);
 }
 
 }  // namespace ctb

@@ -80,6 +80,7 @@ EXTRA_PROTOTYPES = {
     "ctb_quantize_row_q8_1": (C.c_int, [_P, _P, C.c_int]),
     "ctb_norm": (C.c_int, [C.c_int, _P, _P, _P, _P, C.c_int, C.c_float]),
     "ctb_norm_path": (C.c_int, [C.c_int, C.c_int, _P, _P, _P, _P, C.c_int, C.c_float]),
+    "ctb_norm_path_cluster": (C.c_int, [C.c_int]),
     "ctb_rope": (C.c_int, [_P, C.c_int, C.c_int, C.c_int, C.c_int, C.c_float, C.c_float]),
     "ctb_attention": (C.c_int, [_P, _P, _P, _P, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_float]),
     "ctb_attention_path": (C.c_int, [C.c_int, _P, _P, _P, _P, _P, _P, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, _P, C.c_int,
@@ -87,8 +88,10 @@ EXTRA_PROTOTYPES = {
     "ctb_prefill_mul_mat": (C.c_int, [C.c_int, _P, _P, _P, C.c_int, C.c_int, _P, _P, C.c_int, _P, _P, C.c_float, _P, _P, _P, _P, C.c_int,
                                       C.c_int, _P]),
     "ctb_llm_paths": (C.c_long, [_P, _IP, C.c_int]),
+    "ctb_llm_step_cluster": (C.c_int, [_P]),
     "ctb_ffn_gate": (C.c_int, [C.c_int, _P, _P, _P, _P, C.c_int, C.c_int]),
     "ctb_matvec_partition": (C.c_int, [_IP, _IP, C.c_int, C.c_int, C.c_int, _IP, _IP]),
+    "ctb_stage_pair_split": (C.c_int, [C.c_int, _IP]),
     "ctb_get_row": (C.c_int, [C.c_int, _P, C.c_int, C.c_int, C.c_int, _P]),
     "ctb_argmax_path": (C.c_int, [C.c_int, _P, C.c_int, _IP]),
     "ctb_sample_topk": (C.c_int, [_P, C.c_int, _IP, C.c_int, C.c_float, C.c_int, _IP, _P]),

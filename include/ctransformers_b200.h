@@ -105,6 +105,9 @@ double ctb_llm_time_matvec_kinds(LLM* llm, int reps, long* launches, unsigned ki
  * kernel (ST_W per slot depth), batched prefill available (tries to set it up), batched prefill launches so far, tokens
  * evaluated by single-token steps so far}.  Returns the entries written (6), or -6 when cap is smaller, < 0 on error. */
 long ctb_llm_paths(LLM* llm, int* out, int cap);
+/* CTAs per cluster the decode-step kernel is launched with: 2 = pairs that stage each mat-vec input together, 1 = single CTAs
+ * (CTB_ST_CLUSTER=0, or the GPU or the model does not allow pairs) */
+int ctb_llm_step_cluster(LLM* llm);
 
 /* Host-only pieces of the boundary, callable without a GPU: the GGUF vocabulary with its SPM / BPE tokenizer
  * (llama.cpp:1648-1760, 3080-3427, 6151-6187) and the sampler chain of llama_llm::Sample (llama.cc:53-84). */
@@ -134,6 +137,8 @@ int ctb_norm(int mode, const float* x, const float* w, const float* b, float* y,
  *           the normalised vector CTA 0 writes, as the engine's result_norm / embeddings; n a positive multiple of 256
  * 0 on success, -1 (with a message on stderr) otherwise. */
 int ctb_norm_path(int path, int mode, const float* x, const float* w, const float* b, float* y, int n, float eps);
+/* CTAs per cluster of the step-kernel launch ctb_norm_path's path 1 makes at width n (2 = a CTA pair stages the input), -1 on error. */
+int ctb_norm_path_cluster(int n);
 /* ggml_rope_custom on [n_heads][head_dim] at position pos; mode 0 or 2 (neox) (ggml.c:12430-12566). */
 int ctb_rope(float* x, int n_heads, int head_dim, int pos, int mode, float freq_base, float freq_scale);
 /* One query token (at position T-1) against T cached positions, all heads, exactly as the reference's attention block:
@@ -184,6 +189,8 @@ int ctb_ffn_gate(int type, const void* w1_blocks, const void* w3_blocks, const f
  * bytes, tiles alive per CTA (mailboxes), tiles, consumer warps per CTA, rows per tile, work items of the largest CTA,
  * blocks per work item as Q4_K | Q5_K << 8 | Q6_K << 16 | Q3_K << 24}.  0 on success. */
 int ctb_matvec_partition(const int* types, const int* rows, int nseg, int K, int n_sm, int* first_tile, int* meta);
+/* the paired step kernel's split of a K-wide input's staging: block0[0..2] = first block of cluster rank 0, 1, end; 1 = pairable */
+int ctb_stage_pair_split(int K, int* block0);
 
 int ctb_get_row(int type, const void* table_blocks, int K, int n_rows, int row, float* out);
 
