@@ -815,7 +815,12 @@ __device__ __forceinline__ float dot_f32_row(const DevMat& w, int row, const uin
   return sumf;
 }
 
-__device__ __forceinline__ float table_f16(const uint16_t* tab, float x) { return h2f(__ldg(tab + f2h(x))); }
+// The table entry as F16C widens it: a NaN keeps its sign and payload (h2f's conversion would give the canonical NaN).  The
+// tables hold NaNs where the reference's activation of an out-of-range index is one, e.g. SiLU(-inf) = -inf / inf.
+__device__ __forceinline__ float table_f16(const uint16_t* tab, float x) {
+  const uint16_t h = __ldg(tab + f2h(x));
+  return (h & 0x7fffu) > 0x7c00u ? __uint_as_float(((uint32_t)(h & 0x8000u) << 16) | 0x7f800000u | ((uint32_t)(h & 0x3ffu) << 13)) : h2f(h);
+}
 
 // The value an output element stores: the row's sum v with the segment's epilogue.  res / res2 point at this element's
 // residuals (read by EPI_ADD / EPI_ADD2 only); they may have been written earlier in the same persistent kernel: L2-coherent loads.

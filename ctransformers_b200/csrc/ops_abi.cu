@@ -114,8 +114,8 @@ StepLaunch plan_phases(const std::vector<Phase>& phs) {
   return L;
 }
 
-// a program of phases through the persistent step kernel, exactly as the engine launches it
-void run_phases(std::vector<Phase> phs) {
+// a program of phases through the persistent step kernel, exactly as the engine launches it; returns the launch it made
+StepLaunch run_phases(std::vector<Phase> phs) {
   unsigned* d_sync = sync_words();
   const StepLaunch L = plan_phases(phs);
   const std::vector<int> hb = step_bounds(phs.data(), (int)phs.size(), L.grid);
@@ -126,14 +126,20 @@ void run_phases(std::vector<Phase> phs) {
   OPS_CUDA(launch_step(L, 0, dprog.as<Phase>(), dbounds.as<int>(), (int)phs.size(), d_sync));
   OPS_CUDA(cudaGetLastError());
   OPS_CUDA(cudaDeviceSynchronize());
+  return L;
 }
 
-void run_matvec(MVParams& p) {
+// which kernel ran a mat-vec: k_step (1) or k_matvec (0), and the CTAs per cluster of its launch
+struct MatvecLaunch { int kernel, cluster; };
+
+// a mat-vec routed as Engine::push_matvec routes it, run `repeat` times back to back: one step-kernel program of that many
+// phases, or that many k_matvec launches
+MatvecLaunch run_matvec(MVParams& p, int repeat = 1) {
   p.silu_tab = tables().silu;
   p.gelu_tab = tables().gelu;
   if (step_supports(p)) {
-    run_phases({matvec_phase(p)});
-    return;
+    const StepLaunch L = run_phases(std::vector<Phase>(repeat, matvec_phase(p)));
+    return {1, step_paired(L, false) ? 2 : 1};
   }
   static bool attr = false;
   if (!attr) {
@@ -141,8 +147,9 @@ void run_matvec(MVParams& p) {
     attr = true;
   }
   const MVLaunch L = matvec_launch_shape(p, sm_count());
-  OPS_CUDA(launch_matvec_kernel(L, 0, p));
+  for (int r = 0; r < repeat; r++) OPS_CUDA(launch_matvec_kernel(L, 0, p));
   OPS_CUDA(cudaGetLastError());
+  return {0, 1};
 }
 
 // standalone wrappers around the prologue pieces, so the activation quantizers can be checked bit-for-bit
@@ -604,6 +611,62 @@ int ctb_prefill_mul_mat(int nseg, const int* types, const void* const* w_blocks,
       OPS_CUDA(cudaMemcpy(out + (size_t)b * W, dout.get(), (size_t)n * W * 4, cudaMemcpyDeviceToHost));
     }
     if (n_slots) *n_slots = slots;
+  });
+}
+
+int ctb_decode_mul_mat(int nseg, const int* types, const void* const* w_blocks, const int* rows, int K, int n_tok, const float* x,
+                       const float* x2, int norm_mode, const float* norm_w, const float* norm_b, float eps, const int* epi,
+                       const float* res, const float* res2, float* out, float* norm_out, int repeat, int* launch) {
+  return guarded("ctb_decode_mul_mat", [&] {
+    if (nseg < 1 || nseg > MV_MAX_SEG) throw std::runtime_error("1 to 3 segments");
+    if (K < 1) throw std::runtime_error("K must be positive");
+    if (n_tok < 1) throw std::runtime_error("n_tok must be at least 1");
+    if (repeat < 1 || repeat > 4) throw std::runtime_error("repeat must be 1 to 4");
+    if (norm_mode < NORM_NONE || norm_mode > NORM_LAYER || (x2 && norm_mode != NORM_NONE)) throw std::runtime_error("norm mode 0, 1 or 2, and 0 with x2");
+    if ((norm_mode != NORM_NONE && !norm_w) || (norm_mode == NORM_LAYER && !norm_b)) throw std::runtime_error("RMSNorm needs norm_w, LayerNorm norm_w and norm_b");
+    if (norm_mode == NORM_NONE) norm_w = nullptr;
+    if (norm_mode != NORM_LAYER) norm_b = nullptr;
+    int off[MV_MAX_SEG + 1] = {0};
+    for (int s = 0; s < nseg; s++) {
+      if (act_format_for(types[s]) != act_format_for(types[0])) throw std::runtime_error("the segments of one phase share an activation format");
+      if (rows[s] < 1) throw std::runtime_error("every segment needs at least one row");
+      if (epi[s] < EPI_STORE || epi[s] > EPI_SILU) throw std::runtime_error("unknown epilogue");
+      if ((epi[s] == EPI_ADD || epi[s] == EPI_ADD2) && !res) throw std::runtime_error("ADD / ADD2 need res");
+      if (epi[s] == EPI_ADD2 && !res2) throw std::runtime_error("ADD2 needs res2");
+      off[s + 1] = off[s] + rows[s];
+    }
+    const int W = off[nseg];
+    std::vector<DevMem> keep;
+    DevMat mats[MV_MAX_SEG];
+    for (int s = 0; s < nseg; s++) mats[s] = upload(keep, types[s], w_blocks[s], K, rows[s]);
+    // one buffer of each kind, reused by every token's launch like the engine's decode buffers
+    DevMem dx((size_t)K * 4), dx2((size_t)K * 4), dnw((size_t)K * 4), dnb((size_t)K * 4), dnorm((size_t)K * 4), dout((size_t)W * 4),
+        dres((size_t)W * 4), dres2((size_t)W * 4);
+    OPS_CUDA(cudaMemset(dout.get(), 0xff, (size_t)W * 4));
+    OPS_CUDA(cudaMemset(dnorm.get(), 0xff, (size_t)K * 4));
+    if (norm_w) OPS_CUDA(cudaMemcpy(dnw.get(), norm_w, (size_t)K * 4, cudaMemcpyHostToDevice));
+    if (norm_b) OPS_CUDA(cudaMemcpy(dnb.get(), norm_b, (size_t)K * 4, cudaMemcpyHostToDevice));
+    MVParams p{};
+    p.x = dx.as<float>(); p.x2 = x2 ? dx2.as<float>() : nullptr; p.x_mode = x2 ? 1 : 0;
+    p.norm_w = norm_w ? dnw.as<float>() : nullptr; p.norm_b = norm_b ? dnb.as<float>() : nullptr; p.norm_out = norm_out ? dnorm.as<float>() : nullptr;
+    p.norm_mode = norm_mode; p.eps = eps; p.K = K; p.act = act_format_for(types[0]); p.nseg = nseg;
+    for (int s = 0; s < nseg; s++) {
+      p.seg[s].w = mats[s]; p.seg[s].out = dout.as<float>() + off[s]; p.seg[s].epi = epi[s];
+      if (epi[s] == EPI_ADD || epi[s] == EPI_ADD2) p.seg[s].res = dres.as<float>() + off[s];
+      if (epi[s] == EPI_ADD2) p.seg[s].res2 = dres2.as<float>() + off[s];
+    }
+    MatvecLaunch ran{};
+    for (int i = 0; i < n_tok; i++) {   // one launch per token, as decode steps come
+      OPS_CUDA(cudaMemcpy(dx.get(), x + (size_t)i * K, (size_t)K * 4, cudaMemcpyHostToDevice));
+      if (x2) OPS_CUDA(cudaMemcpy(dx2.get(), x2 + (size_t)i * K, (size_t)K * 4, cudaMemcpyHostToDevice));
+      if (res) OPS_CUDA(cudaMemcpy(dres.get(), res + (size_t)i * W, (size_t)W * 4, cudaMemcpyHostToDevice));
+      if (res2) OPS_CUDA(cudaMemcpy(dres2.get(), res2 + (size_t)i * W, (size_t)W * 4, cudaMemcpyHostToDevice));
+      ran = run_matvec(p, repeat);
+      OPS_CUDA(cudaDeviceSynchronize());
+      OPS_CUDA(cudaMemcpy(out + (size_t)i * W, dout.get(), (size_t)W * 4, cudaMemcpyDeviceToHost));
+      if (norm_out) OPS_CUDA(cudaMemcpy(norm_out + (size_t)i * K, dnorm.get(), (size_t)K * 4, cudaMemcpyDeviceToHost));
+    }
+    if (launch) { launch[0] = ran.kernel; launch[1] = ran.cluster; }
   });
 }
 

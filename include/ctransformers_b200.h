@@ -181,6 +181,23 @@ int ctb_attention_path(int path, const float* q, const float* k_new, const float
 int ctb_prefill_mul_mat(int nseg, const int* types, const void* const* w_blocks, const int* rows, int K, int n_tok, const float* x,
                         const float* x2, int norm_mode, const float* norm_w, const float* norm_b, float eps, const int* epi,
                         const float* res, const float* res2, float* out, int n_ctx, int head_dim, int* n_slots);
+/* n_tok activation rows through one mat-vec phase of a decode step, routed and launched as the engine does it: K-quant matrices
+ * (Q3_K / Q4_K / Q5_K / Q6_K) go to the persistent step kernel (k_step), its launch shape chosen as the engine chooses it
+ * (clusters of two CTAs that split the input's staging unless CTB_ST_CLUSTER=0, the input is wider than 80 Q8_K blocks, or a
+ * matrix is Q3_K); every other type goes to k_matvec with its own activation format (Q8_0, Q8_1, F16 or F32).  Each token is
+ * a launch of its own on the same device buffers.  The first arguments and the result are those of ctb_prefill_mul_mat, with
+ * any weight type and K a whole number of the types' blocks; then:
+ *   norm_out  optional [n_tok][K]: the phase's input after the prologue (the normalised vector, x * x2, or x), as the output
+ *             head writes the embeddings
+ *   repeat    1..4: the phase runs that many times back to back (one step-kernel program of that many phases, or that many
+ *             k_matvec launches); every run writes the same values
+ *   launch    output [2] (may be null): {kernel: 1 k_step, 0 k_matvec; CTAs per cluster: 1 or 2}
+ * 0 on success, -1 (with a message on stderr) for what the engine never builds: segments of different activation formats, x2
+ * with a norm, ADD / ADD2 without res / res2, K not a whole number of blocks, 0 or more than 3 segments, or a K too wide for
+ * the step kernel's shared memory. */
+int ctb_decode_mul_mat(int nseg, const int* types, const void* const* w_blocks, const int* rows, int K, int n_tok, const float* x,
+                       const float* x2, int norm_mode, const float* norm_w, const float* norm_b, float eps, const int* epi,
+                       const float* res, const float* res2, float* out, float* norm_out, int repeat, int* launch);
 /* silu(W1 x) * (W3 x) with the fp16 SiLU table (ggml.c:3625-3632) — the fused FFN gate. */
 int ctb_ffn_gate(int type, const void* w1_blocks, const void* w3_blocks, const float* x, float* out, int K, int M);
 /* ggml_get_rows on a quantized table (ggml.c:11615-11642). */

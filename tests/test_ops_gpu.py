@@ -10,8 +10,12 @@ import functools
 import numpy as np
 import pytest
 
+import q3k_refs
+import q41_q51_refs
 import refs
 from conftest import ptr
+from q3k_refs import Q3_K
+from q41_q51_refs import Q4_1, Q5_1
 from refs import F16, F32, Q4_0, Q4_K, Q5_0, Q5_K, Q6_K, Q8_0, Q8_K, row_bytes
 
 pytestmark = pytest.mark.gpu
@@ -62,10 +66,13 @@ def test_quantize_q8_0_bit_exact(lib, k):
         assert np.array_equal(a, b)
 
 
-def _same_bits(got, want):
+def _same_bits(got, want, what=""):
     got, want = np.ascontiguousarray(got, np.float32), np.ascontiguousarray(want, np.float32)
     bad = got.view(np.uint32) != want.view(np.uint32)
-    assert not bad.any(), f"{int(bad.sum())} of {bad.size} values differ; max |diff| {np.abs(got - want).max():.3e}"
+    if bad.any():
+        at = tuple(int(i) for i in np.argwhere(bad)[0])
+        raise AssertionError(f"{what}{': ' if what else ''}{int(bad.sum())} of {bad.size} values differ, the first at {at} "
+                             f"({got[at]!r} for {want[at]!r}); max |diff| {np.abs(got - want).max():.3e}")
 
 
 @pytest.mark.parametrize("t", [Q4_K, Q5_K, Q6_K, Q4_0, Q5_0, Q8_0])
@@ -363,12 +370,25 @@ PF_SHAPES = {
     # the Falcon-7B-shaped Q5_K_M layer: LayerNorm + fused wqkv and up (GELU), down + attention output + layer input
     "falcon7b-qkv-up": ([(Q5_K, 4736, STORE), (Q5_K, 18432, GELU)], 4608, 3, 2, False, "random"),
     "falcon7b-down": ([(Q6_K, 4608, ADD2)], 18432, 3, 0, False, "random"),
+    # the output heads: the 7B's (RMSNorm, the embeddings written beside the logits) and the Falcon-7B-shaped one (LayerNorm)
+    "7b-head": ([(Q6_K, 32000, STORE)], 4096, 3, 1, False, "random"),
+    "falcon7b-head": ([(Q6_K, 65024, STORE)], 4608, 3, 2, False, "random"),
 }
+
+
+def _weights(t, k, m, seed, src):
+    """m rows of k type-t weights from source src (PF_SOURCES); Q3_K, Q4_1 and Q5_1 from their checkers' own block makers."""
+    if t == Q3_K:
+        return q3k_refs.blocks(src, k, m, seed)
+    if t in (Q4_1, Q5_1):
+        Q = q41_q51_refs
+        return {"random": Q.random_blocks, "refq": Q.reference_quantized_blocks, "edge": Q.edge_blocks}[src](t, k, m, seed)
+    return np.ascontiguousarray(PF_SOURCES[src](t, k, m, seed))
 
 
 def _pf_inputs(segs, k, n_tok, norm, with_x2, src, seed):
     rng = np.random.default_rng(seed)
-    ws = [np.ascontiguousarray(PF_SOURCES[src](t, k, m, seed + 10 * i)) for i, (t, m, _) in enumerate(segs)]
+    ws = [_weights(t, k, m, seed + 10 * i, src) for i, (t, m, _) in enumerate(segs)]
     x = np.stack([_act(rng, k, [1e-3, 1.0, 300.0][i % 3]) for i in range(n_tok)])
     x[0, :256] = 0.0                                                  # an all-zero block: Q8_K d = 0
     x2 = np.stack([_act(rng, k, 0.5) for _ in range(n_tok)]) if with_x2 else None
@@ -380,7 +400,25 @@ def _pf_inputs(segs, k, n_tok, norm, with_x2, src, seed):
     return ws, x, x2, nw, nb, res, res2
 
 
+def _oracle_mul_mat(t, w, y, k, m):
+    """[n_tok][m]: ggml_mul_mat of m rows of type-t weights by the rows y, each quantized to the type's activation format; F16
+    weights take ggml_vec_dot_f16 on y rounded to f16, as in test_mul_mat_f16_weights."""
+    n_tok = y.shape[0]
+    if t == F16:
+        o = refs.oracle()
+        o.orc_vec_dot_f16.restype = C.c_float
+        w16, y16 = w.view(np.float16).reshape(m, k), y.astype(np.float16)
+        return np.array([[o.orc_vec_dot_f16(k, ptr(w16[j]), ptr(y16[i])) for j in range(m)] for i in range(n_tok)], np.float32)
+    if t in (Q3_K, Q4_1, Q5_1):
+        return (q3k_refs if t == Q3_K else q41_q51_refs).mul_mat(t, w, y, k, m, n_tok).reshape(n_tok, m)
+    v = np.zeros((n_tok, m), np.float32)
+    assert refs.oracle().orc_mul_mat(t, ptr(w), ptr(y), ptr(v), k, m, n_tok) == 0
+    return v
+
+
 def _pf_expected(segs, ws, k, x, x2, norm, nw, nb, res, res2, eps=1e-5):
+    """(out, y): y = the rows the mat-muls take (the normalised rows, x * x2, or x), out = every segment's mat-mul of y with its
+    epilogue, side by side."""
     o = refs.oracle()
     n_tok = x.shape[0]
     y = np.zeros_like(x)
@@ -393,8 +431,7 @@ def _pf_expected(segs, ws, k, x, x2, norm, nw, nb, res, res2, eps=1e-5):
             y[i] = x[i] if x2 is None else x[i] * x2[i]
     outs, off = [], 0
     for (t, m, epi), w in zip(segs, ws):
-        v = np.zeros((n_tok, m), np.float32)
-        assert o.orc_mul_mat(t, ptr(w), ptr(y), ptr(v), k, m, n_tok) == 0
+        v = _oracle_mul_mat(t, w, y, k, m)
         if epi == ADD:
             v = v + res[:, off:off + m]
         elif epi == ADD2:
@@ -405,7 +442,7 @@ def _pf_expected(segs, ws, k, x, x2, norm, nw, nb, res, res2, eps=1e-5):
             v = a
         outs.append(v)
         off += m
-    return np.concatenate(outs, axis=1)
+    return np.concatenate(outs, axis=1), y
 
 
 def _pf_run(lib, segs, ws, k, x, x2, norm, nw, nb, res, res2, n_ctx=512, hd=128, eps=1e-5):
@@ -425,7 +462,7 @@ def _pf_run(lib, segs, ws, k, x, x2, norm, nw, nb, res, res2, n_ctx=512, hd=128,
 def _pf_case(t, src):
     segs = [(t, 37, STORE)]
     ws, x, x2, nw, nb, res, res2 = _pf_inputs(segs, 11008, max(PF_TOKENS), 0, False, src, seed=t)
-    return segs, ws, x, res, res2, nw, nb, _pf_expected(segs, ws, 11008, x, None, 0, nw, nb, res, res2)
+    return segs, ws, x, res, res2, nw, nb, _pf_expected(segs, ws, 11008, x, None, 0, nw, nb, res, res2)[0]
 
 
 @pytest.mark.parametrize("src", list(PF_SOURCES))
@@ -439,10 +476,7 @@ def test_prefill_mul_mat_types_and_weight_sources(lib, t, src):
     for n in PF_TOKENS:
         rc, got, _ = _pf_run(lib, segs, ws, 11008, x[:n], None, 0, nw, nb, res[:n], res2[:n])
         assert rc == 0
-        try:
-            _same_bits(got, want[:n])
-        except AssertionError as e:
-            raise AssertionError(f"n_tok {n}: {e}") from None
+        _same_bits(got, want[:n], f"n_tok {n}")
 
 
 @functools.lru_cache(maxsize=None)
@@ -452,12 +486,19 @@ def _pf_shape_expected(case):
     return (ws, x, x2, nw, nb, res, res2), _pf_expected(segs, ws, k, x, x2, norm, nw, nb, res, res2)
 
 
-@pytest.mark.parametrize("case", list(PF_SHAPES))
-def test_prefill_mul_mat_shapes(lib, case):
+@pytest.mark.parametrize("case,kernel", [pytest.param(c, "prefill", id=c) for c in PF_SHAPES] +
+                         [pytest.param(c, "decode", id=f"decode-{c}") for c in PF_SHAPES])
+def test_prefill_mul_mat_shapes(lib, monkeypatch, case, kernel):
     """Rows below one tile, single-tile grids, several segments of different types and epilogues in one phase, x_mode 1, RMSNorm
-    and LayerNorm prologues, and the 7B-shaped projections the prefill2048 bench runs: bit-exact with the oracle."""
+    and LayerNorm prologues, the 7B-shaped projections the prefill2048 bench runs and the output heads: bit-exact with the
+    oracle, through the batched prefill kernel and through the decode step's mat-vec phase in both its launch shapes (there
+    the phase's input, as norm_out, too)."""
     segs, k, n_tok, norm, with_x2, src = PF_SHAPES[case]
-    (ws, x, x2, nw, nb, res, res2), want = _pf_shape_expected(case)
+    (ws, x, x2, nw, nb, res, res2), (want, y) = _pf_shape_expected(case)
+    if kernel == "decode":
+        for paired in _launch_shapes(monkeypatch):
+            _dec_check(lib, segs, ws, k, (x, x2, norm, nw, nb, res, res2), (want, y), _dec_launch(paired, k), f"paired {paired}")
+        return
     rc, got, _ = _pf_run(lib, segs, ws, k, x, x2, norm, nw, nb, res, res2)
     assert rc == 0
     _same_bits(got, want)
@@ -485,7 +526,7 @@ def test_prefill_mul_mat_deepest_and_shallowest_ring(lib):
             hi = mid
     segs = [(Q6_K, 40, STORE), (Q5_K, 24, ADD), (Q4_K, 20, SILU)]
     ws, x, x2, nw, nb, res, res2 = _pf_inputs(segs, 11008, 70, 1, False, "edge", seed=5)
-    want = _pf_expected(segs, ws, 11008, x, None, 1, nw, nb, res, res2)
+    want, _ = _pf_expected(segs, ws, 11008, x, None, 1, nw, nb, res, res2)
     depths = {}
     for n_ctx in (16, lo):
         rc, got, depths[n_ctx] = _pf_run(lib, segs, ws, 11008, x, None, 1, nw, nb, res, res2, n_ctx=n_ctx, hd=hd)
@@ -507,3 +548,239 @@ def test_prefill_mul_mat_refuses_what_the_kernel_cannot_take(lib):
                                    None, None, ptr(r), 512, 128, None) == -1
     assert _pf_run(lib, [(Q4_K, 4, STORE)] * 4, [w] * 4, 512, x, None, 0, x[0], x[0], r, r)[0] == -1
     assert _pf_run(lib, [(Q4_K, 16, STORE)], [w], 512, x[:0], None, 0, x[0], x[0], r, r)[0] == -1
+
+
+# ---- the decode step's mat-vec phase through ctb_decode_mul_mat: routed as the engine routes it, K-quant matrices to the
+# persistent step kernel (csrc/stream.cuh k_step), the other types to k_matvec, one launch per token.  The step kernel runs in
+# clusters of two CTAs that split the input's norm, normalisation and Q8_K quantization (csrc/matvec.cuh stage_q8k_pair) unless
+# CTB_ST_CLUSTER=0 or the input is wider than 80 Q8_K blocks; every test runs both launch shapes in one process and checks the
+# launch it meant to test.  Expected values: _pf_expected, as for the batched prefill kernel.
+DEC_PAIR_MAX_NB = 80                           # widest input a pair stages: 40 blocks per rank, two groups of 16 per thread
+DEC_SEGS = [(Q4_K, 17, ADD), (Q6_K, 5, SILU), (Q5_K, 30, GELU)]
+DEC_NORMS = {"none": (0, False), "rms": (1, False), "layer": (2, False), "x_mode1": (0, True)}   # name: (norm mode, x2)
+NORM_KS = (256, 512, 1024, 4096, 4608, 8192, 11008)   # test_norm_order.KS that the step kernel takes
+
+
+def _launch_shapes(monkeypatch):
+    """Yields False with CTB_ST_CLUSTER=0, then True with pairs wanted (the default); step_pair_wanted reads the variable on
+    every plan."""
+    monkeypatch.setenv("CTB_ST_CLUSTER", "0")
+    yield False
+    monkeypatch.delenv("CTB_ST_CLUSTER")
+    yield True
+
+
+def _dec_launch(paired, k):
+    """The {kernel, CTAs per cluster} a K-quant phase of width k must get: k_step, paired when pairs are wanted and k fits."""
+    return 1, 2 if paired and k // 256 <= DEC_PAIR_MAX_NB else 1
+
+
+def _pair_block0(nb, rank):
+    """csrc/matvec.cuh pair_block0: the first Q8_K block rank 0 / 1 stages (rank 0 takes the odd block); 2 gives nb."""
+    return (0, (nb + 1) // 2, nb)[rank]
+
+
+def _dec_run(lib, segs, ws, k, x, x2, norm, nw, nb, res, res2, repeat=1, eps=1e-5):
+    """ctb_decode_mul_mat on the rows of x; returns (rc, out, norm_out, (kernel, CTAs per cluster))."""
+    n_tok, nseg = x.shape[0], len(segs)
+    types, rows, epi = (np.array([s[j] for s in segs] or [0], np.int32) for j in range(3))
+    wp = (C.c_void_p * max(nseg, 1))(*[w.ctypes.data for w in ws])
+    out = np.full((n_tok, int(rows[:nseg].sum())), np.nan, np.float32)
+    y = np.full((n_tok, k), np.nan, np.float32)
+    launch = np.full(2, -1, np.int32)
+    opt = lambda a: None if a is None else ptr(a)
+    rc = lib.ctb_decode_mul_mat(nseg, ptr(types), C.cast(wp, C.c_void_p), ptr(rows), k, n_tok, ptr(x), opt(x2), norm, opt(nw), opt(nb), eps,
+                                ptr(epi), opt(res), opt(res2), ptr(out), ptr(y), repeat, ptr(launch))
+    return rc, out, y, tuple(int(v) for v in launch)
+
+
+def _dec_check(lib, segs, ws, k, inputs, expected, launch, what, repeat=1, eps=1e-5):
+    """One ctb_decode_mul_mat call: the launch it reports, out and norm_out against expected = (out, y) bit for bit."""
+    rc, got, got_y, ran = _dec_run(lib, segs, ws, k, *inputs, repeat=repeat, eps=eps)
+    assert rc == 0, what
+    assert ran == launch, f"{what}: launched {ran}, meant {launch}"
+    _same_bits(got, expected[0], f"{what}: out")
+    _same_bits(got_y, expected[1], f"{what}: norm_out")
+
+
+@functools.lru_cache(maxsize=None)
+def _dec_inputs(nb):
+    """_pf_inputs for DEC_SEGS at width 256·nb (tokens at scales 1e-3, 1 and 300, edge weights), with planted blocks: token 0 has
+    block 0 and rank 1's first block all zero, token 1 the block a pair's rank 0 stages beyond rank 1's count (nb odd), and
+    token 2 |max| ties in the first two blocks of each rank (one warp's two half-warps): in each block the largest |x| twice,
+    with both signs, in two threads of the block, the first one negative in one block and positive in the next.  The norm
+    weights are 1 at the tied elements, so that RMSNorm keeps the ties, and so is x2."""
+    k = 256 * nb
+    ws, x, x2, nw, nbias, res, res2 = _pf_inputs(DEC_SEGS, k, 3, 0, True, "edge", seed=7000 + nb)
+    b1 = _pair_block0(nb, 1)
+    if b1 < nb:
+        x[0, 256 * b1:256 * (b1 + 1)] = 0.0
+    if nb % 2:
+        x[1, 256 * (b1 - 1):256 * b1] = 0.0
+    big = np.float32(4 * np.abs(x[2]).max())
+    for b in sorted({0, b1} - {nb}):
+        for j, (first, second) in enumerate([(16 * 2 + 3, 16 * 9 + 1), (16 * 1 + 5, 16 * 14 + 2)][:min(2, nb - b)]):
+            i0, i1 = 256 * (b + j) + first, 256 * (b + j) + second
+            sign = np.float32(-1 if j == 0 else 1)
+            x[2, i0], x[2, i1] = sign * big, -sign * big
+            nw[[i0, i1]] = 1.0
+            x2[2, [i0, i1]] = 1.0
+    return ws, x, x2, nw, nbias, res, res2
+
+
+def _dec_modes(nb):
+    """(name, inputs, expected) of every DEC_NORMS mode on _dec_inputs(nb)."""
+    ws, x, x2, nw, nbias, res, res2 = _dec_inputs(nb)
+    for name, (norm, with_x2) in DEC_NORMS.items():
+        inputs = (x, x2 if with_x2 else None, norm, nw, nbias, res, res2)
+        yield name, inputs, _pf_expected(DEC_SEGS, ws, 256 * nb, *inputs)
+
+
+@pytest.mark.parametrize("nb", list(range(1, DEC_PAIR_MAX_NB + 2)) + [112])
+def test_decode_mul_mat_widths(lib, monkeypatch, nb):
+    """Every input width the paired staging splits differently, K = 256·nb: nb odd (rank 0 stages the extra block), nb = 1 (rank
+    1 stages nothing), nb >= 41 (a thread's second group of 16), nb = 80 (40 blocks per rank fill both groups), nb = 81 and the
+    28672-wide down projection's 112 (unpaired).  Each width runs three segments of different types and epilogues without a
+    norm, with RMSNorm, with LayerNorm and on x * x2 (x_mode 1); at the widths of NORM_KS also the rows whose fp64 norm sums
+    round differently in another order (refs.norm_order_rows), so that the element-order fallback runs in the paired build."""
+    k = 256 * nb
+    ws = _dec_inputs(nb)[0]
+    cases = list(_dec_modes(nb))
+    if k in NORM_KS:
+        for mode in (1, 2):
+            rows, w, b = refs.norm_order_rows(mode, k, seed=k + mode)
+            z = np.zeros((rows.shape[0], sum(m for _, m, _ in DEC_SEGS)), np.float32)
+            inputs = (rows, None, mode, w, b, z, z)
+            cases.append((f"planted {mode}", inputs, _pf_expected(DEC_SEGS, ws, k, *inputs, eps=refs.NORM_ORDER_EPS)))
+    for paired in _launch_shapes(monkeypatch):
+        for name, inputs, expected in cases:
+            eps = refs.NORM_ORDER_EPS if name.startswith("planted") else 1e-5
+            _dec_check(lib, DEC_SEGS, ws, k, inputs, expected, _dec_launch(paired, k), f"nb {nb}, {name}, paired {paired}", eps=eps)
+
+
+def _dec_accepts(lib, nb):
+    segs = [(t, 1, STORE) for t, _, _ in DEC_SEGS]
+    ws = [refs.edge_blocks(t, 256 * nb, 1, 0) for t, _, _ in segs]
+    x = np.ones((1, 256 * nb), np.float32)
+    z = np.zeros((1, len(segs)), np.float32)
+    return _dec_run(lib, segs, ws, 256 * nb, x, None, 0, None, None, z, z)[0] == 0
+
+
+def test_decode_mul_mat_widest_input(lib, monkeypatch):
+    """The widest input the step kernel's shared memory takes beside its ring (found by bisection, in each launch shape: the
+    paired builds hold more static shared memory) runs every mode bit-exact, and one block wider is refused."""
+    for paired in _launch_shapes(monkeypatch):
+        lo, hi = 112, 1024
+        assert _dec_accepts(lib, lo) and not _dec_accepts(lib, hi)
+        while hi - lo > 1:
+            mid = (lo + hi) // 2
+            lo, hi = (mid, hi) if _dec_accepts(lib, mid) else (lo, mid)
+        for name, inputs, expected in _dec_modes(lo):
+            _dec_check(lib, DEC_SEGS, _dec_inputs(lo)[0], 256 * lo, inputs, expected, (1, 1), f"nb {lo}, {name}, paired {paired}")
+
+
+@pytest.mark.parametrize("nb", [43, 72])
+def test_decode_mul_mat_exchange_rounds(lib, monkeypatch, nb):
+    """A pair's exchange rounds alternate two mbarriers and two partial buffers, and a phase takes one round (no norm), two
+    (RMSNorm) or three (LayerNorm): the same phase 1, 2 and 3 times in one launch reaches every parity sequence, and every
+    repeat must give the oracle's bits."""
+    ws = _dec_inputs(nb)[0]
+    for paired in _launch_shapes(monkeypatch):
+        for name, inputs, expected in _dec_modes(nb):
+            for repeat in (1, 2, 3):
+                _dec_check(lib, DEC_SEGS, ws, 256 * nb, inputs, expected, _dec_launch(paired, 256 * nb), f"{name}, repeat {repeat}, paired {paired}",
+                           repeat=repeat)
+
+
+def _pow2_scaled(t, w, m):
+    """Edge blocks of type t with each row's d (and dmin) set to ±2^e, e cycling from -24 (the smallest f16 subnormal) to 15."""
+    blk = w.reshape(-1, refs.BLOCK[t][1]).copy()
+    rows = blk.reshape(m, -1, blk.shape[1])
+    e = np.arange(m) % 40 - 24
+    d = (np.exp2(e) * np.where(np.arange(m) % 3 == 1, -1, 1)).astype(np.float16).view(np.uint8).reshape(m, 1, 2)
+    for at in ((208,) if t == Q6_K else (0, 2)):
+        rows[:, :, at:at + 2] = d
+    return np.ascontiguousarray(rows.reshape(-1))
+
+
+def test_mul_mat_epilogue_fp16_range(lib, monkeypatch):
+    """Row values across the whole fp16 range meet the SiLU / GELU tables (indexed by the value rounded to fp16): zeros,
+    subnormals, normals and values past 65504 (the index is ±inf; SiLU(-inf) and GELU(-inf) are NaNs whose sign and payload
+    the output keeps, as the reference's F16C conversion does); and the ADD / ADD2 residual sums with residuals that cancel
+    the row value exactly.  Through the decode step's mat-vec phase in both launch shapes and the batched prefill."""
+    k, m = 1024, 40
+    base = [(Q4_K, m, STORE), (Q5_K, m, STORE), (Q6_K, m, STORE)]
+    ws, x, _, nw, nbias, res, res2 = _pf_inputs(base, k, 3, 0, False, "edge", seed=99)
+    ws = [_pow2_scaled(t, w, m) for (t, _, _), w in zip(base, ws)]
+    x[0] *= np.float32(1e-3)
+    v, _ = _pf_expected(base, ws, k, x, None, 0, nw, nbias, res, res2)
+    a = np.abs(v)
+    ranges = {"fp16 zero": a < 2.0 ** -25, "fp16 subnormal": (a >= 2.0 ** -25) & (a < 2.0 ** -14), "fp16 normal": (a >= 2.0 ** -14) & (a <= 65504),
+              "fp16 inf": a >= 65520}
+    assert all(r.any() for r in ranges.values()), {n: int(r.sum()) for n, r in ranges.items()}
+    cancel = np.arange(3 * m) % 2 == 0
+    res = np.where(cancel, -v, res).astype(np.float32)              # v + res: exactly 0
+    res2 = np.where(cancel, np.float32(-0.0), res2).astype(np.float32)
+    res2[:, 1::4] = -(v + res)[:, 1::4]                               # (v + res) + res2: exactly 0
+    for segs in ([(Q4_K, m, SILU), (Q5_K, m, GELU), (Q6_K, m, ADD)], [(Q4_K, m, ADD2), (Q5_K, m, ADD), (Q6_K, m, ADD2)]):
+        inputs = (x, None, 0, nw, nbias, res, res2)
+        want, y = _pf_expected(segs, ws, k, *inputs)
+        for paired in _launch_shapes(monkeypatch):
+            _dec_check(lib, segs, ws, k, inputs, (want, y), _dec_launch(paired, k), f"{segs}, paired {paired}")
+        rc, got, _ = _pf_run(lib, segs, ws, k, x, None, 0, nw, nbias, res, res2)
+        assert rc == 0
+        _same_bits(got, want, f"{segs}, prefill")
+
+
+# name: (segments, K, weight source); the activation formats Q8_0 (Q4_0 / Q5_0 / Q8_0), Q8_1 (Q4_1 / Q5_1) and F16
+DEC_LEGACY = {
+    "q8_0-k4544": ([(Q4_0, 21, ADD), (Q5_0, 9, SILU), (Q8_0, 36, GELU)], 4544, "refq"),
+    "q8_0-k11008": ([(Q8_0, 21, ADD2), (Q4_0, 9, GELU), (Q5_0, 36, SILU)], 11008, "refq"),
+    "q8_1-k4544": ([(Q4_1, 21, ADD), (Q5_1, 9, SILU), (Q4_1, 36, GELU)], 4544, "edge"),
+    "q8_1-k11008": ([(Q5_1, 21, ADD2), (Q4_1, 9, GELU), (Q5_1, 36, SILU)], 11008, "random"),
+    "f16-k1000": ([(F16, 7, ADD2), (F16, 9, GELU)], 1000, "random"),
+    "f16-k4544": ([(F16, 5, SILU), (F16, 12, ADD)], 4544, "random"),
+}
+
+
+@pytest.mark.parametrize("case", list(DEC_LEGACY))
+def test_decode_mul_mat_legacy_types(lib, monkeypatch, case):
+    """The weight types the step kernel does not take run through k_matvec with the same prologues, x_mode 1 and epilogues,
+    at Falcon-7B's 4544 and Llama-7B's 11008 (neither a multiple of k_matvec's 8192 elements per pass)."""
+    segs, k, src = DEC_LEGACY[case]
+    ws, x, x2, nw, nbias, res, res2 = _pf_inputs(segs, k, 3, 0, True, src, seed=k + len(case))
+    for name, (norm, with_x2) in DEC_NORMS.items():
+        inputs = (x, x2 if with_x2 else None, norm, nw, nbias, res, res2)
+        expected = _pf_expected(segs, ws, k, *inputs)
+        for paired in _launch_shapes(monkeypatch):
+            _dec_check(lib, segs, ws, k, inputs, expected, (0, 1), f"{name}, paired {paired}")
+
+
+@pytest.mark.parametrize("k", [4096, 11008])
+def test_decode_mul_mat_q3k_unpaired(lib, monkeypatch, k):
+    """A phase with a Q3_K matrix (beside Q4_K and Q6_K ones, as in a Q3_K_M layer) runs k_step's Q3 build, never paired."""
+    segs = [(Q3_K, 17, ADD), (Q4_K, 5, SILU), (Q6_K, 30, GELU)]
+    ws, x, x2, nw, nbias, res, res2 = _pf_inputs(segs, k, 3, 0, True, "edge", seed=k + 3)
+    for name, (norm, with_x2) in DEC_NORMS.items():
+        inputs = (x, x2 if with_x2 else None, norm, nw, nbias, res, res2)
+        expected = _pf_expected(segs, ws, k, *inputs)
+        for paired in _launch_shapes(monkeypatch):
+            _dec_check(lib, segs, ws, k, inputs, expected, (1, 1), f"{name}, paired {paired}")
+
+
+def test_decode_mul_mat_refuses_what_the_engine_never_builds(lib):
+    w = refs.edge_blocks(Q4_K, 512, 16, 0)
+    x = np.ones((2, 512), np.float32)
+    r = np.zeros((2, 64), np.float32)
+    run = lambda segs, ws, k=512, x=x, x2=None, norm=0, res=r, res2=r, repeat=1: _dec_run(lib, segs, ws, k, x, x2, norm, x[0], x[0], res, res2,
+                                                                                         repeat=repeat)[0]
+    assert run([(Q4_K, 16, STORE)], [w]) == 0
+    assert run([(Q4_K, 16, STORE), (Q8_0, 16, STORE)], [w, _rand_weights(Q8_0, 512, 16, 0)]) == -1     # Q8_K beside Q8_0 activations
+    assert run([(Q4_K, 16, STORE)], [w], x2=x, norm=1) == -1
+    assert run([(Q4_K, 16, ADD)], [w], res=None) == -1
+    assert run([(Q4_K, 16, ADD2)], [w], res2=None) == -1
+    assert run([(Q4_K, 16, STORE)], [w], k=384, x=np.ones((2, 384), np.float32)) == -1
+    assert run([(Q4_0, 16, STORE)], [_rand_weights(Q4_0, 512, 16, 0)], k=48, x=np.ones((2, 48), np.float32)) == -1
+    assert run([], []) == -1
+    assert run([(Q4_K, 4, STORE)] * 4, [w] * 4) == -1
+    assert run([(Q4_K, 16, STORE)], [w], repeat=0) == -1 and run([(Q4_K, 16, STORE)], [w], repeat=5) == -1
