@@ -24,9 +24,9 @@
 #include <stdlib.h>
 #include <string.h>
 
+#include "ggml_oracle.h"
+
 /* from ggml_oracle.c */
-float orc_fp16_to_fp32(uint16_t h);
-uint16_t orc_fp32_to_fp16(float f);
 int orc_mul_mat(int type, const void *w, const float *x, float *dst, int K, int M, int N);
 void orc_rms_norm_mul(const float *x, const float *w, float *y, int n, float eps);
 void orc_layer_norm_mul_add(const float *x, const float *w, const float *b, float *y, int n, float eps);
@@ -42,6 +42,7 @@ void orc_dequantize_row_q4_K(const void *vx, float *y, int k);
 void orc_dequantize_row_q5_K(const void *vx, float *y, int k);
 void orc_dequantize_row_q6_K(const void *vx, float *y, int k);
 int orc_sizeof_block(int type);
+int orc_blck_size(int type);
 
 typedef struct { int type; int K; int M; const void *data; } orc_mat;
 
@@ -109,12 +110,14 @@ static void get_row(const orc_mat *t, int row, float *out) {
     const int K = t->K;
     if (t->type == 0) { memcpy(out, (const float *)t->data + (size_t)row * K, (size_t)K * 4); return; }
     if (t->type == 1) { const uint16_t *h = (const uint16_t *)t->data + (size_t)row * K; for (int i = 0; i < K; i++) out[i] = orc_fp16_to_fp32(h[i]); return; }
-    const int be = (t->type == 2 || t->type == 6 || t->type == 8) ? 32 : 256;
-    const char *p = (const char *)t->data + (size_t)row * (K / be) * orc_sizeof_block(t->type);
+    const char *p = (const char *)t->data + (size_t)row * (K / orc_blck_size(t->type)) * orc_sizeof_block(t->type);
     switch (t->type) {
         case 2: orc_dequantize_row_q4_0(p, out, K); break;
+        case 3: orc_dequantize_row_q4_1(p, out, K); break;
         case 6: orc_dequantize_row_q5_0(p, out, K); break;
+        case 7: orc_dequantize_row_q5_1(p, out, K); break;
         case 8: orc_dequantize_row_q8_0(p, out, K); break;
+        case 11: orc_dequantize_row_q3_K(p, out, K); break;
         case 12: orc_dequantize_row_q4_K(p, out, K); break;
         case 13: orc_dequantize_row_q5_K(p, out, K); break;
         case 14: orc_dequantize_row_q6_K(p, out, K); break;
@@ -142,7 +145,7 @@ static void matvec(const orc_mat *w, const float *x, float *y) {
 
 /* x = all-reduce over ranks of (rank 0: x + W_0 a_0; rank r: W_r a_r), W_r = columns [split[r], split[r+1]) of w (quantized types only) */
 static void matvec_row_parallel(const orc_mat *w, const float *a, float *x, int world, const int *split) {
-    const int be = (w->type == 2 || w->type == 6 || w->type == 8) ? 32 : 256, bb = orc_sizeof_block(w->type);
+    const int be = orc_blck_size(w->type), bb = orc_sizeof_block(w->type);
     const size_t full_row = (size_t)(w->K / be) * bb;
     float *part = (float *)malloc(sizeof(float) * w->M);
     for (int r = 0; r < world; r++) {
@@ -231,6 +234,17 @@ int orc_eval(orc_model *m, const int *tokens, int n, int n_past, float *logits, 
     for (int i = 0; i < n; i++) {
         if (tokens[i] < 0 || tokens[i] >= m->n_vocab) return -2;
         eval_token(m, tokens[i], n_past + i, n_past + n, i == n - 1, logits, embd);
+    }
+    return 0;
+}
+
+/* llama_eval with the context flag logits_all (llama.cpp:2949-2960): the same graph, with the output row of every token of
+ * the call copied out.  Token i's logits go to logits[i * n_vocab]; embd gets the last token's result_norm row. */
+int orc_eval_rows(orc_model *m, const int *tokens, int n, int n_past, float *logits, float *embd) {
+    if (n_past + n > m->n_ctx) return -1;
+    for (int i = 0; i < n; i++) {
+        if (tokens[i] < 0 || tokens[i] >= m->n_vocab) return -2;
+        eval_token(m, tokens[i], n_past + i, n_past + n, 1, logits + (size_t)i * m->n_vocab, i == n - 1 ? embd : NULL);
     }
     return 0;
 }

@@ -69,11 +69,6 @@ def _small_blocks(t, w):
     return out
 
 
-def oracle(name, path, n_ctx):
-    import refs
-    return refs.OracleModel(path, n_ctx) if name == SMALL else LA.oracle(name, path, n_ctx)
-
-
 def eos_of(name):
     return 11 if arch_of(name) == "falcon" else 2
 

@@ -24,7 +24,6 @@ import q3k_refs as Q  # noqa: E402
 import refs  # noqa: E402
 from refs import ptr  # noqa: E402
 
-refs.BLOCK.update(Q.BLOCK)   # the reference helpers size rows by refs.BLOCK
 KAT_K, KAT_M = 2048, 16
 
 

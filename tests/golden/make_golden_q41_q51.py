@@ -24,7 +24,6 @@ import q41_q51_refs as Q  # noqa: E402
 import refs  # noqa: E402
 from refs import ptr  # noqa: E402
 
-refs.BLOCK.update(Q.BLOCK)   # the reference helpers size rows by refs.BLOCK
 KAT_K, KAT_M = 1024, 8
 
 
@@ -57,7 +56,7 @@ def blocks():
         rng = np.random.default_rng(200 + t)
         scale = np.exp(rng.uniform(np.log(0.002), np.log(0.1), (32, 1)))   # weights of a model that stays finite and untied
         w = (rng.standard_normal((32, 1024)) * scale + rng.uniform(-0.5, 0.5, (32, 1)) * scale).astype(np.float32)
-        out[f"blocks_{t}"] = refs.ref_quantize(t, w).reshape(-1, Q.BLOCK[t][1])
+        out[f"blocks_{t}"] = refs.ref_quantize(t, w).reshape(-1, refs.BLOCK[t][1])
     np.savez_compressed(HERE / "q41_q51_blocks.npz", **out)
 
 

@@ -1,65 +1,17 @@
 """Model cases whose attention heads are neither 64 nor 128 wide (test infrastructure, never the product).
 
 Each case is a synthetic GGUF written from a seed; tests/golden/make_golden_head_dims.py runs it through the unmodified
-reference and stores what it computed in golden/head_dims_runs.npz.
-
-  * ``oracle()``     tests/head_dims_oracle.c (the unchanged oracle, whose whole-model attention can take a K·q tail the
-                     reference does not use), compiled on first use into a private temporary directory
-  * ``OracleModel``  refs.OracleModel on that library; ``variant`` selects the K·q tail (0: the reference's)
+reference and stores what it computed in golden/head_dims_runs.npz.  The oracle's whole-model attention can take a K·q tail
+the reference does not use: refs.variant("orc_hd_set_variant", TAIL_FP32 or TAIL_IN_LANES).
 """
-import atexit
-import ctypes as C
-import shutil
-import subprocess
-import tempfile
 from pathlib import Path
 
 import numpy as np
 
-import refs
-
-HERE = Path(__file__).resolve().parent
-GOLD = HERE / "golden"
-SRC = HERE / "head_dims_oracle.c"
+from refs import GOLD
 
 N_NEW = 8
 TAIL_FP32, TAIL_IN_LANES = 1, 2   # orc_hd_set_variant: the K·q tail summed in fp32, or folded into the SIMD lanes
-
-_lib = None
-
-
-def oracle():
-    global _lib
-    if _lib is None:
-        d = Path(tempfile.mkdtemp(prefix="head_dims_oracle_"))
-        atexit.register(shutil.rmtree, d, True)
-        so = d / "libheaddimsoracle.so"
-        subprocess.check_call(["gcc", "-O2", "-std=gnu11", "-fPIC", "-shared", "-mf16c", "-mavx2", "-mfma", "-ffp-contract=off",
-                               "-o", str(so), str(SRC), "-lm"])
-        o = C.CDLL(str(so))
-        o.orc_hd_set_variant.argtypes = [C.c_int]
-        _lib = o
-    return _lib
-
-
-class OracleModel(refs.OracleModel):
-    """refs.OracleModel whose attention heads go through orc_attn_head_hd with the given K·q tail variant."""
-
-    def __init__(self, path, n_ctx, variant=0):
-        saved = refs._oracle
-        refs._oracle = oracle()
-        try:
-            super().__init__(path, n_ctx)
-        finally:
-            refs._oracle = saved
-        self.variant = variant
-
-    def eval(self, *args, **kwargs):
-        self.o.orc_hd_set_variant(self.variant)
-        try:
-            return super().eval(*args, **kwargs)
-        finally:
-            self.o.orc_hd_set_variant(0)
 
 
 def model_cases():

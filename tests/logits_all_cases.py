@@ -10,18 +10,18 @@ BATCH_SIZES = (8, 64, 5)
 
 
 def _table(name):
-    """(arch, shape, ftype, ctx, prompt, builder, batch sizes, oracle class)"""
+    """(arch, shape, ftype, ctx, prompt, builder, batch sizes)"""
     if name in modelcases.CASES:
         arch, shape, ftype, ctx = modelcases.CASES[name]
-        return arch, shape, ftype, ctx, modelcases.prompt_for(name), modelcases.build, BATCH_SIZES, None
+        return arch, shape, ftype, ctx, modelcases.prompt_for(name), modelcases.build, BATCH_SIZES
     if name in H.model_cases():
         arch, shape, ftype, ctx, _, bss = H.model_cases()[name]
-        return arch, shape, ftype, ctx, H.prompt_for(name), H.build_model, bss, H.OracleModel
+        return arch, shape, ftype, ctx, H.prompt_for(name), H.build_model, bss
     if name in Q.model_cases():
         arch, shape, ftype, ctx, _, bss, _ = Q.model_cases()[name]
-        return arch, shape, ftype, ctx, Q.prompt_for(name), Q.build_model, bss, Q.OracleModel
+        return arch, shape, ftype, ctx, Q.prompt_for(name), Q.build_model, bss
     arch, shape, ftype, _, ctx, _ = Q1.model_cases()[name]
-    return arch, shape, ftype, ctx, Q1.prompt_for(name), Q1.build_model, Q1.BATCH_SIZES, Q1.OracleModel
+    return arch, shape, ftype, ctx, Q1.prompt_for(name), Q1.build_model, Q1.BATCH_SIZES
 
 
 def names():
@@ -46,56 +46,6 @@ def ctx(name):
 
 def prompt(name):
     return _table(name)[4]
-
-
-_libs = {}
-
-
-def oracle_lib(tu):
-    """tests/logits_all_oracle.c (the oracle plus orc_eval_all) on the oracle translation unit tu (None: the plain oracle)."""
-    if tu not in _libs:
-        import atexit
-        import ctypes as C
-        import shutil
-        import subprocess
-        import tempfile
-        from pathlib import Path
-        here = Path(__file__).resolve().parent
-        d = Path(tempfile.mkdtemp(prefix="logits_all_oracle_"))
-        atexit.register(shutil.rmtree, d, True)
-        so = d / "liblogitsalloracle.so"
-        define = [f'-DORACLE_TU="{tu}"'] if tu else []
-        subprocess.check_call(["gcc", "-O2", "-std=gnu11", "-fPIC", "-shared", "-mf16c", "-mavx2", "-mfma", "-ffp-contract=off", *define,
-                               "-o", str(so), str(here / "logits_all_oracle.c"), "-lm"])
-        o = C.CDLL(str(so))
-        o.orc_eval_all.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_void_p]
-        _libs[tu] = o
-    return _libs[tu]
-
-
-_TU = {H: "head_dims_oracle.c", Q: "q3k_oracle.c", Q1: "q41_q51_oracle.c"}
-
-
-def oracle(name, path, n_ctx=None):
-    """The whole-model oracle of the case (refs.OracleModel or its per-type subclass), at its context length by default, on a
-    library that also has orc_eval_all: the subclass's own oracle source with orc_eval_all appended."""
-    import refs
-    cls = _table(name)[7]
-    n_ctx = n_ctx or ctx(name)
-    if cls is None:
-        saved = refs._oracle
-        refs._oracle = oracle_lib(None)
-        try:
-            return refs.OracleModel(path, n_ctx)
-        finally:
-            refs._oracle = saved
-    mod = next(m for m in _TU if m.OracleModel is cls)
-    saved = mod._lib                 # the subclass loads its module's library through mod.oracle(), which returns mod._lib
-    mod._lib = oracle_lib(_TU[mod])
-    try:
-        return cls(path, n_ctx)
-    finally:
-        mod._lib = saved
 
 
 OVERFLOW = "overflow_llama_tiny_q4km"
@@ -150,15 +100,15 @@ def logprob_ref(rows, targets):
 
 
 def oracle_rows(model, tokens, batch_size, n_ctx):
-    """orc_eval_all, chunked and clamped as LLM::BatchEval: the row block of each chunk."""
+    """orc_eval_rows, chunked and clamped as LLM::BatchEval: the row block of each chunk."""
     import numpy as np
-    o = model.o   # (a model from oracle())
+    o = model.o   # (a refs.OracleModel)
     bs, blocks = min(n_ctx, batch_size), []
     for start in range(0, len(tokens), bs):
         chunk = np.array(tokens[start:start + bs], np.int32)
         past = min(n_ctx - len(chunk), model.n_past)
         rows = np.zeros((len(chunk), model.n_vocab), np.float32)
-        assert o.orc_eval_all(model.m, chunk.ctypes.data, len(chunk), past, rows.ctypes.data, model.embd.ctypes.data) == 0
+        assert o.orc_eval_rows(model.m, chunk.ctypes.data, len(chunk), past, rows.ctypes.data, model.embd.ctypes.data) == 0
         model.n_past += len(chunk)
         blocks.append(rows)
     return blocks

@@ -1,90 +1,41 @@
 """Checkers for the Q3_K weight type (test infrastructure, never the product).
 
-  * ``oracle()``     the plain-C restatement tests/q3k_oracle.c (which includes the unchanged oracle/ggml_oracle.c and
-                     oracle/llama_oracle.c), compiled on first use into a private temporary directory
+  * oracle helpers   the Q3_K dot, dequantizer and mat-mul of the one oracle library (refs.oracle())
   * block pools      ``reference_quantized_blocks`` (the reference quantizer's blocks, golden/q3k_blocks.npz) and ``edge_blocks``
-  * ``OracleModel``  refs.OracleModel bound to this library, so the whole-model oracle multiplies Q3_K matrices too
   * model cases      synthetic GGUF files in the Q3_K presets; tests/golden/make_golden_q3k.py stores what the unmodified
                      reference computed on them in golden/q3k_runs.npz
 """
-import atexit
-import ctypes as C
-import shutil
-import subprocess
-import tempfile
 from pathlib import Path
 
 import numpy as np
 
 import refs
-from refs import ptr
+from refs import GOLD, Q3_K, ptr
 
-HERE = Path(__file__).resolve().parent
-SRC = HERE / "q3k_oracle.c"
-GOLD = HERE / "golden"
-
-Q3_K = 11
-BLOCK = {Q3_K: (256, 110)}
 SCALE_FOLD_IN_FLOAT = 1   # orc_q3k_set_variant: a fold order the reference does not use
-
-_lib = None
-
-
-def oracle():
-    global _lib
-    if _lib is None:
-        d = Path(tempfile.mkdtemp(prefix="q3k_oracle_"))
-        atexit.register(shutil.rmtree, d, True)
-        so = d / "libq3koracle.so"
-        subprocess.check_call(["gcc", "-O2", "-std=gnu11", "-fPIC", "-shared", "-mf16c", "-mavx2", "-mfma", "-ffp-contract=off",
-                               "-o", str(so), str(SRC), "-lm"])
-        o = C.CDLL(str(so))
-        vp, i = C.c_void_p, C.c_int
-        o.orc_vec_dot_q3_K_q8_K.restype = C.c_float
-        o.orc_vec_dot_q3_K_q8_K.argtypes = [i, vp, vp]
-        o.orc_dequantize_row_q3_K.argtypes = [vp, vp, i]
-        o.orc_q3k_set_variant.argtypes = [i]
-        o.orc_mul_mat.restype = i
-        o.orc_mul_mat.argtypes = [i, vp, vp, vp, i, i, i]
-        o.orc_quantize_row_q8_K.argtypes = [vp, vp, i]
-        _lib = o
-    return _lib
-
-
-def row_bytes(t, k):
-    if t in BLOCK:
-        bs, sz = BLOCK[t]
-        assert k % bs == 0
-        return k // bs * sz
-    return refs.row_bytes(t, k)
 
 
 def quantize_q8_k(x):
     x = np.ascontiguousarray(x, np.float32)
     out = np.zeros(refs.row_bytes(refs.Q8_K, x.size), np.uint8)
-    oracle().orc_quantize_row_q8_K(ptr(x), ptr(out), x.size)
+    refs.oracle().orc_quantize_row_q8_K(ptr(x), ptr(out), x.size)
     return out
 
 
-def vec_dot(k, wrow, act, variant=0):
-    o = oracle()
-    o.orc_q3k_set_variant(variant)
-    try:
-        return float(o.orc_vec_dot_q3_K_q8_K(k, ptr(np.ascontiguousarray(wrow)), ptr(np.ascontiguousarray(act))))
-    finally:
-        o.orc_q3k_set_variant(0)
+def vec_dot(k, wrow, act):
+    return float(refs.oracle().orc_vec_dot_q3_K_q8_K(k, ptr(np.ascontiguousarray(wrow)), ptr(np.ascontiguousarray(act))))
 
 
 def dequantize(blocks, k):
     out = np.zeros(k, np.float32)
-    oracle().orc_dequantize_row_q3_K(ptr(np.ascontiguousarray(blocks)), ptr(out), k)
+    refs.oracle().orc_dequantize_row_q3_K(ptr(np.ascontiguousarray(blocks)), ptr(out), k)
     return out
 
 
 def mul_mat(t, w, x, K, M, N=1):
     x = np.ascontiguousarray(x, np.float32)
     out = np.zeros(M * N, np.float32)
-    assert oracle().orc_mul_mat(t, ptr(np.ascontiguousarray(w)), ptr(x), ptr(out), K, M, N) == 0
+    assert refs.oracle().orc_mul_mat(t, ptr(np.ascontiguousarray(w)), ptr(x), ptr(out), K, M, N) == 0
     return out
 
 
@@ -131,29 +82,6 @@ def random_blocks(k, m, seed, sigma=0.02):
 
 def blocks(src, k, m, seed):
     return {"random": random_blocks, "refq": reference_quantized_blocks, "edge": edge_blocks}[src](k, m, seed)
-
-
-# ------------------------------------------------------------------------------------------------------ whole-model oracle
-class OracleModel(refs.OracleModel):
-    """refs.OracleModel on this library: llama_oracle.c's orc_mul_mat is the one above.  Its get_rows knows only the oracle's
-    original types, so a Q3_K token_embd is handed to it as the F32 table this file's dequantizer makes (ggml_get_rows
-    dequantizes the requested row with the same to_float, ggml.c:11615-11642)."""
-
-    def __init__(self, path, n_ctx):
-        saved_oracle, saved_block = refs._oracle, dict(refs.BLOCK)
-        refs._oracle = oracle()
-        refs.BLOCK.update(BLOCK)            # refs.read_gguf sizes tensors by refs.BLOCK
-        try:
-            super().__init__(path, n_ctx)
-            t, shape, data = refs.read_gguf(path)[1]["token_embd.weight"]
-        finally:
-            refs._oracle = saved_oracle
-            refs.BLOCK.clear()
-            refs.BLOCK.update(saved_block)
-        if t == Q3_K:
-            table = dequantize(np.ascontiguousarray(data), shape[0] * shape[1])
-            self.keep.append(table)
-            self.o.orc_model_set_mat(self.m, -1, 0, 0, shape[0], shape[1], ptr(table))
 
 
 # ------------------------------------------------------------------------------------------------------------ model cases

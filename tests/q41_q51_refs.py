@@ -1,102 +1,44 @@
 """Checkers for the Q4_1 / Q5_1 weights and their Q8_1 activation (test infrastructure, never the product).
 
-  * ``oracle()``  the plain-C restatement tests/q41_q51_oracle.c (which includes the unchanged oracle/ggml_oracle.c and
-                  oracle/llama_oracle.c), compiled on first use into a private temporary directory
-  * block pools  ``reference_quantized_blocks`` / ``edge_blocks`` for types 3 and 7, like refs.py's for the other types
-  * ``OracleModel`` refs.OracleModel bound to this library, so the whole-model oracle multiplies Q4_1 / Q5_1 matrices too
+  * oracle helpers  the Q8_1 quantizer and the Q4_1 / Q5_1 dots, dequantizers and mat-mul of the one oracle library
+                    (refs.oracle())
+  * block pools     ``reference_quantized_blocks`` / ``edge_blocks`` for types 3 and 7, like refs.py's for the other types
 """
-import atexit
-import ctypes as C
-import shutil
-import subprocess
-import tempfile
 from pathlib import Path
 
 import numpy as np
 
 import refs
-from refs import ptr
+from refs import GOLD, Q4_1, Q5_1, Q8_1, ptr
 
-HERE = Path(__file__).resolve().parent
-SRC = HERE / "q41_q51_oracle.c"
-GOLD = HERE / "golden"
-
-Q4_1, Q5_1, Q8_1 = 3, 7, 9
-BLOCK = {Q4_1: (32, 20), Q5_1: (32, 24), Q8_1: (32, 40)}
-TYPE_NAME = {Q4_1: "q4_1", Q5_1: "q5_1"}
 # orc_q1_set_variant bits: the forms the reference does not use
 SUMMS_UNFUSED, DEQ_UNFUSED, DY_FP16, ROUNDF = 1, 2, 4, 8
 
-_lib = None
 
-
-def oracle():
-    global _lib
-    if _lib is None:
-        d = Path(tempfile.mkdtemp(prefix="q41_q51_oracle_"))
-        atexit.register(shutil.rmtree, d, True)
-        so = d / "libq41q51oracle.so"
-        subprocess.check_call(["gcc", "-O2", "-std=gnu11", "-fPIC", "-shared", "-mf16c", "-mavx2", "-mfma", "-ffp-contract=off",
-                               "-o", str(so), str(SRC), "-lm"])
-        o = C.CDLL(str(so))
-        vp, i = C.c_void_p, C.c_int
-        for n in ("orc_vec_dot_q4_1_q8_1", "orc_vec_dot_q5_1_q8_1"):
-            getattr(o, n).restype = C.c_float
-            getattr(o, n).argtypes = [i, vp, vp]
-        for n in ("orc_quantize_row_q8_1", "orc_dequantize_row_q4_1", "orc_dequantize_row_q5_1"):
-            getattr(o, n).argtypes = [vp, vp, i]
-        o.orc_q1_set_variant.argtypes = [i]
-        o.orc_mul_mat.restype = i
-        o.orc_mul_mat.argtypes = [i, vp, vp, vp, i, i, i]
-        _lib = o
-    return _lib
-
-
-def row_bytes(t, k):
-    if t in BLOCK:
-        bs, sz = BLOCK[t]
-        assert k % bs == 0
-        return k // bs * sz
-    return refs.row_bytes(t, k)
-
-
-def quantize_q8_1(x, variant=0):
+def quantize_q8_1(x):
     x = np.ascontiguousarray(x, np.float32)
-    out = np.zeros(row_bytes(Q8_1, x.size), np.uint8)
-    o = oracle()
-    o.orc_q1_set_variant(variant)
-    try:
-        o.orc_quantize_row_q8_1(ptr(x), ptr(out), x.size)
-    finally:
-        o.orc_q1_set_variant(0)
+    out = np.zeros(refs.row_bytes(Q8_1, x.size), np.uint8)
+    refs.oracle().orc_quantize_row_q8_1(ptr(x), ptr(out), x.size)
     return out
 
 
-def vec_dot(t, k, wrow, act, variant=0):
-    o = oracle()
-    o.orc_q1_set_variant(variant)
-    try:
-        return float((o.orc_vec_dot_q4_1_q8_1 if t == Q4_1 else o.orc_vec_dot_q5_1_q8_1)(k, ptr(np.ascontiguousarray(wrow)), ptr(act)))
-    finally:
-        o.orc_q1_set_variant(0)
+def vec_dot(t, k, wrow, act):
+    o = refs.oracle()
+    return float((o.orc_vec_dot_q4_1_q8_1 if t == Q4_1 else o.orc_vec_dot_q5_1_q8_1)(k, ptr(np.ascontiguousarray(wrow)), ptr(act)))
 
 
-def dequantize(t, blocks, k, variant=0):
+def dequantize(t, blocks, k):
     blocks = np.ascontiguousarray(blocks)
     out = np.zeros(k, np.float32)
-    o = oracle()
-    o.orc_q1_set_variant(variant)
-    try:
-        (o.orc_dequantize_row_q4_1 if t == Q4_1 else o.orc_dequantize_row_q5_1)(ptr(blocks), ptr(out), k)
-    finally:
-        o.orc_q1_set_variant(0)
+    o = refs.oracle()
+    (o.orc_dequantize_row_q4_1 if t == Q4_1 else o.orc_dequantize_row_q5_1)(ptr(blocks), ptr(out), k)
     return out
 
 
 def mul_mat(t, w, x, K, M, N=1):
     x = np.ascontiguousarray(x, np.float32)
     out = np.zeros(M * N, np.float32)
-    assert oracle().orc_mul_mat(t, ptr(np.ascontiguousarray(w)), ptr(x), ptr(out), K, M, N) == 0
+    assert refs.oracle().orc_mul_mat(t, ptr(np.ascontiguousarray(w)), ptr(x), ptr(out), K, M, N) == 0
     return out
 
 
@@ -132,7 +74,7 @@ def planted_rows(k, seed):
 # -------------------------------------------------------------------------------------------------------- weight blocks
 def reference_quantized_blocks(t, k, m, seed):
     """m rows of k weights of type t, drawn from the blocks the reference's quantizer wrote (golden/q41_q51_blocks.npz)."""
-    bs, sz = BLOCK[t]
+    bs, sz = refs.BLOCK[t]
     pool = np.load(GOLD / "q41_q51_blocks.npz")[f"blocks_{t}"]
     idx = np.random.default_rng(seed).integers(0, len(pool), m * (k // bs))
     return np.ascontiguousarray(pool[idx].reshape(-1))
@@ -143,7 +85,7 @@ def edge_blocks(t, k, m, seed):
     about a tenth of the blocks), whole blocks of all-0 or all-15 nibbles, and for Q5_1 qh drawn from every pattern class
     (all clear, all set, alternating, random)."""
     rng = np.random.default_rng(seed)
-    bs, sz = BLOCK[t]
+    bs, sz = refs.BLOCK[t]
     nb = m * (k // bs)
     out = rng.integers(0, 256, (nb, sz), dtype=np.uint8)
     out[:, 0:2] = refs._f16_edge(rng, nb).view(np.uint8).reshape(nb, 2)
@@ -163,29 +105,6 @@ def edge_blocks(t, k, m, seed):
 def random_blocks(t, k, m, seed, sigma=0.02):
     from ctransformers_b200 import synth
     return np.ascontiguousarray(synth.random_blocks(t, k, m, sigma, np.random.default_rng(seed)))
-
-
-# ------------------------------------------------------------------------------------------------------ whole-model oracle
-class OracleModel(refs.OracleModel):
-    """refs.OracleModel on this library: llama_oracle.c's orc_mul_mat is the one above.  Its get_rows knows only the oracle's
-    original types, so a Q4_1 / Q5_1 token_embd is handed to it as the F32 table this file's dequantizer makes (ggml_get_rows
-    dequantizes the requested row with the same to_float, ggml.c:11615-11642)."""
-
-    def __init__(self, path, n_ctx):
-        saved_oracle, saved_block = refs._oracle, dict(refs.BLOCK)
-        refs._oracle = oracle()
-        refs.BLOCK.update(BLOCK)            # refs.read_gguf sizes tensors by refs.BLOCK
-        try:
-            super().__init__(path, n_ctx)
-            t, shape, data = refs.read_gguf(path)[1]["token_embd.weight"]
-        finally:
-            refs._oracle = saved_oracle
-            refs.BLOCK.clear()
-            refs.BLOCK.update(saved_block)
-        if t in (Q4_1, Q5_1):
-            table = dequantize(t, np.ascontiguousarray(data), shape[0] * shape[1])
-            self.keep.append(table)
-            self.o.orc_model_set_mat(self.m, -1, 0, 0, shape[0], shape[1], ptr(table))
 
 
 # ------------------------------------------------------------------------------------------------------------ model cases
@@ -225,7 +144,7 @@ def build_model(name, directory):
         quantizer = None
         if weights == "reference":
             def quantizer(t, w):   # the Q5_1 matrices from the pool; the Q6_K head random (the K-quant pool's scales reach 2)
-                if t not in BLOCK:
+                if t not in (Q4_1, Q5_1):
                     return synth.random_blocks(t, w.shape[1], w.shape[0], 0.04, np.random.default_rng(w.shape[0] * 7 + t))
                 return reference_quantized_blocks(t, w.shape[1], w.shape[0], seed=w.shape[0] * 7 + t)
         (synth.write_llama if arch == "llama" else synth.write_falcon)(path, shape, ftype, seed=11, quantizer=quantizer, tensor_types=types)

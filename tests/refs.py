@@ -1,13 +1,15 @@
 """ctypes loaders for the two CHECKERS (test infrastructure, never the product):
 
-  * ``oracle()``  — oracle/_build/liboracle.so, our plain-C restatement (oracle/ggml_oracle.c)
+  * ``oracle()``  — oracle/_build/liboracle.so, our plain-C restatement (oracle/*.c) of every
+                    weight type and of the whole-model eval; ``variant()`` selects, for one block of code, arithmetic the
+                    reference does not use
   * ``ref()``     — oracle/_ref/libctransformers_ref.so, the unmodified reference compiled by oracle/Makefile where its
                     sources are available; only tests/golden/make_golden.py uses it.  The tests compare with what it
                     computed, stored under tests/golden/.
 """
+import contextlib
 import ctypes as C
 import hashlib
-import os
 import subprocess
 from pathlib import Path
 
@@ -18,9 +20,9 @@ ORACLE_SO = ROOT / "oracle" / "_build" / "liboracle.so"
 REF_SO = ROOT / "oracle" / "_ref" / "libctransformers_ref.so"
 
 # ggml type ids (ggml.h enum ggml_type)
-F32, F16, Q4_0, Q5_0, Q8_0, Q4_K, Q5_K, Q6_K, Q8_K = 0, 1, 2, 6, 8, 12, 13, 14, 15
-BLOCK = {Q4_0: (32, 18), Q5_0: (32, 22), Q8_0: (32, 34), Q4_K: (256, 144), Q5_K: (256, 176), Q6_K: (256, 210), Q8_K: (256, 292),
-         F32: (1, 4), F16: (1, 2)}
+F32, F16, Q4_0, Q4_1, Q5_0, Q5_1, Q8_0, Q8_1, Q3_K, Q4_K, Q5_K, Q6_K, Q8_K = 0, 1, 2, 3, 6, 7, 8, 9, 11, 12, 13, 14, 15
+BLOCK = {Q4_0: (32, 18), Q4_1: (32, 20), Q5_0: (32, 22), Q5_1: (32, 24), Q8_0: (32, 34), Q8_1: (32, 40), Q3_K: (256, 110),
+         Q4_K: (256, 144), Q5_K: (256, 176), Q6_K: (256, 210), Q8_K: (256, 292), F32: (1, 4), F16: (1, 2)}
 TYPE_NAME = {Q4_0: "q4_0", Q5_0: "q5_0", Q8_0: "q8_0", Q4_K: "q4_K", Q5_K: "q5_K", Q6_K: "q6_K"}
 
 
@@ -37,27 +39,54 @@ _ref = None
 def oracle():
     global _oracle
     if _oracle is None:
-        if not ORACLE_SO.exists():
-            subprocess.check_call(["make", "-C", str(ROOT / "oracle"), "oracle"])
+        # make rebuilds the library when a source is newer than it, and does nothing otherwise
+        subprocess.check_call(["make", "-s", "-C", str(ROOT / "oracle"), "oracle"], stdout=subprocess.DEVNULL)
         o = C.CDLL(str(ORACLE_SO))
-        fp, vp, i = C.POINTER(C.c_float), C.c_void_p, C.c_int
-        o.orc_fp16_to_fp32.restype = C.c_float
-        o.orc_fp16_to_fp32.argtypes = [C.c_uint16]
-        o.orc_fp32_to_fp16.restype = C.c_uint16
-        o.orc_fp32_to_fp16.argtypes = [C.c_float]
-        for n in ("orc_vec_dot_q4_0_q8_0", "orc_vec_dot_q5_0_q8_0", "orc_vec_dot_q8_0_q8_0", "orc_vec_dot_q4_K_q8_K", "orc_vec_dot_q5_K_q8_K",
-                  "orc_vec_dot_q6_K_q8_K"):
-            getattr(o, n).restype = C.c_float
-            getattr(o, n).argtypes = [i, vp, vp]
-        o.orc_mul_mat.restype = i
-        o.orc_mul_mat.argtypes = [i, vp, vp, vp, i, i, i]
-        o.orc_rms_norm_mul.argtypes = [vp, vp, vp, i, C.c_float]
-        o.orc_layer_norm_mul_add.argtypes = [vp, vp, vp, vp, i, C.c_float]
-        o.orc_rope.argtypes = [vp, i, i, i, i, C.c_float, C.c_float]
-        o.orc_rope_table.argtypes = [vp, i, i, C.c_float, C.c_float]
-        o.orc_attn_head.argtypes = [vp, vp, C.c_size_t, vp, C.c_size_t, i, i, C.c_float, vp]
+        f, vp, i, sz = C.c_float, C.c_void_p, C.c_int, C.c_size_t
+        sig = {"orc_fp16_to_fp32": (f, [C.c_uint16]), "orc_fp32_to_fp16": (C.c_uint16, [f]),
+               "orc_sizeof_block": (i, [i]), "orc_blck_size": (i, [i]),
+               "orc_vec_dot_f16": (f, [i, vp, vp]),
+               "orc_mul_mat": (i, [i, vp, vp, vp, i, i, i]),
+               "orc_rms_norm_mul": (None, [vp, vp, vp, i, f]),
+               "orc_layer_norm_mul_add": (None, [vp, vp, vp, vp, i, f]),
+               "orc_rope": (None, [vp, i, i, i, i, f, f]),
+               "orc_rope_table": (None, [vp, i, i, f, f]),
+               "orc_silu": (None, [vp, vp, i]), "orc_gelu": (None, [vp, vp, i]), "orc_soft_max": (None, [vp, vp, i]),
+               "orc_attn_head": (None, [vp, vp, sz, vp, sz, i, i, f, vp]),
+               "orc_attn_head_n": (None, [vp, vp, sz, vp, sz, i, i, i, f, vp]),
+               "orc_model_new": (vp, [i] * 8 + [f] * 3),
+               "orc_model_set_mat": (None, [vp, i, i, i, i, i, vp]),
+               "orc_model_set_vec": (None, [vp, i, i, vp]),
+               "orc_model_set_tp": (i, [vp, i, vp, vp]),
+               "orc_model_set_trace": (None, [vp, vp, vp]),
+               "orc_model_free": (None, [vp]),
+               "orc_eval": (i, [vp, vp, i, i, vp, vp]),
+               "orc_eval_rows": (i, [vp, vp, i, i, vp, vp])}
+        for w, a in (("q4_0", "q8_0"), ("q4_1", "q8_1"), ("q5_0", "q8_0"), ("q5_1", "q8_1"), ("q8_0", "q8_0"), ("q3_K", "q8_K"),
+                     ("q4_K", "q8_K"), ("q5_K", "q8_K"), ("q6_K", "q8_K")):
+            sig[f"orc_vec_dot_{w}_{a}"] = (f, [i, vp, vp])
+            sig[f"orc_dequantize_row_{w}"] = (None, [vp, vp, i])
+        for a in ("q8_0", "q8_1", "q8_K"):
+            sig[f"orc_quantize_row_{a}"] = (None, [vp, vp, i])
+        for v in ("q3k", "q1", "hd"):
+            sig[f"orc_{v}_set_variant"] = (None, [i])
+        for name, (res, args) in sig.items():
+            fn = getattr(o, name)
+            fn.restype, fn.argtypes = res, args
         _oracle = o
     return _oracle
+
+
+@contextlib.contextmanager
+def variant(setter, v):
+    """Run the body with the oracle's arithmetic variant v selected by setter ("orc_q3k_set_variant", "orc_q1_set_variant" or
+    "orc_hd_set_variant"; oracle/variants.c), and the reference's arithmetic (0) restored after it."""
+    fn = getattr(oracle(), setter)
+    fn(v)
+    try:
+        yield
+    finally:
+        fn(0)
 
 
 class _Traits(C.Structure):
@@ -212,7 +241,6 @@ def attention_expected(q, k_new, v_new, kcache, vcache, n_head, n_kv, hd, pos0, 
     orc_attn_head_n per head over the chunk row length n_total[i].  Arguments as ctb_attention_path (kcache [n_ctx][n_kv*hd],
     vcache [n_kv*hd][n_ctx], uint16 fp16 bits); returns (out [n_tok][n_head*hd], kcache, vcache) with the new rows stored."""
     o = oracle()
-    o.orc_attn_head_n.argtypes = [C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p, C.c_size_t, C.c_int, C.c_int, C.c_int, C.c_float, C.c_void_p]
     n_tok, n_ctx = q.shape[0], kcache.shape[0]
     kc, vc = kcache.copy(), vcache.copy()
     for i in range(n_tok):
@@ -304,13 +332,6 @@ class OracleModel:
         eps = g("attention.layer_norm_epsilon") if self.falcon else g("attention.layer_norm_rms_epsilon")
         rope_base = g("rope.freq_base", 10000.0)
         lin = g("rope.scale_linear", 1.0)
-        o.orc_model_new.restype = C.c_void_p
-        o.orc_model_new.argtypes = [C.c_int] * 8 + [C.c_float] * 3
-        o.orc_model_set_mat.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_void_p]
-        o.orc_model_set_vec.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_void_p]
-        o.orc_model_set_trace.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p]
-        o.orc_model_free.argtypes = [C.c_void_p]
-        o.orc_eval.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_void_p]
         self.o, self.keep = o, []
         self.m = o.orc_model_new(int(self.falcon), self.n_vocab, self.n_embd, self.n_ff, self.n_head, self.n_head_kv, self.n_layer, n_ctx,
                                  eps, rope_base, 1.0 / lin if lin != 1.0 else 1.0)
@@ -353,7 +374,6 @@ class OracleModel:
         sh = tp_plan.plan(self.n_embd, self.n_head, self.n_head_kv, self.n_ff, self.n_vocab, world)
         wo = (C.c_int * (world + 1))(*([s.attn_k[0] for s in sh] + [sh[-1].attn_k[1]]))
         w2 = (C.c_int * (world + 1))(*([s.ff[0] for s in sh] + [sh[-1].ff[1]]))
-        self.o.orc_model_set_tp.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p]
         assert self.o.orc_model_set_tp(self.m, world, wo, w2) == 0
 
     def eval(self, tokens, batch_size=8):

@@ -21,7 +21,7 @@ def golden():
 def oracle_search(name, prompt, n_beams, n_predict, model_dir):
     """The restatement on the oracle: the prompt in chunks of B.BATCH_SIZE, then one oracle eval per chunk the reference evaluates."""
     path, ctx = B.build(name, model_dir)
-    model = B.oracle(name, path, ctx)
+    model = refs.OracleModel(path, ctx)
     model.eval(prompt, batch_size=B.BATCH_SIZE)
 
     def eval_fn(tokens, n_past):

@@ -31,7 +31,7 @@ def stored(key):
 @pytest.mark.parametrize("name,bs", RUNS, ids=[f"{n}-bs{b}" for n, b in RUNS])
 def test_whole_model_oracle_matches_reference(name, bs, model_dir):
     path, ctx = H.build_model(name, model_dir)
-    run = modelcases.oracle_greedy(H.OracleModel(path, ctx), H.prompt_for(name), H.N_NEW, bs)
+    run = modelcases.oracle_greedy(refs.OracleModel(path, ctx), H.prompt_for(name), H.N_NEW, bs)
     assert results(run) == stored(f"{name}_bs{bs}")
 
 
@@ -42,7 +42,8 @@ def test_other_tails_give_other_bits(variant, model_dir):
     changed = []
     for name in ("llama_hd100_q4_0", "llama_hd80_q4km_gqa"):
         path, ctx = H.build_model(name, model_dir)
-        run = modelcases.oracle_greedy(H.OracleModel(path, ctx, variant), H.prompt_for(name), H.N_NEW, 8)
+        with refs.variant("orc_hd_set_variant", variant):
+            run = modelcases.oracle_greedy(refs.OracleModel(path, ctx), H.prompt_for(name), H.N_NEW, 8)
         got, want = results(run), stored(f"{name}_bs8")
         changed += [f"{name}:{k}" for k in want if got[k] != want[k]]
     assert changed, "the stored results do not tell this tail from the reference's"

@@ -132,7 +132,6 @@ def test_attention_hd100_bit_exact(lib, n_head, n_kv, T, n_total):
     want = np.zeros((n_head, hd), np.float32)
     vpad = np.zeros((n_kv * hd, n_total), np.float16)
     vpad[:, :T] = vt
-    o.orc_attn_head_n.argtypes = [C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p, C.c_size_t, C.c_int, C.c_int, C.c_int, C.c_float, C.c_void_p]
     for h in range(n_head):
         kvh = h // (n_head // n_kv)
         kslice = np.ascontiguousarray(kc[:, kvh, :])

@@ -20,7 +20,7 @@ def model_dir(tmp_path_factory):
 def test_oracle_rows_match_reference_digests(key, model_dir):
     name, calls = LA.runs()[key]
     path, ctx = LA.build(name, model_dir)
-    model = LA.oracle(name, path)
+    model = refs.OracleModel(path, ctx)
     got = []
     for toks, bs in calls:
         blocks = LA.oracle_rows(model, toks, bs, ctx)
@@ -35,13 +35,13 @@ def test_oracle_rows_match_reference_digests(key, model_dir):
 def test_last_row_is_the_golden_first_logits(name, model_dir):
     """The last row of the prompt eval at batch_size 8 is the logits the reference's ordinary eval leaves (model_<name>.npz)."""
     path, ctx = modelcases.build(name, model_dir)
-    model = LA.oracle(name, path)
+    model = refs.OracleModel(path, ctx)
     gold = np.load(refs.GOLD / f"model_{name}.npz")
     blocks = LA.oracle_rows(model, gold["prompt"].tolist(), 8, ctx)
     assert np.array_equal(blocks[-1][-1].view(np.uint32), gold["first_logits"].view(np.uint32))
     assert np.array_equal(model.embd.view(np.uint32), gold["first_embd"].view(np.uint32))
     toks, cur = [], blocks[-1][-1]
-    for _ in range(4):   # greedy steps through orc_eval_all: the single row of each is the ordinary eval's
+    for _ in range(4):   # greedy steps through orc_eval_rows: the single row of each is the ordinary eval's
         toks.append(LA.greedy_ref(cur))
         cur = LA.oracle_rows(model, [toks[-1]], 8, ctx)[0][0]
     assert toks == gold["tokens"][:4].tolist()

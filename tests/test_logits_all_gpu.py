@@ -1,5 +1,5 @@
 """Every-token rows (the reference's logits_all) and their scores on the GPU: each row bit for bit the reference's (digests) and the
-oracle's (orc_eval_all) on every path an eval can take; nothing an ordinary eval leaves behind moves; MultiLLM rows equal a
+oracle's (orc_eval_rows) on every path an eval can take; nothing an ordinary eval leaves behind moves; MultiLLM rows equal a
 single-sequence LLM's; the device scores equal float64 numpy over the same rows."""
 import ctypes as C
 
@@ -8,6 +8,7 @@ import pytest
 
 import logits_all_cases as LA
 import modelcases
+import refs
 
 pytestmark = pytest.mark.gpu
 
@@ -74,7 +75,7 @@ def check_run(key, model_dir, monkeypatch, env, ctx_override):
     if ctx_override is None:
         assert LA.digests(rows, sizes) == gold[f"{key}_chunks"].tolist(), f"{key}: rows are not the reference's"
     if sum(len(t) for t, _ in calls) <= ORACLE_MAX:
-        model = LA.oracle(name, path, ctx)
+        model = refs.OracleModel(path, ctx)
         want = np.concatenate([b for toks, bs in calls for b in LA.oracle_rows(model, toks, bs, ctx)])
         same(rows, want, f"{key} rows against the oracle")
     return before, after

@@ -110,7 +110,6 @@ def test_mul_mat_full_size_partitions(lib, t, k, m):
 def test_mul_mat_f16_weights(lib, k):
     """F16 weights take ggml_vec_dot_f16 with the activation row rounded to f16 (ggml.c:1665-1675, 2392-2426)."""
     o = refs.oracle()
-    o.orc_vec_dot_f16.restype = C.c_float
     m = 24
     rng = np.random.default_rng(k)
     w = (rng.standard_normal((m, k)) * 0.05).astype(np.float16)
@@ -178,7 +177,6 @@ def test_attention_bit_exact(lib, n_head, n_kv, hd, T, n_total):
     # the oracle's V·P dot runs over n_total entries: pad the transposed cache with zeros probabilities beyond T
     vpad = np.zeros((n_kv * hd, n_total), np.float16)
     vpad[:, :T] = vt
-    o.orc_attn_head_n.argtypes = [C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p, C.c_size_t, C.c_int, C.c_int, C.c_int, C.c_float, C.c_void_p]
     for h in range(n_head):
         kvh = h // (n_head // n_kv)
         kslice = np.ascontiguousarray(kc[:, kvh, :])
@@ -406,11 +404,8 @@ def _oracle_mul_mat(t, w, y, k, m):
     n_tok = y.shape[0]
     if t == F16:
         o = refs.oracle()
-        o.orc_vec_dot_f16.restype = C.c_float
         w16, y16 = w.view(np.float16).reshape(m, k), y.astype(np.float16)
         return np.array([[o.orc_vec_dot_f16(k, ptr(w16[j]), ptr(y16[i])) for j in range(m)] for i in range(n_tok)], np.float32)
-    if t in (Q3_K, Q4_1, Q5_1):
-        return (q3k_refs if t == Q3_K else q41_q51_refs).mul_mat(t, w, y, k, m, n_tok).reshape(n_tok, m)
     v = np.zeros((n_tok, m), np.float32)
     assert refs.oracle().orc_mul_mat(t, ptr(w), ptr(y), ptr(v), k, m, n_tok) == 0
     return v

@@ -1,4 +1,4 @@
-"""Q3_K on the CPU: the oracle's restatement (tests/q3k_oracle.c) against what the unmodified reference computed
+"""Q3_K on the CPU: the oracle's restatement (oracle/q3k_oracle.c) against what the unmodified reference computed
 (golden/q3k_kat.npz, q3k_runs.npz), and a check that those stored results tell the reference's fp32 order from another."""
 import numpy as np
 import pytest
@@ -42,9 +42,10 @@ def test_fixtures_tell_the_fold_order_apart(kat):
     differ = 0
     for src in SRCS:
         w, want = kat[f"w_{src}"], kat[f"dot_{src}"]
-        for j, a in enumerate(kat["dot_q8k"]):
-            for i in range(len(w)):
-                differ += np.float32(Q.vec_dot(k, w[i], a, variant=Q.SCALE_FOLD_IN_FLOAT)).view(np.uint32) != want[j, i].view(np.uint32)
+        with refs.variant("orc_q3k_set_variant", Q.SCALE_FOLD_IN_FLOAT):
+            for j, a in enumerate(kat["dot_q8k"]):
+                for i in range(len(w)):
+                    differ += np.float32(Q.vec_dot(k, w[i], a)).view(np.uint32) != want[j, i].view(np.uint32)
     assert differ > 0
 
 
@@ -69,7 +70,7 @@ SMALL = [(name, bs) for name, case in Q.model_cases().items() if case[4] <= 70 f
 def test_whole_model_oracle_equals_reference(name, bs, model_dir):
     """The whole-model oracle on the small cases gives the reference's stored digests at the same chunkings."""
     path, ctx = Q.build_model(name, model_dir)
-    first_logits, first_embd, toks, last_logits, _ = modelcases.oracle_greedy(Q.OracleModel(path, ctx), Q.prompt_for(name), Q.N_NEW, bs)
+    first_logits, first_embd, toks, last_logits, _ = modelcases.oracle_greedy(refs.OracleModel(path, ctx), Q.prompt_for(name), Q.N_NEW, bs)
     gold, key = Q.golden_runs(), f"{name}_bs{bs}"
     assert toks == gold[f"{key}_tokens"].tolist()
     for k, v in (("first_logits", first_logits), ("first_embd", first_embd), ("last_logits", last_logits)):

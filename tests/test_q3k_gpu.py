@@ -1,5 +1,5 @@
 """Q3_K on the GPU (the step kernel's block code, the batched prefill, embedding rows), bit-exact with the oracle
-(tests/q3k_oracle.c) at op level and with the reference's runs of the model cases through the public Python API."""
+(oracle/q3k_oracle.c) at op level and with the reference's runs of the model cases through the public Python API."""
 import ctypes as C
 
 import numpy as np
@@ -81,9 +81,7 @@ def test_ffn_gate(lib):
     got = np.zeros(M, np.float32)
     assert lib.ctb_ffn_gate(Q.Q3_K, ptr(w1), ptr(w3), ptr(x), ptr(got), K, M) == 0
     g, u = Q.mul_mat(Q.Q3_K, w1, x, K, M), Q.mul_mat(Q.Q3_K, w3, x, K, M)
-    o = refs.oracle()
-    o.orc_silu.argtypes = [C.c_void_p, C.c_void_p, C.c_int]
-    o.orc_silu(ptr(g), ptr(g), M)
+    refs.oracle().orc_silu(ptr(g), ptr(g), M)
     same(got, g * u)
 
 
@@ -91,7 +89,7 @@ def test_ffn_gate(lib):
 def test_get_row(lib, src):
     K, rows = 4096, 12
     table = Q.blocks(src, K, rows, seed=9)
-    rb = Q.row_bytes(Q.Q3_K, K)
+    rb = refs.row_bytes(Q.Q3_K, K)
     for r in (0, 5, rows - 1):
         got = np.zeros(K, np.float32)
         assert lib.ctb_get_row(Q.Q3_K, ptr(table), K, rows, r, ptr(got)) == 0
@@ -159,7 +157,7 @@ def test_whole_model_against_oracle(name, model_dir):
     path, ctx = Q.build_model(name, model_dir)
     llm = AutoModelForCausalLM.from_pretrained(str(path), context_length=ctx)
     run = modelcases.run_greedy(llm, Q.prompt_for(name), 8, batch_size=64)
-    want = modelcases.oracle_greedy(Q.OracleModel(path, ctx), Q.prompt_for(name), 8, 64)
+    want = modelcases.oracle_greedy(refs.OracleModel(path, ctx), Q.prompt_for(name), 8, 64)
     for i, what in ((0, "logits after the prompt"), (1, "embeddings after the prompt"), (3, "last logits")):
         same(run[i], want[i], what)
     assert run[2] == want[2]
@@ -173,7 +171,7 @@ def test_q2k_file_is_refused(model_dir, capfd):
     synth.BLOCK.setdefault(10, (256, 84))
     try:
         synth.write_llama(path, synth.LlamaShape(n_vocab=400, n_embd=256, n_head=4, n_head_kv=4, n_ff=512, n_layer=1, n_ctx_train=64), "Q3_K_S",
-                          seed=1, quantizer=lambda t, w: np.zeros(Q.row_bytes(t, w.shape[1]) * w.shape[0] if t != 10 else w.shape[0] * 84, np.uint8),
+                          seed=1, quantizer=lambda t, w: np.zeros(refs.row_bytes(t, w.shape[1]) * w.shape[0] if t != 10 else w.shape[0] * 84, np.uint8),
                           tensor_types={"ffn_up": 10})
     finally:
         synth.BLOCK.pop(10)

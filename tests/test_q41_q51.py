@@ -1,4 +1,4 @@
-"""Q4_1 / Q5_1 weights and their Q8_1 activation, without a GPU: the plain-C restatement (tests/q41_q51_oracle.c) against the
+"""Q4_1 / Q5_1 weights and their Q8_1 activation, without a GPU: the plain-C restatement (oracle/q41_q51_oracle.c) against the
 reference's known-answer vectors (golden/kat_q8_1.npz) and, where oracle/_ref is built, against the reference live; the forms the
 restatement rejected against the same vectors; and the whole-model oracle against the reference's runs of the model cases."""
 import ctypes as C
@@ -53,7 +53,7 @@ def test_vec_dot_and_dequantize_match_reference_kat(t, src):
 
 def test_edge_blocks_reach_the_edges():
     for t in (Q.Q4_1, Q.Q5_1):
-        b = Q.edge_blocks(t, 1024, 8, seed=t).reshape(-1, Q.BLOCK[t][1])
+        b = Q.edge_blocks(t, 1024, 8, seed=t).reshape(-1, refs.BLOCK[t][1])
         d, m = b[:, 0:2].copy().view(np.float16)[:, 0], b[:, 2:4].copy().view(np.float16)[:, 0]
         for v in (d, m):
             assert (v > 0).any() and (v < 0).any() and (v == 0).any()
@@ -70,13 +70,15 @@ def test_rejected_forms_give_other_bits():
     round-half-even each change some result."""
     g = np.load(KAT)
     for variant in (Q.DY_FP16, Q.ROUNDF):
-        assert any(not np.array_equal(Q.quantize_q8_1(x, variant), want) for x, want in zip(g["x_1024"], g["q81_1024"])), variant
+        with refs.variant("orc_q1_set_variant", variant):
+            assert any(not np.array_equal(Q.quantize_q8_1(x), want) for x, want in zip(g["x_1024"], g["q81_1024"])), variant
     for t in (Q.Q4_1, Q.Q5_1):
         w, k = g[f"w_refq_{t}"], 1024
         differ = 0
         for a, x in enumerate(g["dot_x"]):
             act = Q.quantize_q8_1(x)
-            got = np.array([Q.vec_dot(t, k, w[i], act, Q.SUMMS_UNFUSED) for i in range(len(w))], np.float32)
+            with refs.variant("orc_q1_set_variant", Q.SUMMS_UNFUSED):
+                got = np.array([Q.vec_dot(t, k, w[i], act) for i in range(len(w))], np.float32)
             differ += int((bits(got) != bits(g[f"dot_refq_{t}"][a])).sum())
         assert differ > 0, t
 
@@ -94,42 +96,36 @@ def test_dequantize_forms_cannot_differ():
         for src in SOURCES:
             w = g[f"w_{src}_{t}"]
             for i in range(len(w)):
-                assert np.array_equal(bits(Q.dequantize(t, w[i], 1024, Q.DEQ_UNFUSED)), bits(Q.dequantize(t, w[i], 1024)))
+                with refs.variant("orc_q1_set_variant", Q.DEQ_UNFUSED):
+                    unfused = Q.dequantize(t, w[i], 1024)
+                assert np.array_equal(bits(unfused), bits(Q.dequantize(t, w[i], 1024)))
 
 
 @pytest.mark.skipif(not refs.have_ref(), reason="oracle/_ref (the compiled reference) is not built here")
 def test_against_live_reference():
     """Fresh seeded rows and blocks through the compiled reference: Q8_1 bytes, dots and dequantized rows, bit for bit."""
-    saved = dict(refs.BLOCK)
-    refs.BLOCK.update(Q.BLOCK)
-    try:
-        rng = np.random.default_rng(77)
-        for x in Q.planted_rows(2048, seed=77):
-            assert np.array_equal(Q.quantize_q8_1(x), refs.ref_quantize_act(Q.Q8_1, x))
-        for t in (Q.Q4_1, Q.Q5_1):
-            for w in (Q.edge_blocks(t, 2048, 4, seed=5), Q.reference_quantized_blocks(t, 2048, 4, seed=6), Q.random_blocks(t, 2048, 4, seed=7)):
-                w = w.reshape(4, -1)
-                x = (rng.standard_normal(2048) * 3).astype(np.float32)
-                act = refs.ref_quantize_act(Q.Q8_1, x)
-                for i in range(4):
-                    assert np.float32(Q.vec_dot(t, 2048, w[i], act)) == np.float32(refs.ref_vec_dot(t, 2048, w[i], act))
-                deq = np.zeros(4 * 2048, np.float32)
-                refs.ref_traits(t)["to_float"](refs.ptr(np.ascontiguousarray(w)), refs.ptr(deq), deq.size)
-                assert np.array_equal(bits(deq), bits(np.concatenate([Q.dequantize(t, w[i], 2048) for i in range(4)])))
-    finally:
-        refs.BLOCK.clear()
-        refs.BLOCK.update(saved)
+    rng = np.random.default_rng(77)
+    for x in Q.planted_rows(2048, seed=77):
+        assert np.array_equal(Q.quantize_q8_1(x), refs.ref_quantize_act(Q.Q8_1, x))
+    for t in (Q.Q4_1, Q.Q5_1):
+        for w in (Q.edge_blocks(t, 2048, 4, seed=5), Q.reference_quantized_blocks(t, 2048, 4, seed=6), Q.random_blocks(t, 2048, 4, seed=7)):
+            w = w.reshape(4, -1)
+            x = (rng.standard_normal(2048) * 3).astype(np.float32)
+            act = refs.ref_quantize_act(Q.Q8_1, x)
+            for i in range(4):
+                assert np.float32(Q.vec_dot(t, 2048, w[i], act)) == np.float32(refs.ref_vec_dot(t, 2048, w[i], act))
+            deq = np.zeros(4 * 2048, np.float32)
+            refs.ref_traits(t)["to_float"](refs.ptr(np.ascontiguousarray(w)), refs.ptr(deq), deq.size)
+            assert np.array_equal(bits(deq), bits(np.concatenate([Q.dequantize(t, w[i], 2048) for i in range(4)])))
 
 
 def test_mul_mat_routes_other_types_to_the_original_oracle():
-    """The combined library's orc_mul_mat is the original one for every other type."""
-    from ctransformers_b200 import synth
-    x = np.random.default_rng(3).standard_normal(512).astype(np.float32)
-    for t in (synth.Q4_0, synth.Q8_0, synth.Q4_K, synth.Q6_K):
-        w = Q.random_blocks(t, 512, 8, seed=t)
-        want = np.zeros(8, np.float32)
-        assert refs.oracle().orc_mul_mat(t, refs.ptr(w), refs.ptr(x), refs.ptr(want), 512, 8, 1) == 0
-        assert np.array_equal(bits(Q.mul_mat(t, w, x, 512, 8)), bits(want))
+    """orc_mul_mat, which also takes Q4_1 / Q5_1, gives the reference's known answers for every other type (golden/kat_quant.npz:
+    the reference's quantized weights dotted with its quantization of x)."""
+    kat = np.load(refs.GOLD / "kat_quant.npz")
+    for t in (refs.Q4_0, refs.Q5_0, refs.Q8_0, refs.Q4_K, refs.Q5_K, refs.Q6_K):
+        w = kat[f"wq_{t}"]
+        assert np.array_equal(bits(Q.mul_mat(t, w, kat["x_1024"], 1024, len(w))), bits(kat[f"dot_{t}"])), t
 
 
 @pytest.fixture(scope="module")
@@ -149,7 +145,7 @@ def same_as_reference(key, run):
 @pytest.mark.parametrize("name", list(Q.model_cases()))
 def test_whole_model_oracle_matches_reference(name, bs, model_dir):
     path, ctx = Q.build_model(name, model_dir)
-    same_as_reference(f"{name}_bs{bs}", modelcases.oracle_greedy(Q.OracleModel(path, ctx), Q.prompt_for(name), Q.N_NEW, bs))
+    same_as_reference(f"{name}_bs{bs}", modelcases.oracle_greedy(refs.OracleModel(path, ctx), Q.prompt_for(name), Q.N_NEW, bs))
 
 
 @pytest.mark.skipif(not refs.have_ref(), reason="oracle/_ref (the compiled reference) is not built here")
@@ -171,14 +167,8 @@ def test_model_cases_have_the_promised_types(model_dir):
         "falcon_narrow_mixed": {"attn_qkv": Q.Q5_1, "ffn_up": Q.Q5_1, "ffn_down": synth.Q5_K, "output": synth.Q8_0},
         "llama_qkv_mixed": {"attn_q": Q.Q5_1, "attn_k": synth.Q4_0, "attn_v": Q.Q5_1},
     }
-    saved = dict(refs.BLOCK)
-    refs.BLOCK.update(Q.BLOCK)
-    try:
-        for name, kinds in want.items():
-            tensors = refs.read_gguf(Q.build_model(name, model_dir)[0])[1]
-            for kind, t in kinds.items():
-                names = [n for n in tensors if n.split(".")[-2] == kind]
-                assert names and all(tensors[n][0] == t for n in names), (name, kind)
-    finally:
-        refs.BLOCK.clear()
-        refs.BLOCK.update(saved)
+    for name, kinds in want.items():
+        tensors = refs.read_gguf(Q.build_model(name, model_dir)[0])[1]
+        for kind, t in kinds.items():
+            names = [n for n in tensors if n.split(".")[-2] == kind]
+            assert names and all(tensors[n][0] == t for n in names), (name, kind)

@@ -1,5 +1,5 @@
 """Q4_1 / Q5_1 on the GPU (k_matvec with a Q8_1 activation, Q4_1 / Q5_1 embedding rows), bit-exact with the oracle
-(tests/q41_q51_oracle.c) at op level, at Falcon-7B's real projection shapes among others, and with the reference's runs of the
+(oracle/q41_q51_oracle.c) at op level, at Falcon-7B's real projection shapes among others, and with the reference's runs of the
 model cases through the public Python API."""
 import ctypes as C
 
@@ -28,7 +28,7 @@ def weights(src, t, k, m, seed):
 @pytest.mark.parametrize("k", [32, 4096, 4544, 18176])
 def test_quantize_row_q8_1(lib, k):
     for x in Q.planted_rows(k, seed=k):
-        got = np.zeros(Q.row_bytes(Q.Q8_1, k), np.uint8)
+        got = np.zeros(refs.row_bytes(Q.Q8_1, k), np.uint8)
         assert lib.ctb_quantize_row_q8_1(ptr(x), ptr(got), k) == 0
         assert np.array_equal(got, Q.quantize_q8_1(x))
 
@@ -56,9 +56,7 @@ def test_ffn_gate(lib, t):
     got = np.zeros(M, np.float32)
     assert lib.ctb_ffn_gate(t, ptr(w1), ptr(w3), ptr(x), ptr(got), K, M) == 0
     g, u = Q.mul_mat(t, w1, x, K, M), Q.mul_mat(t, w3, x, K, M)
-    o = refs.oracle()
-    o.orc_silu.argtypes = [C.c_void_p, C.c_void_p, C.c_int]
-    o.orc_silu(ptr(g), ptr(g), M)
+    refs.oracle().orc_silu(ptr(g), ptr(g), M)
     same(got, g * u, f"type {t}")
 
 
@@ -67,7 +65,7 @@ def test_ffn_gate(lib, t):
 def test_get_row(lib, t, src):
     K, rows = 4544, 12
     table = weights(src, t, K, rows, seed=9 + t)
-    rb = Q.row_bytes(t, K)
+    rb = refs.row_bytes(t, K)
     for r in (0, 5, rows - 1):
         got = np.zeros(K, np.float32)
         assert lib.ctb_get_row(t, ptr(table), K, rows, r, ptr(got)) == 0
@@ -120,7 +118,7 @@ def test_whole_model_against_oracle(name, model_dir):
     path, ctx = Q.build_model(name, model_dir)
     llm = AutoModelForCausalLM.from_pretrained(str(path), context_length=ctx)
     run = modelcases.run_greedy(llm, Q.prompt_for(name), 8, batch_size=8)
-    want = modelcases.oracle_greedy(Q.OracleModel(path, ctx), Q.prompt_for(name), 8, 8)
+    want = modelcases.oracle_greedy(refs.OracleModel(path, ctx), Q.prompt_for(name), 8, 8)
     for i, what in ((0, "logits after the prompt"), (1, "embeddings after the prompt"), (3, "last logits")):
         same(run[i], want[i], what)
     assert run[2] == want[2]
