@@ -188,9 +188,7 @@ DevMat Engine::upload_matrix(const GGUFTensor& t, Uploader& up, int want_K, int 
   const uint8_t* src = t.data + (size_t)row0 * full_row_bytes;
   std::vector<uint8_t> gathered;
   if (m.K != full_K) {   // a K range: the kept blocks of every row, packed
-    gathered.resize(m.bytes);
-    const size_t off = (size_t)(k0 / be) * type_block_bytes(t.type);
-    for (int r = 0; r < m.M; r++) memcpy(gathered.data() + (size_t)r * row_bytes, src + (size_t)r * full_row_bytes + off, row_bytes);
+    gathered = gather_k_range(src, m.M, full_row_bytes, (size_t)(k0 / be) * type_block_bytes(t.type), row_bytes);
     src = gathered.data();
   }
   int rows_per_chunk = (int)std::max<size_t>(ST_ROWS, UP_CHUNK / row_bytes / ST_ROWS * ST_ROWS);   // whole 16-row tiles

@@ -13,6 +13,7 @@
 #include "../../include/ctransformers_b200.h"
 #include "attention.cuh"
 #include "cuda_owned.cuh"
+#include "engine.cuh"
 #include "matvec.cuh"
 #include "prefill.cuh"
 #include "repack.cuh"
@@ -90,6 +91,20 @@ DevMat upload(std::vector<DevMem>& keep, int type, const void* blocks, int K, in
   OPS_CUDA(cudaDeviceSynchronize());
   m.qs = (const uint8_t*)pl[0]; m.qh = (const uint8_t*)pl[1]; m.d = pl[2]; m.mn = pl[3];
   return m;
+}
+
+// the step kernel's watchdog words of this translation unit (stream.cuh st_fail), in host-mapped memory, so that a launch that
+// trapped still tells which wait timed out; set once per process, like the tables
+const int* watchdog_words() {
+  static int* words = nullptr;
+  if (!words) {
+    OPS_CUDA(cudaHostAlloc((void**)&words, 16, cudaHostAllocMapped));
+    memset(words, 0, 16);
+    int* d = nullptr;
+    OPS_CUDA(cudaHostGetDevicePointer((void**)&d, words, 0));
+    OPS_CUDA(st_set_debug_words(d));
+  }
+  return words;
 }
 
 int sm_count() {
@@ -667,6 +682,176 @@ int ctb_decode_mul_mat(int nseg, const int* types, const void* const* w_blocks, 
       if (norm_out) OPS_CUDA(cudaMemcpy(norm_out + (size_t)i * K, dnorm.get(), (size_t)K * 4, cudaMemcpyDeviceToHost));
     }
     if (launch) { launch[0] = ran.kernel; launch[1] = ran.cluster; }
+  });
+}
+
+int ctb_xchg_mul_mat(int world, int rank, int n_embd, int n_head, int n_head_kv, int n_ff, int n_vocab, int n_layers, const int* types,
+                     const void* const* w_blocks, const float* attn, const float* res0, const float* norm_w, float eps, const float* const* peers,
+                     unsigned xc_base, int steps, float* out, float* sum_out, unsigned* ll, unsigned* sync2, int* launch) {
+  return guarded("ctb_xchg_mul_mat", [&] {
+    // everything is checked before the first device allocation: a program whose peers' entries are not all written would
+    // spin until the watchdog traps
+    if (world < 2 || world > XC_MAX_WORLD || rank < 0 || rank >= world) throw std::runtime_error("world must be 2 to 8 and rank below world");
+    if (n_layers < 1 || steps < 1) throw std::runtime_error("n_layers and steps must be at least 1");
+    if (n_vocab < 1) throw std::runtime_error("the head needs at least one row");
+    const TPShard sh = tp_shard(n_embd, n_head, n_head_kv, n_ff, rank, world);   // (throws on a shape it does not split)
+    const int hd = n_embd / n_head, per_kv = n_head / n_head_kv;
+    if (sh.head1 <= sh.head0 || sh.ff1 <= sh.ff0) throw std::runtime_error("more ranks than 256-element blocks to share out");
+    if (sh.head0 % per_kv || sh.head1 % per_kv) throw std::runtime_error("a rank's query heads must cover whole KV groups");
+    const int q0 = sh.head0 * hd, q1 = sh.head1 * hd, g0 = sh.kv0 * hd, g1 = sh.kv1 * hd, f0 = sh.ff0, f1 = sh.ff1;
+    const int qw = q1 - q0, gw = g1 - g0, fw = f1 - f0;
+    if (q0 % 256 || q1 % 256 || f0 % 256 || f1 % 256) throw std::runtime_error("a K range off the 256-element block boundaries");
+    const int n_mats = 7 * n_layers - 2, n_xchg = 2 * n_layers;
+    for (int i = 0; i < n_mats; i++) {
+      if (!w_blocks[i]) throw std::runtime_error("matrix " + std::to_string(i) + " is missing");
+      if (!type_is_kquant(types[i])) throw std::runtime_error("the exchange runs in the step kernel: K-quant matrices only (matrix " + std::to_string(i) + ")");
+    }
+    if (!attn || !res0 || !norm_w) throw std::runtime_error("attention inputs, first residual and norm weights are required");
+    for (int k = 0; k < n_xchg; k++)
+      for (int r = 0; r < world; r++)
+        if (r != rank && !peers[(size_t)k * world + r]) throw std::runtime_error("peer vector of rank " + std::to_string(r) + " in exchange " + std::to_string(k) + " is missing");
+
+    std::vector<DevMem> keep;
+    // rows [r0, r1) of a full K-wide matrix (column-parallel), or the blocks [k0, k1) of each of its M rows (row-parallel), packed
+    // by the gather the engine's upload_matrix uses
+    auto rows_of = [&](int i, int K, int r0, int r1) {
+      return upload(keep, types[i], (const uint8_t*)w_blocks[i] + (size_t)r0 * raw_row_bytes(types[i], K), K, r1 - r0);
+    };
+    auto k_range_of = [&](int i, int K, int M, int k0, int k1) {
+      const std::vector<uint8_t> g = gather_k_range((const uint8_t*)w_blocks[i], M, raw_row_bytes(types[i], K), raw_row_bytes(types[i], k0),
+                                                    raw_row_bytes(types[i], k1 - k0));
+      return upload(keep, types[i], g.data(), k1 - k0, M);
+    };
+    // consumer outputs side by side: per layer C_up {silu(w1), w3}, then C_qkv {wq, wk, wv}, or the head after the last layer
+    std::vector<size_t> out_off(n_xchg + 1, 0);
+    for (int c = 0; c < n_xchg; c++) out_off[c + 1] = out_off[c] + (c % 2 == 0 ? 2 * (size_t)fw : (c == n_xchg - 1 ? (size_t)n_vocab : (size_t)qw + 2 * gw));
+    const size_t n_out = out_off[n_xchg], region = (size_t)2 * world * n_embd;   // region: uint2 ll[2][world][n_embd]
+    DevMem dattn((size_t)n_layers * qw * 4), dres0((size_t)n_embd * 4), dnorm((size_t)n_xchg * n_embd * 4), dsum((size_t)n_xchg * n_embd * 4),
+        dout(n_out * 4), dprod((size_t)n_embd * 4), dll((size_t)n_layers * world * region * 8), dsync(64);
+    OPS_CUDA(cudaMemcpy(dattn.get(), attn, (size_t)n_layers * qw * 4, cudaMemcpyHostToDevice));
+    OPS_CUDA(cudaMemcpy(dres0.get(), res0, (size_t)n_embd * 4, cudaMemcpyHostToDevice));
+    OPS_CUDA(cudaMemcpy(dnorm.get(), norm_w, (size_t)n_xchg * n_embd * 4, cudaMemcpyHostToDevice));
+    OPS_CUDA(cudaMemset(dsum.get(), 0xff, (size_t)n_xchg * n_embd * 4));
+    OPS_CUDA(cudaMemset(dout.get(), 0xff, n_out * 4));
+    OPS_CUDA(cudaMemset(dll.get(), 0, (size_t)n_layers * world * region * 8));   // as the engine's regions start
+    OPS_CUDA(cudaMemset(dsync.get(), 0, 64));
+    OPS_CUDA(cudaMemcpy(dsync.as<unsigned>() + 2, &xc_base, 4, cudaMemcpyHostToDevice));
+    // The engine's regions hold two exchanges, one per parity half; a peer overwrites its slots of exchange k with those of
+    // k + 2 once this rank has consumed k.  One launch on one GPU cannot wait for that, so each layer's pair of exchanges gets
+    // its own W regions, laid out and used as the engine's: [layer][region of rank R][parity][slot of rank r][n_embd].
+    auto ll_of = [&](int layer, int R) { return dll.as<uint2>() + ((size_t)layer * world + R) * region; };
+    float* sums = dsum.as<float>();
+    float* outs = dout.as<float>();
+
+    // the program, numbered as Engine::build_ops numbers a fused tensor-parallel Llama layer (fill_xc, push_xchg, take_input,
+    // mark_exchange), without the attention phase: per layer P_wo, C_up, P_down, then C_qkv or, after the last layer, the head
+    std::vector<Phase> phs;
+    int n_x = 0;              // exchanges so far in the program
+    float* x_sum_into = nullptr;
+    auto fill_xc = [&](XchgParams& xc, int role) {
+      xc.world = world; xc.rank = rank; xc.index = n_x; xc.n = n_embd; xc.role = role;
+      for (int r = 0; r < world; r++) xc.ll[r] = ll_of(n_x / 2, r);
+    };
+    auto push = [&](MVParams& p) {
+      p.silu_tab = tables().silu; p.gelu_tab = tables().gelu;
+      phs.push_back(matvec_phase(p));
+    };
+    auto push_xchg = [&](float* buf) { fill_xc(phs.back().xc, 2); x_sum_into = buf; };
+    auto take_input = [&](MVParams& p) {
+      p.x = (const float*)ll_of(n_x / 2, rank); p.x_mode = 2; p.x_parts = world; p.x_stride = n_embd; p.sum_out = x_sum_into;
+    };
+    auto mark_exchange = [&] { fill_xc(phs.back().xc, 1); n_x++; x_sum_into = nullptr; };
+    const float* res = dres0.as<float>();   // the residual rank 0's next producer adds
+    for (int l = 0; l < n_layers; l++) {
+      const int m = 7 * l;
+      {  // P_wo: the attention output's K range of wo (+ residual on rank 0)
+        MVParams p{};
+        p.x = dattn.as<float>() + (size_t)l * qw; p.norm_mode = NORM_NONE; p.K = qw; p.nseg = 1;
+        p.seg[0] = MVSeg{k_range_of(m, n_embd, n_embd, q0, q1), dprod.as<float>(), rank == 0 ? res : nullptr, nullptr, rank == 0 ? EPI_ADD : EPI_STORE};
+        push(p);
+        push_xchg(sums + (size_t)n_x * n_embd);
+      }
+      {  // C_up: RMSNorm of the summed vector into this rank's rows of w1 (SiLU) and w3
+        MVParams p{};
+        p.norm_w = dnorm.as<float>() + (size_t)n_x * n_embd; p.norm_mode = NORM_RMS; p.eps = eps; p.K = n_embd;
+        take_input(p);
+        float* o = outs + out_off[n_x];
+        p.nseg = 2;
+        p.seg[0] = MVSeg{rows_of(m + 1, n_embd, f0, f1), o, nullptr, nullptr, EPI_SILU};
+        p.seg[1] = MVSeg{rows_of(m + 2, n_embd, f0, f1), o + fw, nullptr, nullptr, EPI_STORE};
+        res = p.sum_out;
+        push(p);
+        mark_exchange();
+      }
+      {  // P_down: w2's K range on silu(gate) * up (+ C_up's sum on rank 0)
+        const float* gate = outs + out_off[n_x - 1];
+        MVParams p{};
+        p.x = gate; p.x2 = gate + fw; p.x_mode = 1; p.norm_mode = NORM_NONE; p.K = fw; p.nseg = 1;
+        p.seg[0] = MVSeg{k_range_of(m + 3, n_ff, n_embd, f0, f1), dprod.as<float>(), rank == 0 ? res : nullptr, nullptr, rank == 0 ? EPI_ADD : EPI_STORE};
+        push(p);
+        push_xchg(sums + (size_t)n_x * n_embd);
+      }
+      {  // C_qkv into this rank's wq / wk / wv rows, or the replicated head after the last layer
+        MVParams p{};
+        p.norm_w = dnorm.as<float>() + (size_t)n_x * n_embd; p.norm_mode = NORM_RMS; p.eps = eps; p.K = n_embd;
+        take_input(p);
+        float* o = outs + out_off[n_x];
+        if (l < n_layers - 1) {
+          p.nseg = 3;
+          p.seg[0] = MVSeg{rows_of(m + 4, n_embd, q0, q1), o, nullptr, nullptr, EPI_STORE};
+          p.seg[1] = MVSeg{rows_of(m + 5, n_embd, g0, g1), o + qw, nullptr, nullptr, EPI_STORE};
+          p.seg[2] = MVSeg{rows_of(m + 6, n_embd, g0, g1), o + qw + gw, nullptr, nullptr, EPI_STORE};
+        } else {
+          p.nseg = 1;
+          p.seg[0] = MVSeg{rows_of(m + 4, n_embd, 0, n_vocab), o, nullptr, nullptr, EPI_STORE};
+        }
+        res = p.sum_out;
+        push(p);
+        mark_exchange();
+      }
+    }
+
+    const StepLaunch L = plan_phases(phs);   // (the exchange build is never paired, whatever the plan says about pairs)
+    const std::vector<int> hb = step_bounds(phs.data(), (int)phs.size(), L.grid);
+    DevMem dbounds(hb.size() * 4), dprog((phs.size() + 1) * sizeof(Phase));
+    OPS_CUDA(cudaMemcpy(dbounds.get(), hb.data(), hb.size() * 4, cudaMemcpyHostToDevice));
+    OPS_CUDA(cudaMemcpy(dprog.get(), phs.data(), phs.size() * sizeof(Phase), cudaMemcpyHostToDevice));
+    const int* wd = watchdog_words();
+    std::vector<uint2> slot(n_embd);
+    for (int s = 0; s < steps; s++) {
+      // the peers' entries of this launch's exchanges, numbered as the kernel numbers them, in this rank's regions
+      const unsigned base = xc_base + (unsigned)s * (unsigned)n_xchg;
+      for (int k = 0; k < n_xchg; k++) {
+        const unsigned e = xc_epoch(base, k);
+        for (int r = 0; r < world; r++) {
+          if (r == rank) continue;
+          const float* v = peers[(size_t)k * world + r];
+          for (int i = 0; i < n_embd; i++) {
+            memcpy(&slot[i].x, v + i, 4);
+            slot[i].y = e;
+          }
+          OPS_CUDA(cudaMemcpy(ll_of(k / 2, rank) + ((size_t)(e & 1u) * world + r) * n_embd, slot.data(), (size_t)n_embd * 8, cudaMemcpyHostToDevice));
+        }
+      }
+      OPS_CUDA(launch_step(L, 0, dprog.as<Phase>(), dbounds.as<int>(), (int)phs.size(), dsync.as<unsigned>(), false, nullptr, true));
+      OPS_CUDA(cudaGetLastError());
+      if (cudaDeviceSynchronize() != cudaSuccess) {
+        const int* w = wd;
+        throw std::runtime_error(std::string("launch ") + std::to_string(s) + " failed: " + cudaGetErrorString(cudaGetLastError()) + "; watchdog: wait " +
+                                 std::to_string(w[0]) + " (" + WAIT_TEXT[w[0] > 0 && w[0] < W_CODES ? w[0] : 0] + ") in CTA " + std::to_string(w[1]) +
+                                 ", aux " + std::to_string(w[2]) + ", thread " + std::to_string(w[3]));
+      }
+    }
+    OPS_CUDA(cudaMemcpy(out, dout.get(), n_out * 4, cudaMemcpyDeviceToHost));
+    OPS_CUDA(cudaMemcpy(sum_out, dsum.get(), (size_t)n_xchg * n_embd * 4, cudaMemcpyDeviceToHost));
+    OPS_CUDA(cudaMemcpy(ll, dll.get(), (size_t)n_layers * world * region * 8, cudaMemcpyDeviceToHost));
+    OPS_CUDA(cudaMemcpy(sync2, dsync.as<unsigned>() + 2, 4, cudaMemcpyDeviceToHost));
+    if (launch) {
+      const StepKernel k = step_kernel(L, true);
+      launch[0] = k == k_step<true, false, false> || k == k_step<true, false, true>;
+      launch[1] = k == k_step<true, false, true> || k == k_step<false, false, true> || k == k_step<false, true, true>;
+      launch[2] = step_paired(L, true) ? 2 : 1;
+    }
   });
 }
 

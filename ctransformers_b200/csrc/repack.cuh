@@ -1,11 +1,22 @@
 // GGUF array-of-blocks → device planes (layout table in device_types.cuh).  Shared by the engine's model
 // upload and the op-level entry points.
 #pragma once
+#include <cstring>
+#include <vector>
+
 #include "device_types.cuh"
 
 namespace ctb {
 
 struct PlaneSizes { size_t qs, qh, d, mn; };
+
+// The row-parallel shard of a tensor-parallel rank (wo / w2: a K range of every row): from each of `rows` rows that lie
+// full_row_bytes apart, the row_bytes that start `off` bytes into the row, packed row after row.
+inline std::vector<uint8_t> gather_k_range(const uint8_t* src, int rows, size_t full_row_bytes, size_t off, size_t row_bytes) {
+  std::vector<uint8_t> g((size_t)rows * row_bytes);
+  for (int r = 0; r < rows; r++) memcpy(g.data() + (size_t)r * row_bytes, src + (size_t)r * full_row_bytes + off, row_bytes);
+  return g;
+}
 
 inline PlaneSizes plane_sizes(int type, int M, int nb, size_t raw_bytes) {
   const size_t nblk = (size_t)M * nb;

@@ -636,6 +636,9 @@ struct XchgParams {
   int role;                            // 0 none, 1 this phase consumes the exchange (sums it while staging), 2 it produces it
   uint2* ll[XC_MAX_WORLD];             // region base of every rank as mapped here
 };
+// The number an element of exchange `index` (0-based inside the program) carries in a launch that starts after `base` exchanges
+// (StepArgs::sync[2]); its parity half of the regions is the number's low bit.  The numbers wrap past 2^32 without a break.
+__host__ __device__ inline unsigned xc_epoch(unsigned base, int index) { return base + (unsigned)index + 1u; }
 struct PickParams { const float* logits; int* state; int* out_tokens; int n; };
 struct alignas(16) Phase {
   int kind;
@@ -898,7 +901,7 @@ __device__ __forceinline__ void st_matvec_phase(const Phase& ph, const NormPre& 
                                                 unsigned xc_base, PairX& px) {
   const MVParams& p = ph.mv;
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const unsigned epoch = XC ? xc_base + (unsigned)ph.xc.index + 1u : 0u;   // number of the exchange this phase consumes / produces (if any)
+  const unsigned epoch = XC ? xc_epoch(xc_base, ph.xc.index) : 0u;   // number of the exchange this phase consumes / produces (if any)
   if constexpr (PAIR) stage_q8k_pair<ST_NT, ST_BAR>(p, np, act_smem, red, px, blockIdx.x < 2);
   else stage_activation<ST_NT, ST_BAR, XC>(p, np, ACT_Q8_K, act_smem, red, blockIdx.x == 0, epoch);
   StAct a = st_act_extras<ST_NT, ST_BAR>(act_smem, p.K, ph.q6 != 0);

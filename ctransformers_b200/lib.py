@@ -89,6 +89,8 @@ EXTRA_PROTOTYPES = {
                                       C.c_int, _P]),
     "ctb_decode_mul_mat": (C.c_int, [C.c_int, _P, _P, _P, C.c_int, C.c_int, _P, _P, C.c_int, _P, _P, C.c_float, _P, _P, _P, _P, _P, C.c_int,
                                      _P]),
+    "ctb_xchg_mul_mat": (C.c_int, [C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, _P, _P, _P, _P, _P, C.c_float, _P,
+                                   C.c_uint, C.c_int, _P, _P, _P, _P, _P]),
     "ctb_llm_paths": (C.c_long, [_P, _IP, C.c_int]),
     "ctb_llm_step_cluster": (C.c_int, [_P]),
     "ctb_ffn_gate": (C.c_int, [C.c_int, _P, _P, _P, _P, C.c_int, C.c_int]),

@@ -198,6 +198,34 @@ int ctb_prefill_mul_mat(int nseg, const int* types, const void* const* w_blocks,
 int ctb_decode_mul_mat(int nseg, const int* types, const void* const* w_blocks, const int* rows, int K, int n_tok, const float* x,
                        const float* x2, int norm_mode, const float* norm_w, const float* norm_b, float eps, const int* epi,
                        const float* res, const float* res2, float* out, float* norm_out, int repeat, int* launch);
+/* One rank's side of the tensor-sharded mode's fused exchange (DESIGN.md §8), on one GPU: rank `rank` of `world` (2..8) runs
+ * n_layers of the mat-vec phases of a fused tensor-parallel Llama layer, attention left out, through the exchange build of the
+ * step kernel (k_step<true, ...>), programmed and numbered as the engine programs it:
+ *   P_wo    producer: this rank's attention slice attn[l] by wo's K range (+ the residual on rank 0)
+ *   C_up    consumer: RMSNorm of the rank-order sum of every rank's P_wo rows, into this rank's rows of w1 (SiLU table) and w3
+ *   P_down  producer: w2's K range by silu(gate) * up (+ C_up's sum on rank 0)
+ *   C_qkv   consumer: RMSNorm of the P_down sum into this rank's rows of wq / wk / wv; after the last layer the head instead
+ * Shards as tp_shard cuts them (ctb_tp_shard).  The matrices are given whole, n_mats = 7·n_layers - 2 of them, entry 7·l + {0 wo
+ * [n_embd x n_embd], 1 w1 [n_ff x n_embd], 2 w3, 3 w2 [n_embd x n_ff], 4 wq [n_embd x n_embd], 5 wk [n_head_kv·hd x n_embd],
+ * 6 wv} of layer l, where layer n_layers - 1 has the head [n_vocab x n_embd] at entry 4 and no 5, 6; types[n_mats] K-quant only.
+ *   attn      [n_layers][this rank's query width]; res0 [n_embd]: the residual of the first P_wo
+ *   norm_w    [2·n_layers][n_embd]: the RMSNorm weight of each consumer, in program order; eps its epsilon
+ *   peers     [2·n_layers · world] pointers: peers[k·world + r] = rank r's partial vector [n_embd] of exchange k (entries of
+ *             `rank` itself are not read); before each launch they are written with that launch's exchange numbers
+ *             (xc_epoch) into the peers' slots of this rank's regions
+ *   xc_base   the exchange count the first launch starts from (the step kernel's sync[2]); steps >= 1 launches back to back,
+ *             each continuing the numbers of the one before
+ * Outputs of the last launch: out = every consumer's segments side by side (C_up: silu(w1) then w3 rows; C_qkv: wq, wk, wv rows;
+ * the head's rows); sum_out [2·n_layers][n_embd] = each consumer's summed input; ll = the regions as uint32 pairs {float bits,
+ * exchange number}, [n_layers][world][2][world][n_embd][2]: region R of the layer's two exchanges, parity half, slot of each
+ * rank (each layer has its own regions: one launch cannot wait for a peer to overwrite its slots); sync2 = sync[2] after the
+ * run; launch [3] (may be null) = {exchange build, Q3_K build, CTAs per cluster}.
+ * 0 on success; -1 (with a message on stderr, before anything reaches the GPU) for a world outside 2..8 or rank >= world, a
+ * matrix that is not K-quant, a shard tp_shard refuses or one that leaves a rank without heads or whole KV groups, a K range
+ * off 256-element blocks, a missing matrix or peer vector, n_layers or steps below 1. */
+int ctb_xchg_mul_mat(int world, int rank, int n_embd, int n_head, int n_head_kv, int n_ff, int n_vocab, int n_layers, const int* types,
+                     const void* const* w_blocks, const float* attn, const float* res0, const float* norm_w, float eps, const float* const* peers,
+                     unsigned xc_base, int steps, float* out, float* sum_out, unsigned* ll, unsigned* sync2, int* launch);
 /* silu(W1 x) * (W3 x) with the fp16 SiLU table (ggml.c:3625-3632) — the fused FFN gate. */
 int ctb_ffn_gate(int type, const void* w1_blocks, const void* w3_blocks, const float* x, float* out, int K, int M);
 /* ggml_get_rows on a quantized table (ggml.c:11615-11642). */
